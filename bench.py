@@ -1,12 +1,18 @@
 """bench.py -- BASELINE metric: 64x64 images/sec, IAN_simple encode -> decode @ batch 256 (fp32 semantics),
 plus latent-edit steps/sec as a secondary block.  Contract: see the task statement / DESIGN.md section 5.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--global-batch G]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--global-batch G] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Default: weak scaling, 256 images per GPU (BASELINE configs[1] on every GPU).  `--global-batch G` shards a FIXED global
 batch (BASELINE configs[4]: 4096) over the ranks (strong scaling); the default run also reports that configuration as
-the secondary block `config5`, so the driver's 1/2/4/8-GPU runs carry the same-global-batch curve.
+the secondary block `config5`, so 1/2/4/8-GPU runs carry the same-global-batch curve.
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step (seeded inputs: identical from run to
+run) as DIR/z.npy (latents, float32) and DIR/xhat.npy (decoded images, float32), so two builds can be compared output
+for output.  Both hold the whole batch in the same sample order (at N > 1 the gathered batch of all ranks).  When the
+two together would exceed 64 MB, both keep the same fixed sample of rows: dump_rows() below, a seeded choice that depends
+only on the batch size.
 """
 from __future__ import annotations
 
@@ -36,55 +42,55 @@ EDGE_KERNELS = ("enc_conv1", "dec_out")
 # algorithmic HBM bytes per image of the two HBM-bound end kernels: x in + a1 planes out / h3 planes in + x_hat out
 EDGE_BYTES_PER_IMAGE = {"enc_conv1": 49152 + 32 * 32 * 128 * 4, "dec_out": 32 * 32 * 128 * 4 + 49152}
 CONFIG5_GLOBAL = 4096            # BASELINE configs[4]
-NCU_SUMMARY = os.path.join(ROOT, "profiles", "r2_ncu_tc_kernels_full_summary.csv")
 METRIC = "64x64 images/sec IAN encode->decode @ batch 256"
+DUMP_MAX_BYTES = 64 << 20       # --dump-outputs: the arrays of one dump together stay within this
+DUMP_SEED = 20240917
+
+
+def dump_rows(n, bytes_per_row, max_bytes=DUMP_MAX_BYTES):
+    """Rows of an n-sample batch that --dump-outputs writes: all of them when they fit in max_bytes, else a fixed sample
+    of the largest count that fits -- np.random.default_rng(DUMP_SEED).choice(n, k, replace=False), sorted -- which
+    depends only on n, so two builds (or two runs) dump the same samples."""
+    k = min(n, max_bytes // bytes_per_row)
+    if k == n:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(DUMP_SEED).choice(n, k, replace=False))
+
+
+def write_dump(directory, arrays, max_bytes=DUMP_MAX_BYTES):
+    """arrays: name -> numpy array, all with the batch as first dimension; written as float32 directory/<name>.npy"""
+    arrays = {k: np.asarray(v, dtype=np.float32) for k, v in arrays.items()}
+    n = next(iter(arrays.values())).shape[0]
+    rows = dump_rows(n, sum(a[0].nbytes for a in arrays.values()), max_bytes)
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a[rows])
+    return rows
 
 
 def peaks():
+    """Roofline denominators: MEASURED_PEAKS.json beside this file when a peak measurement of this machine is present,
+    else NVIDIA's data-sheet figures for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16.  Data-sheet rates
+    are not reached under a lower power limit; `clocks` and `gpu` in the result line say what the card ran at."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback"}
-
-
-def ncu_traffic(kernel_substr, launches_per_step):
-    """dram__bytes_read + dram__bytes_write of the first `launches_per_step` launches whose kernel name contains
-    `kernel_substr`, from the committed `ncu --set full` summary of this same command (tools/ncu_summary.py); None if the
-    file is absent.  Not a measurement of the run that prints it -- the file it came from is named beside it."""
-    import csv
-    if not os.path.exists(NCU_SUMMARY):
-        return None
-    rows = list(csv.reader(open(NCU_SUMMARY)))
-    hdr = rows[0]
-    try:
-        kn = [i for i, h in enumerate(hdr) if h.startswith("Kernel Name")][0]
-        rd = [i for i, h in enumerate(hdr) if h.startswith("dram__bytes_read.sum")][0]
-        wr = [i for i, h in enumerate(hdr) if h.startswith("dram__bytes_write.sum")][0]
-    except IndexError:
-        return None
-    scale = {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}
-    unit_r = hdr[rd].split("[")[-1].rstrip("]")
-    unit_w = hdr[wr].split("[")[-1].rstrip("]")
-    tot, n = 0.0, 0
-    for r in rows[1:]:
-        if kernel_substr in r[kn] and n < launches_per_step:
-            tot += float(r[rd]) * scale.get(unit_r, 1.0) + float(r[wr]) * scale.get(unit_w, 1.0)
-            n += 1
-    return tot if n == launches_per_step else None
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe): one
-    background `nvidia-smi -lms 20` process; samples are selected by wall-clock window."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region: one background `nvidia-smi -lms 20` query process
+    (stopped by summary() or, whatever happens, at interpreter exit); samples are selected by wall-clock window."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
 
     def __init__(self, index):
-        self.path = "/tmp/ian_clocks_%d_%d.csv" % (os.getpid(), index)
-        self.f = open(self.path, "w")
+        import tempfile
+        fd, self.path = tempfile.mkstemp(prefix="ian_clocks_%d_" % index, suffix=".csv")
+        self.f = os.fdopen(fd, "w")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(index), "--query-gpu=" + self.Q,
                                           "--format=csv,noheader,nounits", "-lms", "20"], stdout=self.f,
@@ -92,6 +98,16 @@ class ClockSampler:
         except Exception:
             self.proc = None
         self.t0 = self.t1 = None
+        import atexit
+        atexit.register(self._stop_proc)
+
+    def _stop_proc(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            try:
+                self.proc.wait(timeout=5)
+            except Exception:
+                self.proc.kill()
 
     def start(self):
         self.t0 = time.time()
@@ -103,11 +119,7 @@ class ClockSampler:
         import datetime
         if self.proc is not None:
             time.sleep(0.05)
-            self.proc.terminate()
-            try:
-                self.proc.wait(timeout=5)
-            except Exception:
-                self.proc.kill()
+        self._stop_proc()
         self.f.close()
         rows_all, rows_in = [], []
         for line in open(self.path):
@@ -138,6 +150,18 @@ class ClockSampler:
                 "power_w_max": max(r[2] for r in rows) if rows else None,
                 "reasons": sorted(reasons), "samples": len(rows),
                 "window": "timed region" if rows_in else "whole run (timed region shorter than the sampling period)"}
+
+
+def gpu_info(index):
+    """name and power limit of the card the numbers were measured on (they belong beside every absolute figure)"""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out)
+    except Exception:
+        pass
+    return info
 
 
 def _cpu_setup():
@@ -238,6 +262,9 @@ def main():
     ap.add_argument("--no-edit", action="store_true")
     ap.add_argument("--no-full", action="store_true", help="skip the full-IAN (BASELINE configs[2]) block")
     ap.add_argument("--no-config5", action="store_true", help="skip the global-batch-4096 block (BASELINE configs[4])")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write z.npy and xhat.npy of the last timed step into DIR (the whole batch, gathered over the ranks at "
+                         "N>1; a fixed seeded row sample when both would exceed 64 MB)")
     ap.add_argument("--gather", default="p2p_async", choices=["p2p_async", "p2p", "nccl"],
                     help="N>1: p2p_async = decoded shard pushed to the peers on a side stream (copy engines + stream memory "
                          "operations; IAN_PUSH=kernel: a copy kernel) while the next step computes (default); p2p = peer stores fused into the dec_out kernel; nccl = separate NCCL all_gather")
@@ -307,19 +334,30 @@ def main():
                 gather_mode = "nccl"
                 check = "p2p setup failed: %s" % (str(e)[:120],)
 
+        last = {}                                           # what the most recent step produced: local z, (gathered) images
+
         def step():
             if world > 1 and gather_mode == "p2p_async":
                 model.reconstruct_gather_async_dev(x.data_ptr(), n_local, z.data_ptr(), stream)
             elif world > 1 and gather_mode == "p2p":
-                model.reconstruct_gather_dev(x.data_ptr(), n_local, z.data_ptr(), stream)
+                last["ptr"] = model.reconstruct_gather_dev(x.data_ptr(), n_local, z.data_ptr(), stream)
             else:
                 model.reconstruct_dev(x.data_ptr(), n_local, z.data_ptr(), xhat.data_ptr(), stream)
                 if world > 1:
-                    par.gather_images(xhat, global_n)       # the one collective of the path (north_star), via NCCL
+                    last["gathered"] = par.gather_images(xhat, global_n)   # the one collective of the path, via NCCL
 
         def finish():
             if world > 1 and gather_mode == "p2p_async":
-                model.gather_wait_dev(stream)               # the last step's gather must land inside the timed region
+                last["ptr"] = model.gather_wait_dev(stream)   # the last step's gather must land inside the timed region
+
+        def outputs():                                      # every rank calls this (the z gather is a collective)
+            if world == 1:
+                return {"z": z, "xhat": xhat}
+            if "ptr" in last:
+                images = par.as_cuda_tensor(last["ptr"], (global_n, 3, 64, 64), dev)
+            else:
+                images = last["gathered"]
+            return {"z": par.gather_images(z, global_n), "xhat": images}
 
         for _ in range(warmup):
             step()
@@ -339,7 +377,7 @@ def main():
             sampler.stop()
         launches = model.launch_count() - l0
         (ms,) = max_over_ranks(e0.elapsed_time(e1))
-        return ms, launches, check, gather_mode, step, x
+        return ms, launches, check, gather_mode, step, outputs()
 
     strong = args.global_batch > 0
     global_n = args.global_batch if strong else BATCH * world
@@ -351,9 +389,12 @@ def main():
     torch.cuda.synchronize()
 
     sampler = ClockSampler(local_rank)
-    ms, launches, gather_check, gather_mode, step, x = timed_job(model, n_local, global_n, 1234, args.steps, args.warmup,
-                                                                 args.gather if world > 1 else "none", sampler)
+    ms, launches, gather_check, gather_mode, step, outs = timed_job(model, n_local, global_n, 1234, args.steps, args.warmup,
+                                                                    args.gather if world > 1 else "none", sampler)
     value = global_n * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:                     # before anything else runs on these buffers
+        write_dump(args.dump_outputs, {name: t.float().cpu().numpy() for name, t in outs.items()})
+    del outs
 
     # ---- roofline of the dominant kernel (tap-GEMM), CUDA events on the launch stream, same loop
     model.set_layer_timing(True)
@@ -371,7 +412,6 @@ def main():
     achieved = tg_flops / (tg_ms / 1e3) / 1e12 if tg_ms > 0 else 0.0
     peak_burst, peak_sust = pk["bf16_tflops"] / 3.0, pk["bf16_tflops_sustained"] / 3.0
     timed_region_ms = ms
-    traffic = ncu_traffic("tapgemm_tc", len(TAPGEMM_LAYERS)) if (n_local == BATCH and world == 1) else None
     hbm = pk["hbm_gbs"]
     edge_roof = {k: {"ms": round(edge_ms[k], 4), "algorithmic_mb": round(EDGE_BYTES_PER_IMAGE[k] * per_launch_imgs / 1e6, 1),
                      "achieved_gbs": round(EDGE_BYTES_PER_IMAGE[k] * per_launch_imgs / (edge_ms[k] / 1e3) / 1e9, 1),
@@ -387,8 +427,6 @@ def main():
                              "bf16 split, so one algorithmic MAC costs 3 tensor-core MACs" % (pk["src"], pk["bf16_tflops"], pk["bf16_tflops_sustained"]),
                 "tensor_executed_tflops": 3 * achieved, "kernel_ms_per_step": tg_ms,
                 "algorithmic_flop_per_step": tg_flops,
-                "traffic": traffic, "traffic_unit": "bytes per step, dram read+write summed over the 9 tap-GEMM launches",
-                "traffic_src": os.path.relpath(NCU_SUMMARY, ROOT) if traffic is not None else None,
                 "traffic_algorithmic": 943.0e6 if n_local == BATCH else None,
                 # share among the kernels event-timed in this same pass (tap-GEMMs + enc_conv1 + dec_out)
                 "kernel_share_of_step": tg_ms / (tg_ms + chunks * sum(v for v in edge_ms.values() if v > 0)),
@@ -549,7 +587,7 @@ def main():
                          "layer_ms": {k: round(fm.layer_time_ms(k), 4) for k in names}}
         diff = (outs["bf16"] - outs["fp32"]).abs()
         full = {"metric": "64x64 images/sec full IAN (IAN.py) encode->decode @ batch 512 (BASELINE configs[2])",
-                "unit": "images/sec", "value": res["bf16"]["value"], "dtype": "bf16 operands, fp32 accumulate (single tcgen05 pass)",
+                "unit": "images/sec", "value": res["bf16"]["value"], "dtype": "bf16 operands, fp32 accumulate (single wgmma pass)",
                 "bf16": res["bf16"], "fp32_split": res["fp32"],
                 "bf16_vs_fp32_max_abs": float(diff.max().item()), "bf16_vs_fp32_mean_abs": float(diff.mean().item()),
                 "bf16_vs_fp32_psnr_db": _psnr(outs["bf16"], outs["fp32"])}
@@ -563,11 +601,11 @@ def main():
         line = {"metric": METRIC, "value": value, "unit": "images/sec", "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
                 "scaling": "strong" if strong else "weak",
-                "vs_baseline": None, "dtype": "f32 (3-pass bf16 split on tcgen05, fp32 accumulate)", "data": "synthetic",
+                "vs_baseline": None, "dtype": "f32 (3-pass bf16 split on wgmma, fp32 accumulate)", "data": "synthetic",
                 "config": {"workload": ("IAN_simple encode->decode, global batch %d sharded over the ranks (BASELINE configs[4])" % global_n)
                            if strong else "IAN_simple encode->decode, batch 256 per GPU (BASELINE configs[1])",
                            "global_batch": global_n, "per_gpu": n_local, "parallelism": "dp%d" % world,
-                           "l2": "no flush: one step streams 211 MB of weights + ~1 GB of activations (> 126 MB L2)",
+                           "l2": "no flush: one step streams 211 MB of weights + ~1 GB of activations (> 50 MB L2)",
                            "collective": {"none": "none", "nccl": "NCCL all_gather of decoded images after dec_out",
                                           "p2p": "all-gather fused into dec_out: st.global to every rank's buffer over NVLink "
                                                  "peer memory + flag barrier",
@@ -576,7 +614,7 @@ def main():
                                                        "the last step's gather completes inside the timed region"}[gather_mode],
                            "gather_check_max_abs_vs_nccl": gather_check},
                 "tflops_algorithmic": value * GFLOP_PER_IMAGE / 1e3, "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e,
-                "gpu_launches": launches, "clocks": sampler.summary(), "config5": config5, "edit": edit, "full_ian": full,
+                "gpu_launches": launches, "clocks": sampler.summary(), "gpu": gpu_info(local_rank), "config5": config5, "edit": edit, "full_ian": full,
                 "single_image_latency": lat}
         print(json.dumps(line), flush=True)
     model.close()

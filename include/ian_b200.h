@@ -1,5 +1,5 @@
 /*
- * ian_b200.h -- C-ABI of libian_b200.so: the B200-native (sm_100a) implementation of the IAN hot path
+ * ian_b200.h -- C-ABI of libian_b200.so: the H100-native (sm_90a) implementation of the IAN hot path
  * of ajbrock/Neural-Photo-Editor.
  *
  * The reference has NO native boundary for this path: its contract is the Python class API.IAN
@@ -21,14 +21,12 @@
  *   - results are reproducible: a call repeated with the same batch size returns the same bits (split-K and
  *     stream-K partial sums are added in a fixed order; there are no atomics on the path).
  *   - environment, read by ian_create: IAN_CHUNK=<n> images per internal chunk (default 512); IAN_PATH=simt selects
- *     the FFMA verification kernels; IAN_STREAMK=0 disables stream-K scheduling; IAN_GRAPHS=0 disables the CUDA-graph
- *     replay that *_host calls with <= 32 images use; IAN_TC2=0 keeps every layer on the one-CTA tap-GEMM kernel
- *     (default: layers with >= IAN_TC2_MIN (37) whole pair-tiles run on CTA pairs, tcgen05 cta_group::2);
- *     IAN_TC2_SKIP=<layer,layer> exempts layers; IAN_TC2_BF16=0 keeps bf16-mode layers off the 256x256 pair tiles;
+ *     the FFMA verification kernels; IAN_STREAMK=0 disables stream-K scheduling, IAN_STREAMK=2 uses it on every eligible
+ *     launch (tests); IAN_GRAPHS=0 disables the CUDA-graph replay that *_host calls with <= 32 images use;
  *     IAN_SPLITK=0 disables split-K (tests); IAN_PUSH=kernel makes the pipelined all-gather push with a copy kernel
  *     (IAN_PUSH_CTAS=<n> CTAs) instead of copy engines + stream memory operations; IAN_PDL=0 launches the kernel chains
- *     plainly instead of with programmatic dependent launch; IAN_TC2_SPLITK=0 / IAN_TC2_OVER_SPLIT=0 / IAN_FINALIZE8=0 choose
- *     the older split-K forms.  All of these select schedules or launch forms of the same kernels (DESIGN.md section 5.8);
+ *     plainly instead of with programmatic dependent launch; IAN_FINALIZE8=0 chooses the one-thread split-K finalize.
+ *     All of these select schedules or launch forms of the same kernels (DESIGN.md section 5.8);
  *     results do not depend on IAN_GRAPHS, IAN_PDL or IAN_FINALIZE8 (bit-identical), the others change float32 summation
  *     order within the tolerances of the parity tests.
  *   - stream semantics of *_dev calls: kernels of one call are chained with programmatic dependent launch among themselves;
@@ -66,7 +64,7 @@ typedef enum ian_model_kind {
 
 /* Compute path of the dense contractions (enc_conv2-4, dec_conv1-3, fully-connected layers).
  * Both are CUDA on the GPU; there is no CPU path.
- *   IAN_PATH_TC   : tcgen05 tensor-core kernels, fp32 emulated by a 3-pass bf16 split (default)
+ *   IAN_PATH_TC   : wgmma tensor-core kernels, fp32 emulated by a 3-pass bf16 split (default)
  *   IAN_PATH_SIMT : fp32 FFMA kernels (verification path, bit-for-bit independent of IAN_PATH_TC) */
 typedef enum ian_path { IAN_PATH_TC = 0, IAN_PATH_SIMT = 1 } ian_path;
 

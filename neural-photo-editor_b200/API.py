@@ -1,4 +1,4 @@
-"""Plat-style model API of the Neural Photo Editor, backed by libian_b200.so (sm_100a CUDA).
+"""Plat-style model API of the Neural Photo Editor, backed by libian_b200.so (sm_90a CUDA).
 
 Drop-in for the reference `API.py` (reference API.py:11-110): same class name, constructor signature
 and method surface (`encode_images`, `sample_at`, `get_zdim`, `imgrad`, `imgradRGB`, attributes `cfg`,
@@ -179,7 +179,7 @@ class IAN:
             pass
 
     def set_path(self, path):
-        """'tc' (tcgen05, default) or 'simt' (fp32 FFMA verification path); both are CUDA."""
+        """'tc' (wgmma tensor cores, default) or 'simt' (fp32 FFMA verification path); both are CUDA."""
         self._check(self._lib.ian_set_path(self._h, {'tc': _lib.IAN_PATH_TC, 'simt': _lib.IAN_PATH_SIMT}[path]))
 
     def set_precision(self, precision):

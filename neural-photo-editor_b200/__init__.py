@@ -1,4 +1,4 @@
-"""neural-photo-editor_b200: B200-native (sm_100a) implementation of the IAN hot path of
+"""neural-photo-editor_b200: H100-native (sm_90a) implementation of the IAN hot path of
 ajbrock/Neural-Photo-Editor behind the reference's own API.IAN surface.
 
     import importlib; npe = importlib.import_module("neural-photo-editor_b200")

@@ -1,12 +1,12 @@
 """ctypes binding of libian_b200.so (C-ABI: include/ian_b200.h).  No CPU fallback: if the library is
-missing or no sm_100 GPU is present, construction fails loudly."""
+missing or no sm_90 (H100) GPU is present, construction fails loudly."""
 from __future__ import annotations
 
 import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# IAN_B200_LIB: another in-tree BUILD of the same sources/ABI (tools/r2_ab.sh compares two builds on one box); the
+# IAN_B200_LIB: another in-tree BUILD of the same sources/ABI (to compare two builds in one process run); the
 # default is the library build.py produces.  It is never a different implementation: there is no fallback.
 LIB_PATH = os.environ.get("IAN_B200_LIB") or os.path.join(HERE, "libian_b200.so")
 

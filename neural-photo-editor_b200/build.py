@@ -1,9 +1,9 @@
-"""Build libian_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libian_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python neural-photo-editor_b200/build.py [--force]
 
 Every .cu is compiled to its own object (in parallel, only when stale) and the objects are linked into the shared
-library; objects live under csrc/_obj/ (git-ignored; they travel to the GPU box with the .so so nothing rebuilds there).
+library; objects live under csrc/_obj/ (git-ignored), so a rebuild only recompiles what changed.
 """
 from __future__ import annotations
 
@@ -13,12 +13,13 @@ import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = ["ian_api.cu", "tapgemm_simt.cu", "tapgemm_tc.cu", "tapgemm_tc2.cu", "decout_tc.cu", "conv1_tc.cu", "edge_kernels.cu",
+SRC = ["ian_api.cu", "tapgemm_simt.cu", "tapgemm_tc.cu", "decout_tc.cu", "conv1_tc.cu", "edge_kernels.cu",
        "head_tc.cu", "train_kernels.cu"]
 HDR = ["tapgemm.h", "edge.h", "tc_ptx.cuh", "../../include/ian_b200.h"]
 LIB = os.path.join(HERE, "libian_b200.so")
 OBJ_DIR = os.path.join(HERE, "csrc", "_obj")
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-O3", "-std=c++17"] + ARCH + ["-lineinfo",
               "-Xcompiler", "-fPIC"]
 
 
@@ -52,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=max(1, min(len(todo), os.cpu_count() or 1))) as ex:
         list(ex.map(cc, todo))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+    cmd = [nvcc, "-shared"] + ARCH + ["-o", LIB] + objs
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.run(cmd, check=True)
@@ -65,7 +66,7 @@ C_HOST_BIN = os.path.join(HERE, "..", "examples", "c_host", "ian_cli")
 
 def build_c_host(force: bool = False) -> str:
     """the plain-C host program over the C-ABI (examples/c_host): strict C99 against include/ian_b200.h, linked to
-    the in-tree library with an $ORIGIN-relative rpath so it runs from the snapshot on the GPU box."""
+    the in-tree library with an $ORIGIN-relative rpath so it runs from wherever the tree is copied."""
     lib = build()
     deps = [C_HOST_SRC, os.path.join(HERE, "..", "include", "ian_b200.h"), lib]
     if not force and os.path.exists(C_HOST_BIN) and all(os.path.getmtime(d) <= os.path.getmtime(C_HOST_BIN) for d in deps):

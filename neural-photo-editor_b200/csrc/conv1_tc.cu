@@ -4,20 +4,19 @@
 // K = 3*25 = 75 is too thin for a TMA-fed tap GEMM (the input has 3 channels, not a multiple of 64), so the im2col
 // tile is built by threads: 16 producer warps stage the 11 x 67 x 3 float32 input patch of a 4-row x 32-column output
 // tile in shared memory, expand it to the 128 x 80 (K padded) operand, split every value into bf16 hi|lo and write it
-// straight into the 128B-swizzled K-major layout tcgen05 reads (the same layout TMA would produce), then
-// fence.proxy.async + mbarrier hand it to the MMA warp.  Weights (128 x 80, hi|lo) are TMA-loaded once per CTA.
-// 15 MMAs per tile (5 K-slices x 3 passes), two TMEM accumulator buffers, epilogue = bias + LReLU + re-split.
-// Roles: warp 0 weight TMA, warp 1 MMA, warps 2-9 epilogue, warps 10-25 im2col (four threads per operand row).
+// straight into the 128B-swizzled K-major layout wgmma reads (the same layout TMA would produce), then
+// fence.proxy.async + mbarrier hand it to the consumers.  Weights (128 x 80, hi|lo) are TMA-loaded once per CTA.
+// Roles: warps 0-7 two consumer warpgroups (64 operand rows each; per 64-channel half of the output 15 wgmma = 5 K-slices
+// x 3 passes into main|cross register accumulators, then the epilogue = bias + LReLU + re-split), warps 8-15 im2col
+// (two threads per operand row and quarter pair).
 //
 // Operand layout: K = 80 is one 64-wide chunk (hi plane, lo plane) plus a 16-wide tail.  The tail's hi AND lo slices share
 // ONE 128-byte-row plane (hi at K-slice position 0, lo at position 1: a K = 16 slice is just a +32 B start offset in the
 // descriptor), so a stage is 48 KB instead of 64 KB -- which pays for the output staging below.
 //
-// Output: the 128 pixels x 128 channels of a tile are 32 KB CONTIGUOUS per plane in the NHWC activation.  Round 2's
-// first form stored them from registers, 16 B per lane at a 256 B stride: ncu showed 16 of 32 bytes used per sector, the
-// L1 store path 65 % busy and every role (producers' LDS/STS included) queueing behind it ("stall_mio").  Now the
-// epilogue writes the tile into four 128B-swizzled staging tiles in shared memory (conflict-free 16-byte stores) and one
-// thread per half issues two TMA stores: no global store instruction is left in the kernel.
+// Output: the 128 pixels x 128 channels of a tile are 32 KB CONTIGUOUS per plane in the NHWC activation.  The epilogue
+// writes the tile into four 128B-swizzled staging tiles in shared memory and one thread issues four TMA stores: whole
+// lines leave the SM and no global store instruction is left in the kernel.
 #include <cstdio>
 #include <cstring>
 
@@ -37,8 +36,8 @@ namespace {
 
 using namespace tc;
 
-constexpr int kProducers = 512;
-constexpr int kThreads = 320 + kProducers;
+constexpr int kProducers = 256;
+constexpr int kThreads = 256 + kProducers;
 constexpr int kChunkPlane = 128 * 64 * 2;          // one 128-row x 64-k bf16 plane: 16 KB
 constexpr int kAStage = 3 * kChunkPlane;           // k 0..63 hi | k 0..63 lo | tail plane (hi, lo slices): 48 KB
 constexpr int kBBytes = 3 * kChunkPlane;           // weights, same three blocks x 128 rows: 48 KB
@@ -47,7 +46,7 @@ constexpr int kPatchRows = 11, kPatchCols = 67;    // input rows 2*p0-2 .. 2*p0+
 constexpr int kPatchFloats = 3 * kPatchRows * kPatchCols;
 constexpr int kPatchBytes = (kPatchFloats * 4 + 15) / 16 * 16;
 // no alignment slack: the kernel has no static shared memory, so the dynamic window starts 1024-aligned (the kernel traps
-// if it ever does not); 227 KB per CTA minus the 1 KB the toolchain reserves per block on sm_100
+// if it ever does not); 227 KB per CTA minus 1 KB of margin
 constexpr int kSmemBytes = 2 * kAStage + kBBytes + kOutBytes + 2 * kPatchBytes + 128 + 512;   // + barriers + staged bias
 static_assert(kSmemBytes <= 232448 - 1024, "conv1_tc: shared memory budget");
 constexpr int kTilesPerImage = 8;                  // 32 output rows / 4
@@ -85,7 +84,8 @@ __device__ __forceinline__ void put_unit(uint8_t* stage, const float* patch, int
   }
 }
 
-// the 10 sixteen-byte units (K = 80) of an operand row are split 3 | 3 | 2 | 2 over the row's four producer threads
+// the 10 sixteen-byte units (K = 80) of an operand row are split into quarters 3 | 3 | 2 | 2; a producer thread builds
+// quarters q and q + 2 of its row
 __device__ __forceinline__ void build_quarter(int quarter, uint8_t* stage, const float* patch, int m, int r, int c) {
   if (quarter == 0) {
     put_unit<0>(stage, patch, m, r, c); put_unit<8>(stage, patch, m, r, c); put_unit<16>(stage, patch, m, r, c);
@@ -109,12 +109,9 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
   const uint32_t bar_base = p_base + 2 * kPatchBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (2 + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (4 + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (6 + b); };
-  const uint32_t b_bar = bar_base + 64u, tmem_slot = bar_base + 72u;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_al + (tmem_slot - smem_base));
+  const uint32_t b_bar = bar_base + 64u;
   float* bias_s = reinterpret_cast<float*>(smem_al + (bar_base + 128u - smem_base));   // 128 floats, 16-byte aligned
-  if (threadIdx.x < 128) bias_s[threadIdx.x] = __ldg(bias + threadIdx.x);   // the epilogue reads it 2048 times per thread
+  if (threadIdx.x < 128) bias_s[threadIdx.x] = __ldg(bias + threadIdx.x);   // the epilogue reads it for every tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total = n_img * kTilesPerImage;
@@ -123,139 +120,98 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
     pdl_trigger();                                      // tapgemm.h: PDL
     for (int s = 0; s < 2; ++s) {
       mbar_init(full_bar(s), kProducers / 32);
-      mbar_init(empty_bar(s), 1);
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);
+      mbar_init(empty_bar(s), 2);                       // one arrival per consumer warpgroup
     }
     mbar_init(b_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
-    if (lane == 0) {                                    // weights, once: three 16 KB blocks in one box (constants: no pdl_wait)
+  if (warp < 8) {
+    // ======= consumers: wgmma per channel half, bias + LeakyRectify(0.2) + hi|lo re-split -> swizzled staging -> TMA store =======
+    const int wg = warp >> 2, wtid = threadIdx.x & 127;
+    const bool issuer = threadIdx.x == 0;
+    if (issuer) {                                       // weights, once: three 16 KB blocks in one box (constants: no pdl_wait)
       mbar_expect_tx(b_bar, kBBytes);
       tma_load_3d(&maps.b, b_bar, b_base, 0, 0, 0);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp in uniform control flow; one elected lane issues) =====================
-    {
-      constexpr uint32_t idesc = make_idesc_bf16_m128(128);
-      mbar_wait(b_bar, 0);
-      uint32_t t = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++t) {
-        const uint32_t s = t & 1u, use = t >> 1;
-        const uint32_t acc_main = tmem_base + s * 256, acc_cross = acc_main + 128;
-        mbar_wait(tempty_bar(s), (use & 1u) ^ 1u);
-        mbar_wait(full_bar(s), use & 1u);
-        tc_fence_after();
-        const uint32_t sa = a_base + s * kAStage;
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int ks = 0; ks < 5; ++ks) {              // K = 80: slices 0..3 of the 64-wide chunk, then the tail
-            const bool tail = ks == 4;
-            const uint64_t ko = (uint64_t)((ks & 3) * 2);   // a K = 16 slice is 32 B = 2 descriptor address units
-            const uint64_t a_hi = tail ? make_sw128_desc(sa + 2 * kChunkPlane) : make_sw128_desc(sa) + ko;
-            const uint64_t a_lo = tail ? make_sw128_desc(sa + 2 * kChunkPlane) + 2 : make_sw128_desc(sa + kChunkPlane) + ko;
-            const uint64_t b_hi = tail ? make_sw128_desc(b_base + 2 * kChunkPlane) : make_sw128_desc(b_base) + ko;
-            const uint64_t b_lo = tail ? make_sw128_desc(b_base + 2 * kChunkPlane) + 2 : make_sw128_desc(b_base + kChunkPlane) + ko;
-            const uint32_t acc = ks > 0 ? 1u : 0u;
-            umma_bf16(acc_main, a_hi, b_hi, idesc, acc);
-            umma_bf16(acc_cross, a_lo, b_hi, idesc, acc);
-            umma_bf16(acc_cross, a_hi, b_lo, idesc, 1u);
-          }
-          umma_commit(empty_bar(s));
-          umma_commit(tfull_bar(s));
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 10) {
-    // ============ epilogue: bias + LeakyRectify(0.2) + hi|lo re-split -> swizzled staging tiles -> TMA store ============
-    const int ew = warp - 2, lg = warp & 3, half = ew >> 2;
-    const int m = lg * 32 + lane;
-    const bool issuer = (ew & 3) == 0 && lane == 0;     // one thread per channel half issues that half's two TMA stores
-    const uint32_t o_hi = o_base + (uint32_t)(half * 2) * kChunkPlane, o_lo = o_hi + kChunkPlane;
-    const uint32_t row_hi = o_hi + (uint32_t)m * 128u, row_lo = o_lo + (uint32_t)m * 128u;
-    const uint32_t mx = (uint32_t)(m & 7);
-    const int group_bar = 3 + half;                      // named barrier of the half's four warps
-    pdl_wait();                                          // a1 may still be read by the previous step's enc_conv2 only transitively; be exact
+    pdl_wait();                                         // a1 may still be read by the previous step's enc_conv2 only transitively; be exact
+    mbar_wait(b_bar, 0);
     uint32_t t = 0;
     for (int w = blockIdx.x; w < total; w += gridDim.x, ++t) {
       const int n = w / kTilesPerImage, p0 = (w % kTilesPerImage) * 4;
       const uint32_t s = t & 1u, use = t >> 1;
-      const uint32_t lane_addr = tmem_base + s * 256 + ((uint32_t)(lg * 32) << 16);
-      mbar_wait(tfull_bar(s), use & 1u);
-      tc_fence_after();
-      // software-pipelined drain: the TMEM loads of chunk k+1 are in flight while chunk k is converted and staged
-      uint32_t vm[2][16], vc[2][16];
-      __syncwarp();
-      tmem_ld16(lane_addr + half * 64, vm[0]);
-      tmem_ld16(lane_addr + 128 + half * 64, vc[0]);
-      if (t > 0) {                                      // the previous tile's TMA stores have read the staging tiles
-        if (issuer) bulk_wait_group_read0();
-        asm volatile("bar.sync %0, 128;" ::"r"(group_bar) : "memory");
-      }
+      mbar_wait(full_bar(s), use & 1u);
+      const uint32_t sa = a_base + s * kAStage + wg * 64 * 128;
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {                     // output channels [64h, 64h + 64)
+        float am[32], ac[32];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int cb = half * 64 + 16 * k;
-        tmem_ld_wait();
-        if (k < 3) {
-          __syncwarp();
-          tmem_ld16(lane_addr + cb + 16, vm[(k + 1) & 1]);
-          tmem_ld16(lane_addr + 128 + cb + 16, vc[(k + 1) & 1]);
-        } else {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(s));
+        for (int j = 0; j < 32; ++j) { am[j] = 0.f; ac[j] = 0.f; }
+        wgmma_fence_regs(am);
+        wgmma_fence_regs(ac);
+        const uint32_t sb = b_base + h * 64 * 128;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 5; ++ks) {                // K = 80: slices 0..3 of the 64-wide chunk, then the tail
+          const bool tail = ks == 4;
+          const uint64_t ko = (uint64_t)((ks & 3) * 2);   // a K = 16 slice is 32 B = 2 descriptor address units
+          const uint64_t a_hi = tail ? make_sw128_desc(sa + 2 * kChunkPlane) : make_sw128_desc(sa) + ko;
+          const uint64_t a_lo = tail ? make_sw128_desc(sa + 2 * kChunkPlane) + 2 : make_sw128_desc(sa + kChunkPlane) + ko;
+          const uint64_t b_hi = tail ? make_sw128_desc(sb + 2 * kChunkPlane) : make_sw128_desc(sb) + ko;
+          const uint64_t b_lo = tail ? make_sw128_desc(sb + 2 * kChunkPlane) + 2 : make_sw128_desc(sb + kChunkPlane) + ko;
+          const uint32_t acc = ks > 0 ? 1u : 0u;
+          wgmma_bf16<64>(am, a_hi, b_hi, acc);
+          wgmma_bf16<64>(ac, a_lo, b_hi, acc);
+          wgmma_bf16<64>(ac, a_hi, b_lo, 1u);
         }
-        const uint32_t* am = vm[k & 1];
-        const uint32_t* ac = vc[k & 1];
-        __align__(16) __nv_bfloat162 hi[8], lo[8];
-        __align__(16) float bv[16];
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(am);
+        wgmma_fence_regs(ac);
+        if (h == 1 && wtid == 0) mbar_arrive(empty_bar(s));   // this warpgroup no longer reads the operand stage
+        if (h == 0 && t > 0) {                          // the previous tile's TMA stores have read the staging tiles
+          if (issuer) bulk_wait_group_read0();
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+        }
+        const uint32_t o_hi = o_base + (uint32_t)(h * 2) * kChunkPlane, o_lo = o_hi + kChunkPlane;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) reinterpret_cast<float4*>(bv)[j] = reinterpret_cast<const float4*>(bias_s + cb)[j];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float v0 = __uint_as_float(am[2 * j]) + __uint_as_float(ac[2 * j]) + bv[2 * j];
-          float v1 = __uint_as_float(am[2 * j + 1]) + __uint_as_float(ac[2 * j + 1]) + bv[2 * j + 1];
+        for (int j = 0; j < 32; j += 2) {
+          const int row = wg * 64 + frag_row(wtid, j), col = frag_col(wtid, j);
+          float v0 = am[j] + ac[j] + bias_s[h * 64 + col];
+          float v1 = am[j + 1] + ac[j + 1] + bias_s[h * 64 + col + 1];
           v0 = fmaf(0.4f, fabsf(v0), 0.6f * v0);
           v1 = fmaf(0.4f, fabsf(v1), 0.6f * v1);
-          hi[j] = __floats2bfloat162_rn(v0, v1);
-          const float2 hf = __bfloat1622float2(hi[j]);
-          lo[j] = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
+          const __nv_bfloat162 hi = __floats2bfloat162_rn(v0, v1);
+          const float2 hf = __bfloat1622float2(hi);
+          const __nv_bfloat162 lo = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
+          // channel col of the pixel's 128-byte row: 16-byte unit col/8 (128B swizzle: unit ^ row%8), 2 bytes per channel
+          const uint32_t off = (uint32_t)row * 128u + ((((uint32_t)col >> 3) ^ ((uint32_t)row & 7u)) << 4) + ((uint32_t)col & 7u) * 2u;
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(o_hi + off), "r"(*reinterpret_cast<const uint32_t*>(&hi)) : "memory");
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(o_lo + off), "r"(*reinterpret_cast<const uint32_t*>(&lo)) : "memory");
         }
-        // channels 16k .. 16k+15 of this half = 16-byte units 2k, 2k+1 of the pixel's 128-byte row (128B swizzle: unit ^ row%8;
-        // the 32 lanes of a warp are 32 consecutive rows -> 8 bank groups x 4 lanes: conflict-free)
-        const uint32_t u0 = ((uint32_t)(2 * k) ^ mx) << 4, u1 = ((uint32_t)(2 * k + 1) ^ mx) << 4;
-        st_shared_v4(row_hi + u0, reinterpret_cast<const uint4*>(hi)[0]);
-        st_shared_v4(row_hi + u1, reinterpret_cast<const uint4*>(hi)[1]);
-        st_shared_v4(row_lo + u0, reinterpret_cast<const uint4*>(lo)[0]);
-        st_shared_v4(row_lo + u1, reinterpret_cast<const uint4*>(lo)[1]);
       }
       fence_proxy_async_smem();                          // generic-proxy writes -> visible to the TMA store
-      asm volatile("bar.sync %0, 128;" ::"r"(group_bar) : "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");
       if (issuer) {
         const int pix0 = (n * 32 + p0) * 32;             // the tile's 128 pixels are consecutive in NHWC
-        tma_store_3d(&omap.out, o_hi, half * 64, pix0, 0);
-        tma_store_3d(&omap.out, o_lo, half * 64, pix0, 1);
+        for (int h = 0; h < 2; ++h) {
+          tma_store_3d(&omap.out, o_base + (uint32_t)(h * 2) * kChunkPlane, h * 64, pix0, 0);
+          tma_store_3d(&omap.out, o_base + (uint32_t)(h * 2 + 1) * kChunkPlane, h * 64, pix0, 1);
+        }
         bulk_commit_group();
       }
     }
     if (issuer) bulk_wait_group0();                      // every byte has left before the CTA retires its shared memory
   } else {
-    // ===================== im2col producers (warps 10..25) =====================
-    const int pt = threadIdx.x - 320;                   // 0..511
+    // ===================== im2col producers (warps 8..15) =====================
+    const int pt = threadIdx.x - 256;                   // 0..255
     // quarter-major: the 32 lanes of a warp build the SAME unit group of 32 consecutive rows (no divergence, and the
     // patch reads of a warp walk consecutive columns)
     const int quarter = pt >> 7, m = pt & 127;
     const int r = m >> 5, c = m & 31;
     // the patch of tile t+1 is fetched into registers while tile t is being expanded (global latency hidden)
-    constexpr int kPer = (kPatchFloats + kProducers - 1) / kProducers;    // 5 floats per thread
+    constexpr int kPer = (kPatchFloats + kProducers - 1) / kProducers;    // 9 floats per thread
     float pre[kPer];
     auto fetch = [&](int w) {
       const int n = w / kTilesPerImage, p0 = (w % kTilesPerImage) * 4;
@@ -282,18 +238,15 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
 #pragma unroll
       for (int e = 0; e < kPer; ++e)
         if (pt + e * kProducers < kPatchFloats) patch[pt + e * kProducers] = pre[e];
-      asm volatile("bar.sync 2, 512;" ::: "memory");    // patch complete (producer warps only)
+      asm volatile("bar.sync 2, 256;" ::: "memory");    // patch complete (producer warps only)
       if (w + (int)gridDim.x < total) fetch(w + gridDim.x);
       build_quarter(quarter, stage, patch, m, r, c);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to tcgen05
+      build_quarter(quarter + 2, stage, patch, m, r, c);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
       __syncwarp();
       if (lane == 0) mbar_arrive(full_bar(s));
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace

@@ -1,5 +1,5 @@
 // decout_tc.cu -- dec_out (reference IAN_simple.py:171-181: DeconvLayer 128 -> 3 ch, 5x5, stride 2, tanh;
-// layers.py:436-483) as ONE dense tcgen05 GEMM plus an on-chip col2im, reading its input once.
+// layers.py:436-483) as ONE dense wgmma GEMM plus an on-chip col2im, reading its input once.
 //
 // The output has only 3 channels, so the layer is bandwidth work: h3 is 512 KB/image, x_hat 48 KB.
 // Running it as a shifted-tap GEMM would re-stage every input pixel once per tap (25x).  Instead:
@@ -11,9 +11,9 @@
 // TMA zero-fills rows outside the image) and finishes the 4 output rows that depend only on it
 // (input rows p0, p0+1): 2x redundant GEMM work, which is free next to the saved traffic.
 //
-// Roles (persistent CTA, one per SM): warp 0 TMA producer (weights once, then an A ring), warp 1 MMA
-// issuer (3-pass bf16 split, main|cross accumulators, two TMEM buffers), warps 2-9 epilogue
-// (TMEM -> smem T tile -> col2im -> tanh -> store).
+// Roles (persistent CTA, one per SM): warp 8 TMA producer (weights once, then an A ring), warps 0-7 two consumer
+// warpgroups (64 rows each; 3-pass bf16 split into main|cross register accumulators), which then run the epilogue
+// (registers -> smem T tile -> col2im -> tanh -> store).
 #include <cstdio>
 #include <cstring>
 
@@ -40,9 +40,8 @@ namespace {
 
 using namespace tc;
 
-constexpr int kThreads = 320;
-constexpr int kEpiThreads = 256;
-constexpr int BN = 80;                       // 25 taps x 3 channels = 75, padded to a legal UMMA N
+constexpr int kThreads = 288;               // 8 consumer warps + 1 TMA warp
+constexpr int BN = 80;                       // 25 taps x 3 channels = 75, padded to a multiple of 16
 constexpr int kAStage = 128 * 64 * 2 * 2;    // one K chunk of the A tile, hi+lo: 32 KB
 constexpr int kAStages = 4;                  // 2 work items of look-ahead (an item is two K chunks): hides the TMA round trip
 constexpr int kBChunk = BN * 64 * 2 * 2;     // one K chunk of the weights, hi+lo: 20 KB
@@ -63,29 +62,20 @@ decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant_
   float* Ts = reinterpret_cast<float*>(smem_al + (t_base - smem_base));
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kAStages + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * kAStages + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * kAStages + 2 + b); };
-  const uint32_t b_bar = bar_base + 8u * (2 * kAStages + 4);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kAStages + 5);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_al + (tmem_slot - smem_base));
+  const uint32_t b_bar = bar_base + 8u * (2 * kAStages);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total = n_img * kItemsPerImage;
 
   if (threadIdx.x == 0) {
     pdl_trigger();                                      // tapgemm.h: PDL
-    for (int s = 0; s < kAStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), kEpiThreads / 32); }
+    for (int s = 0; s < kAStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }
     mbar_init(b_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       mbar_expect_tx(b_bar, 2 * kBChunk);
@@ -103,108 +93,79 @@ decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp in uniform control flow; one elected lane issues) =====================
-    {
-      constexpr uint32_t idesc = make_idesc_bf16_m128(BN);
-      mbar_wait(b_bar, 0);
-      uint32_t i = 0, t = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++t) {
-        const uint32_t buf = t & 1u, use = t >> 1;
-        const uint32_t acc_main = tmem_base + buf * 256, acc_cross = acc_main + 128;
-        mbar_wait(tempty_bar(buf), (use & 1u) ^ 1u);
-        tc_fence_after();
-        for (int c = 0; c < 2; ++c, ++i) {
-          const int s = i % kAStages;
-          mbar_wait(full_bar(s), (i / kAStages) & 1u);
-          tc_fence_after();
-          const uint32_t sa = a_base + s * kAStage, sb = b_base + c * kBChunk;
-          const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + 128 * 64 * 2);
-          const uint64_t b_hi = make_sw128_desc(sb), b_lo = make_sw128_desc(sb + BN * 64 * 2);
-          if (elect_one_sync()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t ko = (uint64_t)(k * 2);
-              const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-              umma_bf16(acc_main, a_hi + ko, b_hi + ko, idesc, acc);
-              umma_bf16(acc_cross, a_lo + ko, b_hi + ko, idesc, acc);
-              umma_bf16(acc_cross, a_hi + ko, b_lo + ko, idesc, 1u);
-            }
-            umma_commit(empty_bar(s));
-          }
-          __syncwarp();
-        }
-        if (elect_one_sync()) umma_commit(tfull_bar(buf));
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue: TMEM -> smem T tile -> col2im -> tanh -> NCHW store =====================
-    pdl_wait();                                         // the destinations may still be read by an earlier kernel of the stream
-    const int et = threadIdx.x - 64;                    // 0..255
-    const int ew = warp - 2;
-    const int lg = warp & 3;                            // TMEM lane group
-    const int half = ew >> 2;                           // columns [0,48) or [48,80)
-    const int row = lg * 32 + lane;                     // T tile row = pixel (pr*32 + q), pr = 0..3 <-> input row p0-1+pr
-    // output element handled in the col2im: out row ur (0..3) of the item, out col v (0..63)
-    const int ur = et >> 6, v = et & 63;
-    const int q = v >> 1, sx = v & 1, pr = 1 + (ur >> 1), ry = ur & 1;
-    uint32_t t = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x, ++t) {
-      const int n = w / kItemsPerImage, p0 = (w % kItemsPerImage) * 2;
-      const uint32_t buf = t & 1u, use = t >> 1;
-      const uint32_t lane_addr = tmem_base + buf * 256 + ((uint32_t)(lg * 32) << 16);
-      mbar_wait(tfull_bar(buf), use & 1u);
-      tc_fence_after();
-      // this warp's columns: half 0 -> [0,48), half 1 -> [48,80)
-      const int c_begin = half ? 48 : 0, c_end = half ? 80 : 48;
-#pragma unroll 1
-      for (int cb = c_begin; cb < c_end; cb += 16) {
-        uint32_t vm[16], vc[16];
-        __syncwarp();
-        tmem_ld16(lane_addr + cb, vm);
-        tmem_ld16(lane_addr + 128 + cb, vc);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (cb + j < 75) Ts[row * kTLd + cb + j] = __uint_as_float(vm[j]) + __uint_as_float(vc[j]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(buf));       // TMEM buffer free: next item's MMAs may start
-      asm volatile("bar.sync 1, 256;" ::: "memory");     // T tile complete (epilogue warps only)
-
-      // y[co, 2p+ry, 2q+sx] = sum_{d,e} T[(p+d, q+e)][(ki*5+kj)*3+co], ki = 2+2d-ry, kj = 2+2e-sx
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-#pragma unroll
-      for (int d = -1; d <= 1; ++d) {
-        if (ry && d < 0) continue;
-        const int ki = 2 + 2 * d - ry;
-#pragma unroll
-        for (int e = -1; e <= 1; ++e) {
-          if (sx && e < 0) continue;
-          const int qq = q + e;
-          if (qq < 0 || qq > 31) continue;               // image border (rows are handled by TMA zero fill)
-          const int kj = 2 + 2 * e - sx;
-          const float* tp = Ts + ((pr + d) * 32 + qq) * kTLd + (ki * 5 + kj) * 3;
-          a0 += tp[0]; a1 += tp[1]; a2 += tp[2];
-        }
-      }
-      const long long off = ((long long)n * 3 * 64 + (2 * p0 + ur)) * 64 + v;
-      const float y0 = tanhf(a0), y1 = tanhf(a1), y2 = tanhf(a2);
-      for (int d = 0; d < dst.n; ++d) {                  // d > 0: peer GPUs' gather buffers (st.global over NVLink)
-        float* o = dst.base[d] + off;
-        o[0] = y0;
-        o[4096] = y1;
-        o[8192] = y2;
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");     // T tile consumed: may be overwritten
-    }
+    return;
   }
+  // ===================== consumers: wgmma -> smem T tile -> col2im -> tanh -> NCHW store =====================
+  pdl_wait();                                           // the destinations may still be read by an earlier kernel of the stream
+  const int et = threadIdx.x;                           // 0..255
+  const int wg = warp >> 2, wtid = threadIdx.x & 127;
+  // output element handled in the col2im: out row ur (0..3) of the item, out col v (0..63)
+  const int ur = et >> 6, v = et & 63;
+  const int q = v >> 1, sx = v & 1, pr = 1 + (ur >> 1), ry = ur & 1;
+  mbar_wait(b_bar, 0);
+  uint32_t i = 0;
+  for (int w = blockIdx.x; w < total; w += gridDim.x) {
+    const int n = w / kItemsPerImage, p0 = (w % kItemsPerImage) * 2;
+    float am[BN / 2], ac[BN / 2];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) { am[j] = 0.f; ac[j] = 0.f; }
+    wgmma_fence_regs(am);
+    wgmma_fence_regs(ac);
+    for (int c = 0; c < 2; ++c, ++i) {
+      const int s = i % kAStages;
+      mbar_wait(full_bar(s), (i / kAStages) & 1u);
+      const uint32_t sa = a_base + s * kAStage + wg * 64 * 128, sb = b_base + c * kBChunk;
+      const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + 128 * 64 * 2);
+      const uint64_t b_hi = make_sw128_desc(sb), b_lo = make_sw128_desc(sb + BN * 64 * 2);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t ko = (uint64_t)(k * 2);
+        const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
+        wgmma_bf16<BN>(am, a_hi + ko, b_hi + ko, acc);
+        wgmma_bf16<BN>(ac, a_lo + ko, b_hi + ko, acc);
+        wgmma_bf16<BN>(ac, a_hi + ko, b_lo + ko, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(am);
+      wgmma_fence_regs(ac);
+      if (wtid == 0) mbar_arrive(empty_bar(s));         // this warpgroup no longer reads the stage
+    }
+    // T tile row = pixel (pr*32 + q), pr = 0..3 <-> input row p0-1+pr; columns tap*3+co (75 used)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) {
+      const int row = wg * 64 + frag_row(wtid, j), col = frag_col(wtid, j);
+      if (col < 75) Ts[row * kTLd + col] = am[j] + ac[j];
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");     // T tile complete (consumer warps only)
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
+    // y[co, 2p+ry, 2q+sx] = sum_{d,e} T[(p+d, q+e)][(ki*5+kj)*3+co], ki = 2+2d-ry, kj = 2+2e-sx
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+#pragma unroll
+    for (int d = -1; d <= 1; ++d) {
+      if (ry && d < 0) continue;
+      const int ki = 2 + 2 * d - ry;
+#pragma unroll
+      for (int e = -1; e <= 1; ++e) {
+        if (sx && e < 0) continue;
+        const int qq = q + e;
+        if (qq < 0 || qq > 31) continue;               // image border (rows are handled by TMA zero fill)
+        const int kj = 2 + 2 * e - sx;
+        const float* tp = Ts + ((pr + d) * 32 + qq) * kTLd + (ki * 5 + kj) * 3;
+        a0 += tp[0]; a1 += tp[1]; a2 += tp[2];
+      }
+    }
+    const long long off = ((long long)n * 3 * 64 + (2 * p0 + ur)) * 64 + v;
+    const float y0 = tanhf(a0), y1 = tanhf(a1), y2 = tanhf(a2);
+    for (int d = 0; d < dst.n; ++d) {                  // d > 0: peer GPUs' gather buffers (st.global over NVLink)
+      float* o = dst.base[d] + off;
+      o[0] = y0;
+      o[4096] = y1;
+      o[8192] = y2;
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");     // T tile consumed: may be overwritten
+  }
 }
 
 // ---- cross-GPU barrier over peer memory: every rank owns flags[kMaxPeers]; rank r writes its epoch into slot r of
@@ -253,8 +214,8 @@ __device__ __forceinline__ int ld_acquire_sys(const int* p) {
   return v;
 }
 
-// Footprint: the push runs NEXT TO the persistent tensor kernels of the following step (1 CTA per SM, 168 registers x 320
-// threads, or 72 x 832 for enc_conv1), so a push CTA must fit in what they leave free -- 128 threads, <= 40 registers, no
+// Footprint: the push runs NEXT TO the persistent tensor kernels of the following step (1 CTA per SM, up to 168 registers x
+// 288 threads, or 128 x 512 for enc_conv1), so a push CTA must fit in what they leave free -- 128 threads, <= 40 registers, no
 // shared memory -- or it would hold an SM back from a statically scheduled persistent kernel (measured: +57 us on
 // enc_conv2 with 256-thread / 60-register push CTAs).
 __global__ void __launch_bounds__(128, 12) peer_push_kernel(const PushArgs a) {

@@ -35,7 +35,7 @@ HeadMaps* head_build_maps(const __nv_bfloat16* fh4, long long fh4_plane, int n_i
                           char* err, int errlen);
 void head_free_maps(HeadMaps*);
 int launch_head_tc(const HeadMaps* maps, int passes, float* ha, int n, cudaStream_t st);
-// enc_conv1 on the tensor-core path (conv1_tc.cu): thread-built im2col tile + tcgen05
+// enc_conv1 on the tensor-core path (conv1_tc.cu): thread-built im2col tile + wgmma
 struct Conv1Maps;
 struct Conv1OutMap;
 // wt: three blocks of [128 cout][64 k] bf16 (hi k<64 | lo k<64 | tail: hi k 64..79, lo k 64..79, zeros)

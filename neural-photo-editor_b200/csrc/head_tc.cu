@@ -11,9 +11,9 @@
 // shifts, the feature map is staged exactly once per conv), drains T to shared memory, and every epilogue thread adds
 // the taps that land on ITS 16 output pixels,  ha[p][f] += T[p + off_t][t*2+f],  into registers (weight rows are sorted by
 // the taps' row offset; the [2,3,4]-scale tap set is analytic, so the gather needs no table).  No atomics, fixed order.
-// Roles as in decout_tc.cu: warp 0 TMA (weights per item, A ring), warp 1 tcgen05 issue (float32 = 3-pass bf16 split,
-// main|cross accumulators; or single pass), warps 2-9 epilogue; two TMEM buffers so tile i+1 multiplies while tile i
-// is gathered.
+// Roles: warp 16 TMA (weights per item, A ring); warps 0-15 four consumer warpgroups, one per (64-row half, 40-column
+// half) of the tile's 128 x 80 result (float32 = 3-pass bf16 split into main|cross register accumulators, or single
+// pass), which then drain their fragments into the shared T tile and run the gather.
 // The autoregressive part (sigmoid R; G from 33 taps of R; B from 33 taps of [R,G]; Beta means) stays the three per-pixel
 // kernels of edge_kernels.cu, reading this kernel's planar output: a one-CTA-per-image version with R and G in shared
 // memory was tried and measured 3x slower (512 CTAs of dependent shared-memory chains vs 2 M independent threads on L2).
@@ -34,18 +34,17 @@ namespace {
 
 using namespace tc;
 
-constexpr int kEpiThreads = 512;              // 16 epilogue warps: the drain + gather is latency-bound, more warps hide it
-constexpr int kThreads = 64 + kEpiThreads;
-constexpr int BN = 80;                        // 33 taps x 2 filters = 66, padded to a legal UMMA N
+constexpr int kEpiThreads = 512;              // 16 consumer warps: the drain + gather is latency-bound, more warps hide it
+constexpr int kThreads = 32 + kEpiThreads;
+constexpr int BN = 80;                        // 33 taps x 2 filters = 66, padded to a multiple of 16
 constexpr int kNT = 33;
 constexpr int kTLd = 67;                      // T row pitch in floats (odd: conflict-free column access)
 constexpr int kTBytes = 128 * kTLd * 4;
 constexpr int kTilesPerImage = 32;
 
 template <int PASSES> struct HeadCfg {
-  // the A ring is what hides the TMA round trip: a tile is only two K chunks, so its depth in TILES is kAStages / 2.  Round
-  // 2's first version had 3 stages (1.5 tiles) and ran at ~3.5 k clocks per tile whatever the epilogue did -- TMA-latency
-  // bound.  Now the ring takes all the shared memory left: 4 stages of 32 KB in float32 mode, 8 of 16 KB in bf16 mode.
+  // the A ring is what hides the TMA round trip: a tile is only two K chunks, so its depth in TILES is kAStages / 2.  The
+  // ring takes the shared memory left: 4 stages of 32 KB in float32 mode, 8 of 16 KB in bf16 mode.
   static constexpr int kAStages = PASSES == 3 ? 4 : 8;
   static constexpr int kPlanes = PASSES == 3 ? 2 : 1;
   static constexpr int kAStage = 128 * 64 * 2 * kPlanes;      // one K chunk of an A tile
@@ -68,32 +67,23 @@ head_tc_kernel(const __grid_constant__ HeadMaps maps, float* __restrict__ ha /*[
   float* Ts = reinterpret_cast<float*>(smem_al + (t_base - smem_base));
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kAStages + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * kAStages + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * kAStages + 2 + b); };
-  const uint32_t bfull_bar = bar_base + 8u * (2 * kAStages + 4);
-  const uint32_t bempty_bar = bar_base + 8u * (2 * kAStages + 5);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kAStages + 6);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_al + (tmem_slot - smem_base));
+  const uint32_t bfull_bar = bar_base + 8u * (2 * kAStages);
+  const uint32_t bempty_bar = bar_base + 8u * (2 * kAStages + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total = n_img * 3;
 
   if (threadIdx.x == 0) {
     pdl_trigger();                                      // tapgemm.h: PDL
-    for (int s = 0; s < kAStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), kEpiThreads / 32); }
+    for (int s = 0; s < kAStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4); }
     mbar_init(bfull_bar, 1);
     mbar_init(bempty_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   pdl_wait();                                           // prologue done; the feature map / ha below belong to the chain
 
-  if (warp == 0) {
+  if (warp == kEpiThreads / 32) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t i = 0, it = 0;
@@ -112,135 +102,108 @@ head_tc_kernel(const __grid_constant__ HeadMaps maps, float* __restrict__ ha /*[
           }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp in uniform control flow; one elected lane issues) =====================
-    {
-      constexpr uint32_t idesc = make_idesc_bf16_m128(BN);
-      uint32_t i = 0, t = 0, it = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        mbar_wait(bfull_bar, it & 1u);
-        tc_fence_after();
-        for (int mt = 0; mt < kTilesPerImage; ++mt, ++t) {
-          const uint32_t buf = t & 1u, use = t >> 1;
-          const uint32_t acc_main = tmem_base + buf * 256, acc_cross = acc_main + 128;
-          mbar_wait(tempty_bar(buf), (use & 1u) ^ 1u);
-          tc_fence_after();
-          for (int c = 0; c < 2; ++c, ++i) {
-            const int s = i % kAStages;
-            mbar_wait(full_bar(s), (i / kAStages) & 1u);
-            tc_fence_after();
-            const uint32_t sa = a_base + s * Cfg::kAStage, sb = b_base + c * Cfg::kBChunk;
-            const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + 128 * 64 * 2);
-            const uint64_t b_hi = make_sw128_desc(sb), b_lo = make_sw128_desc(sb + BN * 64 * 2);
-            if (elect_one_sync()) {
+    return;
+  }
+  // ===================== consumers: wgmma -> smem T tile -> tap gather into registers =====================
+  constexpr int NW = BN / 2;                            // columns of one warpgroup's accumulator
+  const int et = threadIdx.x;                           // 0..511
+  const int wg = warp >> 2, wtid = threadIdx.x & 127;
+  const int row0 = (wg & 1) * 64, col0 = (wg >> 1) * NW;
+  const int q = et & 63, r0 = et >> 6;                  // this thread's output pixels: column q, rows r0 + 8*i, i = 0..7
+  uint32_t si = 0, it = 0;   // si: running A-stage counter
+  for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
+    const int n = w / 3, k = w % 3;
+    float acc[8][2];
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t ko = (uint64_t)(k * 2);
-                const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-                umma_bf16(acc_main, a_hi + ko, b_hi + ko, idesc, acc);
-                if (PASSES == 3) {
-                  umma_bf16(acc_cross, a_lo + ko, b_hi + ko, idesc, acc);
-                  umma_bf16(acc_cross, a_hi + ko, b_lo + ko, idesc, 1u);
-                }
-              }
-              umma_commit(empty_bar(s));
-            }
-            __syncwarp();
+    for (int i = 0; i < 8; ++i) { acc[i][0] = 0.f; acc[i][1] = 0.f; }
+    mbar_wait(bfull_bar, it & 1u);
+    for (int mt = 0; mt < kTilesPerImage; ++mt) {
+      float am[NW / 2], ac[PASSES == 3 ? NW / 2 : 1];
+#pragma unroll
+      for (int j = 0; j < NW / 2; ++j) am[j] = 0.f;
+#pragma unroll
+      for (int j = 0; j < (PASSES == 3 ? NW / 2 : 1); ++j) ac[j] = 0.f;
+      wgmma_fence_regs(am);
+      if (PASSES == 3) wgmma_fence_regs(ac);
+      for (int c = 0; c < 2; ++c, ++si) {
+        const int s = si % kAStages;
+        mbar_wait(full_bar(s), (si / kAStages) & 1u);
+        const uint32_t sa = a_base + s * Cfg::kAStage + row0 * 128, sb = b_base + c * Cfg::kBChunk + col0 * 128;
+        const uint64_t a_hi = make_sw128_desc(sa), a_lo = make_sw128_desc(sa + 128 * 64 * 2);
+        const uint64_t b_hi = make_sw128_desc(sb), b_lo = make_sw128_desc(sb + BN * 64 * 2);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t ko = (uint64_t)(kk * 2);
+          const uint32_t a = (c > 0 || kk > 0) ? 1u : 0u;
+          wgmma_bf16<NW>(am, a_hi + ko, b_hi + ko, a);
+          if constexpr (PASSES == 3) {
+            wgmma_bf16<NW>(ac, a_lo + ko, b_hi + ko, a);
+            wgmma_bf16<NW>(ac, a_hi + ko, b_lo + ko, 1u);
           }
-          if (elect_one_sync()) umma_commit(tfull_bar(buf));
-          __syncwarp();
         }
-        if (elect_one_sync()) umma_commit(bempty_bar);   // weights of this item no longer read once these MMAs retire
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(am);
+        if (PASSES == 3) wgmma_fence_regs(ac);
+        if (wtid == 0) mbar_arrive(empty_bar(s));       // this warpgroup no longer reads the stage
       }
-    }
-  } else {
-    // ===================== epilogue: TMEM -> smem T tile -> tap gather into registers =====================
-    const int et = threadIdx.x - 64;                    // 0..511
-    const int ew = warp - 2;
-    const int lg = warp & 3;                            // TMEM lane group
-    const int quarter = ew >> 2;                        // T columns [16*quarter, +16); quarter 0 also takes [64, 80)
-    const int row = lg * 32 + lane;                     // T tile row = pixel (pr*64 + q) of input rows 2mt + pr
-    const int q = et & 63, r0 = et >> 6;                // this thread's output pixels: column q, rows r0 + 8*i, i = 0..7
-    uint32_t t = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x) {
-      const int n = w / 3, k = w % 3;
-      float acc[8][2];
+      // T tile row = pixel (pr*64 + q) of input rows 2mt + pr; columns tap*2 + filter (66 used)
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { acc[i][0] = 0.f; acc[i][1] = 0.f; }
-      for (int mt = 0; mt < kTilesPerImage; ++mt, ++t) {
-        const uint32_t buf = t & 1u, use = t >> 1;
-        const uint32_t lane_addr = tmem_base + buf * 256 + ((uint32_t)(lg * 32) << 16);
-        mbar_wait(tfull_bar(buf), use & 1u);
-        tc_fence_after();
-#pragma unroll 1
-        for (int cb = 16 * quarter; cb < 80; cb += 64) {
-          if (cb >= 64 && quarter != 0) break;
-          uint32_t vm[16], vc[16];
-          __syncwarp();
-          tmem_ld16(lane_addr + cb, vm);
-          if (PASSES == 3) tmem_ld16(lane_addr + 128 + cb, vc);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (cb + j < 2 * kNT)
-              Ts[row * kTLd + cb + j] = PASSES == 3 ? __uint_as_float(vm[j]) + __uint_as_float(vc[j]) : __uint_as_float(vm[j]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(buf));     // TMEM buffer free: the next tile's MMAs may start
-        asm volatile("bar.sync 1, 512;" ::: "memory");   // T tile complete (epilogue warps only)
+      for (int j = 0; j < NW / 2; ++j) {
+        const int row = row0 + frag_row(wtid, j), col = col0 + frag_col(wtid, j);
+        float v = am[j];
+        if constexpr (PASSES == 3) v += ac[j];
+        if (col < 2 * kNT) Ts[row * kTLd + col] = v;
+      }
+      asm volatile("bar.sync 1, 512;" ::: "memory");   // T tile complete (consumer warps only)
+      if (mt == kTilesPerImage - 1 && threadIdx.x == 0) mbar_arrive(bempty_bar);   // every MMA of this item has retired
 
-        // ha[p][f] += T[(p + dy, q + dx)][j*2 + f] for the taps whose input row p + dy lies in this tile (rows 2mt, 2mt+1).
-        // The scales-[2,3,4] MDC has an analytic tap set (checked on the host against the sorted table): a row offset
-        // dy != 0 belongs to exactly one dilation s = |dy| with dx in {-s, 0, +s} (T columns j0, j0+1, j0+2); dy = 0 has
-        // dx in {-1,0,1,-2,2,-3,3,-4,4} (columns 12..20).  No table look-ups, independent loads per hit.
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int p = r0 + 8 * i;
-#pragma unroll
-          for (int pr = 0; pr < 2; ++pr) {
-            const int dy = 2 * mt + pr - p;              // the row offset that reaches input row 2mt + pr from p (warp-uniform)
-            if (dy < -4 || dy > 4) continue;
-            const float* trow = Ts + (pr * 64 + q) * kTLd;
-            if (dy != 0) {
-              const int sdil = dy < 0 ? -dy : dy;
-              const int j0 = dy < 0 ? 3 * (dy + 4) : 21 + 3 * (dy - 1);
-              const float* tc0 = trow + 2 * j0;
-              float a0 = tc0[2], a1 = tc0[3];            // dx = 0
-              if (q - sdil >= 0) { a0 += tc0[-sdil * kTLd]; a1 += tc0[-sdil * kTLd + 1]; }          // dx = -s
-              if (q + sdil <= 63) { a0 += tc0[sdil * kTLd + 4]; a1 += tc0[sdil * kTLd + 5]; }       // dx = +s
-              acc[i][0] += a0;
-              acc[i][1] += a1;
-            } else {
-              const float* tc0 = trow + 2 * 12;
-              float a0 = tc0[2], a1 = tc0[3];            // dx = 0 (column 13)
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {              // dx = -(e+1) / +(e+1): columns {12,14}, {15,16}, {17,18}, {19,20}
-                const int d = e + 1;
-                const int cm = e == 0 ? 0 : 2 * (2 * e + 1), cp = e == 0 ? 4 : 2 * (2 * e + 2);
-                if (q - d >= 0) { a0 += tc0[-d * kTLd + cm]; a1 += tc0[-d * kTLd + cm + 1]; }
-                if (q + d <= 63) { a0 += tc0[d * kTLd + cp]; a1 += tc0[d * kTLd + cp + 1]; }
-              }
-              acc[i][0] += a0;
-              acc[i][1] += a1;
-            }
-          }
-        }
-        asm volatile("bar.sync 1, 512;" ::: "memory");   // T tile consumed: may be overwritten
-      }
-      float* o0 = ha + ((long long)n * 6 + 2 * k) * 4096 + q;
+      // ha[p][f] += T[(p + dy, q + dx)][j*2 + f] for the taps whose input row p + dy lies in this tile (rows 2mt, 2mt+1).
+      // The scales-[2,3,4] MDC has an analytic tap set (checked on the host against the sorted table): a row offset
+      // dy != 0 belongs to exactly one dilation s = |dy| with dx in {-s, 0, +s} (T columns j0, j0+1, j0+2); dy = 0 has
+      // dx in {-1,0,1,-2,2,-3,3,-4,4} (columns 12..20).  No table look-ups, independent loads per hit.
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        o0[(r0 + 8 * i) * 64] = acc[i][0];
-        o0[4096 + (r0 + 8 * i) * 64] = acc[i][1];
+        const int p = r0 + 8 * i;
+#pragma unroll
+        for (int pr = 0; pr < 2; ++pr) {
+          const int dy = 2 * mt + pr - p;              // the row offset that reaches input row 2mt + pr from p (warp-uniform)
+          if (dy < -4 || dy > 4) continue;
+          const float* trow = Ts + (pr * 64 + q) * kTLd;
+          if (dy != 0) {
+            const int sdil = dy < 0 ? -dy : dy;
+            const int j0 = dy < 0 ? 3 * (dy + 4) : 21 + 3 * (dy - 1);
+            const float* tc0 = trow + 2 * j0;
+            float a0 = tc0[2], a1 = tc0[3];            // dx = 0
+            if (q - sdil >= 0) { a0 += tc0[-sdil * kTLd]; a1 += tc0[-sdil * kTLd + 1]; }          // dx = -s
+            if (q + sdil <= 63) { a0 += tc0[sdil * kTLd + 4]; a1 += tc0[sdil * kTLd + 5]; }       // dx = +s
+            acc[i][0] += a0;
+            acc[i][1] += a1;
+          } else {
+            const float* tc0 = trow + 2 * 12;
+            float a0 = tc0[2], a1 = tc0[3];            // dx = 0 (column 13)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {              // dx = -(e+1) / +(e+1): columns {12,14}, {15,16}, {17,18}, {19,20}
+              const int d = e + 1;
+              const int cm = e == 0 ? 0 : 2 * (2 * e + 1), cp = e == 0 ? 4 : 2 * (2 * e + 2);
+              if (q - d >= 0) { a0 += tc0[-d * kTLd + cm]; a1 += tc0[-d * kTLd + cm + 1]; }
+              if (q + d <= 63) { a0 += tc0[d * kTLd + cp]; a1 += tc0[d * kTLd + cp + 1]; }
+            }
+            acc[i][0] += a0;
+            acc[i][1] += a1;
+          }
+        }
       }
+      asm volatile("bar.sync 1, 512;" ::: "memory");   // T tile consumed: may be overwritten
+    }
+    float* o0 = ha + ((long long)n * 6 + 2 * k) * 4096 + q;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o0[(r0 + 8 * i) * 64] = acc[i][0];
+      o0[4096 + (r0 + 8 * i) * 64] = acc[i][1];
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace

@@ -168,16 +168,10 @@ struct ian_handle {
   float* sk_ws = nullptr;      // stream-K partial-sum slots + arrival flags (shared by all layers of the handle)
   int* sk_flags = nullptr;
   int sk_epoch = 0;
-  bool streamk = true;
+  int streamk = 1;             // 0: whole tiles only; 1: stream-K where the makespan test asks for it; 2: wherever eligible (tests)
   bool splitk = true;          // split-K for small-M layers (IAN_SPLITK=0: whole tiles everywhere; used by tests)
-  bool tc2_bf16 = true;        // bf16 mode: Cout % 256 == 0 layers on 256 x 256 pair tiles (IAN_TC2_BF16=0: one-CTA kernel)
-  bool tc2 = true;             // CTA-pair tap-GEMM for layers with enough whole tiles (IAN_TC2=0 turns it off)
   bool coop_finalize = true;   // deep split-K layers: cooperative finalize kernel (IAN_FINALIZE8=0: one thread per output everywhere)
   bool pdl = true;             // programmatic dependent launch along the kernel chains (tapgemm.h; IAN_PDL=0 turns it off)
-  bool tc2_splitk = true;      // float32 mode: deep-K layers with few tiles split K over the SM pairs in the pair kernel (IAN_TC2_SPLITK=0)
-  bool tc2_over_split = true;  // float32 mode: the pair kernel (un-split, stream-K) also takes layers choose_ksplit() would split (IAN_TC2_OVER_SPLIT=0)
-  int tc2_min_tiles = 37;      // pair-tiles needed before a layer moves to the pair kernel (IAN_TC2_MIN); half a wave: stream-K fills it
-  std::string tc2_skip;        // comma-separated layer names kept on the one-CTA kernel (IAN_TC2_SKIP)
   bool graphs = true;          // replay small-batch host calls as CUDA graphs (IAN_GRAPHS=0 turns it off)
   bool capturing = false;
   bool finalized = false;
@@ -280,8 +274,6 @@ struct Plan {
   Planes dha2, d4, ds3, du3, dx3, ds2, du2, dx2, ds1, du1, dx1, dfh0;
   TapGemm g[L_COUNT];
   TcMaps* maps[L_COUNT] = {nullptr};
-  Tc2Maps* maps2[L_COUNT] = {nullptr};   // CTA-pair kernel (only for layers with enough whole tiles; see build_pair_maps)
-  int pair_ksplit[L_COUNT] = {0};        // K split the pair kernel runs the layer with (1 = un-split; build_pair_maps)
   DecOutMaps* decout_maps = nullptr;
   Conv1OutMap* conv1_out = nullptr;       // TMA-store view of a1 (conv1_tc.cu)
   HeadMaps* head_maps = nullptr;
@@ -408,8 +400,8 @@ void set_io(TapGemm& g, const Planes& a, int n, int Hin, int Win, int Cin, int H
 }
 
 int choose_ksplit(const TapGemm& g) {
-  // fill ~one wave of 148 SMs when the output tile count is small; keep >= 4 K steps per CTA
-  const int bn = (g.Cout % 256 == 0) ? 256 : (g.Cout % 128 == 0) ? 128 : 16;
+  // fill ~one wave of the SMs when the output tile count is small; keep >= 4 K steps per CTA
+  const int bn = (g.Cout % 128 == 0) ? 128 : 16;   // the tile width tc_build_maps picks
   const int M = g.n_img * g.Hg * g.Wg;
   const int ctas = ((M + 127) / 128) * (g.Cout / bn) * g.nphase;
   int min_it = 1 << 30;
@@ -417,7 +409,7 @@ int choose_ksplit(const TapGemm& g) {
     const int it = g.phase[p].ntaps * (g.Cin / 64);
     if (it < min_it) min_it = it;
   }
-  int ks = 148 / ctas;
+  int ks = tc_num_sms() / ctas;
   if (ks > min_it / 4) ks = min_it / 4;
   if (ks < 1) ks = 1;
   if (ks > 64) ks = 64;
@@ -455,53 +447,12 @@ int alloc_splitk_workspace(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
-// A layer moves to the CTA-pair kernel when it has no channel-major output, its channel counts fit the 256 x 128 pair
-// tile and it has at least tc2_min_tiles pair-tiles (half of the SM pairs).  A split-K factor that choose_ksplit() picked
-// to fill the one-CTA kernel's wave (37..74 tiles: e.g. the decoder's backward-data layers of the batch-128 edit loop)
-// does not hold a layer back: in float32 mode the pair kernel runs it un-split, balanced by stream-K, without the
-// workspace round trip and the finalize launch (run_gemm); bf16 mode keeps the split one-CTA form.
-int build_pair_maps(ian_handle* h, Plan* pl, int l) {
-  const TapGemm& g = pl->g[l];
-  if (!h->tc2 || g.out_f32_t || g.Cout % 128 || g.Cin % 64) return IAN_OK;
-  if (g.ksplit != 1 && !h->tc2_over_split) return IAN_OK;
-  if (!h->tc2_skip.empty() && h->tc2_skip.find(std::string(",") + kLayerNames[l] + ",") != std::string::npos) return IAN_OK;
-  char err[256] = {0};
-  Tc2Maps* m = tc2_build_maps(g, err, sizeof(err));
-  if (!m) return fail(h, IAN_ERR_CUDA, "layer %s (pair kernel): %s", kLayerNames[l], err);
-  const long long pt = tc2_pair_tiles(g, m);
-  if (pt >= h->tc2_min_tiles) {
-    pl->maps2[l] = m;
-    pl->pair_ksplit[l] = 1;
-    return IAN_OK;
-  }
-  // Few tiles but a deep K (enc_fc1 at batch 256: 8 pair-tiles x 256 K steps): split K over the SM pairs in the pair kernel
-  // too.  The one-CTA kernel's 256-wide float32 tiles leave room for only 2 x 96 KB stages -- the TMA ring covers half of the
-  // load latency and enc_fc1 ran at 35 % tensor activity; the pair kernel's 48 KB stages are four deep.  Same slab /
-  // finalize protocol (the plan's workspace is sized for the one-CTA split, which is never smaller).  Batches above the
-  // graph-replayed sizes only, so the single-image latency path keeps one schedule.
-  if (h->tc2_splitk && g.ksplit > 1 && g.n_img > 32 && (long long)g.n_img * g.Hg * g.Wg >= 256) {
-    int min_it = 1 << 30;
-    for (int p = 0; p < g.nphase; ++p) min_it = std::min(min_it, g.phase[p].ntaps * (g.Cin / 64));
-    int ks = (int)((tc_num_sms() / 2) / pt);
-    ks = std::min(ks, std::min(min_it / 8, g.ksplit));
-    if (ks >= 2 && pt * ks >= h->tc2_min_tiles) {
-      pl->maps2[l] = m;
-      pl->pair_ksplit[l] = ks;
-      return IAN_OK;
-    }
-  }
-  tc2_free_maps(m);
-  return IAN_OK;
-}
-
 int finish_maps(ian_handle* h, Plan* pl, std::initializer_list<int> layers) {
   for (int l : layers) {
     char err[256] = {0};
     pl->maps[l] = tc_build_maps(pl->g[l], err, sizeof(err));
     if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
     if (pl->g[l].ksplit == 0) pl->g[l].ksplit = h->splitk ? choose_ksplit(pl->g[l]) : 1;
-    int rc = build_pair_maps(h, pl, l);
-    if (rc != IAN_OK) return rc;
   }
   return alloc_splitk_workspace(h, pl);
 }
@@ -711,7 +662,6 @@ int build_plan(ian_handle* h, int n, Plan** out) {
     pl->maps[l] = tc_build_maps(g[l], err, sizeof(err));
     if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
     if (g[l].ksplit == 0) g[l].ksplit = h->splitk ? choose_ksplit(g[l]) : 1;
-    if ((rc = build_pair_maps(h, pl, l)) != IAN_OK) return rc;
   }
   if ((rc = alloc_splitk_workspace(h, pl)) != IAN_OK) return rc;
   {
@@ -731,7 +681,6 @@ void free_plan(Plan* pl) {
     if (pl->ev_d2h[s]) cudaEventDestroy(pl->ev_d2h[s]);
   }
   for (int l = 0; l < L_COUNT; ++l) if (pl->maps[l]) tc_free_maps(pl->maps[l]);
-  for (int l = 0; l < L_COUNT; ++l) if (pl->maps2[l]) tc2_free_maps(pl->maps2[l]);
   if (pl->decout_maps) decout_free_maps(pl->decout_maps);
   if (pl->conv1_out) conv1_free_out_map(pl->conv1_out);
   if (pl->head_maps) head_free_maps(pl->head_maps);
@@ -768,6 +717,7 @@ int run_gemm(ian_handle* h, Plan* pl, int l, cudaStream_t st) {
   g.passes = h->passes;
   g.out_t_bf16 = (g.out_f32_t && h->passes == 1) ? 1 : 0;   // bf16 mode: the head's tap table travels as bf16
   g.sk_ws = (h->streamk && !h->capturing) ? h->sk_ws : nullptr;   // the stream-K epoch is a kernel argument: not replayable
+  g.sk_force = h->streamk == 2 ? 1 : 0;
   g.sk_flags = h->sk_flags;
   g.sk_epoch = ++h->sk_epoch;
   ian_handle::Timed tm{};
@@ -783,20 +733,7 @@ int run_gemm(ian_handle* h, Plan* pl, int l, cudaStream_t st) {
     if (h->timing) CUDA_TRY(h, cudaEventRecord(tm.e1, st));
   } else {
     if (h->timing) CUDA_TRY(h, cudaEventRecord(tm.e0, st));
-    // pair kernel: float32-split mode (256 x 128 tiles, double-buffered main|cross accumulators) and, in bf16 mode, the
-    // Cout % 256 == 0 layers on 256 x 256 tiles (32 KB per 512-clock stage instead of 48 KB: the 192 KB ring then covers
-    // ~3 k clocks of TMA latency instead of ~2 k; measured +5 % on enc_conv2-4 once the MMA issue was fixed).  Cout = 128
-    // single-pass layers stay on the one-CTA kernel's paired-M tiles (256 x 128 pair tiles: 24 KB stages, measured slower).
-    const int pks = pl->pair_ksplit[l];
-    const bool pair = pl->maps2[l] && (h->passes == 3 || (pks == 1 && g.ksplit == 1 && h->tc2_bf16 && g.Cout % 256 == 0 &&
-                                                          tc2_pair_tiles(g, pl->maps2[l]) / 2 >= h->tc2_min_tiles));
-    if (pair) {
-      g.ksplit = pks;                                       // see build_pair_maps: un-split (1) or the pair kernel's own split
-      if (pks == 1) g.ws = nullptr;
-      LAUNCH_TRY(h, launch_tapgemm_tc2(g, pl->maps2[l], st));
-    } else {
-      LAUNCH_TRY(h, launch_tapgemm_tc(g, pl->maps[l], st));
-    }
+    LAUNCH_TRY(h, launch_tapgemm_tc(g, pl->maps[l], st));
     if (h->timing) CUDA_TRY(h, cudaEventRecord(tm.e1, st));
     if (g.ksplit > 1) LAUNCH_TRY(h, launch_splitk_finalize(g, st));
   }
@@ -1532,8 +1469,8 @@ int ian_create(int model_kind, int device, ian_handle** out) {
   if (device < 0 || device >= ndev) return fail(nullptr, IAN_ERR_INVALID, "device %d out of range [0,%d)", device, ndev);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10)
-    return fail(nullptr, IAN_ERR_UNSUPPORTED, "device %d is sm_%d%d; libian_b200 is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, IAN_ERR_UNSUPPORTED, "device %d is sm_%d%d; libian_b200 is built for sm_90a only", device, prop.major, prop.minor);
   ian_handle* h = new ian_handle();
   h->device = device;
   h->model_kind = model_kind;
@@ -1546,16 +1483,10 @@ int ian_create(int model_kind, int device, ian_handle** out) {
   }
   if (const char* c = getenv("IAN_CHUNK")) { int v = atoi(c); if (v > 0) h->max_chunk = v > 4096 ? 4096 : v; }
   if (const char* c = getenv("IAN_PATH")) { if (!strcmp(c, "simt")) h->path = IAN_PATH_SIMT; }
-  if (const char* c = getenv("IAN_STREAMK")) h->streamk = atoi(c) != 0;
+  if (const char* c = getenv("IAN_STREAMK")) { const int v = atoi(c); h->streamk = v < 0 ? 0 : v > 2 ? 2 : v; }
   if (const char* c = getenv("IAN_SPLITK")) h->splitk = atoi(c) != 0;
-  if (const char* c = getenv("IAN_TC2")) h->tc2 = atoi(c) != 0;
-  if (const char* c = getenv("IAN_TC2_BF16")) h->tc2_bf16 = atoi(c) != 0;
   if (const char* c = getenv("IAN_PDL")) h->pdl = atoi(c) != 0;
   if (const char* c = getenv("IAN_FINALIZE8")) h->coop_finalize = atoi(c) != 0;
-  if (const char* c = getenv("IAN_TC2_SPLITK")) h->tc2_splitk = atoi(c) != 0;
-  if (const char* c = getenv("IAN_TC2_OVER_SPLIT")) h->tc2_over_split = atoi(c) != 0;
-  if (const char* c = getenv("IAN_TC2_MIN")) { int v = atoi(c); if (v > 0) h->tc2_min_tiles = v; }
-  if (const char* c = getenv("IAN_TC2_SKIP")) h->tc2_skip = std::string(",") + c + ",";
   if (const char* c = getenv("IAN_GRAPHS")) h->graphs = atoi(c) != 0;
   *out = h;
   return IAN_OK;
@@ -2159,7 +2090,7 @@ int ian_reconstruct_gather_async_dev(ian_handle* h, const float* x, int n_local,
       CUDA_TRY(h, cudaEventCreateWithFlags(&h->g_comp[b], cudaEventDisableTiming));
       CUDA_TRY(h, cudaEventCreateWithFlags(&h->g_done[b], cudaEventDisableTiming));
     }
-    if (const char* c = getenv("IAN_PUSH_CTAS")) { int v = atoi(c); if (v >= 1 && v <= 148) h->push_ctas = v; }
+    if (const char* c = getenv("IAN_PUSH_CTAS")) { int v = atoi(c); if (v >= 1 && v <= tc_num_sms()) h->push_ctas = v; }
     if (const char* c = getenv("IAN_PUSH")) h->push_mode = !strcmp(c, "kernel") ? 1 : 0;
   }
   const int half_id = h->gcur;
@@ -2173,7 +2104,7 @@ int ian_reconstruct_gather_async_dev(ian_handle* h, const float* x, int n_local,
   const MemOps& mo = memops();
   if (h->push_mode == 0 && mo.write && mo.wait) {
     // copy engines + stream memory operations: nothing of the push occupies an SM, so the next step's persistent tensor
-    // kernels keep all 148 (a co-resident copy KERNEL held its SMs' shared-memory configuration and cost the first three
+    // kernels keep all SMs (a co-resident copy KERNEL held its SMs' shared-memory configuration and cost the first three
     // tap-GEMMs of the next step +60 % at 8 GPUs).  Order on the side stream: publish free[t] to every peer; per peer wait
     // for ITS free[t], then DMA the shard into its buffer; publish pushed[t]; wait for everybody's pushed[t].
     CUstream ps = (CUstream)h->push_stream;

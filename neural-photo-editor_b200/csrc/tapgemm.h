@@ -13,7 +13,7 @@
 //
 // Operands are bf16 SPLIT PLANES: a float32 value v is stored as hi=bf16(v), lo=bf16(v-hi) in two
 // planes of the same NHWC tensor (4 bytes/element, 16 significand bits).  The tensor-core path
-// computes hi*hi + lo*hi + hi*lo with fp32 accumulation (3 tcgen05 MMAs per K step); the SIMT path
+// computes hi*hi + lo*hi + hi*lo with fp32 accumulation (3 wgmma per K step); the SIMT path
 // computes (hi+lo)*(hi+lo) in fp32 FFMA.
 #pragma once
 #include <cuda_bf16.h>
@@ -42,7 +42,7 @@ struct DeviceOnce {
 };
 
 // Programmatic dependent launch (PDL).  A step is a chain of 13-15 short kernels on one stream; with plain launches each
-// boundary costs the launch latency plus the next kernel's prologue (barrier init, TMEM allocation, first descriptor
+// boundary costs the launch latency plus the next kernel's prologue (barrier init, first descriptor
 // fetch) plus the previous kernel's tail, with the SMs idle.  Kernels on the hot chains therefore
 //   * call pdl_trigger() first thing (griddepcontrol.launch_dependents: "my successor may be scheduled as soon as every
 //     CTA of mine has said so or exited" -- for the persistent kernels that means: as my CTAs retire, SM by SM), and
@@ -150,6 +150,7 @@ struct TapGemm {
   float* sk_ws;
   int* sk_flags;
   int sk_epoch;
+  int sk_force;                 // 1: stream-K on every eligible launch, skipping the makespan test (tests use it)
 };
 
 // 128-row M tiles are boxes {Nt images, Ht rows, Wt cols} of the (n, p, q) output grid
@@ -181,16 +182,9 @@ TcMaps* tc_build_maps(const TapGemm& g, char* err, int errlen);
 void tc_free_maps(TcMaps*);
 int launch_tapgemm_tc(const TapGemm& g, const TcMaps* maps, cudaStream_t st);
 int launch_splitk_finalize(const TapGemm& g, cudaStream_t st);
-// CTA-pair path (tapgemm_tc2.cu): tcgen05.mma.cta_group::2, 256 x 128 tiles, double-buffered accumulators in float32
-// mode; whole tiles only (ksplit == 1, no channel-major output)
-struct Tc2Maps;
-Tc2Maps* tc2_build_maps(const TapGemm& g, char* err, int errlen);
-void tc2_free_maps(Tc2Maps*);
-long long tc2_pair_tiles(const TapGemm& g, const Tc2Maps* maps);
-int launch_tapgemm_tc2(const TapGemm& g, const Tc2Maps* maps, cudaStream_t st);
 int tc_tile_width(const TcMaps* maps);
 int tc_num_sms();
-size_t tc_sk_workspace_floats();   // per handle: 148 slots x 128 x 256 fp32
+size_t tc_sk_workspace_floats();   // per handle: one 128 x 256 fp32 slot per SM
 size_t tc_sk_flag_ints();
 
 }  // namespace ian

@@ -1,5 +1,5 @@
 // tapgemm_simt.cu -- fp32 FFMA implementation of the shifted-tap GEMM (see tapgemm.h).
-// This is the verification path (IAN_PATH_SIMT): it shares no arithmetic with the tcgen05 kernel
+// This is the verification path (IAN_PATH_SIMT): it shares no arithmetic with the wgmma kernel
 // (operands are re-joined to fp32, products and sums are plain FFMA), so the two check each other on
 // the GPU.  Also hosts the split-K finalize kernel used by the tensor-core path.
 #include "tapgemm.h"

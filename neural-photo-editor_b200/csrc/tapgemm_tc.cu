@@ -1,21 +1,23 @@
-// tapgemm_tc.cu -- tcgen05 / TMEM / TMA implementation of the shifted-tap GEMM (see tapgemm.h).
+// tapgemm_tc.cu -- wgmma / TMA implementation of the shifted-tap GEMM (see tapgemm.h) for Hopper (sm_90a).
 //
 // A persistent CTA (one per SM) computes 128 (pixels) x BN (output channels) tiles of the output phases:
-//   warp 0     : TMA producer.  Per K step (one tap x 64 input channels) two bulk-tensor loads:
+//   warp 8     : TMA producer.  Per K step (one tap x 64 input channels) two bulk-tensor loads:
 //                a 5-D box {64 ch, Wt, Ht, Nt, 2 planes} of the activation view the tap reads -- the
 //                tap shift is just a coordinate offset and the zero padding of the convolution is
 //                TMA's out-of-bounds fill -- and a 3-D box {64 ch, BN, 2 planes} of the tap's weights.
-//                Both land in the 128B-swizzled K-major layout tcgen05 consumes; no im2col buffer
+//                Both land in the 128B-swizzled K-major layout wgmma consumes; no im2col buffer
 //                ever exists in HBM or shared memory.
-//   warp 1     : TMEM allocation + single-thread tcgen05.mma issue.  fp32 fidelity from bf16 tensor
+//   warps 0..7 : two consumer warpgroups, one per 64-row half of the tile.  fp32 fidelity from bf16 tensor
 //                cores: per K=16 slice   main  += A_hi * B_hi
 //                                         cross += A_lo * B_hi ;  cross += A_hi * B_lo
-//                in two separate TMEM accumulators (the 2^-9-smaller cross terms get their own
-//                accumulator so their rounding does not ride on the main sum's exponent).
-//   warps 2..9 : epilogue.  tcgen05.ld both accumulators, add, BatchNorm scale/shift + activation
-//                (or backward scale * ReLU-mask), re-split to bf16 hi/lo planes and store NHWC at
-//                the phase's output stride; or store raw sums to this K split's workspace slab.
-// Pipeline: STAGES-deep smem ring with full/empty mbarriers (TMA -> MMA -> tcgen05.commit).
+//                in two separate register accumulators (the 2^-9-smaller cross terms get their own
+//                accumulator so their rounding does not ride on the main sum's exponent).  After the last K
+//                step the sum main + cross goes through a float32 staging tile in shared memory, and the same
+//                eight warps run the epilogue one pixel row per thread: BatchNorm scale/shift + activation
+//                (or backward scale * ReLU-mask), re-split to bf16 hi/lo planes and store NHWC at the phase's
+//                output stride; or store raw sums to this K split's workspace slab.
+// Pipeline: STAGES-deep smem ring with full/empty mbarriers (TMA -> wgmma -> release after wgmma.wait_group); the
+// producer runs ahead across work items, so the next tile's operands load while the epilogue of this one runs.
 #include <cuda.h>
 
 #include <cstdio>
@@ -43,46 +45,40 @@ using namespace tc;
 constexpr int BM = 128;
 constexpr int BK = 64;
 
-
-constexpr int kEpiWarps = 8;
+constexpr int kEpiWarps = 8;                 // the two consumer warpgroups
+constexpr int kThreadsCta = 32 * kEpiWarps + 32;
 
 // PASSES = 3: float32 fidelity, operands are bf16 hi|lo planes, 3 MMAs per K slice, main|cross accumulators.
 // PASSES = 1: plain bf16 (BASELINE configs[2]): hi planes only, 1 MMA per K slice, one accumulator.
-// MT = M tiles (128 pixels each) per work item sharing ONE weight tile: MT = 2 turns the Cout = 128 layers from
-// operand-feed-bound (64 KB of smem fill per 128x128x64 MMA block) into the 128x256-equivalent intensity.
-template <int BN, int PASSES, int MT, int EW = 8> struct TcCfg {
+// BN <= 128: a warpgroup holds 64 x BN float32 accumulators (BN / 2 registers per thread, twice that in float32 mode).
+template <int BN, int PASSES> struct TcCfg {
   static constexpr int kPlanes = PASSES == 3 ? 2 : 1;
   static constexpr int kATileBytes = BM * BK * 2 * kPlanes;
   static constexpr int kBTileBytes = BN * BK * 2 * kPlanes;
-  static constexpr int kStageBytes = MT * kATileBytes + kBTileBytes;
-  static constexpr int kStagesFit = (196 * 1024) / kStageBytes;
+  static constexpr int kStageBytes = kATileBytes + kBTileBytes;
+  static constexpr int kLd = BN + 8;                           // staging row pitch in floats (conflict-free fragment stores)
+  static constexpr int kStagingBytes = BM * kLd * 4;
+  static constexpr int kStageSmem = kEpiWarps * 1024;          // per-warp scale|shift staging
+  static constexpr int kStagesFit = (220 * 1024 - kStagingBytes - kStageSmem) / kStageBytes;
   static constexpr int kStages = kStagesFit > 6 ? 6 : kStagesFit;
-  static constexpr int kTileCols = (PASSES == 3 ? 2 : 1) * BN; // TMEM columns of one tile's accumulators: main | cross
-  static constexpr int kAccCols = MT * kTileCols;              // ... of one buffer
-  static constexpr int kAccBufs = (2 * kAccCols <= 512) ? 2 : 1;
-  static constexpr int kTmemCols = (kAccBufs * kAccCols <= 32) ? 32 : (kAccBufs * kAccCols <= 64) ? 64 : 512;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + EW * 1024;
-  static constexpr int kThreadsCta = 64 + 32 * EW;     // producer, MMA, EW epilogue warps
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kStageSmem + kStagingBytes;
+  static_assert(kStages >= 2 && kSmemBytes <= 232448, "tapgemm_tc: shared memory budget");
 };
-
-template <int BN> __device__ __forceinline__ constexpr uint32_t make_idesc() { return tc::make_idesc_bf16_m128(BN); }
 
 // ---------------------------------------------------------------- kernel
 // Persistent, warp-specialised.  Work items w = blockIdx.x + i*gridDim.x over
-// (phase | k-split | n-tile | m-tile), longest phases first.  The smem ring and the TMEM accumulator
-// buffers run ACROSS work items: the producer prefetches the next tile's operands while the epilogue
-// of the current tile drains TMEM, and (when two accumulator buffers fit in the 512 TMEM columns) the
-// MMA warp starts the next tile while the epilogue warps are still converting/storing the previous one.
+// (phase | k-split | n-tile | m-tile), longest phases first.  The smem ring runs ACROSS work items: the producer
+// prefetches the next tile's operands while the consumers run the epilogue of the current one.
 struct WorkItem {
   int phase, ks, co0, it0, it1;
-  int n0[2], p0[2], q0[2], mtile[2];   // up to MT = 2 M tiles
+  int n0, p0, q0, mtile;
   // stream-K (SK): 0 = the segment is a whole tile; 1 = contributor (a later part of a tile: raw sums go to this
   // CTA's workspace slot); 2 = finisher (the first part of a tile cut by a CTA boundary: adds the partial sums of
   // CTAs blockIdx.x+1 .. sk_last, then runs the epilogue)
   int sk_role, sk_last;
 };
 
-// CH float32 values -> bf16 hi|lo planes (hi only in single-pass mode), packed bf16x2 conversions, 16-byte stores
+// CH float32 values -> bf16 hi|lo planes (hi only in single-pass mode), packed bf16x2 conversions, 32-byte sector stores
 template <int CH, int PASSES>
 __device__ __forceinline__ void store_split(__nv_bfloat16* dst, long long plane, const float (&v)[CH]) {
   __align__(16) __nv_bfloat162 hi[CH / 2], lo[CH / 2];
@@ -104,31 +100,22 @@ __device__ __forceinline__ void store_split(__nv_bfloat16* dst, long long plane,
   }
 }
 
-template <int BN, int MT>
+template <int BN>
 __device__ __forceinline__ WorkItem decode_work(const TapGemm& g, const TcMaps& maps, int w) {
   WorkItem wi;
   const int tiles_q = g.Wg / maps.Wt, tiles_p = g.Hg / maps.Ht;
   const int tiles_m = tiles_q * tiles_p * ((g.n_img + maps.Nt - 1) / maps.Nt);
-  const int groups_m = (tiles_m + MT - 1) / MT;
   const int tiles_n = g.Cout / BN;
-  const int per_phase = groups_m * tiles_n * g.ksplit;
+  const int per_phase = tiles_m * tiles_n * g.ksplit;
   wi.phase = w / per_phase;
   int r = w % per_phase;
-  const int mg = r % groups_m; r /= groups_m;
+  int mt = r % tiles_m; r /= tiles_m;
   const int nt = r % tiles_n; r /= tiles_n;
   wi.ks = r;
-#pragma unroll
-  for (int j = 0; j < MT; ++j) {
-    int mt = mg * MT + j;
-    wi.mtile[j] = mt;
-    if (mt >= tiles_m) {                                // odd tile count: phantom tile, fully out of range
-      wi.n0[j] = g.n_img; wi.p0[j] = 0; wi.q0[j] = 0;
-      continue;
-    }
-    const int qb = mt % tiles_q; mt /= tiles_q;
-    const int pb = mt % tiles_p; mt /= tiles_p;
-    wi.n0[j] = mt * maps.Nt; wi.p0[j] = pb * maps.Ht; wi.q0[j] = qb * maps.Wt;
-  }
+  wi.mtile = mt;
+  const int qb = mt % tiles_q; mt /= tiles_q;
+  const int pb = mt % tiles_p; mt /= tiles_p;
+  wi.n0 = mt * maps.Nt; wi.p0 = pb * maps.Ht; wi.q0 = qb * maps.Wt;
   wi.co0 = nt * BN;
   const int total_it = g.phase[wi.phase].ntaps * (g.Cin / BK);
   wi.it0 = (int)((long long)total_it * wi.ks / g.ksplit);
@@ -138,11 +125,11 @@ __device__ __forceinline__ WorkItem decode_work(const TapGemm& g, const TcMaps& 
 
 // Work iteration of one CTA.  SK = false: whole tiles, w = blockIdx.x + i*gridDim.x (longest phases first).
 // SK = true (stream-K): the launch is ONE linear space of T K-steps over (phase | n-tile | m-tile | K step) and CTA c
-// owns steps [T*c/G, T*(c+1)/G): every SM gets the same tensor work however the tile count divides by 148 and
+// owns steps [T*c/G, T*(c+1)/G): every SM gets the same tensor work however the tile count divides by the SM count and
 // however unequal the phases are.  A tile cut by a CTA boundary is finished by the CTA holding its FIRST K steps
 // (which it reaches at the END of its range), after the CTAs holding the later steps (which they run FIRST) have
 // published their raw partial sums -- an ordered, atomic-free, deterministic fix-up.
-template <int BN, int MT, bool SK>
+template <int BN, bool SK>
 struct WorkIter {
   int w, total, stride;                 // !SK
   int T, G, cur, end, iters[kMaxPhases], tiles_per_phase, tiles_m, tiles_q, tiles_p;   // SK
@@ -165,7 +152,7 @@ struct WorkIter {
   __device__ __forceinline__ bool next(const TapGemm& g, const TcMaps& maps, WorkItem& wi) {
     if (!SK) {
       if (w >= total) return false;
-      wi = decode_work<BN, MT>(g, maps, w);
+      wi = decode_work<BN>(g, maps, w);
       wi.sk_role = 0; wi.sk_last = 0;
       w += stride;
       return true;
@@ -180,10 +167,10 @@ struct WorkIter {
     wi.phase = ph; wi.ks = 0; wi.it0 = it; wi.it1 = it + len;
     int mt = tile % tiles_m;
     const int nt = tile / tiles_m;
-    wi.mtile[0] = mt;
+    wi.mtile = mt;
     const int qb = mt % tiles_q; mt /= tiles_q;
     const int pb = mt % tiles_p; mt /= tiles_p;
-    wi.n0[0] = mt * maps.Nt; wi.p0[0] = pb * maps.Ht; wi.q0[0] = qb * maps.Wt; wi.co0 = nt * BN;
+    wi.n0 = mt * maps.Nt; wi.p0 = pb * maps.Ht; wi.q0 = qb * maps.Wt; wi.co0 = nt * BN;
     wi.sk_role = it > 0 ? 1 : (len < ip ? 2 : 0);
     wi.sk_last = wi.sk_role == 2 ? owner(phase_start + tile * ip + ip - 1) : 0;
     cur = gi + len;
@@ -191,13 +178,10 @@ struct WorkIter {
   }
 };
 
-// EW = epilogue warps: 8, or 16 for the short-K single-pass layers whose epilogue (convert + store of 2 x 128 x 128 outputs) is
-// longer than their main loop -- four warps per TMEM lane group, each draining a quarter of the columns.
-template <int BN, int PASSES, int MT, bool SK, int EW = 8>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+template <int BN, int PASSES, bool SK>
+__global__ void __launch_bounds__(kThreadsCta, 1)
 tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcMaps maps, const int total_work) {
-  using Cfg = TcCfg<BN, PASSES, MT, EW>;
-  static_assert(EW == 8 || (EW == 16 && !SK && BN >= 128), "16 epilogue warps: whole-tile schedule, >= 128 columns");
+  using Cfg = TcCfg<BN, PASSES>;
   constexpr int kATileBytes = Cfg::kATileBytes;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -205,13 +189,10 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
   const uint32_t bar_base = smem_base + S * Cfg::kStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * S + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * S + 2 + b); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * S + 4);
   const uint32_t stage_smem = bar_base + 256u;       // per-epilogue-warp scale|shift staging: 8 x (128 + 128) floats
   uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_al + (tmem_slot - smem_base));
   float* stage_ptr = reinterpret_cast<float*>(smem_al + (stage_smem - smem_base));
+  float* acc_tile = stage_ptr + kEpiWarps * 256;     // [BM][kLd] float32: the finished accumulators of one tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -219,311 +200,274 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
     pdl_trigger();                                      // the next kernel of the chain may move in as this grid's CTAs retire
     for (int s = 0; s < S; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), EW);
+      mbar_init(empty_bar(s), 2);                       // one arrival per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   pdl_wait();                                           // prologue done; everything below reads / writes activations (tapgemm.h: PDL)
   const int nchunk = g.Cin / BK;
 
-  if (warp == 0) {
+  if (warp == kEpiWarps) {
     // ===================== TMA producer (whole warp in uniform control flow, one elected lane issues) =====================
-    {
-      uint32_t i = 0;                                   // running K-step counter across work items
-      WorkIter<BN, MT, SK> iter;
-      iter.init(g, maps, total_work);
-      WorkItem wi;
-      while (iter.next(g, maps, wi)) {
-        const Phase ph = g.phase[wi.phase];
-        for (int it = wi.it0; it < wi.it1; ++it, ++i) {
-          const int s = i % S;
-          const uint32_t par = (i / S) & 1u;
-          const Tap tap = g.taps[ph.tap_begin + it / nchunk];
-          const int c0 = (it % nchunk) * BK;
-          mbar_wait(empty_bar(s), par ^ 1u);
-          const uint32_t sa = smem_base + s * Cfg::kStageBytes;
-          if (elect_one_sync()) {
-            mbar_expect_tx(full_bar(s), Cfg::kStageBytes);
-#pragma unroll
-            for (int j = 0; j < MT; ++j)
-              tma_load_5d(PASSES == 3 ? &maps.a[tap.view] : &maps.a1[tap.view], full_bar(s), sa + j * kATileBytes, c0,
-                          wi.q0[j] + tap.dw, wi.p0[j] + tap.dh, wi.n0[j], 0);
-            tma_load_3d(PASSES == 3 ? &maps.b : &maps.b1, full_bar(s), sa + MT * kATileBytes, c0, tap.wtile * g.Cout + wi.co0, 0);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp walks the schedule; one elected lane issues: descriptors stay in
-    // uniform registers instead of an ELECT + R2UR waterfall per UTCHMMA) =====================
-    {
-      constexpr uint32_t idesc = make_idesc<BN>();
-      uint32_t i = 0, t = 0;
-      WorkIter<BN, MT, SK> iter;
-      iter.init(g, maps, total_work);
-      WorkItem wi;
-      for (; iter.next(g, maps, wi); ++t) {
-        const uint32_t buf = t % Cfg::kAccBufs, use = t / Cfg::kAccBufs;
-        const uint32_t acc_base = tmem_base + buf * Cfg::kAccCols;
-        mbar_wait(tempty_bar(buf), (use & 1u) ^ 1u);    // epilogue has drained this buffer
-        tc_fence_after();
-        for (int it = wi.it0; it < wi.it1; ++it, ++i) {
-          const int s = i % S;
-          const uint32_t par = (i / S) & 1u;
-          mbar_wait(full_bar(s), par);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * Cfg::kStageBytes;
-          const uint64_t b_hi = make_sw128_desc(sa + MT * kATileBytes), b_lo = make_sw128_desc(sa + MT * kATileBytes + BN * BK * 2);
-          const uint32_t first = (it == wi.it0) ? 0u : 1u;
-          if (elect_one_sync()) {
-#pragma unroll
-            for (int j = 0; j < MT; ++j) {
-              const uint64_t a_hi = make_sw128_desc(sa + j * kATileBytes), a_lo = make_sw128_desc(sa + j * kATileBytes + BM * BK * 2);
-              const uint32_t acc_main = acc_base + j * Cfg::kTileCols, acc_cross = acc_main + BN;
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t ko = (uint64_t)(k * 2);   // 32 bytes per K=16 slice, in 16-byte units
-                const uint32_t acc = k > 0 ? 1u : first;
-                umma_bf16(acc_main, a_hi + ko, b_hi + ko, idesc, acc);
-                if (PASSES == 3) {
-                  umma_bf16(acc_cross, a_lo + ko, b_hi + ko, idesc, acc);
-                  umma_bf16(acc_cross, a_hi + ko, b_lo + ko, idesc, 1u);
-                }
-              }
-            }
-            umma_commit(empty_bar(s));                    // frees the smem stage when these MMAs retire
-          }
-          __syncwarp();
-        }
-        if (elect_one_sync()) umma_commit(tfull_bar(buf));   // accumulators of this work item complete
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    constexpr int CH = (BN >= 64) ? 32 : 16;            // columns per tcgen05.ld
-    constexpr int COLS_PER_WARP = (BN >= 64) ? BN / (EW / 4) : BN;
-    const int ew = warp - 2;
-    const int lg = warp & 3;                            // TMEM lane group this warp may access
-    const int half = ew >> 2;                           // which slice (half, or quarter with 16 warps) of the tile's columns
-    const bool has_cols = (BN >= 64) || half == 0;
-    float* my_stage = stage_ptr + ew * 256;             // [0,128): scale, [128,256): shift of this warp's columns
-    // activation as a branch-free a*t + b*|t| (none / LeakyRectify(0.2) / rectify; lasagne forms, SURVEY C.5)
-    const float act_a = g.act == ACT_LRELU ? 0.6f : g.act == ACT_RELU ? 0.5f : 1.f;
-    const float act_b = g.act == ACT_LRELU ? 0.4f : g.act == ACT_RELU ? 0.5f : 0.f;
-    const int ml = lg * 32 + lane;                      // tile row
-    const int wl = ml % maps.Wt;
-    const int hl = (ml / maps.Wt) % maps.Ht;
-    const int nl = ml / (maps.Wt * maps.Ht);
-    uint32_t t = 0;
-    WorkIter<BN, MT, SK> iter;
+    uint32_t i = 0;                                     // running K-step counter across work items
+    WorkIter<BN, SK> iter;
     iter.init(g, maps, total_work);
     WorkItem wi;
-    for (; iter.next(g, maps, wi); ++t) {
+    while (iter.next(g, maps, wi)) {
       const Phase ph = g.phase[wi.phase];
-      const uint32_t buf = t % Cfg::kAccBufs, use = t / Cfg::kAccBufs;
-      if (has_cols && g.scale_pix_stride == 0) {         // stage this tile's per-channel scale/shift while the MMAs run
-        __syncwarp();
-        const int cbase = wi.co0 + half * COLS_PER_WARP;
-        for (int c = lane; c < COLS_PER_WARP; c += 32) {
-          my_stage[c] = g.scale ? __ldg(g.scale + cbase + c) : 1.f;
-          my_stage[128 + c] = g.shift ? __ldg(g.shift + cbase + c) : 0.f;
+      for (int it = wi.it0; it < wi.it1; ++it, ++i) {
+        const int s = i % S;
+        const uint32_t par = (i / S) & 1u;
+        const Tap tap = g.taps[ph.tap_begin + it / nchunk];
+        const int c0 = (it % nchunk) * BK;
+        mbar_wait(empty_bar(s), par ^ 1u);
+        const uint32_t sa = smem_base + s * Cfg::kStageBytes;
+        if (elect_one_sync()) {
+          mbar_expect_tx(full_bar(s), Cfg::kStageBytes);
+          tma_load_5d(PASSES == 3 ? &maps.a[tap.view] : &maps.a1[tap.view], full_bar(s), sa, c0, wi.q0 + tap.dw,
+                      wi.p0 + tap.dh, wi.n0, 0);
+          tma_load_3d(PASSES == 3 ? &maps.b : &maps.b1, full_bar(s), sa + kATileBytes, c0, tap.wtile * g.Cout + wi.co0, 0);
         }
         __syncwarp();
       }
-      mbar_wait(tfull_bar(buf), use & 1u);
-      tc_fence_after();
-      if (has_cols && wi.it1 > wi.it0) {
-       if (SK && wi.sk_role == 2) {                      // finisher: the later parts were computed first; wait for them
-         for (int k = (int)blockIdx.x + 1 + lane; k <= wi.sk_last; k += 32) {
-           const int* fl = g.sk_flags + k * kEpiWarps + ew;
-           const long long t0 = clock64();
-           int fv;
-           do {
-             asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(fv) : "l"(fl) : "memory");
-             if (clock64() - t0 > 4000000000LL) __trap();
-           } while (fv != g.sk_epoch);
-         }
-         __syncwarp();
-       }
+    }
+    return;
+  }
+
+  // ===================== consumers (warps 0..7): wgmma main loop, then the epilogue =====================
+  constexpr int R = BN / 2;                             // accumulator registers per thread and accumulator
+  constexpr int CH = (BN >= 64) ? 32 : 16;              // columns per epilogue chunk
+  constexpr int COLS_PER_WARP = (BN >= 64) ? BN / 2 : BN;
+  const int wg = warp >> 2, wtid = threadIdx.x & 127;
+  const int ew = warp;
+  const int lg = warp & 3;                              // 32-row group of the tile this warp's epilogue handles
+  const int half = ew >> 2;                             // which half of the tile's columns
+  const bool has_cols = (BN >= 64) || half == 0;
+  float* my_stage = stage_ptr + ew * 256;               // [0,128): scale, [128,256): shift of this warp's columns
+  // activation as a branch-free a*t + b*|t| (none / LeakyRectify(0.2) / rectify; lasagne forms, SURVEY C.5)
+  const float act_a = g.act == ACT_LRELU ? 0.6f : g.act == ACT_RELU ? 0.5f : 1.f;
+  const float act_b = g.act == ACT_LRELU ? 0.4f : g.act == ACT_RELU ? 0.5f : 0.f;
+  const int ml = lg * 32 + lane;                        // tile row of this thread's epilogue
+  const int wl = ml % maps.Wt;
+  const int hl = (ml / maps.Wt) % maps.Ht;
+  const int nl = ml / (maps.Wt * maps.Ht);
+  uint32_t i = 0;
+  WorkIter<BN, SK> iter;
+  iter.init(g, maps, total_work);
+  WorkItem wi;
+  while (iter.next(g, maps, wi)) {
+    const Phase ph = g.phase[wi.phase];
+    if (wi.it1 <= wi.it0) continue;                     // (uniform over the CTA)
+    if (has_cols && g.scale_pix_stride == 0) {          // stage this tile's per-channel scale/shift while the MMAs run
+      __syncwarp();
+      const int cbase = wi.co0 + half * COLS_PER_WARP;
+      for (int c = lane; c < COLS_PER_WARP; c += 32) {
+        my_stage[c] = g.scale ? __ldg(g.scale + cbase + c) : 1.f;
+        my_stage[128 + c] = g.shift ? __ldg(g.shift + cbase + c) : 0.f;
+      }
+      __syncwarp();
+    }
+    // ---- main loop: this warpgroup's 64 rows x BN columns (declared per tile: dead during the epilogue)
+    float acc_m[R], acc_c[PASSES == 3 ? R : 1];
+#pragma unroll
+    for (int j = 0; j < R; ++j) acc_m[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (PASSES == 3 ? R : 1); ++j) acc_c[j] = 0.f;
+    wgmma_fence_regs(acc_m);
+    if (PASSES == 3) wgmma_fence_regs(acc_c);
+    for (int it = wi.it0; it < wi.it1; ++it, ++i) {
+      const int s = i % S;
+      mbar_wait(full_bar(s), (i / S) & 1u);
+      const uint32_t sa = smem_base + s * Cfg::kStageBytes;
+      const uint64_t a_hi = make_sw128_desc(sa + wg * 64 * 128), a_lo = make_sw128_desc(sa + BM * BK * 2 + wg * 64 * 128);
+      const uint64_t b_hi = make_sw128_desc(sa + kATileBytes), b_lo = make_sw128_desc(sa + kATileBytes + BN * BK * 2);
+      const uint32_t first = (it == wi.it0) ? 0u : 1u;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t ko = (uint64_t)(k * 2);         // 32 bytes per K=16 slice, in 16-byte units
+        const uint32_t acc = k > 0 ? 1u : first;
+        wgmma_bf16<BN>(acc_m, a_hi + ko, b_hi + ko, acc);
+        if constexpr (PASSES == 3) {
+          wgmma_bf16<BN>(acc_c, a_lo + ko, b_hi + ko, acc);
+          wgmma_bf16<BN>(acc_c, a_hi + ko, b_lo + ko, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                  // the previous K step's MMAs have retired: free its stage
+      if (it > wi.it0 && wtid == 0) mbar_arrive(empty_bar((i - 1) % S));
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc_m);
+    if (PASSES == 3) wgmma_fence_regs(acc_c);
+    if (wtid == 0) mbar_arrive(empty_bar((i - 1) % S));
+    // ---- accumulators -> float32 staging tile (row-per-thread access for the epilogue)
+    asm volatile("bar.sync 1, 256;" ::: "memory");      // the previous tile's epilogue has read the staging tile
+#pragma unroll
+    for (int j = 0; j < R; j += 2) {
+      const int row = wg * 64 + frag_row(wtid, j), col = frag_col(wtid, j);
+      float2 v = make_float2(acc_m[j], acc_m[j + 1]);
+      if constexpr (PASSES == 3) { v.x += acc_c[j]; v.y += acc_c[j + 1]; }
+      *reinterpret_cast<float2*>(acc_tile + row * Cfg::kLd + col) = v;
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (!has_cols) continue;
+    // ===================== epilogue =====================
+    if (SK && wi.sk_role == 2) {                        // finisher: the later parts were computed first; wait for them
+      for (int k = (int)blockIdx.x + 1 + lane; k <= wi.sk_last; k += 32) {
+        if (iter.boundary(k) == iter.boundary(k + 1)) continue;   // a CTA without K steps (T < G) publishes nothing
+        const int* fl = g.sk_flags + k * kEpiWarps + ew;
+        const long long t0 = clock64();
+        int fv;
+        do {
+          asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(fv) : "l"(fl) : "memory");
+          if (clock64() - t0 > 4000000000LL) __trap();
+        } while (fv != g.sk_epoch);
+      }
+      __syncwarp();
+    }
+    const int n = wi.n0 + nl, p = wi.p0 + hl, q = wi.q0 + wl;
+    const bool valid = n < g.n_img;
+    const int oh = p * g.osh + ph.oh0, ow = q * g.osw + ph.ow0;
+    const long long pix = (long long)(n * g.Hout + oh) * g.Wout + ow;
 #pragma unroll 1
-       for (int tj = 0; tj < MT; ++tj) {
-        const int n = wi.n0[tj] + nl, p = wi.p0[tj] + hl, q = wi.q0[tj] + wl;
-        const bool valid = n < g.n_img;
-        const int oh = p * g.osh + ph.oh0, ow = q * g.osw + ph.ow0;
-        const long long pix = (long long)(n * g.Hout + oh) * g.Wout + ow;
-        const uint32_t lane_addr = tmem_base + buf * Cfg::kAccCols + tj * Cfg::kTileCols + ((uint32_t)(lg * 32) << 16);
-#pragma unroll 1
-        for (int cc = 0; cc < COLS_PER_WARP; cc += CH) {
-          const int cb = half * COLS_PER_WARP + cc;
-          const int co = wi.co0 + cb;
-          float v[CH];
-          __syncwarp();                                 // tcgen05.ld is .aligned: reconverge first
-          if (PASSES == 3) {
-            uint32_t vm[CH], vc[CH];
-            tmem_ld<CH>(lane_addr + cb, vm);
-            tmem_ld<CH>(lane_addr + BN + cb, vc);
-            tmem_ld_wait();
+    for (int cc = 0; cc < COLS_PER_WARP; cc += CH) {
+      const int cb = half * COLS_PER_WARP + cc;
+      const int co = wi.co0 + cb;
+      float v[CH];
+      const float* srow = acc_tile + ml * Cfg::kLd + cb;
 #pragma unroll
-            for (int j = 0; j < CH; ++j) v[j] = __uint_as_float(vm[j]) + __uint_as_float(vc[j]);
-          } else {
-            uint32_t vm[CH];
-            tmem_ld<CH>(lane_addr + cb, vm);
-            tmem_ld_wait();
+      for (int j = 0; j < CH / 4; ++j) {
+        const float4 t4 = *reinterpret_cast<const float4*>(srow + 4 * j);
+        v[4 * j] = t4.x; v[4 * j + 1] = t4.y; v[4 * j + 2] = t4.z; v[4 * j + 3] = t4.w;
+      }
+      if (SK && wi.sk_role == 1) {                     // contributor: raw partial sums -> this CTA's workspace slot
+        float4* wp = reinterpret_cast<float4*>(g.sk_ws + (((long long)blockIdx.x * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
 #pragma unroll
-            for (int j = 0; j < CH; ++j) v[j] = __uint_as_float(vm[j]);
+        for (int j = 0; j < CH / 4; ++j) __stcg(wp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+        continue;
+      }
+      if (SK && wi.sk_role == 2) {                     // finisher: add the later parts, in CTA order
+        for (int k = (int)blockIdx.x + 1; k <= wi.sk_last; ++k) {
+          if (iter.boundary(k) == iter.boundary(k + 1)) continue;
+          const float4* rp = reinterpret_cast<const float4*>(g.sk_ws + (((long long)k * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
+#pragma unroll
+          for (int j = 0; j < CH / 4; ++j) {
+            const float4 a = __ldcg(rp + j);
+            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
           }
-          if (tj == MT - 1 && cc + CH >= COLS_PER_WARP) { // last TMEM read of this work item: release the buffer
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(buf));
-          }
-          if (SK && wi.sk_role == 1) {                   // contributor: raw partial sums -> this CTA's workspace slot
-            float4* wp = reinterpret_cast<float4*>(g.sk_ws + (((long long)blockIdx.x * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
+        }
+      }
+      if (g.ksplit > 1) {
+        if (valid) {                                    // this K split's slab; the finalize kernel adds them in order
+          float4* wsp = reinterpret_cast<float4*>(g.ws + (long long)wi.ks * g.ws_slab + pix * g.Cout + co);
 #pragma unroll
-            for (int j = 0; j < CH / 4; ++j) __stcg(wp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-            continue;
-          }
-          if (SK && wi.sk_role == 2) {                   // finisher: add the later parts, in CTA order
-            for (int k = (int)blockIdx.x + 1; k <= wi.sk_last; ++k) {
-              const float4* rp = reinterpret_cast<const float4*>(g.sk_ws + (((long long)k * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
+          for (int j = 0; j < CH / 4; ++j) __stcg(wsp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+        }
+        continue;
+      }
+      if (valid) {
+        const long long off = pix * g.Cout + co;
+        if (g.out_raw) store_split<CH, PASSES>(g.out_raw + off, g.out_raw_plane, v);   // pre-BN value (MDBLOCK residual input)
+        if (g.res && !g.res_after) {                                   // residual add before BatchNorm (MDBLOCK, layers.py:411-416)
+          const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
+          const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
 #pragma unroll
-              for (int j = 0; j < CH / 4; ++j) {
-                const float4 a = __ldcg(rp + j);
-                v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-              }
-            }
-          }
-          if (g.ksplit > 1) {
-            if (valid) {                                  // this K split's slab; the finalize kernel adds them in order
-              float4* wsp = reinterpret_cast<float4*>(g.ws + (long long)wi.ks * g.ws_slab + pix * g.Cout + co);
+          for (int j8 = 0; j8 < CH / 8; ++j8) {
+            const uint4 h4 = __ldg(rh + j8);
+            const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
+            if (PASSES == 3) {
+              const uint4 l4 = __ldg(rl + j8);
+              const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
 #pragma unroll
-              for (int j = 0; j < CH / 4; ++j) __stcg(wsp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-            }
-            continue;
-          }
-          if (valid) {
-            const long long off = pix * g.Cout + co;
-            if (g.out_raw) store_split<CH, PASSES>(g.out_raw + off, g.out_raw_plane, v);   // pre-BN value (MDBLOCK residual input)
-            if (g.res && !g.res_after) {                                   // residual add before BatchNorm (MDBLOCK, layers.py:411-416)
-              const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
-              const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
-#pragma unroll
-              for (int j8 = 0; j8 < CH / 8; ++j8) {
-                const uint4 h4 = __ldg(rh + j8);
-                const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
-                if (PASSES == 3) {
-                  const uint4 l4 = __ldg(rl + j8);
-                  const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
-                }
-              }
-            }
-            if (g.act == ACT_MASK) {
-              const int si = co + (oh * g.Wout + ow) * g.scale_pix_stride;
-              const uint4* mk = reinterpret_cast<const uint4*>(g.mask + off);
-#pragma unroll
-              for (int j8 = 0; j8 < CH / 8; ++j8) {
-                const uint4 m4 = __ldg(mk + j8);
-                const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float sc = g.scale_pix_stride ? __ldg(g.scale + si + j8 * 8 + j) : my_stage[cc + j8 * 8 + j];
-                  v[j8 * 8 + j] = v[j8 * 8 + j] * sc * (__bfloat162float(mb[j]) > 0.f ? 1.f : g.mask_slope);
-                }
-              }
-              if (g.res && g.res_after) {                    // gradient of the block's residual branch joins after the mask/scale
-                const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
-                const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
-#pragma unroll
-                for (int j8 = 0; j8 < CH / 8; ++j8) {
-                  const uint4 h4 = __ldg(rh + j8);
-                  const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
-                  if (PASSES == 3) {
-                    const uint4 l4 = __ldg(rl + j8);
-                    const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
-                  } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
-                  }
-                }
-              }
+              for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
             } else {
 #pragma unroll
-              for (int j4 = 0; j4 < CH / 4; ++j4) {
-                const float4 sc = *reinterpret_cast<const float4*>(my_stage + cc + 4 * j4);
-                const float4 sf = *reinterpret_cast<const float4*>(my_stage + 128 + cc + 4 * j4);
-                v[4 * j4 + 0] = fmaf(v[4 * j4 + 0], sc.x, sf.x);
-                v[4 * j4 + 1] = fmaf(v[4 * j4 + 1], sc.y, sf.y);
-                v[4 * j4 + 2] = fmaf(v[4 * j4 + 2], sc.z, sf.z);
-                v[4 * j4 + 3] = fmaf(v[4 * j4 + 3], sc.w, sf.w);
-              }
-              if (g.act == ACT_ELU) {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.f ? v[j] : expm1f(v[j]);
-              } else if (g.act != ACT_NONE) {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) v[j] = fmaf(act_b, fabsf(v[j]), act_a * v[j]);
-              }
-            }
-            if (g.out) store_split<CH, PASSES>(g.out + off, g.out_plane, v);
-            if (g.out_f32_t) {                           // tile-blocked channel-major table: [m-tile][co][128 rows]
-              const long long tbase = ((long long)wi.mtile[tj] * g.cout_real + co) * BM + ml;
-              if (g.out_t_bf16) {
-                __nv_bfloat16* ot = reinterpret_cast<__nv_bfloat16*>(g.out_f32_t) + tbase;
-#pragma unroll
-                for (int j = 0; j < CH; ++j)
-                  if (co + j < g.cout_real) ot[j * BM] = __float2bfloat16_rn(v[j]);   // a warp writes 64 contiguous bytes per column
-              } else {
-                float* ot = g.out_f32_t + tbase;
-#pragma unroll
-                for (int j = 0; j < CH; ++j)
-                  if (co + j < g.cout_real) ot[j * BM] = v[j];   // a warp writes 128 contiguous bytes per column
-              }
-            }
-            if (g.out_f32) {
-              float4* of = reinterpret_cast<float4*>(g.out_f32 + off);
-#pragma unroll
-              for (int j = 0; j < CH / 4; ++j) of[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+              for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
             }
           }
         }
-       }
-       if (SK && wi.sk_role == 1) {                      // publish this warp's sub-block of partial sums
-         __threadfence();
-         __syncwarp();
-         if (lane == 0) {
-           int* fl = g.sk_flags + (int)blockIdx.x * kEpiWarps + ew;
-           asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(fl), "r"(g.sk_epoch) : "memory");
-         }
-       }
-      } else {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(buf));
+        if (g.act == ACT_MASK) {
+          const int si = co + (oh * g.Wout + ow) * g.scale_pix_stride;
+          const uint4* mk = reinterpret_cast<const uint4*>(g.mask + off);
+#pragma unroll
+          for (int j8 = 0; j8 < CH / 8; ++j8) {
+            const uint4 m4 = __ldg(mk + j8);
+            const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float sc = g.scale_pix_stride ? __ldg(g.scale + si + j8 * 8 + j) : my_stage[cc + j8 * 8 + j];
+              v[j8 * 8 + j] = v[j8 * 8 + j] * sc * (__bfloat162float(mb[j]) > 0.f ? 1.f : g.mask_slope);
+            }
+          }
+          if (g.res && g.res_after) {                    // gradient of the block's residual branch joins after the mask/scale
+            const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
+            const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
+#pragma unroll
+            for (int j8 = 0; j8 < CH / 8; ++j8) {
+              const uint4 h4 = __ldg(rh + j8);
+              const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
+              if (PASSES == 3) {
+                const uint4 l4 = __ldg(rl + j8);
+                const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
+              } else {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
+              }
+            }
+          }
+        } else {
+#pragma unroll
+          for (int j4 = 0; j4 < CH / 4; ++j4) {
+            const float4 sc = *reinterpret_cast<const float4*>(my_stage + cc + 4 * j4);
+            const float4 sf = *reinterpret_cast<const float4*>(my_stage + 128 + cc + 4 * j4);
+            v[4 * j4 + 0] = fmaf(v[4 * j4 + 0], sc.x, sf.x);
+            v[4 * j4 + 1] = fmaf(v[4 * j4 + 1], sc.y, sf.y);
+            v[4 * j4 + 2] = fmaf(v[4 * j4 + 2], sc.z, sf.z);
+            v[4 * j4 + 3] = fmaf(v[4 * j4 + 3], sc.w, sf.w);
+          }
+          if (g.act == ACT_ELU) {
+#pragma unroll
+            for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.f ? v[j] : expm1f(v[j]);
+          } else if (g.act != ACT_NONE) {
+#pragma unroll
+            for (int j = 0; j < CH; ++j) v[j] = fmaf(act_b, fabsf(v[j]), act_a * v[j]);
+          }
+        }
+        if (g.out) store_split<CH, PASSES>(g.out + off, g.out_plane, v);
+        if (g.out_f32_t) {                           // tile-blocked channel-major table: [m-tile][co][128 rows]
+          const long long tbase = ((long long)wi.mtile * g.cout_real + co) * BM + ml;
+          if (g.out_t_bf16) {
+            __nv_bfloat16* ot = reinterpret_cast<__nv_bfloat16*>(g.out_f32_t) + tbase;
+#pragma unroll
+            for (int j = 0; j < CH; ++j)
+              if (co + j < g.cout_real) ot[j * BM] = __float2bfloat16_rn(v[j]);   // a warp writes 64 contiguous bytes per column
+          } else {
+            float* ot = g.out_f32_t + tbase;
+#pragma unroll
+            for (int j = 0; j < CH; ++j)
+              if (co + j < g.cout_real) ot[j * BM] = v[j];   // a warp writes 128 contiguous bytes per column
+          }
+        }
+        if (g.out_f32) {
+          float4* of = reinterpret_cast<float4*>(g.out_f32 + off);
+#pragma unroll
+          for (int j = 0; j < CH / 4; ++j) of[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+        }
+      }
+    }
+    if (SK && wi.sk_role == 1) {                        // publish this warp's sub-block of partial sums
+      __threadfence();
+      __syncwarp();
+      if (lane == 0) {
+        int* fl = g.sk_flags + (int)blockIdx.x * kEpiWarps + ew;
+        asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(fl), "r"(g.sk_epoch) : "memory");
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::kTmemCols);
 }
 
 }  // namespace
@@ -536,7 +480,7 @@ TcMaps* tc_build_maps(const TapGemm& g, char* err, int errlen) {
   memset(m, 0, sizeof(*m));
   tile_shape(g.Hg, g.Wg, m->Wt, m->Ht, m->Nt);
   m->sk_choice = -1;
-  m->BN = (g.Cout % 256 == 0) ? 256 : (g.Cout % 128 == 0) ? 128 : 16;
+  m->BN = (g.Cout % 128 == 0) ? 128 : 16;   // 128: the widest tile whose float32-mode accumulators fit a warpgroup's registers
   if (g.Wg % m->Wt || g.Hg % m->Ht || m->Wt * m->Ht * m->Nt != BM) {
     snprintf(err, errlen, "M grid %dx%d does not tile into 128-row boxes", g.Hg, g.Wg);
     delete m; return nullptr;
@@ -603,13 +547,13 @@ int tc_num_sms() {
 size_t tc_sk_workspace_floats() { return (size_t)tc_num_sms() * kEpiWarps * 32 * 128; }
 size_t tc_sk_flag_ints() { return (size_t)tc_num_sms() * kEpiWarps; }
 
-template <int BN, int PASSES, int MT, bool SK, int EW = 8>
+template <int BN, int PASSES, bool SK>
 static int launch_one(const TapGemm& g, const TcMaps* maps, int tiles_m, int num_sms, cudaStream_t st) {
-  using Cfg = TcCfg<BN, PASSES, MT, EW>;
+  using Cfg = TcCfg<BN, PASSES>;
   static DeviceOnce attr_set;
   const int dev = cur_device();
   if (!attr_set.is_done(dev)) {
-    if (cudaFuncSetAttribute(tapgemm_tc_kernel<BN, PASSES, MT, SK, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess)
+    if (cudaFuncSetAttribute(tapgemm_tc_kernel<BN, PASSES, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) != cudaSuccess)
       return -1;
     attr_set.set_done(dev);
   }
@@ -620,10 +564,10 @@ static int launch_one(const TapGemm& g, const TcMaps* maps, int tiles_m, int num
     total_work = (int)T;
     grid = num_sms;
   } else {
-    total_work = ((tiles_m + MT - 1) / MT) * (g.Cout / maps->BN) * g.nphase * g.ksplit;
+    total_work = tiles_m * (g.Cout / maps->BN) * g.nphase * g.ksplit;
     grid = total_work < num_sms ? total_work : num_sms;
   }
-  if (launch_pdl(tapgemm_tc_kernel<BN, PASSES, MT, SK, EW>, dim3(grid), dim3(Cfg::kThreadsCta), Cfg::kSmemBytes, st, g, *maps, total_work) != cudaSuccess)
+  if (launch_pdl(tapgemm_tc_kernel<BN, PASSES, SK>, dim3(grid), dim3(kThreadsCta), Cfg::kSmemBytes, st, g, *maps, total_work) != cudaSuccess)
     return -1;
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
@@ -632,17 +576,14 @@ int launch_tapgemm_tc(const TapGemm& g, const TcMaps* maps, cudaStream_t st) {
   const int num_sms = tc_num_sms();
   const int tiles_m = (g.Wg / maps->Wt) * (g.Hg / maps->Ht) * ((g.n_img + maps->Nt - 1) / maps->Nt);
   const long long tiles = (long long)tiles_m * (g.Cout / maps->BN) * g.nphase;
-  // Cout = 128 layers in bf16 mode: pair M tiles on one weight tile (halves the weight refills of these
-  // operand-feed-bound layers) once there is enough work to keep every SM busy.  In float32 mode the pair would need
-  // all 512 TMEM columns and lose the epilogue overlap -- measured slower, so it keeps single tiles.
-  const bool pair = maps->BN == 128 && g.passes == 1 && g.ksplit == 1 && tiles >= 2LL * num_sms;
-  // stream-K pays for one extra partial-sum round trip and one un-overlapped epilogue per CTA, so it is used only where
-  // whole-tile scheduling leaves >= 20 % of the SM-time idle (measured: +14 % on dec_conv1 of IAN_simple, whose 9/6/6/4-tap
-  // phases and 256 tiles map badly onto 148 SMs; -4 % on layers with a 1.16x imbalance).
+  // stream-K pays for one extra partial-sum round trip per cut tile, so it is used only where whole-tile scheduling
+  // leaves >= 20 % of the SM-time idle (e.g. dec_conv1 of IAN_simple, whose 9/6/6/4-tap phases map badly onto the SMs).
   bool sk = false;
-  if (maps->sk_choice >= 0) {
+  if (g.sk_force) {
+    sk = g.sk_ws && g.ksplit == 1 && maps->BN == 128 && !g.out_f32_t;
+  } else if (maps->sk_choice >= 0) {
     sk = maps->sk_choice == 1 && g.sk_ws != nullptr;
-  } else if (g.sk_ws && g.ksplit == 1 && !pair && maps->BN == 256 && tiles >= num_sms / 2 && !g.out_f32_t) {
+  } else if (g.sk_ws && g.ksplit == 1 && maps->BN == 128 && tiles >= num_sms / 2 && !g.out_f32_t) {
     const int per_phase = tiles_m * (g.Cout / maps->BN);
     std::vector<long long> load(num_sms, 0);
     long long T = 0;
@@ -659,17 +600,11 @@ int launch_tapgemm_tc(const TapGemm& g, const TcMaps* maps, cudaStream_t st) {
     maps->sk_choice = 0;
   }
   if (g.passes == 1) {
-    if (maps->BN == 256) return sk ? launch_one<256, 1, 1, true>(g, maps, tiles_m, num_sms, st) : launch_one<256, 1, 1, false>(g, maps, tiles_m, num_sms, st);
-    if (maps->BN == 128) {
-      // short-K single-pass layers (dec_conv4 / dec_conv4a* of IAN.py: 8-50 K steps per tile) are epilogue-bound on 8 warps
-      if (pair) return launch_one<128, 1, 2, false, 16>(g, maps, tiles_m, num_sms, st);
-      return sk ? launch_one<128, 1, 1, true>(g, maps, tiles_m, num_sms, st) : launch_one<128, 1, 1, false>(g, maps, tiles_m, num_sms, st);
-    }
-    return launch_one<16, 1, 1, false>(g, maps, tiles_m, num_sms, st);
+    if (maps->BN == 128) return sk ? launch_one<128, 1, true>(g, maps, tiles_m, num_sms, st) : launch_one<128, 1, false>(g, maps, tiles_m, num_sms, st);
+    return launch_one<16, 1, false>(g, maps, tiles_m, num_sms, st);
   }
-  if (maps->BN == 256) return sk ? launch_one<256, 3, 1, true>(g, maps, tiles_m, num_sms, st) : launch_one<256, 3, 1, false>(g, maps, tiles_m, num_sms, st);
-  if (maps->BN == 128) return sk ? launch_one<128, 3, 1, true>(g, maps, tiles_m, num_sms, st) : launch_one<128, 3, 1, false>(g, maps, tiles_m, num_sms, st);
-  return launch_one<16, 3, 1, false>(g, maps, tiles_m, num_sms, st);
+  if (maps->BN == 128) return sk ? launch_one<128, 3, true>(g, maps, tiles_m, num_sms, st) : launch_one<128, 3, false>(g, maps, tiles_m, num_sms, st);
+  return launch_one<16, 3, false>(g, maps, tiles_m, num_sms, st);
 }
 
 }  // namespace ian

@@ -3,7 +3,7 @@
 PARITY: PINNED TO THE EXECUTED REFERENCE, with one stated limit.  Theano 0.9 / Lasagne 0.2.dev1 (and Python 2)
 are absent and the trained weights are git-LFS pointers, so the reference cannot run as shipped and has no golden
 vectors (SURVEY.md F2/F3/F5).  Instead the reference's OWN files -- API.py, IAN_simple.py, IANv1.py, IAN.py,
-layers.py, mask_generator.py, GANcheckpoints.py -- are executed unmodified from /root/reference on numpy stand-ins
+layers.py, mask_generator.py, GANcheckpoints.py -- are executed unmodified from the original project on numpy stand-ins
 for those two third-party packages (oracle/refshim/), with the synthetic seeded checkpoint loaded by the reference's
 own loader; the outputs are committed as tests/golden/ref_exec_*.npz (tests/golden/make_golden_ref.py) and this
 file agrees with them to 1e-12 (forward) / 1e-8 (gradients, vs numeric differentiation of the reference forward):

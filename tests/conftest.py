@@ -11,23 +11,23 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100) GPU; run by the driver on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) GPU")
 
 
-def _have_b200():
+def _have_h100():
     try:
         import torch
-        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     except Exception:
         return False
 
 
 def pytest_collection_modifyitems(config, items):
-    """a plain `pytest` on a box without an sm_100 GPU skips the gpu-marked tests instead of erroring in the fixture
+    """a plain `pytest` on a machine without an sm_90 GPU skips the gpu-marked tests instead of erroring in the fixture
     (the product itself still fails loudly there: tests/test_abi.py::test_create_fails_loudly_without_gpu)."""
-    if _have_b200():
+    if _have_h100():
         return
-    skip = pytest.mark.skip(reason="needs a B200 (sm_100) GPU")
+    skip = pytest.mark.skip(reason="needs an H100 (sm_90) GPU")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

@@ -76,8 +76,9 @@ def simple():
         x = on.to_tanh(gold['images'][:k].astype(np.float64)).astype(np.float32)      # NPE.py:257
         z = m.encode_images(x)                            # API.py:78-90
         out['mu_' + tag] = z
-        out['xhat_' + tag] = m.sample_at(np.float32(z))   # API.py:98-110 (NPE.py:261 passes float32)
-        out['xhat_rand_' + tag] = m.sample_at(gold['z_rand'][:k])
+        kx = min(k, 3)                                    # decoded images: the first 3 keep the file under 1 MB
+        out['xhat_' + tag] = m.sample_at(np.float32(z[:kx]))   # API.py:98-110 (NPE.py:261 passes float32)
+        out['xhat_rand_' + tag] = m.sample_at(gold['z_rand'][:kx])
         ls_fn = theano.function([m.X], lasagne.layers.get_output(m.model['l_ls'], {m.model['l_in']: m.X}, deterministic=True))
         out['logsigma_' + tag] = ls_fn(x)
         print(tag, 'forward done in %.1f s' % (time.time() - t0), flush=True)

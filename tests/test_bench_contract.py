@@ -40,19 +40,40 @@ def test_reference_arm_nonzero_ranks_do_no_work():
     assert out.returncode == 0 and not [l for l in out.stdout.splitlines() if l.startswith("{")]
 
 
-def test_roofline_traffic_resolves_from_the_committed_ncu_summary():
-    """`roofline.traffic` is read at run time from profiles/r2_ncu_tc_kernels_full_summary.csv (the ncu --set full capture of
-    the same command), not a constant in the source: the 9 tap-GEMM launches of one batch-256 step must all be there, their
-    DRAM bytes between the algorithmic 0.94 GB and 2x that, and the bench line committed beside it must carry that figure."""
+def _bench():
     sys.path.insert(0, ROOT)
     import importlib
-    bench = importlib.import_module("bench")
-    t = bench.ncu_traffic("tapgemm_tc", 9)
-    assert t is not None and 0.94e9 <= t <= 1.9e9, t
-    assert bench.ncu_traffic("tapgemm_tc", 10) is None           # a step has exactly nine of them: more cannot be resolved
-    line = [l for l in open(os.path.join(ROOT, "profiles", "r2_bench_n1.json")) if l.startswith("{")][-1]
+    return importlib.import_module("bench")
+
+
+def test_dump_outputs_size_rule(tmp_path):
+    """--dump-outputs keeps z and x_hat within 64 MB together: all rows when they fit, else the same fixed, sorted, seeded
+    sample of rows in every array, depending only on the batch size (two builds dump the same samples)."""
+    import numpy as np
+    bench = _bench()
+    row = 100 * 4 + 3 * 64 * 64 * 4                               # one sample of z + one of x_hat, float32
+    assert np.array_equal(bench.dump_rows(256, row), np.arange(256))   # 12.7 MB: everything
+    big = bench.dump_rows(4096, row)                               # 201 MB: a sample
+    assert len(big) * row <= bench.DUMP_MAX_BYTES < (len(big) + 1) * row
+    assert np.all(np.diff(big) > 0) and big[0] >= 0 and big[-1] < 4096
+    assert np.array_equal(big, bench.dump_rows(4096, row))
+    n = 3000                                                       # end to end with small arrays and a small cap
+    z = np.arange(n * 2, dtype=np.float64).reshape(n, 2)
+    x = -np.arange(n * 6, dtype=np.float32).reshape(n, 3, 2)
+    rows = bench.write_dump(str(tmp_path), {"z": z, "xhat": x}, max_bytes=1000 * (2 + 6) * 4)
+    zd, xd = np.load(tmp_path / "z.npy"), np.load(tmp_path / "xhat.npy")
+    assert len(rows) == 1000 and zd.dtype == np.float32 and xd.dtype == np.float32
+    assert np.array_equal(zd, z[rows].astype(np.float32)) and np.array_equal(xd, x[rows])
+    assert zd.nbytes + xd.nbytes <= 1000 * (2 + 6) * 4
+
+
+def test_committed_h100_bench_line():
+    """the bench line committed beside the docs (profiles/h100_bench_n1.json) carries its card, a sane roofline fraction
+    and the launch count of the IAN_simple step: conv1, 3 convs, fc1 + finalize, head + finalize, sample, fc2, 3 deconvs,
+    dec_out"""
+    line = [l for l in open(os.path.join(ROOT, "profiles", "h100_bench_n1.json")) if l.startswith("{")][-1]
     d = json.loads(line)
-    assert abs(d["roofline"]["traffic"] - t) <= 0.1 * t          # (that line was printed just before the capture was refreshed in the same call)
-    assert d["roofline"]["traffic_src"].endswith("r2_ncu_tc_kernels_full_summary.csv")
-    assert d["roofline"]["frac"] == d["roofline"]["frac_burst"] and 0.5 < d["roofline"]["frac_burst"] <= 1.0
-    assert d["gpu_launches"] == 14 * d["steps"]                  # conv1, 3 convs, fc1 + finalize, head + finalize, sample, fc2, 3 deconvs, dec_out
+    assert "H100" in d["gpu"]["name"] and d["gpu"]["power_limit_w"] > 0
+    assert d["roofline"]["frac"] == d["roofline"]["frac_burst"] and 0.1 < d["roofline"]["frac_burst"] <= 1.0
+    assert d["gpu_launches"] == 14 * d["steps"]
+    assert d["n_gpus"] == 1 and d["value"] > 0 and d["unit"] == "images/sec"

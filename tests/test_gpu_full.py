@@ -175,10 +175,9 @@ def test_simple_model_function_set_is_flowless(model, golden):
 
 def test_bf16_mode_tolerance_vs_oracle(full_model, gold):
     """BASELINE configs[2]: full IAN in bf16 with an fp32 tolerance check.  Operands rounded to bf16 (8 significand
-    bits), fp32 accumulation.  Measured on this fixture's [-1,1] images (final round-2 build; the kernels are
-    deterministic, so every B200 gives these bits): max-abs 0.034 (the Beta ratio 2a/(a+b) is steep where both sigmoids
-    are small), mean-abs 2.6e-3.  Bounds stated here: max-abs 0.08, mean-abs 5e-3 (bench.py reports max-abs / mean-abs /
-    PSNR of bf16 vs float32 mode at batch 512: 0.065 / 2.8e-3 / 52.7 dB)."""
+    bits), fp32 accumulation.  The Beta ratio 2a/(a+b) is steep where both sigmoids
+    are small, so single pixels move most.  Bounds stated here: max-abs 0.08, mean-abs 5e-3 (bench.py reports max-abs /
+    mean-abs / PSNR of bf16 vs float32 mode at batch 512; on an H100: 0.064 / 2.8e-3 / 52.7 dB)."""
     x = on.to_tanh(gold["images"].astype(np.float64)).astype(np.float32)
     try:
         full_model.set_precision("bf16")
@@ -229,33 +228,3 @@ def test_ianv1_golden(npe, gold_v1, path):
             assert err.max() <= 0.03 and err.mean() <= 3e-3     # measured 0.0061 / 7.5e-4 (plain deconv decoder: no steep MDC/Beta chain)
     finally:
         m.close()
-
-
-@pytest.mark.parametrize("which", ["full", "v1"])
-def test_pair_kernel_on_the_flow_models(npe, which, monkeypatch):
-    """the CTA-pair tap-GEMM on the IAN.py / IANv1.py graphs (MDC taps, residual + raw-output epilogue of the MDBLOCKs),
-    float32 split and single-pass bf16 mode, against the one-CTA kernel on the same schedule."""
-    from oracle import weights as ow
-    P = (ow.make_v1_weights if which == "v1" else ow.make_full_weights)(0)
-    cfg = "IANv1.py" if which == "v1" else "IAN.py"
-    for k, v in (("IAN_SPLITK", "0"), ("IAN_STREAMK", "0"), ("IAN_GRAPHS", "0")):
-        monkeypatch.setenv(k, v)
-    monkeypatch.setenv("IAN_TC2", "0")
-    one = npe.IAN(cfg, True, weights=P)
-    monkeypatch.setenv("IAN_TC2", "1")
-    monkeypatch.setenv("IAN_TC2_MIN", "1")
-    monkeypatch.setenv("IAN_TC2_BF16", "1")               # also exercise the 256 x 256 single-pass pair tiles
-    pair = npe.IAN(cfg, True, weights=P)
-    rng = np.random.default_rng(43)
-    try:
-        for prec, tol in (("fp32", 1e-6), ("bf16", 1e-6)):
-            one.set_precision(prec)
-            pair.set_precision(prec)
-            for n in (2, 5):
-                x = rng.uniform(-1, 1, (n, 3, 64, 64)).astype(np.float32)
-                xa, za = one.reconstruct(x, return_z=True)
-                xb, zb = pair.reconstruct(x, return_z=True)
-                assert np.abs(za - zb).max() <= tol and np.abs(xa - xb).max() <= tol, (prec, n)
-    finally:
-        one.close()
-        pair.close()

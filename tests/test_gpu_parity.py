@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through API.IAN -> ctypes -> C-ABI,
+"""GPU parity tests (run on an H100): the CUDA path, called through API.IAN -> ctypes -> C-ABI,
 against the float64 oracle's committed golden vectors and against the oracle run live on seeded inputs.
 
 Tolerances (float32 path; stated per BASELINE north_star "within 1e-4 max-abs"):
@@ -320,8 +320,8 @@ def test_config4_edit_loop_at_size(model, weights):
     the rest of the batch is tied to the probe by the independence invariant.
 
     Bound, per sample, relative to that sample's own move max|z_32 - z_0| (BASELINE.md: "within 2 % of the move"):
-    median <= 2e-3, every probe sample <= 2e-2.  Measured on B200 (tc path): median 3.3e-4, max 3.5e-3; the batch-128 run
-    vs the probe run alone: max 7.9e-4 (profiles/r2_config4_parity.json, written by this test when IAN_TEST_RECORD is set).  The drivers of the error are the rare ReLU-mask flips of 16-bit
+    median <= 2e-3, every probe sample <= 2e-2 (the measured values are written to config4_parity.json when IAN_TEST_RECORD
+    names a directory).  The drivers of the error are the rare ReLU-mask flips of 16-bit
     activations (module docstring): one flip perturbs one step's g by ~1 %, and later steps contract it."""
     import json
     import torch
@@ -358,44 +358,57 @@ def test_config4_edit_loop_at_size(model, weights):
     assert rel_alone.max() <= 2e-2, rel_alone
 
 
-def test_pair_kernel_equals_one_cta_kernel(npe, weights, monkeypatch):
-    """tapgemm_tc2 (tcgen05 cta_group::2, 256 x 128 pair tiles) against tapgemm_tc (one CTA per tile) on the same whole-tile
-    schedule: same K order per output element, so the results must agree to the last bits.  Small batches are forced
-    onto the pair kernel (IAN_TC2_MIN=1, split-K off) so that odd tile counts (phantom half of a pair), every phase mix
-    of the deconvs and the backward (ACT_MASK, per-pixel scale) epilogues are covered."""
-    for k, v in (("IAN_SPLITK", "0"), ("IAN_STREAMK", "0"), ("IAN_GRAPHS", "0")):
+def test_stream_k_schedule_matches_whole_tiles(npe, weights, monkeypatch):
+    """stream-K (CTA c owns K steps [T*c/G, T*(c+1)/G) of the whole launch; a cut tile is finished by the CTA holding its
+    first K steps after the others published their partial sums) against the whole-tile schedule.  IAN_STREAMK=2 puts
+    EVERY eligible tap-GEMM launch on stream-K (no makespan test), so batches 1, 3, 9 and 70 cover small launches with
+    fewer K steps than SMs, every deconv phase mix and the backward (ACT_MASK, per-pixel scale) epilogues of grad() and
+    the edit loop.  Cutting every layer changes the float32 summation order everywhere (on z: up to ~6e-5 relative to a
+    whole-tile run), so each schedule is held to the float64 oracle at the standing tolerances on a probe of the batch,
+    the two to each other at those tolerances, and the ordered fix-up must be deterministic."""
+    import torch
+    from oracle import ian_torch as ot
+    for k, v in (("IAN_SPLITK", "0"), ("IAN_GRAPHS", "0")):
         monkeypatch.setenv(k, v)
-    monkeypatch.setenv("IAN_TC2", "0")
-    one = npe.IAN("IAN_simple.py", True, weights=weights)
-    monkeypatch.setenv("IAN_TC2", "1")
-    monkeypatch.setenv("IAN_TC2_MIN", "1")
-    pair = npe.IAN("IAN_simple.py", True, weights=weights)
-    monkeypatch.setenv("IAN_STREAMK", "1")               # third handle: the pair kernel's stream-K schedule (ordered fix-up)
-    pair_sk = npe.IAN("IAN_simple.py", True, weights=weights)
+    monkeypatch.setenv("IAN_STREAMK", "0")
+    whole = npe.IAN("IAN_simple.py", True, weights=weights)
+    monkeypatch.setenv("IAN_STREAMK", "2")
+    sk = npe.IAN("IAN_simple.py", True, weights=weights)
+    P = ot.to_torch(weights, torch.float64)
     rng = np.random.default_rng(41)
     try:
-        x = rng.uniform(-1, 1, (70, 3, 64, 64)).astype(np.float32)
-        xa, za = one.reconstruct(x, return_z=True)
-        xs, zs = pair_sk.reconstruct(x, return_z=True)   # another float32 summation order where a tile is cut: rerun tolerances
-        assert np.abs(za - zs).max() <= Z_RERUN and np.abs(xa - xs).max() <= X_RERUN
-        xs2, zs2 = pair_sk.reconstruct(x, return_z=True)
-        assert np.array_equal(xs, xs2) and np.array_equal(zs, zs2)      # ... and deterministic
         for n in (1, 3, 9, 70):
             x = rng.uniform(-1, 1, (n, 3, 64, 64)).astype(np.float32)
             z = rng.standard_normal((n, 100)).astype(np.float32)
             boxes = np.tile(np.array([[6, 10, 38, 30]], np.int32), (n, 1))
             rgb = rng.uniform(-1, 1, (n, 3)).astype(np.float32)
-            xa, za = one.reconstruct(x, return_z=True)
-            xb, zb = pair.reconstruct(x, return_z=True)
-            assert np.abs(za - zb).max() <= 1e-6 and np.abs(xa - xb).max() <= 1e-6, n
-            ga, gb = one.grad(z, boxes, rgb), pair.grad(z, boxes, rgb)
-            assert np.abs(ga - gb).max() <= 1e-6 * max(1.0, np.abs(ga).max()), n
-            ea, eb = one.edit_steps(z, boxes, rgb, n_steps=3), pair.edit_steps(z, boxes, rgb, n_steps=3)
-            assert np.abs(ea - eb).max() <= 1e-5, n
+            probe = sorted({0, n // 2, n - 1})
+            zr = on.simple_encode(weights, x[probe])
+            xa, za = whole.reconstruct(x, return_z=True)
+            xs, zs = sk.reconstruct(x, return_z=True)
+            for xh, zz in ((xa, za), (xs, zs)):
+                assert np.abs(zz[probe] - zr).max() <= Z_TOL, n
+                assert np.abs(xh[probe] - on.simple_decode(weights, zz[probe])).max() <= X_TOL, n
+            assert np.abs(za - zs).max() <= Z_TOL and np.abs(xa - xs).max() <= X_TOL, n
+            xs2, zs2 = sk.reconstruct(x, return_z=True)
+            assert np.array_equal(xs, xs2) and np.array_equal(zs, zs2), n
+            gs, ga = sk.grad(z, boxes, rgb), whole.grad(z, boxes, rgb)
+            gr = ot.grad_batched(P, torch.from_numpy(z[probe].astype(np.float64)), boxes[probe],
+                                 torch.from_numpy(rgb[probe].astype(np.float64))).numpy()
+            # per-sample relative error; on random latents a ReLU-mask flip of a 16-bit activation inside the brush
+            # footprint moves one sample's gradient by up to ~1 % on EITHER schedule (module docstring), so these are the
+            # per-sample bounds of the config-4 edit-loop test rather than assert_grad_close's golden-input median
+            def rel(a, b):
+                return np.abs(a - b).max(axis=1) / np.abs(b).max(axis=1)
+            for r in (rel(gs[probe], gr), rel(ga[probe], gr), rel(gs, ga)):
+                assert np.median(r) <= 2e-3 and r.max() <= 2e-2, (n, r)
+            assert np.array_equal(gs, sk.grad(z, boxes, rgb)), n
+            ea, es = whole.edit_steps(z, boxes, rgb, n_steps=3), sk.edit_steps(z, boxes, rgb, n_steps=3)
+            r = np.abs(ea - es).max(axis=1) / np.abs(ea - z).max(axis=1)
+            assert np.median(r) <= 2e-3 and r.max() <= 2e-2, (n, r)
     finally:
-        one.close()
-        pair.close()
-        pair_sk.close()
+        whole.close()
+        sk.close()
 
 
 def test_pdl_and_coop_finalize_are_bit_identical(npe, weights, monkeypatch):
@@ -404,8 +417,8 @@ def test_pdl_and_coop_finalize_are_bit_identical(npe, weights, monkeypatch):
         next kernel's prologue overlaps the previous kernel's tail, every kernel waits (griddepcontrol.wait) before
         touching activations -- compared against a handle with plain launches;
       * IAN_FINALIZE8=0 -- the one-thread split-K finalize instead of the cooperative one (same slab order by construction).
-    Plain launches (graphs off) so that PDL is really in effect; batches that cover split-K layers (1, 5), whole pair tiles
-    and stream-K (160) and the batch-128 edit loop's mix."""
+    Plain launches (graphs off) so that PDL is really in effect; batches that cover split-K layers (1, 5), stream-K (160)
+    and the batch-128 edit loop's mix."""
     monkeypatch.setenv("IAN_GRAPHS", "0")
     monkeypatch.setenv("IAN_PDL", "0")
     base = npe.IAN("IAN_simple.py", True, weights=weights)

@@ -1,14 +1,12 @@
 """The oracle against fixtures produced by EXECUTING the reference's own files (tests/golden/make_golden_ref.py):
 API.IAN / IAN_simple.get_model / IANv1.get_model / IAN.get_model / layers.py / mask_generator.py /
-GANcheckpoints.load_weights run unmodified from /root/reference on numpy stand-ins for Theano and Lasagne
+GANcheckpoints.load_weights run unmodified from the original project on numpy stand-ins for Theano and Lasagne
 (oracle/refshim).  This is what pins the oracle: graph wiring, hyper-parameters, parameter names and the loading
 path are the reference's code; only the third-party layer semantics underneath are restated.
 
 The fixtures are float64 evaluations, so the float64 oracle must agree to rounding; the numeric gradients
 (central differences of the reference forward) bound the analytic brush gradients."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -43,8 +41,10 @@ def test_simple_forward_matches_executed_reference(golden, weights):
         assert ref["mu_" + tag].shape == (k, 100)
         assert np.abs(mu[:k] - ref["mu_" + tag]).max() <= 1e-12
         assert np.abs(ls[:k] - ref["logsigma_" + tag]).max() <= 1e-12
-        assert np.abs(on.simple_decode(weights, np.float32(ref["mu_" + tag])) - ref["xhat_" + tag]).max() <= 1e-12
-        assert np.abs(on.simple_decode(weights, golden["z_rand"][:k]) - ref["xhat_rand_" + tag]).max() <= 1e-12
+        kx = ref["xhat_" + tag].shape[0]               # decoded images are stored for the first min(k, 3) only
+        assert kx == min(k, 3) and ref["xhat_rand_" + tag].shape[0] == kx
+        assert np.abs(on.simple_decode(weights, np.float32(ref["mu_" + tag][:kx])) - ref["xhat_" + tag]).max() <= 1e-12
+        assert np.abs(on.simple_decode(weights, golden["z_rand"][:kx]) - ref["xhat_rand_" + tag]).max() <= 1e-12
     assert np.abs(ref["xhat_dnn"][:2] - ref["xhat_nodnn"]).max() <= 1e-12
     _names_match(ref, weights)
 
@@ -99,19 +99,6 @@ def test_made_layer_is_fed_its_own_input_layer():
     as_read = fn.iaf(z_iaf, fn.made_core(P, "l_IAF_mu", z_iaf, masks), fn.made_core(P, "l_IAF_ls", z_iaf, masks))
     assert np.abs(as_read - ref["z_from_mu"]).max() > 0.1
     assert np.abs(fn.full_latent(P, z_iaf, masks) - ref["z_from_mu"]).max() <= 1e-11
-
-
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="needs the reference checkout (build container only)")
-def test_fixture_regenerates_from_the_reference(tmp_path):
-    """re-execute the reference (IANv1.py: encoder, MADE/IAF, decoder, RGB-Beta head) and compare with the committed file"""
-    script = os.path.join(GOLD, "make_golden_ref.py")
-    out = subprocess.run([sys.executable, script, "v1"], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, REF_EXEC_OUT=str(tmp_path), REF_EXEC_GRADS="0"))
-    assert out.returncode == 0, out.stderr[-2000:]
-    committed, fresh = _load("ref_exec_v1.npz"), np.load(tmp_path / "ref_exec_v1.npz")
-    assert set(fresh.files) <= set(committed.files)          # the quick regeneration skips the numeric gradients
-    for k in fresh.files:
-        assert np.array_equal(committed[k], fresh[k]), k
 
 
 def test_product_cfg_dicts_equal_the_reference_config_modules(npe):

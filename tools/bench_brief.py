@@ -1,4 +1,4 @@
-"""one-line digest of a bench.py JSON line (A/B scripts): python tools/bench_brief.py TAG FILE"""
+"""one-line digest of a bench.py JSON line: python tools/bench_brief.py TAG FILE"""
 import json, sys
 tag, path = sys.argv[1], sys.argv[2]
 line = [l for l in open(path) if l.startswith("{")]

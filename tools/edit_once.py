@@ -1,4 +1,4 @@
-"""a few steps of the BASELINE config-4 edit loop at batch 128 (for ncu launch lists)"""
+"""a few steps of the BASELINE config-4 edit loop at batch 128 (a short workload for torch.profiler launch lists)"""
 import importlib, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)

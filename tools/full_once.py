@@ -1,4 +1,4 @@
-"""run the full-IAN reconstruct a few times at batch 512 (for ncu launch lists)"""
+"""run the full-IAN reconstruct a few times at batch 512 (a short workload for torch.profiler launch lists)"""
 import importlib, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)

@@ -1,6 +1,6 @@
-"""profiles/r2_sass_summary.txt: per kernel of the shipped libian_b200.so, the SASS mnemonics that prove the Blackwell
-paths (B200_PROFILING.md: tcgen05.mma -> UTC*MMA, tcgen05.ld -> LDTM, TMA -> UTMALDG/UBLKCP, commit -> UTCBAR,
-TMEM alloc -> UTCATOMSWS) plus registers / shared memory from --dump-resource-usage.
+"""profiles/r2_sass_summary.txt: per kernel of the shipped libian_b200.so, the SASS mnemonics that prove the Hopper
+paths (wgmma.mma_async -> HGMMA, wgmma.fence / wait_group -> WARPGROUP.ARRIVE / WARPGROUP.DEPBAR, TMA -> UTMALDG / UTMASTG /
+UBLKCP) plus registers / shared memory from --dump-resource-usage.
 
 usage: python tools/sass_summary.py > profiles/r2_sass_summary.txt      (no GPU needed)
 """
@@ -12,9 +12,9 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "neural-photo-editor_b200", "libian_b200.so")
-PAT = re.compile(r"\b(UTC[A-Z]*MMA(?:\.2CTA)?|LDTM|STTM|UTMALDG(?:\.[0-9]D)?(?:\.2CTA)?|UTMASTG|UBLKCP|UTCBAR(?:\.2CTA)?(?:\.MULTICAST)?|"
-                 r"UTCATOMSWS(?:\.2CTA)?|UCGABAR_[A-Z]+|SYNCS\.[A-Z]+|HMMA|FFMA|MUFU\.[A-Z0-9]+|LDGSTS|RED|ATOM[GS]?|"
-                 r"STG\.E\.ENL2\.256|PREEXIT|ACQBULK)\b")   # 256-bit stores; griddepcontrol.launch_dependents / .wait (PDL)
+PAT = re.compile(r"\b(HGMMA\.[0-9x]+\.F32\.BF16|WARPGROUP\.ARRIVE|WARPGROUP\.DEPBAR|UTMALDG(?:\.[0-9]D)?|UTMASTG|UBLKCP|"
+                 r"SYNCS\.[A-Z]+|HMMA|FFMA|MUFU\.[A-Z0-9]+|LDGSTS|RED|ATOM[GS]?|"
+                 r"PREEXIT|ACQBULK)\b")   # griddepcontrol.launch_dependents / .wait (PDL)
 
 
 def demangle(names):
@@ -45,7 +45,7 @@ def main():
             continue
         if cur is None:
             continue
-        m = re.search(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.]+)", line)
+        m = re.search(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.x]+)", line)   # x: HGMMA.64x128x16
         if m:
             op = m.group(1)
             counts[cur]["_total"] += 1
@@ -54,8 +54,8 @@ def main():
                 counts[cur][k.group(1)] += 1
     names = list(counts)
     pretty = demangle(names)
-    print("# SASS summary of %s (cuobjdump -sass; CUDA 12.9, sm_100a)" % os.path.relpath(LIB, ROOT))
-    print("# kernel | regs | static smem | instructions | Blackwell / tensor mnemonics (count)")
+    print("# SASS summary of %s (cuobjdump -sass; CUDA 12.9, sm_90a)" % os.path.relpath(LIB, ROOT))
+    print("# kernel | regs | static smem | instructions | Hopper / tensor mnemonics (count)")
     for n, p in sorted(zip(names, pretty), key=lambda t: t[1]):
         c = counts[n]
         key = {k: v for k, v in c.items() if k != "_total" and not k.startswith(("FFMA", "MUFU", "SYNCS", "RED", "ATOM"))}
@@ -66,7 +66,7 @@ def main():
                                              ", ".join("%s x%d" % kv for kv in sorted(other.items())) or "-"))
     tot = collections.Counter()
     for c in counts.values():
-        tot.update({k: v for k, v in c.items() if k.startswith(("UTC", "LDTM", "UTMA", "HMMA"))})
+        tot.update({k: v for k, v in c.items() if k.startswith(("HGMMA", "UTMA", "HMMA"))})
     print("# totals: " + ", ".join("%s x%d" % kv for kv in sorted(tot.items())))
     print("# HMMA (legacy mma.sync) x%d: none expected" % tot.get("HMMA", 0))
 
