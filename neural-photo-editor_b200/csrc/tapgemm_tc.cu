@@ -12,10 +12,11 @@
 //                                         cross += A_lo * B_hi ;  cross += A_hi * B_lo
 //                in two separate register accumulators (the 2^-9-smaller cross terms get their own
 //                accumulator so their rounding does not ride on the main sum's exponent).  After the last K
-//                step the sum main + cross goes through a float32 staging tile in shared memory, and the same
-//                eight warps run the epilogue one pixel row per thread: BatchNorm scale/shift + activation
-//                (or backward scale * ReLU-mask), re-split to bf16 hi/lo planes and store NHWC at the phase's
-//                output stride; or store raw sums to this K split's workspace slab.
+//                step cross is added into main and the sums go through a float32 staging tile in shared memory
+//                (in float32 mode 32 columns at a time, in four rounds), and the same eight warps run the epilogue
+//                one pixel row per thread: BatchNorm scale/shift + activation (or backward scale * ReLU-mask),
+//                re-split to bf16 hi/lo planes and store NHWC at the phase's output stride; or store raw sums to
+//                this K split's workspace slab.
 // Pipeline: STAGES-deep smem ring with full/empty mbarriers (TMA -> wgmma -> release after wgmma.wait_group); the
 // producer runs ahead across work items, so the next tile's operands load while the epilogue of this one runs.
 #include <cuda.h>
@@ -56,7 +57,12 @@ template <int BN, int PASSES> struct TcCfg {
   static constexpr int kATileBytes = BM * BK * 2 * kPlanes;
   static constexpr int kBTileBytes = BN * BK * 2 * kPlanes;
   static constexpr int kStageBytes = kATileBytes + kBTileBytes;
-  static constexpr int kLd = BN + 8;                           // staging row pitch in floats (conflict-free fragment stores)
+  // accumulator columns staged per epilogue round.  Float32 mode stages 32 at a time (a 20 KB tile instead of 68 KB) so
+  // that a third 64 KB operand stage fits; bf16 mode's 32 KB stages fit four deep next to a whole-tile round, and its
+  // short K loops would feel the extra barriers of more rounds.
+  static constexpr int kRound = (PASSES == 3 && BN > 32) ? 32 : BN;
+  static constexpr int kRounds = BN / kRound;
+  static constexpr int kLd = kRound + 8;                       // staging row pitch in floats (conflict-free fragment stores)
   static constexpr int kStagingBytes = BM * kLd * 4;
   static constexpr int kStageSmem = kEpiWarps * 1024;          // per-warp scale|shift staging
   static constexpr int kStagesFit = (220 * 1024 - kStagingBytes - kStageSmem) / kStageBytes;
@@ -64,6 +70,8 @@ template <int BN, int PASSES> struct TcCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kStageSmem + kStagingBytes;
   static_assert(kStages >= 2 && kSmemBytes <= 232448, "tapgemm_tc: shared memory budget");
 };
+// float32 mode at BN = 128 runs the heavy layers: one K step's 64 KB load must not be the only one in flight
+static_assert(TcCfg<128, 3>::kStages == 3 && TcCfg<128, 3>::kSmemBytes == 226560, "tapgemm_tc: three float32-mode stages");
 
 // ---------------------------------------------------------------- kernel
 // Persistent, warp-specialised.  Work items w = blockIdx.x + i*gridDim.x over
@@ -237,14 +245,16 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
 
   // ===================== consumers (warps 0..7): wgmma main loop, then the epilogue =====================
   constexpr int R = BN / 2;                             // accumulator registers per thread and accumulator
-  constexpr int CH = (BN >= 64) ? 32 : 16;              // columns per epilogue chunk
-  constexpr int COLS_PER_WARP = (BN >= 64) ? BN / 2 : BN;
+  constexpr int RW = Cfg::kRound;                     // tile columns per staging round
+  constexpr int TC = RW >= 32 ? RW / 2 : RW;          // columns per thread and round (BN = 16: all 16, on warps 0-3 only)
+  constexpr int CH = TC >= 32 ? 32 : 16;              // columns per epilogue chunk: whole 32-byte sectors per plane
+  constexpr int kThreadCols = Cfg::kRounds * TC;      // columns per thread and tile (its stream-K slot)
   const int wg = warp >> 2, wtid = threadIdx.x & 127;
   const int ew = warp;
   const int lg = warp & 3;                              // 32-row group of the tile this warp's epilogue handles
-  const int half = ew >> 2;                             // which half of the tile's columns
-  const bool has_cols = (BN >= 64) || half == 0;
-  float* my_stage = stage_ptr + ew * 256;               // [0,128): scale, [128,256): shift of this warp's columns
+  const int half = ew >> 2;                           // which half of a round's columns
+  const bool has_cols = RW >= 32 || half == 0;
+  float* my_stage = stage_ptr + ew * 256;             // [0,128): scale, [128,256): shift of the tile's columns
   // activation as a branch-free a*t + b*|t| (none / LeakyRectify(0.2) / rectify; lasagne forms, SURVEY C.5)
   const float act_a = g.act == ACT_LRELU ? 0.6f : g.act == ACT_RELU ? 0.5f : 1.f;
   const float act_b = g.act == ACT_LRELU ? 0.4f : g.act == ACT_RELU ? 0.5f : 0.f;
@@ -261,10 +271,9 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
     if (wi.it1 <= wi.it0) continue;                     // (uniform over the CTA)
     if (has_cols && g.scale_pix_stride == 0) {          // stage this tile's per-channel scale/shift while the MMAs run
       __syncwarp();
-      const int cbase = wi.co0 + half * COLS_PER_WARP;
-      for (int c = lane; c < COLS_PER_WARP; c += 32) {
-        my_stage[c] = g.scale ? __ldg(g.scale + cbase + c) : 1.f;
-        my_stage[128 + c] = g.shift ? __ldg(g.shift + cbase + c) : 0.f;
+      for (int c = lane; c < BN; c += 32) {
+        my_stage[c] = g.scale ? __ldg(g.scale + wi.co0 + c) : 1.f;
+        my_stage[128 + c] = g.shift ? __ldg(g.shift + wi.co0 + c) : 0.f;
       }
       __syncwarp();
     }
@@ -302,19 +311,12 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
     wgmma_fence_regs(acc_m);
     if (PASSES == 3) wgmma_fence_regs(acc_c);
     if (wtid == 0) mbar_arrive(empty_bar((i - 1) % S));
-    // ---- accumulators -> float32 staging tile (row-per-thread access for the epilogue)
-    asm volatile("bar.sync 1, 256;" ::: "memory");      // the previous tile's epilogue has read the staging tile
+    if constexpr (PASSES == 3) {
 #pragma unroll
-    for (int j = 0; j < R; j += 2) {
-      const int row = wg * 64 + frag_row(wtid, j), col = frag_col(wtid, j);
-      float2 v = make_float2(acc_m[j], acc_m[j + 1]);
-      if constexpr (PASSES == 3) { v.x += acc_c[j]; v.y += acc_c[j + 1]; }
-      *reinterpret_cast<float2*>(acc_tile + row * Cfg::kLd + col) = v;
+      for (int j = 0; j < R; ++j) acc_m[j] += acc_c[j];   // main + cross: the one float32 add of every output
     }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (!has_cols) continue;
     // ===================== epilogue =====================
-    if (SK && wi.sk_role == 2) {                        // finisher: the later parts were computed first; wait for them
+    if (SK && wi.sk_role == 2 && has_cols) {          // finisher: the later parts were computed first; wait for them
       for (int k = (int)blockIdx.x + 1 + lane; k <= wi.sk_last; k += 32) {
         if (iter.boundary(k) == iter.boundary(k + 1)) continue;   // a CTA without K steps (T < G) publishes nothing
         const int* fl = g.sk_flags + k * kEpiWarps + ew;
@@ -331,77 +333,61 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
     const bool valid = n < g.n_img;
     const int oh = p * g.osh + ph.oh0, ow = q * g.osw + ph.ow0;
     const long long pix = (long long)(n * g.Hout + oh) * g.Wout + ow;
+    // the sums leave through a BM x RW staging tile, RW columns per round (row-per-thread access for the epilogue)
 #pragma unroll 1
-    for (int cc = 0; cc < COLS_PER_WARP; cc += CH) {
-      const int cb = half * COLS_PER_WARP + cc;
-      const int co = wi.co0 + cb;
-      float v[CH];
-      const float* srow = acc_tile + ml * Cfg::kLd + cb;
+    for (int r = 0; r < Cfg::kRounds; ++r) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");  // every warp has read the staging tile of the previous round
 #pragma unroll
-      for (int j = 0; j < CH / 4; ++j) {
-        const float4 t4 = *reinterpret_cast<const float4*>(srow + 4 * j);
-        v[4 * j] = t4.x; v[4 * j + 1] = t4.y; v[4 * j + 2] = t4.z; v[4 * j + 3] = t4.w;
+      for (int j = 0; j < RW / 2; j += 2) {           // registers [r*RW/2, (r+1)*RW/2) hold this round's columns
+        float2 v = make_float2(acc_m[j], acc_m[j + 1]);
+#pragma unroll
+        for (int rr = 1; rr < Cfg::kRounds; ++rr)
+          if (rr == r) v = make_float2(acc_m[rr * RW / 2 + j], acc_m[rr * RW / 2 + j + 1]);
+        *reinterpret_cast<float2*>(acc_tile + (wg * 64 + frag_row(wtid, j)) * Cfg::kLd + frag_col(wtid, j)) = v;
       }
-      if (SK && wi.sk_role == 1) {                     // contributor: raw partial sums -> this CTA's workspace slot
-        float4* wp = reinterpret_cast<float4*>(g.sk_ws + (((long long)blockIdx.x * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (!has_cols) continue;
+#pragma unroll 1
+      for (int cc = 0; cc < TC; cc += CH) {
+        const int cb = r * RW + half * TC + cc;         // tile column of this chunk's first channel
+        const int co = wi.co0 + cb;
+        const int cs = r * TC + cc;                     // offset in this thread's stream-K slot
+        float v[CH];
+        const float* srow = acc_tile + ml * Cfg::kLd + half * TC + cc;
 #pragma unroll
-        for (int j = 0; j < CH / 4; ++j) __stcg(wp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-        continue;
-      }
-      if (SK && wi.sk_role == 2) {                     // finisher: add the later parts, in CTA order
-        for (int k = (int)blockIdx.x + 1; k <= wi.sk_last; ++k) {
-          if (iter.boundary(k) == iter.boundary(k + 1)) continue;
-          const float4* rp = reinterpret_cast<const float4*>(g.sk_ws + (((long long)k * kEpiWarps + ew) * 32 + lane) * COLS_PER_WARP + cc);
-#pragma unroll
-          for (int j = 0; j < CH / 4; ++j) {
-            const float4 a = __ldcg(rp + j);
-            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-          }
+        for (int j = 0; j < CH / 4; ++j) {
+          const float4 t4 = *reinterpret_cast<const float4*>(srow + 4 * j);
+          v[4 * j] = t4.x; v[4 * j + 1] = t4.y; v[4 * j + 2] = t4.z; v[4 * j + 3] = t4.w;
         }
-      }
-      if (g.ksplit > 1) {
-        if (valid) {                                    // this K split's slab; the finalize kernel adds them in order
-          float4* wsp = reinterpret_cast<float4*>(g.ws + (long long)wi.ks * g.ws_slab + pix * g.Cout + co);
+        if (SK && wi.sk_role == 1) {                   // contributor: raw partial sums -> this CTA's workspace slot
+          float4* wp = reinterpret_cast<float4*>(g.sk_ws + (((long long)blockIdx.x * kEpiWarps + ew) * 32 + lane) * kThreadCols + cs);
 #pragma unroll
-          for (int j = 0; j < CH / 4; ++j) __stcg(wsp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+          for (int j = 0; j < CH / 4; ++j) __stcg(wp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+          continue;
         }
-        continue;
-      }
-      if (valid) {
-        const long long off = pix * g.Cout + co;
-        if (g.out_raw) store_split<CH, PASSES>(g.out_raw + off, g.out_raw_plane, v);   // pre-BN value (MDBLOCK residual input)
-        if (g.res && !g.res_after) {                                   // residual add before BatchNorm (MDBLOCK, layers.py:411-416)
-          const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
-          const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
+        if (SK && wi.sk_role == 2) {                   // finisher: add the later parts, in CTA order
+          for (int k = (int)blockIdx.x + 1; k <= wi.sk_last; ++k) {
+            if (iter.boundary(k) == iter.boundary(k + 1)) continue;
+            const float4* rp = reinterpret_cast<const float4*>(g.sk_ws + (((long long)k * kEpiWarps + ew) * 32 + lane) * kThreadCols + cs);
 #pragma unroll
-          for (int j8 = 0; j8 < CH / 8; ++j8) {
-            const uint4 h4 = __ldg(rh + j8);
-            const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
-            if (PASSES == 3) {
-              const uint4 l4 = __ldg(rl + j8);
-              const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
+            for (int j = 0; j < CH / 4; ++j) {
+              const float4 a = __ldcg(rp + j);
+              v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
             }
           }
         }
-        if (g.act == ACT_MASK) {
-          const int si = co + (oh * g.Wout + ow) * g.scale_pix_stride;
-          const uint4* mk = reinterpret_cast<const uint4*>(g.mask + off);
+        if (g.ksplit > 1) {
+          if (valid) {                                  // this K split's slab; the finalize kernel adds them in order
+            float4* wsp = reinterpret_cast<float4*>(g.ws + (long long)wi.ks * g.ws_slab + pix * g.Cout + co);
 #pragma unroll
-          for (int j8 = 0; j8 < CH / 8; ++j8) {
-            const uint4 m4 = __ldg(mk + j8);
-            const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float sc = g.scale_pix_stride ? __ldg(g.scale + si + j8 * 8 + j) : my_stage[cc + j8 * 8 + j];
-              v[j8 * 8 + j] = v[j8 * 8 + j] * sc * (__bfloat162float(mb[j]) > 0.f ? 1.f : g.mask_slope);
-            }
+            for (int j = 0; j < CH / 4; ++j) __stcg(wsp + j, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
           }
-          if (g.res && g.res_after) {                    // gradient of the block's residual branch joins after the mask/scale
+          continue;
+        }
+        if (valid) {
+          const long long off = pix * g.Cout + co;
+          if (g.out_raw) store_split<CH, PASSES>(g.out_raw + off, g.out_raw_plane, v);   // pre-BN value (MDBLOCK residual input)
+          if (g.res && !g.res_after) {                                   // residual add before BatchNorm (MDBLOCK, layers.py:411-416)
             const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
             const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
 #pragma unroll
@@ -419,47 +405,79 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
               }
             }
           }
-        } else {
+          if (g.act == ACT_MASK) {
+            const int si = co + (oh * g.Wout + ow) * g.scale_pix_stride;
+            const uint4* mk = reinterpret_cast<const uint4*>(g.mask + off);
 #pragma unroll
-          for (int j4 = 0; j4 < CH / 4; ++j4) {
-            const float4 sc = *reinterpret_cast<const float4*>(my_stage + cc + 4 * j4);
-            const float4 sf = *reinterpret_cast<const float4*>(my_stage + 128 + cc + 4 * j4);
-            v[4 * j4 + 0] = fmaf(v[4 * j4 + 0], sc.x, sf.x);
-            v[4 * j4 + 1] = fmaf(v[4 * j4 + 1], sc.y, sf.y);
-            v[4 * j4 + 2] = fmaf(v[4 * j4 + 2], sc.z, sf.z);
-            v[4 * j4 + 3] = fmaf(v[4 * j4 + 3], sc.w, sf.w);
-          }
-          if (g.act == ACT_ELU) {
+            for (int j8 = 0; j8 < CH / 8; ++j8) {
+              const uint4 m4 = __ldg(mk + j8);
+              const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
 #pragma unroll
-            for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.f ? v[j] : expm1f(v[j]);
-          } else if (g.act != ACT_NONE) {
+              for (int j = 0; j < 8; ++j) {
+                const float sc = g.scale_pix_stride ? __ldg(g.scale + si + j8 * 8 + j) : my_stage[cb + j8 * 8 + j];
+                v[j8 * 8 + j] = v[j8 * 8 + j] * sc * (__bfloat162float(mb[j]) > 0.f ? 1.f : g.mask_slope);
+              }
+            }
+            if (g.res && g.res_after) {                  // gradient of the block's residual branch joins after the mask/scale
+              const uint4* rh = reinterpret_cast<const uint4*>(g.res + off);
+              const uint4* rl = reinterpret_cast<const uint4*>(g.res + g.res_plane + off);
 #pragma unroll
-            for (int j = 0; j < CH; ++j) v[j] = fmaf(act_b, fabsf(v[j]), act_a * v[j]);
-          }
-        }
-        if (g.out) store_split<CH, PASSES>(g.out + off, g.out_plane, v);
-        if (g.out_f32_t) {                           // tile-blocked channel-major table: [m-tile][co][128 rows]
-          const long long tbase = ((long long)wi.mtile * g.cout_real + co) * BM + ml;
-          if (g.out_t_bf16) {
-            __nv_bfloat16* ot = reinterpret_cast<__nv_bfloat16*>(g.out_f32_t) + tbase;
+              for (int j8 = 0; j8 < CH / 8; ++j8) {
+                const uint4 h4 = __ldg(rh + j8);
+                const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h4);
+                if (PASSES == 3) {
+                  const uint4 l4 = __ldg(rl + j8);
+                  const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l4);
 #pragma unroll
-            for (int j = 0; j < CH; ++j)
-              if (co + j < g.cout_real) ot[j * BM] = __float2bfloat16_rn(v[j]);   // a warp writes 64 contiguous bytes per column
+                  for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]) + __bfloat162float(lb[j]);
+                } else {
+#pragma unroll
+                  for (int j = 0; j < 8; ++j) v[j8 * 8 + j] += __bfloat162float(hb[j]);
+                }
+              }
+            }
           } else {
-            float* ot = g.out_f32_t + tbase;
 #pragma unroll
-            for (int j = 0; j < CH; ++j)
-              if (co + j < g.cout_real) ot[j * BM] = v[j];   // a warp writes 128 contiguous bytes per column
+            for (int j4 = 0; j4 < CH / 4; ++j4) {
+              const float4 sc = *reinterpret_cast<const float4*>(my_stage + cb + 4 * j4);
+              const float4 sf = *reinterpret_cast<const float4*>(my_stage + 128 + cb + 4 * j4);
+              v[4 * j4 + 0] = fmaf(v[4 * j4 + 0], sc.x, sf.x);
+              v[4 * j4 + 1] = fmaf(v[4 * j4 + 1], sc.y, sf.y);
+              v[4 * j4 + 2] = fmaf(v[4 * j4 + 2], sc.z, sf.z);
+              v[4 * j4 + 3] = fmaf(v[4 * j4 + 3], sc.w, sf.w);
+            }
+            if (g.act == ACT_ELU) {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) v[j] = v[j] > 0.f ? v[j] : expm1f(v[j]);
+            } else if (g.act != ACT_NONE) {
+#pragma unroll
+              for (int j = 0; j < CH; ++j) v[j] = fmaf(act_b, fabsf(v[j]), act_a * v[j]);
+            }
           }
-        }
-        if (g.out_f32) {
-          float4* of = reinterpret_cast<float4*>(g.out_f32 + off);
+          if (g.out) store_split<CH, PASSES>(g.out + off, g.out_plane, v);
+          if (g.out_f32_t) {                         // tile-blocked channel-major table: [m-tile][co][128 rows]
+            const long long tbase = ((long long)wi.mtile * g.cout_real + co) * BM + ml;
+            if (g.out_t_bf16) {
+              __nv_bfloat16* ot = reinterpret_cast<__nv_bfloat16*>(g.out_f32_t) + tbase;
 #pragma unroll
-          for (int j = 0; j < CH / 4; ++j) of[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+              for (int j = 0; j < CH; ++j)
+                if (co + j < g.cout_real) ot[j * BM] = __float2bfloat16_rn(v[j]);   // a warp writes 64 contiguous bytes per column
+            } else {
+              float* ot = g.out_f32_t + tbase;
+#pragma unroll
+              for (int j = 0; j < CH; ++j)
+                if (co + j < g.cout_real) ot[j * BM] = v[j];   // a warp writes 128 contiguous bytes per column
+            }
+          }
+          if (g.out_f32) {
+            float4* of = reinterpret_cast<float4*>(g.out_f32 + off);
+#pragma unroll
+            for (int j = 0; j < CH / 4; ++j) of[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+          }
         }
       }
     }
-    if (SK && wi.sk_role == 1) {                        // publish this warp's sub-block of partial sums
+    if (SK && wi.sk_role == 1 && has_cols) {          // publish this warp's sub-block of partial sums
       __threadfence();
       __syncwarp();
       if (lane == 0) {

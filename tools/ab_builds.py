@@ -1,0 +1,142 @@
+"""A/B of two builds of the library on one GPU, in one command.
+
+    python tools/ab_builds.py build REV
+        (no GPU needed) builds the sources of git revision REV into build/ab/<REV>/libian_b200.so (git-ignored).
+    python tools/ab_builds.py run REV [--rounds 3] [--steps 30] [--warmup 5] [--variant NAME:ENV=V,...] [--out DIR]
+        runs bench.py alternately against build/ab/<REV> ("base") and the in-tree build ("head"), plus any --variant (the
+        in-tree build under extra environment settings, e.g. head_wholetiles:IAN_STREAMK=0), A B A B ... for --rounds
+        rounds.  Prints, per build, the median and range of `value`, of each `roofline.layer_ms` entry and of the
+        secondary blocks, with the card name, power limit and sampled SM clock of every run, and compares the
+        --dump-outputs arrays (z.npy, xhat.npy of the last timed step) of every build with "base" bit for bit.
+        Raw result lines go to DIR/ab_<steps>.jsonl (default DIR: build/ab/results).
+"""
+import argparse
+import json
+import os
+import shutil
+import statistics
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEAD_LIB = os.path.join(ROOT, "neural-photo-editor_b200", "libian_b200.so")
+
+
+def ab_dir(rev):
+    return os.path.join(ROOT, "build", "ab", rev)
+
+
+def cmd_build(rev):
+    out = ab_dir(rev)
+    os.makedirs(out, exist_ok=True)
+    with tempfile.TemporaryDirectory(prefix="ian_ab_") as tmp:
+        arch = subprocess.run(["git", "-C", ROOT, "archive", rev, "neural-photo-editor_b200", "include"], check=True,
+                              capture_output=True).stdout
+        subprocess.run(["tar", "-x", "-C", tmp], input=arch, check=True)
+        pkg = os.path.join(tmp, "neural-photo-editor_b200")
+        code = "import sys; sys.path.insert(0, %r); import build; build.build(force=True)" % pkg
+        subprocess.run([sys.executable, "-c", code], check=True, cwd=pkg)
+        shutil.copy2(os.path.join(pkg, "libian_b200.so"), os.path.join(out, "libian_b200.so"))
+    print(os.path.join(out, "libian_b200.so"))
+
+
+def _bench(lib, env_extra, steps, warmup, dump):
+    env = dict(os.environ, IAN_B200_LIB=lib, **env_extra)
+    cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps), "--warmup", str(warmup),
+           "--no-cpu-baseline"]
+    if dump:
+        cmd += ["--dump-outputs", dump]
+    p = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
+    if p.returncode != 0:
+        raise SystemExit("bench.py failed for %s %s:\n%s" % (lib, env_extra, p.stderr[-3000:]))
+    return json.loads([l for l in p.stdout.splitlines() if l.startswith("{")][-1])
+
+
+def _secondary(line):
+    """the bench blocks besides `value` (higher is better unless the key says ms)"""
+    out = {}
+    if line.get("edit"):
+        out["edit steps/s"] = line["edit"]["value"]
+    f = line.get("full_ian")
+    if f:
+        out["full_ian bf16 img/s"] = f["bf16"]["value"]
+        out["full_ian fp32 img/s"] = f["fp32_split"]["value"]
+    if line.get("config5"):
+        out["config5 img/s"] = line["config5"]["value"]
+    if line.get("e2e"):
+        out["e2e img/s"] = line["e2e"]["value"]
+    lat = line.get("single_image_latency")
+    if lat:
+        out["latency b1 ms"] = lat["median_ms"]
+        out["paint_stroke ms"] = lat["paint_stroke_median_ms"]
+    return out
+
+
+def _fmt(vals):
+    return "median %.4g  range [%.4g, %.4g]" % (statistics.median(vals), min(vals), max(vals))
+
+
+def cmd_run(args):
+    import numpy as np
+    builds = [("base", os.path.join(ab_dir(args.rev), "libian_b200.so"), {}), ("head", HEAD_LIB, {})]
+    for v in args.variant:
+        name, _, envs = v.partition(":")
+        builds.append((name, HEAD_LIB, dict(kv.split("=", 1) for kv in envs.split(",") if kv)))
+    for _, lib, _ in builds:
+        if not os.path.exists(lib):
+            raise SystemExit("missing %s (python tools/ab_builds.py build %s)" % (lib, args.rev))
+    os.makedirs(args.out, exist_ok=True)
+    lines = {b[0]: [] for b in builds}
+    raw = open(os.path.join(args.out, "ab_%d.jsonl" % args.steps), "w")
+    for r in range(args.rounds):
+        for name, lib, env in builds:
+            dump = os.path.join(args.out, "dump_%s" % name) if r == 0 else None
+            line = _bench(lib, env, args.steps, args.warmup, dump)
+            line["ab_build"], line["ab_round"] = name, r
+            raw.write(json.dumps(line) + "\n")
+            raw.flush()
+            lines[name].append(line)
+            g, c = line.get("gpu", {}), line.get("clocks") or {}
+            print("round %d %-16s value %.1f  (%s, %s W, SM clock median %s MHz)" % (r, name, line["value"], g.get("name"),
+                  g.get("power_limit_w"), c.get("sm_mhz")), flush=True)
+    print("\n== --steps %d --warmup %d, %d rounds, builds alternated" % (args.steps, args.warmup, args.rounds))
+    for name, _, env in builds:
+        ls = lines[name]
+        print("%s %s" % (name, env or ""))
+        print("  value (images/s)      %s" % _fmt([l["value"] for l in ls]))
+        print("  SM clock (MHz)        %s" % _fmt([(l.get("clocks") or {}).get("sm_mhz") or 0 for l in ls]))
+        for k in ls[0]["roofline"]["layer_ms"]:
+            print("  layer_ms %-12s %s" % (k, _fmt([l["roofline"]["layer_ms"][k] for l in ls])))
+        for k in _secondary(ls[0]):
+            print("  %-21s %s" % (k, _fmt([_secondary(l)[k] for l in ls])))
+    base_dump = os.path.join(args.out, "dump_base")
+    for name, _, _ in builds[1:]:
+        for f in ("z.npy", "xhat.npy"):
+            a, b = np.load(os.path.join(base_dump, f)), np.load(os.path.join(args.out, "dump_%s" % name, f))
+            same = a.shape == b.shape and np.array_equal(a, b)
+            diff = float(np.abs(a.astype(np.float64) - b).max()) if a.shape == b.shape else float("nan")
+            print("outputs %s vs base %s: %s (max abs diff %.3g)" % (name, f, "bit-identical" if same else "DIFFER", diff))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    sub = ap.add_subparsers(dest="cmd", required=True)
+    b = sub.add_parser("build")
+    b.add_argument("rev")
+    r = sub.add_parser("run")
+    r.add_argument("rev")
+    r.add_argument("--rounds", type=int, default=3)
+    r.add_argument("--steps", type=int, default=30)
+    r.add_argument("--warmup", type=int, default=5)
+    r.add_argument("--variant", action="append", default=[], metavar="NAME:ENV=V,...")
+    r.add_argument("--out", default=os.path.join(ROOT, "build", "ab", "results"))
+    a = ap.parse_args()
+    if a.cmd == "build":
+        cmd_build(a.rev)
+    else:
+        cmd_run(a)
+
+
+if __name__ == "__main__":
+    main()
