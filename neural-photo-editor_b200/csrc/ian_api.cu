@@ -3,6 +3,7 @@
 // IAN_simple graph (reference IAN_simple.py:56-241) for encode, decode, brush gradient and edit loop.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -307,6 +308,11 @@ int alloc_buf(ian_handle* h, Plan* pl, T*& out, long long elems) {
 }
 
 // ---- tap tables --------------------------------------------------------------------------------
+// The strided tables are sorted by view.  The tensor-core path runs K chunk-major (tapgemm.h), so the taps of one view run
+// back to back on the same 64 channels, and their boxes of that view overlap in all but a one-pixel edge.
+void sort_taps_by_view(TapGemm& g) {
+  std::stable_sort(g.taps, g.taps + g.phase[0].ntaps, [](const Tap& x, const Tap& y) { return x.view < y.view; });
+}
 void taps_conv_s2(TapGemm& g) {           // enc_conv: y[p] = sum_i x[2p+i-2] W[i]   (IAN_simple.py:73-116)
   g.nphase = 1;
   g.phase[0] = {0, 25, 0, 0};
@@ -316,6 +322,7 @@ void taps_conv_s2(TapGemm& g) {           // enc_conv: y[p] = sum_i x[2p+i-2] W[
       const int a = (i - 2) >> 1, r = (i - 2) & 1, b = (j - 2) >> 1, s = (j - 2) & 1;
       g.taps[t++] = {(int16_t)(r * 2 + s), (int16_t)a, (int16_t)b, (int16_t)(i * 5 + j)};
     }
+  sort_taps_by_view(g);
   g.sh = g.sw = 2;
   g.osh = g.osw = 1;
 }
@@ -347,6 +354,7 @@ void taps_deconv_bwd(TapGemm& g) {        // dx[a] = sum_ki dy[2+2a-ki] W[ki]   
       const int e = 2 - ki, f = 2 - kj;
       g.taps[t++] = {(int16_t)((e & 1) * 2 + (f & 1)), (int16_t)(e >> 1), (int16_t)(f >> 1), (int16_t)(ki * 5 + kj)};
     }
+  sort_taps_by_view(g);
   g.sh = g.sw = 2;
   g.osh = g.osw = 1;
 }

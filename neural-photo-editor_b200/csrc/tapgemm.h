@@ -176,7 +176,8 @@ __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bflo
 
 // ---- launchers (each returns the number of kernels it launched, or <0 on error) -----------------
 int launch_tapgemm_simt(const TapGemm& g, cudaStream_t st);
-// tensor-core path; maps are built by tc_build_maps() once per plan
+// tensor-core path; maps are built by tc_build_maps() once per plan.  Its K steps run chunk-major: step `it` of a phase
+// is channel chunk it / ntaps of tap it % ntaps (split-K and stream-K ranges are cut on that index).
 struct TcMaps;   // opaque: CUtensorMaps for A views and B
 TcMaps* tc_build_maps(const TapGemm& g, char* err, int errlen);
 void tc_free_maps(TcMaps*);

@@ -214,7 +214,6 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
   }
   __syncthreads();
   pdl_wait();                                           // prologue done; everything below reads / writes activations (tapgemm.h: PDL)
-  const int nchunk = g.Cin / BK;
 
   if (warp == kEpiWarps) {
     // ===================== TMA producer (whole warp in uniform control flow, one elected lane issues) =====================
@@ -224,11 +223,13 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
     WorkItem wi;
     while (iter.next(g, maps, wi)) {
       const Phase ph = g.phase[wi.phase];
+      // K order is chunk-major: step it = channel chunk it / ntaps of tap it % ntaps, so consecutive steps read the same
+      // 64 channels of (almost) the same pixels, which stay hot in L2 across the taps of a chunk
+      int t = wi.it0 % ph.ntaps, c0 = wi.it0 / ph.ntaps * BK;
       for (int it = wi.it0; it < wi.it1; ++it, ++i) {
         const int s = i % S;
         const uint32_t par = (i / S) & 1u;
-        const Tap tap = g.taps[ph.tap_begin + it / nchunk];
-        const int c0 = (it % nchunk) * BK;
+        const Tap tap = g.taps[ph.tap_begin + t];
         mbar_wait(empty_bar(s), par ^ 1u);
         const uint32_t sa = smem_base + s * Cfg::kStageBytes;
         if (elect_one_sync()) {
@@ -238,6 +239,7 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
           tma_load_3d(PASSES == 3 ? &maps.b : &maps.b1, full_bar(s), sa + kATileBytes, c0, tap.wtile * g.Cout + wi.co0, 0);
         }
         __syncwarp();
+        if (++t == ph.ntaps) { t = 0; c0 += BK; }
       }
     }
     return;
