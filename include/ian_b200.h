@@ -201,6 +201,16 @@ int ian_grad_dev(ian_handle* h, const float* z, const int32_t* boxes, const floa
 int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const float* target,
                   int target_is_frame, int n, float* g);
 
+/* ---- decoder vector-Jacobian product: reverse mode through the decoder from l_Z (reference API.py:46), any cotangent --
+ *   dz = (d x_hat / d z)^T . dx_hat
+ * z (n,100), dx_hat (n,3,64,64) float32 NCHW, dz (n,100).  The brush gradients above are the special case
+ * dx_hat = d loss / d x_hat of a box loss; this takes any pixel-space loss (soft or per-pixel weighted brushes, L1, losses
+ * on the whole frame).  Recomputes the forward.  All three graphs, both paths; bf16 precision on the flow graphs as for
+ * ian_grad_*.  A box-loss cotangent formed in float32 exactly as the kernels form it (inv = 1/(3*bh*bw); (2*inv)*(x_hat - t)
+ * or inv inside the box, 0 outside) gives ian_grad_*'s result bit for bit. */
+int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream);
+int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz);
+
 /* ---- latent edit loop: n_steps of the NPE paint rule (reference NPE.py:199-209) per sample:
  *        g = grad(z);  z <- z - weight * g * (1 + (c2 - c1))        (all float32)
  * in place on z (n,100).  `weight` = 0.05 in NPE.py:199.                                          */
@@ -242,7 +252,8 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
 
 /* ---- measurement helpers ----------------------------------------------------------------------- */
 /* Average device time (ms, CUDA events on the launch stream) of the tap-GEMM kernel of layer
- * `layer_name` ("enc_conv2", "dec_conv1", ...) over the launches since the last reset; returns <0 if
+ * `layer_name` ("enc_conv2", "dec_conv1", ...; "enc_conv1", "dec_out" and "brush_seed" -- the loss-seed kernel of the
+ * brush gradients and of ian_decode_vjp_* -- for the edge kernels) over the launches since the last reset; returns <0 if
  * the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);

@@ -8,7 +8,8 @@ later call in NPE.py work unchanged.  All numerics run in the CUDA library throu
 no CPU fallback.
 
 Extensions beyond the reference surface (SURVEY.md section 8b): `reconstruct`, `encode(..., eps)`,
-batched `grad` / `edit_steps`, and `*_dev` variants taking device pointers.
+batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space loss (torch autograd binding:
+`torch_ops.decode`), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -125,6 +126,7 @@ class IAN:
         else:
             raise NotImplementedError("config %r: known graphs are IAN_simple.py, IAN.py and IANv1.py" % base)
         self.kind = kind
+        self.device = int(device)                           # the CUDA device the handle is bound to
         self.weights_fname = str(config_path)[:-3] + '.npz'
         self.model = {k: base[:-3] + '.' + k for k in keys}
         self.dnn = dnn
@@ -384,6 +386,21 @@ class IAN:
                                             _fp(t) if t is not None else None, is_frame, n, _fp(g)))
         return g
 
+    def decode_vjp(self, z, dx_hat):
+        """Vector-Jacobian product of the decoder, dz = (d x_hat / d z)^T . dx_hat, for any pixel-space loss:
+        z float32 (n,100), dx_hat float32 (n,3,64,64) = dL/dx_hat -> dz float32 (n,100).  What T.grad of any loss on
+        X_hat w.r.t. l_Z gives in the reference (API.py:46); grad() is the box-loss special case.  Costs one decoder
+        forward and one backward."""
+        z = _z(z)
+        dx = _img(dx_hat, 'dx_hat')
+        n = z.shape[0]
+        if dx.shape[0] != n:
+            raise ValueError("dx_hat must be (%d,3,64,64), got %r" % (n, dx.shape))
+        dz = np.empty_like(z)
+        if n:
+            self._check(self._lib.ian_decode_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz)))
+        return dz
+
     def edit_steps(self, z, boxes, rgb=None, n_steps=32, weight=0.05):
         """n_steps of the NPE paint rule per sample: Z <- Z - weight*g*(1+(x2-x1)) (reference NPE.py:199-209)."""
         z = _z(z).copy()
@@ -492,6 +509,9 @@ class IAN:
     def grad_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, g_ptr, stream=0):
         self._check(self._lib.ian_grad_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame), n,
                                            g_ptr, stream or None))
+
+    def decode_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, stream=0):
+        self._check(self._lib.ian_decode_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr, stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

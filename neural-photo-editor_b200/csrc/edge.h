@@ -10,7 +10,8 @@ int launch_dec_out(const __nv_bfloat16* h3, long long plane, const float* wt, fl
 int launch_sample(const float* head, const float* eps, float* z, __nv_bfloat16* zp, long long zplane, int n,
                   cudaStream_t st);
 int launch_z_to_planes(const float* z, __nv_bfloat16* zp, long long zplane, int n, cudaStream_t st);
-int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* target, int target_is_frame,
+// loss seed (box form; or, with dxhat != NULL, a caller's (n,3,64,64) cotangent over the whole frame) + dec_out backward
+int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* target, int target_is_frame, const float* dxhat,
                           const float* wt, const float* scale3, const __nv_bfloat16* h3, __nv_bfloat16* d3,
                           long long plane, int n, cudaStream_t st);
 int launch_brush_update(const float* gpad, const int32_t* boxes, float weight, float* g_out, float* z,
@@ -23,10 +24,12 @@ int launch_made_iaf(const float* z0, const float* mw, const float* mb, float* z,
 int launch_head_gather(const float* tt, int tt_is_bf16, const int* taps, int ntaps, float* ha, int n, cudaStream_t st);
 int launch_rgb_beta_head(const float* ha, int ha_planar, float* rg, const int* taps, const float* wgb, const float* wbb, int ntaps,
                          float* xhat, float* bsave /*nullable*/, int n, cudaStream_t st);
-// brush gradient through the RGB-Beta head: seed over the box, beta/sigmoid/autoregressive backward into dpre (n,64,64,8),
-// then the im2col operand a2 (n,64,64,256 split planes) of the dense backward GEMM (see edge_kernels.cu)
-int launch_head_bwd(const float* xhat, const float* rg, const float* bsave, const int32_t* boxes, const float* target,
-                    int target_is_frame, const int* taps, const float* wgb, const float* wbb, int ntaps, float* dpre,
+// brush gradient through the RGB-Beta head: seed over the box (or, with dxhat != NULL, a caller's cotangent over the whole
+// frame) and the Beta backward into dpre (n,64,64,8); then the autoregressive backward and the im2col operand a2
+// (n,64,64,256 split planes) of the dense backward GEMM (see edge_kernels.cu)
+int launch_head_bwd_seed(const float* xhat, const float* rg, const float* bsave, const int32_t* boxes, const float* target,
+                         int target_is_frame, const float* dxhat, float* dpre, int n, cudaStream_t st);
+int launch_head_bwd(const float* rg, const int* taps, const float* wgb, const float* wbb, int ntaps, float* dpre,
                     __nv_bfloat16* a2, long long a2_plane, int n, cudaStream_t st);
 // RGB-Beta head on the tensor-core path (head_tc.cu): dense GEMM per (image, conv) + on-chip tap gather -> ha [n][6][4096]
 // (the autoregressive sigmoid / Beta part stays the three per-pixel kernels of edge_kernels.cu)

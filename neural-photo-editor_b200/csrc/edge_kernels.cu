@@ -210,23 +210,28 @@ __global__ void z_to_planes_kernel(const float* __restrict__ z, __nv_bfloat16* _
 // in shared memory (zero outside the box), every in-reach pixel pair walks the valid taps with warp-uniform control flow
 // (a warp is one pixel pair), and everything else is a coalesced zero fill that does not even read h3.  (Round 2's first
 // form ran one thread per (pixel, 4 channels) over the whole map: 104 us at batch 128, 12 % of an edit step.)
+// kDense (brush_vjp_seed_bwd_kernel, the decoder VJP ian_decode_vjp_*): seed[k,co,u,v] = dx_hat[k,co,u,v] * (1 - x_hat^2)
+// for a caller's cotangent over the whole frame -- the "box" is the frame, so every row and pixel is in reach, and
+// everything after the seed value (tap order, fmaf chain, scale * mask, hi|lo split) is the box form's code.  A box-loss
+// cotangent formed with the kernel's own expression therefore reproduces the box gradient bit for bit.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) brush_seed_bwd_kernel(const float* __restrict__ xhat, const int32_t* __restrict__ boxes,
-                                                             const float* __restrict__ target, int target_is_frame,
-                                                             const float* __restrict__ wt /*[25][128][4]*/,
-                                                             const float* __restrict__ scale3,
-                                                             const __nv_bfloat16* __restrict__ h3,
-                                                             __nv_bfloat16* __restrict__ d3, long long plane, int n) {
+template <bool kDense>
+__device__ __forceinline__ void brush_seed_bwd_body(float* sd /*[3*5*68]*/, float* ws /*[25*3*128], 16-byte aligned*/,
+                                                    const float* __restrict__ xhat, const int32_t* __restrict__ boxes,
+                                                    const float* __restrict__ target, int target_is_frame,
+                                                    const float* __restrict__ dxhat /*kDense: (n,3,64,64)*/,
+                                                    const float* __restrict__ wt /*[25][128][4]*/,
+                                                    const float* __restrict__ scale3,
+                                                    const __nv_bfloat16* __restrict__ h3,
+                                                    __nv_bfloat16* __restrict__ d3, long long plane) {
   pdl_trigger();
   pdl_wait();                                           // tapgemm.h: PDL
-  __shared__ float sd[3 * 5 * 68];                       // [co][row 2a-2 .. 2a+2][col -2 .. 65]
-  __shared__ __align__(16) float ws[25 * 3 * 128];       // dec_out weights of the valid kernel rows, [tap][co][ci] (in-reach rows only)
   const int k = blockIdx.x >> 5, a = blockIdx.x & 31;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // device-resident boxes cannot be validated on the host: clamp to the frame here (never read outside x_hat); an
   // empty box contributes nothing and brush_update_kernel turns its gradient into NaN (mean over an empty slice)
-  const int c1 = max(boxes[k * 4 + 0], 0), r1 = max(boxes[k * 4 + 1], 0);
-  const int c2 = min(boxes[k * 4 + 2], 64), r2 = min(boxes[k * 4 + 3], 64);
+  const int c1 = kDense ? 0 : max(boxes[k * 4 + 0], 0), r1 = kDense ? 0 : max(boxes[k * 4 + 1], 0);
+  const int c2 = kDense ? 64 : min(boxes[k * 4 + 2], 64), r2 = kDense ? 64 : min(boxes[k * 4 + 3], 64);
   const long long row_off = (long long)(k * 32 + a) * 32 * 128;   // this row of the map: 32 pixels x 128 channels
   // rows u = 2+2a-ki, ki in 0..4  ->  u in [2a-2, 2a+2]
   const bool row_reach = r1 < r2 && c1 < c2 && 2 * a + 2 >= r1 && 2 * a - 2 < r2;
@@ -246,7 +251,9 @@ __global__ void __launch_bounds__(256) brush_seed_bwd_kernel(const float* __rest
     if (u >= r1 && u < r2 && v >= c1 && v < c2) {
       const long long xi = ((long long)(k * 3 + co) * 64 + u) * 64 + v;
       const float xv = xhat[xi];
-      if (target) {
+      if (kDense) {
+        sdv = dxhat[xi];
+      } else if (target) {
         const float t = target_is_frame ? target[xi] : target[k * 3 + co];
         sdv = 2.f * inv * (xv - t);
       } else {
@@ -321,6 +328,25 @@ __global__ void __launch_bounds__(256) brush_seed_bwd_kernel(const float* __rest
       *reinterpret_cast<uint2*>(d3 + plane + off) = lv;
     }
   }
+}
+
+__global__ void __launch_bounds__(256) brush_seed_bwd_kernel(const float* __restrict__ xhat, const int32_t* __restrict__ boxes,
+                                                             const float* __restrict__ target, int target_is_frame,
+                                                             const float* __restrict__ wt, const float* __restrict__ scale3,
+                                                             const __nv_bfloat16* __restrict__ h3,
+                                                             __nv_bfloat16* __restrict__ d3, long long plane, int n) {
+  __shared__ float sd[3 * 5 * 68];                       // [co][row 2a-2 .. 2a+2][col -2 .. 65]
+  __shared__ __align__(16) float ws[25 * 3 * 128];       // dec_out weights of the valid kernel rows, [tap][co][ci] (in-reach rows only)
+  brush_seed_bwd_body<false>(sd, ws, xhat, boxes, target, target_is_frame, nullptr, wt, scale3, h3, d3, plane);
+}
+
+__global__ void __launch_bounds__(256) brush_vjp_seed_bwd_kernel(const float* __restrict__ xhat, const float* __restrict__ dxhat,
+                                                                 const float* __restrict__ wt, const float* __restrict__ scale3,
+                                                                 const __nv_bfloat16* __restrict__ h3,
+                                                                 __nv_bfloat16* __restrict__ d3, long long plane, int n) {
+  __shared__ float sd[3 * 5 * 68];
+  __shared__ __align__(16) float ws[25 * 3 * 128];
+  brush_seed_bwd_body<true>(sd, ws, xhat, nullptr, nullptr, 0, dxhat, wt, scale3, h3, d3, plane);
 }
 
 // g fp32 (n,128 padded) -> user g (n,100) and/or z update  z <- z - weight*g*(1+c2-c1)  (NPE.py:206-209)
@@ -637,10 +663,13 @@ int launch_z_to_planes(const float* z, __nv_bfloat16* zp, long long zplane, int 
   return CHECK_LAUNCH();
 }
 
-int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* target, int target_is_frame,
+int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* target, int target_is_frame, const float* dxhat,
                           const float* wt, const float* scale3, const __nv_bfloat16* h3, __nv_bfloat16* d3,
                           long long plane, int n, cudaStream_t st) {
-  if (launch_pdl(brush_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, boxes, target, target_is_frame, wt, scale3, h3, d3, plane, n) != cudaSuccess) return -1;
+  const cudaError_t e = dxhat
+      ? launch_pdl(brush_vjp_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, dxhat, wt, scale3, h3, d3, plane, n)
+      : launch_pdl(brush_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, boxes, target, target_is_frame, wt, scale3, h3, d3, plane, n);
+  if (e != cudaSuccess) return -1;
   return CHECK_LAUNCH();
 }
 
@@ -694,17 +723,19 @@ int launch_rgb_beta_head(const float* ha, int ha_planar, float* rg, const int* t
 //   g    : d[R,G] += MDC_Bb^T(dpreB)   (33 dilated taps, 2 -> 4 channels);  dpreG = dG * G (1-G)
 //   r    : dR     += MDC_Gb^T(dpreG)   (2 -> 2 channels);                   dpreR = dR * R (1-R)
 // and im2col lays dpre out as the K = 33 taps x 6 operand of the dense backward GEMM (dh = A2 * Wcomp).
+// kDense (head_vjp_seed_kernel, the decoder VJP): sd = dx_hat[k,c,p,q], a caller's cotangent over the whole frame; the Beta
+// backward and dpreB after it are the box form's code, so a box-loss cotangent reproduces the box gradient bit for bit.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) head_bwd_seed_kernel(const float* __restrict__ xhat, const float* __restrict__ rg,
-                                                            const float* __restrict__ bsave, const int32_t* __restrict__ boxes,
-                                                            const float* __restrict__ target, int target_is_frame,
-                                                            float* __restrict__ dpre, int n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)n * 4096) return;
+template <bool kDense>
+__device__ __forceinline__ void head_bwd_seed_body(long long i, const float* __restrict__ xhat, const float* __restrict__ rg,
+                                                   const float* __restrict__ bsave, const int32_t* __restrict__ boxes,
+                                                   const float* __restrict__ target, int target_is_frame,
+                                                   const float* __restrict__ dxhat /*kDense: (n,3,64,64)*/,
+                                                   float* __restrict__ dpre) {
   const int q = (int)(i & 63), p = (int)((i >> 6) & 63);
   const int k = (int)(i >> 12);
-  const int c1 = max(boxes[k * 4 + 0], 0), r1 = max(boxes[k * 4 + 1], 0);
-  const int c2 = min(boxes[k * 4 + 2], 64), r2 = min(boxes[k * 4 + 3], 64);
+  const int c1 = kDense ? 0 : max(boxes[k * 4 + 0], 0), r1 = kDense ? 0 : max(boxes[k * 4 + 1], 0);
+  const int c2 = kDense ? 64 : min(boxes[k * 4 + 2], 64), r2 = kDense ? 64 : min(boxes[k * 4 + 3], 64);
   float o[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (p >= r1 && p < r2 && q >= c1 && q < c2) {
     const float inv = 1.f / (3.f * (float)(r2 - r1) * (float)(c2 - c1));
@@ -713,9 +744,11 @@ __global__ void __launch_bounds__(256) head_bwd_seed_kernel(const float* __restr
     const float a[3] = {rgv.x, rgv.z, bv.x}, b[3] = {rgv.y, rgv.w, bv.y};
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float xv = xhat[((long long)(k * 3 + c) * 64 + p) * 64 + q];
       float sd = inv;
-      if (target) {
+      if (kDense) {
+        sd = dxhat[((long long)(k * 3 + c) * 64 + p) * 64 + q];
+      } else if (target) {
+        const float xv = xhat[((long long)(k * 3 + c) * 64 + p) * 64 + q];
         const float t = target_is_frame ? target[((long long)(k * 3 + c) * 64 + p) * 64 + q] : target[k * 3 + c];
         sd = 2.f * inv * (xv - t);
       }
@@ -729,6 +762,22 @@ __global__ void __launch_bounds__(256) head_bwd_seed_kernel(const float* __restr
   float4* dp = reinterpret_cast<float4*>(dpre + i * 8);
   dp[0] = make_float4(o[0], o[1], o[2], o[3]);
   dp[1] = make_float4(o[4], o[5], 0.f, 0.f);
+}
+
+__global__ void __launch_bounds__(256) head_bwd_seed_kernel(const float* __restrict__ xhat, const float* __restrict__ rg,
+                                                            const float* __restrict__ bsave, const int32_t* __restrict__ boxes,
+                                                            const float* __restrict__ target, int target_is_frame,
+                                                            float* __restrict__ dpre, int n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * 4096) return;
+  head_bwd_seed_body<false>(i, xhat, rg, bsave, boxes, target, target_is_frame, nullptr, dpre);
+}
+
+__global__ void __launch_bounds__(256) head_vjp_seed_kernel(const float* __restrict__ rg, const float* __restrict__ bsave,
+                                                            const float* __restrict__ dxhat, float* __restrict__ dpre, int n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * 4096) return;
+  head_bwd_seed_body<true>(i, nullptr, rg, bsave, nullptr, nullptr, 0, dxhat, dpre);
 }
 
 __global__ void __launch_bounds__(256) head_bwd_g_kernel(float* __restrict__ dpre, const float* __restrict__ rg,
@@ -808,15 +857,23 @@ __global__ void __launch_bounds__(256) head_bwd_im2col_kernel(const float* __res
   }
 }
 
-int launch_head_bwd(const float* xhat, const float* rg, const float* bsave, const int32_t* boxes, const float* target,
-                    int target_is_frame, const int* taps, const float* wgb, const float* wbb, int ntaps, float* dpre,
+int launch_head_bwd_seed(const float* xhat, const float* rg, const float* bsave, const int32_t* boxes, const float* target,
+                         int target_is_frame, const float* dxhat, float* dpre, int n, cudaStream_t st) {
+  const unsigned blocks = (unsigned)(((long long)n * 4096 + 255) / 256);
+  if (dxhat)
+    head_vjp_seed_kernel<<<blocks, 256, 0, st>>>(rg, bsave, dxhat, dpre, n);
+  else
+    head_bwd_seed_kernel<<<blocks, 256, 0, st>>>(xhat, rg, bsave, boxes, target, target_is_frame, dpre, n);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_head_bwd(const float* rg, const int* taps, const float* wgb, const float* wbb, int ntaps, float* dpre,
                     __nv_bfloat16* a2, long long a2_plane, int n, cudaStream_t st) {
   const long long npix = (long long)n * 4096;
   const unsigned blocks = (unsigned)((npix + 255) / 256);
-  head_bwd_seed_kernel<<<blocks, 256, 0, st>>>(xhat, rg, bsave, boxes, target, target_is_frame, dpre, n);
   head_bwd_g_kernel<<<blocks, 256, 0, st>>>(dpre, rg, taps, wbb, ntaps, n);
   head_bwd_r_kernel<<<blocks, 256, 0, st>>>(dpre, rg, taps, wgb, ntaps, n);
   head_bwd_im2col_kernel<<<(unsigned)((npix * ntaps + 255) / 256), 256, 0, st>>>(dpre, taps, ntaps, a2, a2_plane, n);
-  return cudaGetLastError() == cudaSuccess ? 4 : -1;
+  return cudaGetLastError() == cudaSuccess ? 3 : -1;
 }
 }  // namespace ian

@@ -138,7 +138,8 @@ enum LayerId {
   F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B, F_BWD_MD2A, F_BWD_CONV2, F_BWD_MD1B, F_BWD_MD1A,
   F_BWD_CONV1, F_BWD_FC2,
   L_COUNT,
-  T_CONV1 = L_COUNT, T_DEC_OUT, T_COUNT   // timing-only slots of the two edge kernels
+  T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_COUNT   // timing-only slots of the edge kernels (brush_seed: the loss-seed
+                                                        // kernel of every decoder backward, box or dense VJP seed)
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
                                     "dec_conv2", "dec_conv3", "bwd_dec_conv3", "bwd_dec_conv2", "bwd_dec_conv1", "bwd_l_dec_fc2",
@@ -147,7 +148,7 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "bwd_rgb_head", "bwd_full_dec_conv4", "bwd_dec_conv4a2", "bwd_dec_conv4a", "bwd_full_dec_conv3",
                                     "bwd_dec_conv3a2", "bwd_dec_conv3a", "bwd_full_dec_conv2", "bwd_dec_conv2a2", "bwd_dec_conv2a",
                                     "bwd_full_dec_conv1", "bwd_full_dec_fc2",
-                                    "enc_conv1", "dec_out"};
+                                    "enc_conv1", "dec_out", "brush_seed"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -283,7 +284,7 @@ struct Plan {
   cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
   // CUDA graphs of the kernel sequences behind the host entry points (small batches only; see run_graphed)
   struct GraphSlot { cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint64_t key = 0; };
-  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_COUNT };
+  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -822,15 +823,21 @@ int run_decode(ian_handle* h, Plan* pl, const float* z, float* xhat, cudaStream_
   return run_decode_from_planes(h, pl, xhat, st);
 }
 
-// decoder forward (from zp) + backward; leaves g (n,128 padded) in pl->gpad
+// decoder forward (from zp) + backward; leaves g (n,128 padded) in pl->gpad.  The loss seed is the box loss of
+// boxes / target (brush gradients), or -- dxhat != NULL -- the caller's cotangent dL/dx_hat (n,3,64,64) over the whole
+// frame (ian_decode_vjp_*); only the seed kernel differs between the two.
 int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* target, int target_is_frame,
-                  cudaStream_t st) {
+                  const float* dxhat, cudaStream_t st) {
   int rc;
   if ((rc = run_decode_from_planes(h, pl, pl->xhat, st)) != IAN_OK) return rc;
   if (has_flow(h)) {
     // the gradient is w.r.t. l_Z, the decoder's input (API.py:46: X_hat = get_output(l_out, {l_Z: Z})): no MADE/IAF backward
-    LAUNCH_TRY(h, launch_head_bwd(pl->xhat, pl->rg, pl->bsave, boxes, target, target_is_frame, h->head_taps, h->head_wgb,
-                                  h->head_wbb, h->head_ntaps, pl->dpre, pl->dha2.p, pl->dha2.plane, pl->n, st));
+    {
+      ScopedTimer tm(h, T_BRUSH_SEED, st);
+      LAUNCH_TRY(h, launch_head_bwd_seed(pl->xhat, pl->rg, pl->bsave, boxes, target, target_is_frame, dxhat, pl->dpre, pl->n, st));
+    }
+    LAUNCH_TRY(h, launch_head_bwd(pl->rg, h->head_taps, h->head_wgb, h->head_wbb, h->head_ntaps, pl->dpre, pl->dha2.p,
+                                  pl->dha2.plane, pl->n, st));
     if (h->model_kind == IAN_MODEL_V1) {
       for (int l : {F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2})
         if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
@@ -841,8 +848,11 @@ int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* ta
     }
     return IAN_OK;
   }
-  LAUNCH_TRY(h, launch_brush_seed_bwd(pl->xhat, boxes, target, target_is_frame, h->decout_wt, h->w[L_DEC_CONV3].scale,
-                                      pl->h3.p, pl->d3.p, pl->d3.plane, pl->n, st));
+  {
+    ScopedTimer tm(h, T_BRUSH_SEED, st);
+    LAUNCH_TRY(h, launch_brush_seed_bwd(pl->xhat, boxes, target, target_is_frame, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale,
+                                        pl->h3.p, pl->d3.p, pl->d3.plane, pl->n, st));
+  }
   for (int l : {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2})
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
   return IAN_OK;
@@ -1773,7 +1783,7 @@ int ian_grad_dev(ian_handle* h, const float* z, const int32_t* boxes, const floa
   const size_t tstride = target_is_frame ? 12288 : 3;
   return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
     LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
-    int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, st);
+    int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, nullptr, st);
     if (r != IAN_OK) return r;
     LAUNCH_TRY(h, launch_brush_update(pl->gpad, boxes + (size_t)off * 4, 0.f, g + (size_t)off * 100, nullptr, nullptr, 0, cn, st));
     return (int)IAN_OK;
@@ -1796,13 +1806,56 @@ int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const flo
     if (target) CUDA_TRY(h, cudaMemcpyAsync(pl->target, target + off * tstride, cn * tstride * 4, cudaMemcpyHostToDevice, st));
     int r = run_graphed(h, pl, Plan::G_GRAD, (target ? 1 : 0) + (target_is_frame ? 2 : 0), st, [&] {
       LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-      int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, st);
+      int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, nullptr, st);
       if (q != IAN_OK) return q;
       LAUNCH_TRY(h, launch_brush_update(pl->gpad, pl->boxes, 0.f, pl->z /*reuse as g staging*/, nullptr, nullptr, 0, cn, st));
       return (int)IAN_OK;
     });
     if (r != IAN_OK) return r;
     CUDA_TRY(h, cudaMemcpyAsync(g + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
+    return (int)IAN_OK;
+  });
+  if (rc != IAN_OK) return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+// ---- decoder vector-Jacobian product --------------------------------------------------------------
+// The brush gradient's kernels with the dense seed (run_grad_core, dxhat set); dz is columns 0..99 of gpad (n,128), a
+// strided copy (no box, so no empty-box NaN rule).
+int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream) {
+  int rc = check_ready(h, n, z, dz);
+  if (rc != IAN_OK) return rc;
+  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
+  if (!dx_hat) return fail(h, IAN_ERR_INVALID, "dx_hat is NULL");
+  DeviceGuard dg(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
+    int r = run_grad_core(h, pl, nullptr, nullptr, 0, dx_hat + (size_t)off * 12288, st);
+    if (r != IAN_OK) return r;
+    CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToDevice, st));
+    return (int)IAN_OK;
+  });
+}
+
+int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz) {
+  int rc = check_ready(h, n, z, dz);
+  if (rc != IAN_OK) return rc;
+  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
+  if (!dx_hat) return fail(h, IAN_ERR_INVALID, "dx_hat is NULL");
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
+    // the plan's frame-target buffer (n,3,64,64) stages the cotangent
+    CUDA_TRY(h, cudaMemcpyAsync(pl->target, dx_hat + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
+    int r = run_graphed(h, pl, Plan::G_VJP, 0, st, [&] {
+      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
+      return run_grad_core(h, pl, nullptr, nullptr, 0, pl->target, st);
+    });
+    if (r != IAN_OK) return r;
+    CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToHost, st));
     return (int)IAN_OK;
   });
   if (rc != IAN_OK) return rc;
@@ -1825,7 +1878,7 @@ int ian_edit_loop_dev(ian_handle* h, float* z, const int32_t* boxes, const float
     float* zc = z + (size_t)off * 100;
     LAUNCH_TRY(h, launch_z_to_planes(zc, pl->zp.p, pl->zp.plane, cn, st));
     for (int s = 0; s < n_steps; ++s) {
-      int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, st);
+      int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, nullptr, st);
       if (r != IAN_OK) return r;
       LAUNCH_TRY(h, launch_brush_update(pl->gpad, boxes + (size_t)off * 4, weight, nullptr, zc, pl->zp.p, pl->zp.plane, cn, st));
     }
@@ -1851,7 +1904,7 @@ int ian_edit_loop_host(ian_handle* h, float* z, const int32_t* boxes, const floa
     const uint64_t key = float_bits(weight) * 4 + (target ? 1 : 0) + (target_is_frame ? 2 : 0);
     for (int s = 0; s < n_steps; ++s) {                    // one graph = one paint step, replayed n_steps times
       int r = run_graphed(h, pl, Plan::G_EDIT_STEP, key, st, [&] {
-        int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, st);
+        int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, nullptr, st);
         if (q != IAN_OK) return q;
         LAUNCH_TRY(h, launch_brush_update(pl->gpad, pl->boxes, weight, nullptr, pl->z, pl->zp.p, pl->zp.plane, cn, st));
         return (int)IAN_OK;
@@ -2231,7 +2284,7 @@ int ian_paint_stroke_host(ian_handle* h, float* z, const int32_t* box, const flo
   CUDA_TRY(h, cudaMemcpyAsync(d_error, error, 12288 * 4, cudaMemcpyHostToDevice, st));
   rc = run_graphed(h, pl, Plan::G_STROKE, float_bits(weight), st, [&] {
     LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, 1, st));
-    int q = run_grad_core(h, pl, pl->boxes, pl->target, 1, st);                                    // NPE.py:205
+    int q = run_grad_core(h, pl, pl->boxes, pl->target, 1, nullptr, st);                                    // NPE.py:205
     if (q != IAN_OK) return q;
     LAUNCH_TRY(h, launch_brush_update(pl->gpad, pl->boxes, weight, nullptr, pl->z, pl->zp.p, pl->zp.plane, 1, st));  // :206-209
     if ((q = run_decode_from_planes(h, pl, pl->xhat, st)) != IAN_OK) return q;                     // NPE.py:218 sample_at
