@@ -720,12 +720,19 @@ struct ScopedTimer {
   }
 };
 
+// Host calls on plans of at most kGraphMaxBatch samples replay a captured CUDA graph (run_graphed).
+constexpr int kGraphMaxBatch = 32;
+
 int run_gemm(ian_handle* h, Plan* pl, int l, cudaStream_t st) {
   TapGemm g = pl->g[l];
   if (g.ksplit < 1) return fail(h, IAN_ERR_INVALID, "layer %s is not part of this plan", kLayerNames[l]);
   g.passes = h->passes;
   g.out_t_bf16 = (g.out_f32_t && h->passes == 1) ? 1 : 0;   // bf16 mode: the head's tap table travels as bf16
-  g.sk_ws = (h->streamk && !h->capturing) ? h->sk_ws : nullptr;   // the stream-K epoch is a kernel argument: not replayable
+  // The stream-K epoch is a kernel argument, so a captured graph cannot replay stream-K.  A plan small enough to be
+  // captured therefore runs whole tiles on every launch form (graph, plain launches, device-pointer calls) unless
+  // stream-K is forced, so all of them compute the same bits.
+  const bool sk_ok = !h->capturing && (h->streamk == 2 || pl->n > kGraphMaxBatch);
+  g.sk_ws = (h->streamk && sk_ok) ? h->sk_ws : nullptr;
   g.sk_force = h->streamk == 2 ? 1 : 0;
   g.sk_flags = h->sk_flags;
   g.sk_epoch = ++h->sk_epoch;
@@ -1432,8 +1439,7 @@ int for_chunks(ian_handle* h, int n, F&& f) {
 // sequence of a host entry point depends only on the plan (fixed buffers, fixed tensor maps) and a few scalars, so it is
 // captured once per (plan, entry point, key) and replayed with one cudaGraphLaunch; the H2D/D2H copies of the
 // caller's buffers stay outside the graph.  Large batches are not launch-bound (and may schedule stream-K, whose
-// epoch is a kernel argument): they keep plain launches.
-constexpr int kGraphMaxBatch = 32;
+// epoch is a kernel argument): they keep plain launches.  kGraphMaxBatch is defined above run_gemm, which also reads it.
 
 template <typename F>
 int run_graphed(ian_handle* h, Plan* pl, int slot, uint64_t key, cudaStream_t st, F&& body) {
