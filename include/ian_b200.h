@@ -211,6 +211,16 @@ int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const flo
 int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream);
 int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz);
 
+/* ---- encoder vector-Jacobian product: reverse mode through the encoder from the image (reference Z_hat, API.py:50) ------
+ *   dx = (d z / d x)^T . dz
+ * x (n,3,64,64) float32 NCHW, eps (n,100) nullable, dz (n,100), dx (n,3,64,64).  z is exactly what ian_encode_* returns for
+ * the same x and eps: mu (+ exp(logsigma) * eps) on IAN_simple; on IAN.py / IANv1.py the MADE/IAF flow of that.  No
+ * gradient w.r.t. eps.  Recomputes the forward.  All three graphs, both paths; bf16 precision on the flow graphs as for
+ * ian_grad_* (enc_conv1 and its adjoint always run in float32).  The first call on a handle builds the backward weight
+ * tiles from the forward ones on the device; the first call per batch size allocates its gradient buffers (~1 MB/image). */
+int ian_encode_vjp_dev(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx, void* stream);
+int ian_encode_vjp_host(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx);
+
 /* ---- latent edit loop: n_steps of the NPE paint rule (reference NPE.py:199-209) per sample:
  *        g = grad(z);  z <- z - weight * g * (1 + (c2 - c1))        (all float32)
  * in place on z (n,100).  `weight` = 0.05 in NPE.py:199.                                          */
@@ -252,9 +262,10 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
 
 /* ---- measurement helpers ----------------------------------------------------------------------- */
 /* Average device time (ms, CUDA events on the launch stream) of the tap-GEMM kernel of layer
- * `layer_name` ("enc_conv2", "dec_conv1", ...; "enc_conv1", "dec_out" and "brush_seed" -- the loss-seed kernel of the
- * brush gradients and of ian_decode_vjp_* -- for the edge kernels) over the launches since the last reset; returns <0 if
- * the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * `layer_name` ("enc_conv2", "dec_conv1", ...; the encoder VJP's "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4",
+ * "bwd_enc_conv3", "bwd_enc_conv2"; "enc_conv1", "dec_out", "brush_seed" -- the loss-seed kernel of the brush gradients
+ * and of ian_decode_vjp_* -- and "enc_conv1_bwd" -- enc_conv1's adjoint in ian_encode_vjp_* -- for the edge kernels) over
+ * the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

@@ -9,7 +9,8 @@ no CPU fallback.
 
 Extensions beyond the reference surface (SURVEY.md section 8b): `reconstruct`, `encode(..., eps)`,
 batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space loss (torch autograd binding:
-`torch_ops.decode`), and `*_dev` variants taking device pointers.
+`torch_ops.decode`), the encoder VJP `encode_vjp` for any loss on the latent (torch autograd binding:
+`torch_ops.encode`), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -401,6 +402,25 @@ class IAN:
             self._check(self._lib.ian_decode_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz)))
         return dz
 
+    def encode_vjp(self, images, dz, eps=None):
+        """Vector-Jacobian product of the encoder, dx = (d z / d x)^T . dz, for any loss on the latent: images as for
+        encode() (n,3,64,64), dz float32 (n,100) = dL/dz, eps as for encode() -> dx float32 (n,3,64,64).  z is what
+        encode(images, eps) returns (on IAN.py / IANv1.py after the MADE/IAF flow), so this is what T.grad of any loss on
+        Z_hat w.r.t. the image gives in the reference (API.py:50).  No gradient w.r.t. eps.  Costs one encoder forward and
+        one backward."""
+        x = _img(images)
+        n = x.shape[0]
+        d = _z(dz, 'dz')
+        if d.shape[0] != n:
+            raise ValueError("dz must be (%d,100), got %r" % (n, d.shape))
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        if n:
+            e = None if eps is None else _z(eps, 'eps')
+            if e is not None and e.shape[0] != n:
+                raise ValueError("eps must be (%d,100), got %r" % (n, e.shape))
+            self._check(self._lib.ian_encode_vjp_host(self._h, _fp(x), n, _fp(e) if e is not None else None, _fp(d), _fp(dx)))
+        return dx
+
     def edit_steps(self, z, boxes, rgb=None, n_steps=32, weight=0.05):
         """n_steps of the NPE paint rule per sample: Z <- Z - weight*g*(1+(x2-x1)) (reference NPE.py:199-209)."""
         z = _z(z).copy()
@@ -512,6 +532,9 @@ class IAN:
 
     def decode_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, stream=0):
         self._check(self._lib.ian_decode_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr, stream or None))
+
+    def encode_vjp_dev(self, x_ptr, dz_ptr, n, dx_ptr, eps_ptr=0, stream=0):
+        self._check(self._lib.ian_encode_vjp_dev(self._h, x_ptr, int(n), eps_ptr or None, dz_ptr, dx_ptr, stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

@@ -55,6 +55,8 @@ SIGNATURES = {
     "ian_grad_host": (C.c_int, [_H, _F, _I, _F, C.c_int, C.c_int, _F]),
     "ian_decode_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ian_decode_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F]),
+    "ian_encode_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_encode_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F]),
     "ian_edit_loop_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float,
                                     C.c_void_p]),
     "ian_edit_loop_host": (C.c_int, [_H, _F, _I, _F, C.c_int, C.c_int, C.c_int, C.c_float]),

@@ -50,8 +50,10 @@ constexpr int kTBytes = 128 * kTLd * 4;
 constexpr int kSmemBytes = 1024 + kAStages * kAStage + 2 * kBChunk + kTBytes + 256;
 constexpr int kItemsPerImage = 16;           // 32 input rows / 2 interior rows per item
 
-__global__ void __launch_bounds__(kThreads, 1)
-decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant__ DecOutDst dst, const int n_img) {
+// kTanh = false (conv1_bwd_tc_kernel): the same GEMM + col2im with an identity epilogue.  enc_conv1's adjoint (3 <- 128
+// channels, 64x64 <- 32x32, stride 2, pad 2) is this transposed convolution on the tap-flipped conv1 weights.
+template <bool kTanh>
+__device__ __forceinline__ void decout_tc_body(const DecOutMaps& maps, const DecOutDst& dst, const int n_img) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -157,7 +159,7 @@ decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant_
       }
     }
     const long long off = ((long long)n * 3 * 64 + (2 * p0 + ur)) * 64 + v;
-    const float y0 = tanhf(a0), y1 = tanhf(a1), y2 = tanhf(a2);
+    const float y0 = kTanh ? tanhf(a0) : a0, y1 = kTanh ? tanhf(a1) : a1, y2 = kTanh ? tanhf(a2) : a2;
     for (int d = 0; d < dst.n; ++d) {                  // d > 0: peer GPUs' gather buffers (st.global over NVLink)
       float* o = dst.base[d] + off;
       o[0] = y0;
@@ -166,6 +168,18 @@ decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant_
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");     // T tile consumed: may be overwritten
   }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant__ DecOutDst dst, const int n_img) {
+  decout_tc_body<true>(maps, dst, n_img);
+}
+
+// encoder VJP: maps.a = e1 (n,32,32,128) split planes, the gradient of enc_conv1's pre-activation; maps.b = rows
+// tap*3 + c holding W1[o][c][24 - tap] over o -> dx (n,3,64,64) float32
+__global__ void __launch_bounds__(kThreads, 1)
+conv1_bwd_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant__ DecOutDst dst, const int n_img) {
+  decout_tc_body<false>(maps, dst, n_img);
 }
 
 // ---- cross-GPU barrier over peer memory: every rank owns flags[kMaxPeers]; rank r writes its epoch into slot r of
@@ -331,6 +345,24 @@ int launch_dec_out_tc(const DecOutMaps* maps, float* const* dsts, int ndst, int 
   dst.n = ndst;
   for (int d = 0; d < ndst; ++d) dst.base[d] = dsts[d];
   if (launch_pdl(decout_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, dst, n) != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_conv1_bwd_tc(const DecOutMaps* maps, float* dx, int n, cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(conv1_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess) return -1;
+    attr_set.set_done(dev);
+  }
+  const int num_sms = tc_num_sms();
+  const int total = n * kItemsPerImage;
+  const int grid = total < num_sms ? total : num_sms;
+  DecOutDst dst;
+  memset(&dst, 0, sizeof(dst));
+  dst.n = 1;
+  dst.base[0] = dx;
+  if (launch_pdl(conv1_bwd_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, dst, n) != cudaSuccess) return -1;
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

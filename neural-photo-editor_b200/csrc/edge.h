@@ -7,6 +7,17 @@ namespace ian {
 int launch_conv1(const float* x, const float* wt, const float* bias, __nv_bfloat16* out, long long plane, int n,
                  cudaStream_t st);
 int launch_dec_out(const __nv_bfloat16* h3, long long plane, const float* wt, float* xhat, int n, cudaStream_t st);
+// enc_conv1's adjoint for the encoder VJP: dec_out's kernel body with an identity epilogue on the conv1 gradient planes e1
+// (n,32,32,128) and the tap-flipped conv1 weights wt[t][o][c(4)] = W[o][c][24-t] -> dx (n,3,64,64) float32
+int launch_conv1_bwd(const __nv_bfloat16* e1, long long plane, const float* wt, float* dx, int n, cudaStream_t st);
+// the rest of the encoder VJP's small kernels (enc_vjp.cu)
+int launch_made_iaf_bwd(const float* z0, const float* mw, const float* mb, const float* dz, float* dzi, int n, cudaStream_t st);
+int launch_enc_vjp_seed(const float* head, const float* eps, const float* dz, const float* scale, __nv_bfloat16* out,
+                        long long plane, int n, cudaStream_t st);
+int launch_enc_fc1_bwd(const float* g, const __nv_bfloat16* f1, long long f1_plane, const float* scale, int elu,
+                       __nv_bfloat16* out, long long plane, int n, cudaStream_t st);
+int launch_permute_tiles(const __nv_bfloat16* in, long long in_plane, __nv_bfloat16* out, int ntiles, int R, int C, int flip,
+                         cudaStream_t st);
 int launch_sample(const float* head, const float* eps, float* z, __nv_bfloat16* zp, long long zplane, int n,
                   cudaStream_t st);
 int launch_z_to_planes(const float* z, __nv_bfloat16* zp, long long zplane, int n, cudaStream_t st);
@@ -55,6 +66,9 @@ DecOutMaps* decout_build_maps(const __nv_bfloat16* h3, long long h3_plane, int n
 void decout_free_maps(DecOutMaps*);
 // dsts[0..ndst): destination base pointers (1 = local only; >1 = every rank's gather buffer incl. peers)
 int launch_dec_out_tc(const DecOutMaps* maps, float* const* dsts, int ndst, int n, cudaStream_t st);
+// enc_conv1's adjoint on the tensor-core path: decout_tc's kernel body with an identity epilogue; maps built by
+// decout_build_maps on the conv1 gradient planes e1 and the [2][80][128] planes of rows tap*3 + c = W1[o][c][24 - tap]
+int launch_conv1_bwd_tc(const DecOutMaps* maps, float* dx, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

@@ -94,9 +94,11 @@ __global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ x,
 // ------------------------------------------------------------------------------------------------
 constexpr int DO_T = 8, DO_P = DO_T + 2, DO_LD = 132;
 
-__global__ void __launch_bounds__(256) dec_out_kernel(const __nv_bfloat16* __restrict__ h3, long long plane,
-                                                      const float* __restrict__ wt /*[25][128][4]*/,
-                                                      float* __restrict__ xhat, int n_img) {
+// kTanh = false (conv1_bwd_kernel): the same transposed convolution with an identity epilogue.  enc_conv1's adjoint
+// (3 <- 128 channels, 64x64 <- 32x32, stride 2, pad 2) is exactly this geometry with the tap-flipped conv1 weights.
+template <bool kTanh>
+__device__ __forceinline__ void dec_out_body(const __nv_bfloat16* __restrict__ h3, long long plane,
+                                             const float* __restrict__ wt, float* __restrict__ xhat) {
   extern __shared__ __align__(16) float smem[];
   float* Xs = smem;                          // [100][132]
   float* Ws = smem + DO_P * DO_P * DO_LD;    // [25*128*4]
@@ -155,9 +157,25 @@ __global__ void __launch_bounds__(256) dec_out_kernel(const __nv_bfloat16* __res
   }
   const int oy = 2 * (py0 + p) + r, ox = 2 * (px0 + q) + s;
   float* o = xhat + (long long)img * 3 * 4096 + oy * 64 + ox;
-  o[0] = tanhf(a0);
-  o[4096] = tanhf(a1);
-  o[8192] = tanhf(a2);
+  o[0] = kTanh ? tanhf(a0) : a0;
+  o[4096] = kTanh ? tanhf(a1) : a1;
+  o[8192] = kTanh ? tanhf(a2) : a2;
+}
+
+__global__ void __launch_bounds__(256) dec_out_kernel(const __nv_bfloat16* __restrict__ h3, long long plane,
+                                                      const float* __restrict__ wt /*[25][128][4]*/,
+                                                      float* __restrict__ xhat, int n_img) {
+  dec_out_body<true>(h3, plane, wt, xhat);
+}
+
+// encoder VJP: e1 (n,32,32,128) split planes = gradient of enc_conv1's pre-activation -> dx (n,3,64,64) float32;
+// wt[t][o][c] = W1[o][c][24 - t] (c < 3, slot 3 zero)
+__global__ void __launch_bounds__(256) conv1_bwd_kernel(const __nv_bfloat16* __restrict__ e1, long long plane,
+                                                        const float* __restrict__ wt /*[25][128][4]*/,
+                                                        float* __restrict__ dx, int n_img) {
+  pdl_trigger();
+  pdl_wait();                                           // tapgemm.h: PDL
+  dec_out_body<false>(e1, plane, wt, dx);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -649,6 +667,18 @@ int launch_dec_out(const __nv_bfloat16* h3, long long plane, const float* wt, fl
     attr_set.set_done(dev);
   }
   dec_out_kernel<<<n * 16, 256, dec_out_smem_bytes(), st>>>(h3, plane, wt, xhat, n);
+  return CHECK_LAUNCH();
+}
+
+int launch_conv1_bwd(const __nv_bfloat16* e1, long long plane, const float* wt, float* dx, int n, cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(conv1_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_out_smem_bytes()) != cudaSuccess) return -1;
+    attr_set.set_done(dev);
+  }
+  if (launch_pdl(conv1_bwd_kernel, dim3((unsigned)n * 16u), dim3(256), (size_t)dec_out_smem_bytes(), st, e1, plane, wt, dx, n) != cudaSuccess)
+    return -1;
   return CHECK_LAUNCH();
 }
 

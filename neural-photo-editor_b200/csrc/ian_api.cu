@@ -137,9 +137,12 @@ enum LayerId {
   // brush gradient through the IAN.py / IANv1.py decoders (T.grad at API.py:59,64 on those graphs)
   F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B, F_BWD_MD2A, F_BWD_CONV2, F_BWD_MD1B, F_BWD_MD1A,
   F_BWD_CONV1, F_BWD_FC2,
+  // encoder VJP (ian_encode_vjp_*): adjoints of the encoder head, enc_fc1 and enc_conv4..2, built on first use
+  E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2,
   L_COUNT,
-  T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_COUNT   // timing-only slots of the edge kernels (brush_seed: the loss-seed
-                                                        // kernel of every decoder backward, box or dense VJP seed)
+  T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD, T_COUNT   // timing-only slots of the edge kernels (brush_seed: the
+                                                        // loss-seed kernel of every decoder backward, box or dense VJP seed;
+                                                        // enc_conv1_bwd: enc_conv1's adjoint, the encoder VJP's last kernel)
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
                                     "dec_conv2", "dec_conv3", "bwd_dec_conv3", "bwd_dec_conv2", "bwd_dec_conv1", "bwd_l_dec_fc2",
@@ -148,7 +151,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "bwd_rgb_head", "bwd_full_dec_conv4", "bwd_dec_conv4a2", "bwd_dec_conv4a", "bwd_full_dec_conv3",
                                     "bwd_dec_conv3a2", "bwd_dec_conv3a", "bwd_full_dec_conv2", "bwd_dec_conv2a2", "bwd_dec_conv2a",
                                     "bwd_full_dec_conv1", "bwd_full_dec_fc2",
-                                    "enc_conv1", "dec_out", "brush_seed"};
+                                    "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4", "bwd_enc_conv3", "bwd_enc_conv2",
+                                    "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -208,6 +212,9 @@ struct ian_handle {
   __nv_bfloat16* conv1_tc_wt = nullptr;    // [3][128 cout][64 k] bf16 blocks (hi | lo | tail), k = c*25+i*5+j (75 used)
   Conv1Maps* conv1_maps = nullptr;
   float* decout_wt = nullptr;  // [25][128][4] fp32 (SIMT forward + brush backward)
+  float* conv1_bwd_wt = nullptr;   // [25][128][4] fp32, W1[o][c][24-t]: enc_conv1's adjoint (built on the first encoder VJP,
+                                   // with the E_BWD_* weight tiles); SIMT path
+  __nv_bfloat16* conv1_bwd_tc_wt = nullptr;   // [2][80][128] bf16 planes, row = tap*3 + c, W1[o][c][24-t]; tensor-core path
   __nv_bfloat16* decout_tc_wt = nullptr;   // [2][80][128] bf16 planes, row = tap*3+co (tensor-core forward)
   // full IAN extras
   std::vector<int32_t> made_ordering;       // MADE input ordering (mask_generator.py:35-38); set by ian_set_made_ordering
@@ -274,9 +281,15 @@ struct Plan {
   // brush backward of the flow models: saved B, head gradient, its im2col operand, and the per-stage gradients
   float *bsave = nullptr, *dpre = nullptr;
   Planes dha2, d4, ds3, du3, dx3, ds2, du2, dx2, ds1, du1, dx1, dfh0;
+  // encoder VJP (allocated on the plan's first ian_encode_vjp_* call): gradient planes of the head's pre-BN output, of
+  // enc_fc1's and enc_conv4..1's pre-activations; dz staging, dz_iaf, enc_fc1's float32 output gradient, split-K slabs
+  bool evjp = false;
+  Planes eh, ef1, e4, e3, e2, e1;
+  float *edz = nullptr, *edzi = nullptr, *eg = nullptr;
   TapGemm g[L_COUNT];
   TcMaps* maps[L_COUNT] = {nullptr};
   DecOutMaps* decout_maps = nullptr;
+  DecOutMaps* conv1_bwd_maps = nullptr;   // encoder VJP: enc_conv1's adjoint on the e1 planes (tensor-core path)
   Conv1OutMap* conv1_out = nullptr;       // TMA-store view of a1 (conv1_tc.cu)
   HeadMaps* head_maps = nullptr;
   // pipelined host API: double-buffered boundary tensors + events (allocated on first use)
@@ -284,7 +297,7 @@ struct Plan {
   cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
   // CUDA graphs of the kernel sequences behind the host entry points (small batches only; see run_graphed)
   struct GraphSlot { cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint64_t key = 0; };
-  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_COUNT };
+  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -691,6 +704,7 @@ void free_plan(Plan* pl) {
   }
   for (int l = 0; l < L_COUNT; ++l) if (pl->maps[l]) tc_free_maps(pl->maps[l]);
   if (pl->decout_maps) decout_free_maps(pl->decout_maps);
+  if (pl->conv1_bwd_maps) decout_free_maps(pl->conv1_bwd_maps);
   if (pl->conv1_out) conv1_free_out_map(pl->conv1_out);
   if (pl->head_maps) head_free_maps(pl->head_maps);
   for (auto& gs : pl->graph) if (gs.exec) cudaGraphExecDestroy(gs.exec);
@@ -1475,6 +1489,155 @@ int run_graphed(ian_handle* h, Plan* pl, int slot, uint64_t key, cudaStream_t st
 
 inline uint64_t float_bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 
+// ---- encoder vector-Jacobian product -------------------------------------------------------------
+// dx = (dz/dx)^T dz through the encoder (and, on IAN.py / IANv1.py, the MADE/IAF flow).  The adjoint of a layer whose
+// forward tile is B[t][co][ci] is the tap-GEMM with tiles B'[t'][ci][co]: for the dense layers t' = t; for the 5x5
+// stride-2 convolutions y[p] = sum_i x[2p+i-2] W[i], the adjoint dx[2q+r] = sum_d dy[q+d] W[2+r-2d] is the decoder's
+// transposed convolution (taps_deconv_s2, tile 2+2d-r) on the flipped tile t' = 24 - t.  ian_finalize has dropped the
+// host parameters by now, so the tiles are permuted on the device from the forward ones: a hi|lo split is per element,
+// so a permuted pair of planes is bit for bit what splitting the re-laid float32 weights would give.
+// Each backward GEMM's epilogue applies the derivative of the activation it lands on (LeakyRectify(0.2) as the mask
+// slope on the stored forward activation) times that layer's BatchNorm scale.
+int ensure_enc_vjp_weights(ian_handle* h) {
+  if (h->conv1_bwd_wt && h->conv1_bwd_tc_wt) return IAN_OK;
+  cudaStream_t st = h->stream;
+  struct Perm { int lb, lf, flip; const float* scale_src; int scale_len, repeat; } perms[] = {
+      {E_BWD_HEAD, L_ENC_HEAD, 0, nullptr, 1024, 1},                   // 256 -> 1024; enc_fc1's derivative: enc_fc1_bwd_kernel
+      {E_BWD_FC1, L_ENC_FC1, 0, h->w[L_ENC_CONV4].scale, 1024, 16},   // 1024 -> 16384 = (4,4,1024) NHWC: bnorm4 scale, per column
+      {E_BWD_CONV4, L_ENC_CONV4, 1, h->w[L_ENC_CONV3].scale, 512, 1},  // -> a3: bnorm3
+      {E_BWD_CONV3, L_ENC_CONV3, 1, h->w[L_ENC_CONV2].scale, 256, 1},  // -> a2: bnorm2
+      {E_BWD_CONV2, L_ENC_CONV2, 1, nullptr, 128, 1}};                 // -> a1: conv1 has a bias and no BatchNorm
+  for (const Perm& p : perms) {
+    const DevWeights& f = h->w[p.lf];
+    DevWeights& b = h->w[p.lb];
+    if (!b.b) {
+      CUDA_TRY(h, cudaMalloc((void**)&b.b, (size_t)f.plane * 2 * sizeof(__nv_bfloat16)));
+      LAUNCH_TRY(h, launch_permute_tiles(f.b, f.plane, b.b, f.ntiles, f.Cout, f.Cin, p.flip, st));
+      b.plane = f.plane; b.ntiles = f.ntiles; b.Cout = f.Cin; b.Cin = f.Cout;
+    }
+    if (!b.scale) {
+      CUDA_TRY(h, cudaMalloc((void**)&b.scale, (size_t)p.scale_len * p.repeat * sizeof(float)));
+      if (p.scale_src) {
+        for (int r = 0; r < p.repeat; ++r)
+          CUDA_TRY(h, cudaMemcpyAsync(b.scale + (size_t)r * p.scale_len, p.scale_src, (size_t)p.scale_len * sizeof(float),
+                                      cudaMemcpyDeviceToDevice, st));
+      } else {
+        const std::vector<float> ones((size_t)p.scale_len, 1.f);
+        CUDA_TRY(h, cudaMemcpyAsync(b.scale, ones.data(), ones.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(h, cudaStreamSynchronize(st));
+      }
+    }
+  }
+  // enc_conv1's adjoint in dec_out's layout: wt[t][o][c] = W1[o][c][24 - t], from conv1_wt[(c*25 + t)*128 + o]
+  std::vector<float> w1(75 * 128), wt(25 * 128 * 4, 0.f);
+  CUDA_TRY(h, cudaMemcpyAsync(w1.data(), h->conv1_wt, w1.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  for (int t = 0; t < 25; ++t)
+    for (int o = 0; o < 128; ++o)
+      for (int c = 0; c < 3; ++c) wt[((size_t)t * 128 + o) * 4 + c] = w1[((size_t)c * 25 + 24 - t) * 128 + o];
+  // tensor-core form (decout_tc.cu's layout): rows tap*3 + c (75, padded to 80), K-major over o; bf16 hi|lo planes
+  std::vector<uint16_t> planes(2 * 80 * 128, 0);
+  for (int t = 0; t < 25; ++t)
+    for (int c = 0; c < 3; ++c)
+      for (int o = 0; o < 128; ++o) {
+        const float w = wt[((size_t)t * 128 + o) * 4 + c];
+        const uint16_t hi = f2bf(w);
+        planes[(t * 3 + c) * 128 + o] = hi;
+        planes[80 * 128 + (t * 3 + c) * 128 + o] = f2bf(w - bf2f(hi));
+      }
+  if (!h->conv1_bwd_tc_wt) {
+    CUDA_TRY(h, cudaMalloc((void**)&h->conv1_bwd_tc_wt, planes.size() * 2));
+    CUDA_TRY(h, cudaMemcpyAsync(h->conv1_bwd_tc_wt, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice, st));
+  }
+  if (!h->conv1_bwd_wt) {
+    CUDA_TRY(h, cudaMalloc((void**)&h->conv1_bwd_wt, wt.size() * sizeof(float)));
+    CUDA_TRY(h, cudaMemcpyAsync(h->conv1_bwd_wt, wt.data(), wt.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+int ensure_enc_vjp_plan(ian_handle* h, Plan* pl) {
+  if (pl->evjp) return IAN_OK;
+  int rc;
+  if ((rc = ensure_enc_vjp_weights(h)) != IAN_OK) return rc;
+  const int n = pl->n;
+  const long long N = n;
+  if ((rc = alloc_planes(h, pl, pl->eh, N * 256)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->ef1, N * 1024)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->e4, N * 16384)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->e3, N * 8 * 8 * 512)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->e2, N * 16 * 16 * 256)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->e1, N * 32 * 32 * 128)) != IAN_OK) return rc;
+  if ((rc = alloc_buf(h, pl, pl->edz, N * 100)) != IAN_OK) return rc;
+  if ((rc = alloc_buf(h, pl, pl->edzi, N * 100)) != IAN_OK) return rc;
+  if ((rc = alloc_buf(h, pl, pl->eg, N * 1024)) != IAN_OK) return rc;
+  TapGemm* g = pl->g;
+  auto mask = [&](int l, const Planes& m, const Planes& out) {
+    g[l].act = ACT_MASK; g[l].mask = m.p; g[l].mask_slope = 0.2f; g[l].out = out.p; g[l].out_plane = out.plane;
+  };
+  set_io(g[E_BWD_HEAD], pl->eh, n, 1, 1, 256, 1, 1, h->w[E_BWD_HEAD], 1, 1); taps_dense(g[E_BWD_HEAD]);
+  g[E_BWD_HEAD].act = ACT_NONE; g[E_BWD_HEAD].out_f32 = pl->eg;
+  set_io(g[E_BWD_FC1], pl->ef1, n, 1, 1, 1024, 1, 1, h->w[E_BWD_FC1], 1, 1); taps_dense(g[E_BWD_FC1]);
+  mask(E_BWD_FC1, pl->a4, pl->e4);                      // a4 (n,4,4,1024) NHWC is the (n,16384) output's geometry
+  set_io(g[E_BWD_CONV4], pl->e4, n, 4, 4, 1024, 4, 4, h->w[E_BWD_CONV4], 8, 8); taps_deconv_s2(g[E_BWD_CONV4]);
+  mask(E_BWD_CONV4, pl->a3, pl->e3);
+  set_io(g[E_BWD_CONV3], pl->e3, n, 8, 8, 512, 8, 8, h->w[E_BWD_CONV3], 16, 16); taps_deconv_s2(g[E_BWD_CONV3]);
+  mask(E_BWD_CONV3, pl->a2, pl->e2);
+  set_io(g[E_BWD_CONV2], pl->e2, n, 16, 16, 256, 16, 16, h->w[E_BWD_CONV2], 32, 32); taps_deconv_s2(g[E_BWD_CONV2]);
+  mask(E_BWD_CONV2, pl->a1, pl->e1);
+  const std::initializer_list<int> layers = {E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2};
+  mark_splitk_candidates(pl, layers);
+  long long need = 0;
+  for (int l : layers) {
+    char err[256] = {0};
+    pl->maps[l] = tc_build_maps(g[l], err, sizeof(err));
+    if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
+    if (g[l].ksplit == 0) g[l].ksplit = h->splitk ? choose_ksplit(g[l]) : 1;
+    if (g[l].ksplit > 1) {
+      g[l].ws_slab = (long long)g[l].n_img * g[l].Hout * g[l].Wout * g[l].Cout;
+      need = std::max(need, g[l].ws_slab * g[l].ksplit);
+    }
+  }
+  if (need) {                                           // the chain's own split-K slabs: the plan's other layers keep theirs
+    float* ws = nullptr;
+    if ((rc = alloc_buf(h, pl, ws, need)) != IAN_OK) return rc;
+    for (int l : layers) if (g[l].ksplit > 1) g[l].ws = ws;
+  }
+  {   // both paths: ian_set_path may switch a live handle
+    char err[256] = {0};
+    pl->conv1_bwd_maps = decout_build_maps(pl->e1.p, pl->e1.plane, n, h->conv1_bwd_tc_wt, 80 * 128, err, sizeof(err));
+    if (!pl->conv1_bwd_maps) return fail(h, IAN_ERR_CUDA, "enc_conv1_bwd: %s", err);
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  pl->evjp = true;
+  return IAN_OK;
+}
+
+// the forward (run_encode) on x, then the backward chain; dz (n,100) is the cotangent of what ian_encode_* returns
+int run_encode_vjp(ian_handle* h, Plan* pl, const float* x, const float* eps, const float* dz, float* dx, cudaStream_t st) {
+  const int n = pl->n;
+  int rc;
+  if ((rc = run_encode(h, pl, x, eps, nullptr, st)) != IAN_OK) return rc;
+  const float* dzi = dz;
+  if (has_flow(h)) {
+    LAUNCH_TRY(h, launch_made_iaf_bwd(pl->z0, h->made_w, h->made_b, dz, pl->edzi, n, st));
+    dzi = pl->edzi;
+  }
+  LAUNCH_TRY(h, launch_enc_vjp_seed(pl->head, eps, dzi, h->w[L_ENC_HEAD].scale, pl->eh.p, pl->eh.plane, n, st));
+  if ((rc = run_gemm(h, pl, E_BWD_HEAD, st)) != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_enc_fc1_bwd(pl->eg, pl->f1.p, pl->f1.plane, h->w[L_ENC_FC1].scale, has_flow(h) ? 0 : 1, pl->ef1.p,
+                                   pl->ef1.plane, n, st));
+  for (int l : {E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2})
+    if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+  ScopedTimer tm(h, T_CONV1_BWD, st);
+  if (h->path == IAN_PATH_TC)
+    LAUNCH_TRY(h, launch_conv1_bwd_tc(pl->conv1_bwd_maps, dx, n, st));
+  else
+    LAUNCH_TRY(h, launch_conv1_bwd(pl->e1.p, pl->e1.plane, h->conv1_bwd_wt, dx, n, st));
+  return IAN_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1618,7 +1781,7 @@ int ian_destroy(ian_handle* h) {
   cudaStreamSynchronize(h->d2h_stream);
   for (auto& kv : h->plans) free_plan(kv.second);
   for (auto& w : h->w) { cudaFree(w.b); cudaFree(w.scale); cudaFree(w.shift); }
-  cudaFree(h->conv1_wt); cudaFree(h->conv1_b); cudaFree(h->decout_wt); cudaFree(h->decout_tc_wt);
+  cudaFree(h->conv1_wt); cudaFree(h->conv1_b); cudaFree(h->decout_wt); cudaFree(h->decout_tc_wt); cudaFree(h->conv1_bwd_wt); cudaFree(h->conv1_bwd_tc_wt);
   cudaFree(h->sk_ws); cudaFree(h->sk_flags);
   cudaFree(h->conv1_tc_wt); if (h->conv1_maps) conv1_free_maps(h->conv1_maps);
   cudaFree(h->made_w); cudaFree(h->made_b); cudaFree(h->head_taps); cudaFree(h->head_wgb); cudaFree(h->head_wbb);
@@ -1862,6 +2025,48 @@ int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int 
     });
     if (r != IAN_OK) return r;
     CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToHost, st));
+    return (int)IAN_OK;
+  });
+  if (rc != IAN_OK) return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+// ---- encoder vector-Jacobian product --------------------------------------------------------------
+// The first call on a handle permutes the backward weight tiles; the first call on a plan allocates its gradient planes
+// and tensor maps (about 1 MB per image).  Both happen before any graph capture; handles and plans that never call these
+// keep their memory as it was.
+int ian_encode_vjp_dev(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx, void* stream) {
+  int rc = check_ready(h, n, x, dx);
+  if (rc != IAN_OK) return rc;
+  if (!dz) return fail(h, IAN_ERR_INVALID, "dz is NULL");
+  DeviceGuard dg(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  return for_chunks(h, n, [&](Plan* pl, int off, int) {
+    int r = ensure_enc_vjp_plan(h, pl);
+    if (r != IAN_OK) return r;
+    return run_encode_vjp(h, pl, x + (size_t)off * 12288, eps ? eps + (size_t)off * 100 : nullptr, dz + (size_t)off * 100,
+                          dx + (size_t)off * 12288, st);
+  });
+}
+
+int ian_encode_vjp_host(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx) {
+  int rc = check_ready(h, n, x, dx);
+  if (rc != IAN_OK) return rc;
+  if (!dz) return fail(h, IAN_ERR_INVALID, "dz is NULL");
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    int r = ensure_enc_vjp_plan(h, pl);
+    if (r != IAN_OK) return r;
+    CUDA_TRY(h, cudaMemcpyAsync(pl->x, x + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
+    if (eps) CUDA_TRY(h, cudaMemcpyAsync(pl->eps, eps + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(h, cudaMemcpyAsync(pl->edz, dz + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
+    // the plan's x_hat buffer (n,3,64,64) stages dx
+    r = run_graphed(h, pl, Plan::G_ENC_VJP, eps ? 1 : 0, st,
+                    [&] { return run_encode_vjp(h, pl, pl->x, eps ? pl->eps : nullptr, pl->edz, pl->xhat, st); });
+    if (r != IAN_OK) return r;
+    CUDA_TRY(h, cudaMemcpyAsync(dx + (size_t)off * 12288, pl->xhat, (size_t)cn * 12288 * 4, cudaMemcpyDeviceToHost, st));
     return (int)IAN_OK;
   });
   if (rc != IAN_OK) return rc;

@@ -1,12 +1,17 @@
-"""torch autograd binding of the IAN decoder, through the C-ABI of libian_b200.so (include/ian_b200.h):
+"""torch autograd binding of the IAN decoder and encoder, through the C-ABI of libian_b200.so (include/ian_b200.h):
 
   * decode(model, z) = X_hat of the reference (API.py:46, sample_at) as a differentiable torch op.  Its backward is the
     decoder's vector-Jacobian product (ian_decode_vjp_dev), so any loss torch can write on the decoded images -- soft or
     per-pixel weighted brushes, L1, losses on the whole frame, refining a latent against a photo -- drives the latent
     through torch.autograd, as any loss on X_hat was one T.grad away in the reference.
+  * encode(model, x, eps=None) = Z_hat of the reference (API.py:50) -- on IAN.py / IANv1.py after the MADE/IAF flow -- as a
+    differentiable torch op.  Its backward is the encoder's vector-Jacobian product (ian_encode_vjp_dev): latent-consistency
+    losses such as |E(G(z)) - z| or |E(x_hat) - E(x)|, saliency of a latent coordinate, optimising a photo against the
+    encoder, and a differentiable decode(encode(x)).  eps is a constant input: it gets no gradient, and an eps that
+    requires grad is refused.
 
-A backward costs one decoder forward plus one backward: the library recomputes the forward from the saved z instead of
-keeping the activations of the forward call.  The op is once-differentiable (no double backward).  Inputs and outputs are
+A backward costs one forward plus one backward of that half of the model: the library recomputes the forward from the
+saved input instead of keeping the activations of the forward call.  The op is once-differentiable (no double backward).  Inputs and outputs are
 torch CUDA float32 tensors on the model's device; torch only carries the device memory and the stream.
 """
 from __future__ import annotations
@@ -14,6 +19,7 @@ from __future__ import annotations
 from .train_ops import _lib_stream
 
 _Decode = None
+_Encode = None
 
 
 def _check_tensor(model, t, what):
@@ -63,6 +69,63 @@ def _function():
 
     _Decode = Decode
     return Decode
+
+
+def _encode_function():
+    global _Encode
+    if _Encode is not None:
+        return _Encode
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class Encode(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, model, x, eps):
+            _check_tensor(model, x, "x")
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 64, 64):
+                raise ValueError("x must be (n,3,64,64), got %r" % (tuple(x.shape),))
+            x = x.contiguous()
+            n = int(x.shape[0])
+            if eps is not None:
+                _check_tensor(model, eps, "eps")
+                if tuple(eps.shape) != (n, 100):
+                    raise ValueError("eps must be (%d,100), got %r" % (n, tuple(eps.shape)))
+                eps = eps.contiguous()
+            z = torch.empty(n, 100, dtype=torch.float32, device=x.device)
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.encode_dev(x.data_ptr(), n, z.data_ptr(), eps.data_ptr() if eps is not None else 0, st)
+            ctx.model = model
+            ctx.has_eps = eps is not None
+            ctx.save_for_backward(x, eps if eps is not None else x.new_empty(0))
+            return z
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            x, eps = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, g, "grad_output")
+            g = g.contiguous()
+            n = int(x.shape[0])
+            dx = torch.empty_like(x)
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.encode_vjp_dev(x.data_ptr(), g.data_ptr(), n, dx.data_ptr(),
+                                         eps.data_ptr() if ctx.has_eps else 0, st)
+            return None, dx, None
+
+    _Encode = Encode
+    return Encode
+
+
+def encode(model, x, eps=None):
+    """z = encoder(x) (what model.encode returns) for x (n,3,64,64) float32 CUDA on the model's device, eps (n,100) or None;
+    differentiable w.r.t. x (one encoder forward + one backward per backward call).  eps is not differentiated: pass a
+    tensor that does not require grad."""
+    if eps is not None and getattr(eps, "requires_grad", False):
+        raise ValueError("torch_ops.encode does not differentiate w.r.t. eps; pass eps.detach() (eps.requires_grad is set)")
+    return _encode_function().apply(model, x, eps)
 
 
 def decode(model, z):
