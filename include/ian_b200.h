@@ -211,6 +211,29 @@ int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const flo
 int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream);
 int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz);
 
+/* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
+ * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
+ * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
+ * BatchNorm, mean / inv_std constant.  z (n,100), dx_hat (n,3,64,64) float32 NCHW as for ian_decode_vjp_*; dz (n,100)
+ * nullable, bit for bit ian_decode_vjp_*'s.  grads is indexed like ian_model_param_spec (ian_model_param_count entries,
+ * NULL = not wanted; grads itself may be NULL); grads[i] receives parameter i in the reference layout and shape.  A
+ * non-NULL entry for a parameter without a gradient -> IAN_ERR_INVALID; IAN_MODEL_FULL / IAN_MODEL_V1 ->
+ * IAN_ERR_UNSUPPORTED; n == 0 does nothing.  Results are overwritten, not accumulated (a batch above the plan chunk is summed
+ * chunk by chunk in chunk order).  Both paths; deterministic (a repeated call is bit-identical).  The first call per batch
+ * size allocates the gradient buffers of that plan (about 2 MB per image plus split-K slabs of at most 64 MB); the first
+ * host call also allocates 75 MB of device gradients on the handle, the first call of either 136 KB of BatchNorm statistics. */
+/* 1 if ian_decode_param_vjp_* computes a gradient for parameter `index` of ian_model_param_spec (handle-free). */
+int ian_param_vjp_supported(int model_kind, int index);
+int ian_decode_param_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                             void* stream);
+int ian_decode_param_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads);
+/* Replace one IAN_simple decoder parameter of a FINALIZED handle: the 13 above or bnorm_dec_fc2 / bnorm_dc1..3 .mean /
+ * .inv_std, in the reference layout and shape.  Re-derives what ian_finalize derives from it and writes it into the same
+ * device buffers, so plans and captured graphs stay valid; afterwards every entry point computes bit for bit what a handle
+ * finalized from the updated parameters computes.  Synchronises the device first (ordered after all earlier work).
+ * Other names -> IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE; IAN_MODEL_FULL / IAN_MODEL_V1 -> IAN_ERR_UNSUPPORTED. */
+int ian_update_param_host(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim);
+
 /* ---- encoder vector-Jacobian product: reverse mode through the encoder from the image (reference Z_hat, API.py:50) ------
  *   dx = (d z / d x)^T . dz
  * x (n,3,64,64) float32 NCHW, eps (n,100) nullable, dz (n,100), dx (n,3,64,64).  z is exactly what ian_encode_* returns for
@@ -264,7 +287,8 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
 /* Average device time (ms, CUDA events on the launch stream) of the tap-GEMM kernel of layer
  * `layer_name` ("enc_conv2", "dec_conv1", ...; the encoder VJP's "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4",
  * "bwd_enc_conv3", "bwd_enc_conv2"; "enc_conv1", "dec_out", "brush_seed" -- the loss-seed kernel of the brush gradients
- * and of ian_decode_vjp_* -- and "enc_conv1_bwd" -- enc_conv1's adjoint in ian_encode_vjp_* -- for the edge kernels) over
+ * and of ian_decode_vjp_* -- "enc_conv1_bwd" -- enc_conv1's adjoint in ian_encode_vjp_* -- for the edge kernels; "wgrad_l_dec_fc2", "wgrad_dec_conv1",
+ * "wgrad_dec_conv2", "wgrad_dec_conv3" and "wgrad_dec_out" for the weight gradients of ian_decode_param_vjp_*) over
  * the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);

@@ -402,6 +402,49 @@ class IAN:
             self._check(self._lib.ian_decode_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz)))
         return dz
 
+    def param_vjp_names(self):
+        """names of the parameters decode_param_vjp returns gradients for, in ian_model_param_spec order: on IAN_simple
+        the 13 tensors of train_IAN_simple.py:353 (`decoder_params`); empty on IAN.py / IANv1.py."""
+        return [name for i, (name, _) in enumerate(model_param_specs(self.kind))
+                if self._lib.ian_param_vjp_supported(self.kind, i)]
+
+    def _param_slots(self, names):
+        specs = model_param_specs(self.kind)
+        index = {name: i for i, (name, _) in enumerate(specs)}
+        for name in names:
+            if name not in index:
+                raise KeyError("%r is not a parameter of this graph" % (name,))
+        return specs, index
+
+    def decode_param_vjp(self, z, dx_hat):
+        """Gradient of a pixel-space loss with respect to the decoder's trainable parameters (IAN_simple):
+        z float32 (n,100), dx_hat float32 (n,3,64,64) = dL/dx_hat -> (dz (n,100), {name: dL/dparam}) with every name of
+        param_vjp_names() in the reference layout.  dz equals decode_vjp(z, dx_hat) bit for bit.  The graph is X_hat_fn's
+        (API.py:46): inference BatchNorm, mean / inv_std held constant."""
+        z = _z(z)
+        dx = _img(dx_hat, 'dx_hat')
+        n = z.shape[0]
+        if dx.shape[0] != n:
+            raise ValueError("dx_hat must be (%d,3,64,64), got %r" % (n, dx.shape))
+        names = self.param_vjp_names()
+        specs, index = self._param_slots(names)
+        grads = {name: np.zeros(specs[index[name]][1], np.float32) for name in names}
+        dz = np.zeros_like(z)
+        ptrs = (C.c_void_p * len(specs))()
+        for name, g in grads.items():
+            ptrs[index[name]] = g.ctypes.data
+        self._check(self._lib.ian_decode_param_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz), ptrs))
+        return dz, grads
+
+    def update_params(self, params):
+        """Replace IAN_simple decoder parameters of this finalized model in place: {name: array in the reference shape}
+        for any of param_vjp_names() and bnorm_dec_fc2 / bnorm_dc1..3 .mean / .inv_std.  Afterwards every call computes
+        what a model built from the updated weights computes, bit for bit; captured graphs stay valid."""
+        for name, value in params.items():
+            arr = np.ascontiguousarray(np.asarray(value, dtype=np.float32))
+            shape = (C.c_int64 * max(arr.ndim, 1))(*arr.shape)
+            self._check(self._lib.ian_update_param_host(self._h, str(name).encode(), _fp(arr), shape, arr.ndim))
+
     def encode_vjp(self, images, dz, eps=None):
         """Vector-Jacobian product of the encoder, dx = (d z / d x)^T . dz, for any loss on the latent: images as for
         encode() (n,3,64,64), dz float32 (n,100) = dL/dz, eps as for encode() -> dx float32 (n,3,64,64).  z is what
@@ -532,6 +575,15 @@ class IAN:
 
     def decode_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, stream=0):
         self._check(self._lib.ian_decode_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr, stream or None))
+
+    def decode_param_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, grad_ptrs, stream=0):
+        """device-pointer form of decode_param_vjp: grad_ptrs {name: device pointer} (any subset of param_vjp_names()),
+        dz_ptr may be 0."""
+        specs, index = self._param_slots(grad_ptrs)
+        ptrs = (C.c_void_p * len(specs))()
+        for name, p in grad_ptrs.items():
+            ptrs[index[name]] = p
+        self._check(self._lib.ian_decode_param_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr or None, ptrs, stream or None))
 
     def encode_vjp_dev(self, x_ptr, dz_ptr, n, dx_ptr, eps_ptr=0, stream=0):
         self._check(self._lib.ian_encode_vjp_dev(self._h, x_ptr, int(n), eps_ptr or None, dz_ptr, dx_ptr, stream or None))

@@ -25,6 +25,20 @@ int launch_z_to_planes(const float* z, __nv_bfloat16* zp, long long zplane, int 
 int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* target, int target_is_frame, const float* dxhat,
                           const float* wt, const float* scale3, const __nv_bfloat16* h3, __nv_bfloat16* d3,
                           long long plane, int n, cudaStream_t st);
+// the dense seed of the parameter VJP: d3 exactly as launch_brush_seed_bwd(dxhat) writes it, plus the seed image
+// dx_hat * (1 - x_hat^2) (n,3,64,64) for dec_out's weight gradient and dL/dh3 before mask and scale (split planes, d3's
+// geometry) for bnorm_dc3
+int launch_brush_param_seed_bwd(const float* xhat, const float* dxhat, const float* wt, const float* scale3,
+                                const __nv_bfloat16* h3, __nv_bfloat16* d3, long long plane, float* seed_out,
+                                __nv_bfloat16* dh3, int n, cudaStream_t st);
+// parameter-VJP reductions (param_vjp.cu); part: per-chunk partial sums, sized by decout_wgrad_chunks / bn_param_chunks
+int decout_wgrad_chunks(int n);                         // part: chunks * 25 * 384 floats
+int bn_param_chunks(int C, long long R);                // part: chunks * 2 * C floats
+int launch_decout_wgrad(const float* seed, const __nv_bfloat16* h3, long long plane, int n, float* part, float* out,
+                        int accumulate, cudaStream_t st);
+int launch_bn_param_bwd(const __nv_bfloat16* dh, long long dh_plane, const __nv_bfloat16* h, const __nv_bfloat16* x,
+                        long long x_plane, const float* mean, const float* istd, int C, long long R, int fc2, float* part,
+                        float* dbeta, float* dgamma, int accumulate, cudaStream_t st);
 int launch_brush_update(const float* gpad, const int32_t* boxes, float weight, float* g_out, float* z,
                         __nv_bfloat16* zp, long long zplane, int n, cudaStream_t st);
 // NPE photo-mode blend + display upsample after a stroke (NPE.py:107-118, 218-231)

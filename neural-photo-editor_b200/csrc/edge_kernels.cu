@@ -233,7 +233,10 @@ __global__ void z_to_planes_kernel(const float* __restrict__ z, __nv_bfloat16* _
 // everything after the seed value (tap order, fmaf chain, scale * mask, hi|lo split) is the box form's code.  A box-loss
 // cotangent formed with the kernel's own expression therefore reproduces the box gradient bit for bit.
 // ------------------------------------------------------------------------------------------------
-template <bool kDense>
+// kParam (brush_param_seed_bwd_kernel, the parameter VJP ian_decode_param_vjp_*): the dense form, and it also stores the seed
+// image rows 2a, 2a+1 to seed_out (dec_out's weight gradient) and the pre-mask, pre-scale sums as dL/dh3 to dh3 (bnorm_dc3);
+// d3 is computed by the same instructions as in the dense form.
+template <bool kDense, bool kParam = false>
 __device__ __forceinline__ void brush_seed_bwd_body(float* sd /*[3*5*68]*/, float* ws /*[25*3*128], 16-byte aligned*/,
                                                     const float* __restrict__ xhat, const int32_t* __restrict__ boxes,
                                                     const float* __restrict__ target, int target_is_frame,
@@ -241,7 +244,9 @@ __device__ __forceinline__ void brush_seed_bwd_body(float* sd /*[3*5*68]*/, floa
                                                     const float* __restrict__ wt /*[25][128][4]*/,
                                                     const float* __restrict__ scale3,
                                                     const __nv_bfloat16* __restrict__ h3,
-                                                    __nv_bfloat16* __restrict__ d3, long long plane) {
+                                                    __nv_bfloat16* __restrict__ d3, long long plane,
+                                                    float* __restrict__ seed_out = nullptr,
+                                                    __nv_bfloat16* __restrict__ dh3 = nullptr) {
   pdl_trigger();
   pdl_wait();                                           // tapgemm.h: PDL
   const int k = blockIdx.x >> 5, a = blockIdx.x & 31;
@@ -280,6 +285,8 @@ __device__ __forceinline__ void brush_seed_bwd_body(float* sd /*[3*5*68]*/, floa
       sdv *= (1.f - xv * xv);
     }
     sd[i] = sdv;
+    if (kParam && (rem / 68 == 2 || rem / 68 == 3) && v >= 0 && v < 64)   // rows 2a, 2a+1: each image row written once
+      seed_out[((long long)(k * 3 + co) * 64 + u) * 64 + v] = sdv;
   }
   // weights through shared memory: every in-reach pixel walks up to the whole 38 KB table, and from L1/L2 each tap was a
   // dependent round trip (the first block-per-row form spent 60 % of its samples there: 32 us for the launch)
@@ -341,6 +348,13 @@ __device__ __forceinline__ void brush_seed_bwd_body(float* sd /*[3*5*68]*/, floa
         }
         hv = *reinterpret_cast<uint2*>(hi4);
         lv = *reinterpret_cast<uint2*>(lo4);
+        if (kParam) {
+          __align__(8) __nv_bfloat16 rh4[4], rl4[4];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) split_bf16(acc[q][c], rh4[c], rl4[c]);
+          *reinterpret_cast<uint2*>(dh3 + off) = *reinterpret_cast<uint2*>(rh4);
+          *reinterpret_cast<uint2*>(dh3 + plane + off) = *reinterpret_cast<uint2*>(rl4);
+        }
       }
       *reinterpret_cast<uint2*>(d3 + off) = hv;
       *reinterpret_cast<uint2*>(d3 + plane + off) = lv;
@@ -365,6 +379,17 @@ __global__ void __launch_bounds__(256) brush_vjp_seed_bwd_kernel(const float* __
   __shared__ float sd[3 * 5 * 68];
   __shared__ __align__(16) float ws[25 * 3 * 128];
   brush_seed_bwd_body<true>(sd, ws, xhat, nullptr, nullptr, 0, dxhat, wt, scale3, h3, d3, plane);
+}
+
+__global__ void __launch_bounds__(256) brush_param_seed_bwd_kernel(const float* __restrict__ xhat, const float* __restrict__ dxhat,
+                                                                   const float* __restrict__ wt, const float* __restrict__ scale3,
+                                                                   const __nv_bfloat16* __restrict__ h3,
+                                                                   __nv_bfloat16* __restrict__ d3, long long plane,
+                                                                   float* __restrict__ seed_out, __nv_bfloat16* __restrict__ dh3,
+                                                                   int n) {
+  __shared__ float sd[3 * 5 * 68];
+  __shared__ __align__(16) float ws[25 * 3 * 128];
+  brush_seed_bwd_body<true, true>(sd, ws, xhat, nullptr, nullptr, 0, dxhat, wt, scale3, h3, d3, plane, seed_out, dh3);
 }
 
 // g fp32 (n,128 padded) -> user g (n,100) and/or z update  z <- z - weight*g*(1+c2-c1)  (NPE.py:206-209)
@@ -700,6 +725,15 @@ int launch_brush_seed_bwd(const float* xhat, const int32_t* boxes, const float* 
       ? launch_pdl(brush_vjp_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, dxhat, wt, scale3, h3, d3, plane, n)
       : launch_pdl(brush_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, boxes, target, target_is_frame, wt, scale3, h3, d3, plane, n);
   if (e != cudaSuccess) return -1;
+  return CHECK_LAUNCH();
+}
+
+int launch_brush_param_seed_bwd(const float* xhat, const float* dxhat, const float* wt, const float* scale3,
+                                const __nv_bfloat16* h3, __nv_bfloat16* d3, long long plane, float* seed_out,
+                                __nv_bfloat16* dh3, int n, cudaStream_t st) {
+  if (launch_pdl(brush_param_seed_bwd_kernel, dim3((unsigned)n * 32u), dim3(256), 0, st, xhat, dxhat, wt, scale3, h3, d3, plane,
+                 seed_out, dh3, n) != cudaSuccess)
+    return -1;
   return CHECK_LAUNCH();
 }
 

@@ -140,9 +140,11 @@ enum LayerId {
   // encoder VJP (ian_encode_vjp_*): adjoints of the encoder head, enc_fc1 and enc_conv4..2, built on first use
   E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2,
   L_COUNT,
-  T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD, T_COUNT   // timing-only slots of the edge kernels (brush_seed: the
+  T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
                                                         // enc_conv1_bwd: enc_conv1's adjoint, the encoder VJP's last kernel)
+  T_WGRAD_FC2, T_WGRAD_CONV1, T_WGRAD_CONV2, T_WGRAD_CONV3, T_WGRAD_DEC_OUT,   // weight gradients of the parameter VJP
+  T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
                                     "dec_conv2", "dec_conv3", "bwd_dec_conv3", "bwd_dec_conv2", "bwd_dec_conv1", "bwd_l_dec_fc2",
@@ -152,7 +154,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "bwd_dec_conv3a2", "bwd_dec_conv3a", "bwd_full_dec_conv2", "bwd_dec_conv2a2", "bwd_dec_conv2a",
                                     "bwd_full_dec_conv1", "bwd_full_dec_fc2",
                                     "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4", "bwd_enc_conv3", "bwd_enc_conv2",
-                                    "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd"};
+                                    "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
+                                    "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -216,6 +219,10 @@ struct ian_handle {
                                    // with the E_BWD_* weight tiles); SIMT path
   __nv_bfloat16* conv1_bwd_tc_wt = nullptr;   // [2][80][128] bf16 planes, row = tap*3 + c, W1[o][c][24-t]; tensor-core path
   __nv_bfloat16* decout_tc_wt = nullptr;   // [2][80][128] bf16 planes, row = tap*3+co (tensor-core forward)
+  std::vector<float> dec_bn[4][4];          // IAN_simple: beta, gamma, mean, inv_std of bnorm_dec_fc2, bnorm_dc1..3, kept after
+                                           // finalize for ian_update_param_host
+  float* dec_bn_stats[4][2] = {};          // their mean, inv_std on the device (first parameter VJP)
+  float* pv_dev[13] = {};                  // the parameter VJP's gradients for the host API (first host call)
   // full IAN extras
   std::vector<int32_t> made_ordering;       // MADE input ordering (mask_generator.py:35-38); set by ian_set_made_ordering
   float *made_w = nullptr, *made_b = nullptr;   // [2][3][100][100] masked weights (in,out), [2][3][100] biases
@@ -297,7 +304,15 @@ struct Plan {
   cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
   // CUDA graphs of the kernel sequences behind the host entry points (small batches only; see run_graphed)
   struct GraphSlot { cudaGraphExec_t exec = nullptr; int64_t launches = 0; uint64_t key = 0; };
-  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_COUNT };
+  // decoder parameter VJP (allocated on the plan's first ian_decode_param_vjp_* call): the raw pre-BN sums x of l_dec_fc2 and
+  // dec_conv1..3, dL/dh of h0..h3 (before mask and scale), the seed image of dec_out, the weight-gradient descriptors and
+  // their split-K slabs, and the partial sums of the small reductions
+  bool pvjp = false;
+  Planes x0r, x1r, x2r, x3r, dh0, dh1, dh2, dh3;
+  float *pseed = nullptr, *pws = nullptr, *ppart = nullptr;
+  WgradGemm wg[4];
+  WgradMaps* wmaps[4] = {nullptr};
+  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -703,6 +718,7 @@ void free_plan(Plan* pl) {
     if (pl->ev_d2h[s]) cudaEventDestroy(pl->ev_d2h[s]);
   }
   for (int l = 0; l < L_COUNT; ++l) if (pl->maps[l]) tc_free_maps(pl->maps[l]);
+  for (auto* m : pl->wmaps) if (m) wgrad_free_maps(m);
   if (pl->decout_maps) decout_free_maps(pl->decout_maps);
   if (pl->conv1_bwd_maps) decout_free_maps(pl->conv1_bwd_maps);
   if (pl->conv1_out) conv1_free_out_map(pl->conv1_out);
@@ -847,8 +863,9 @@ int run_decode(ian_handle* h, Plan* pl, const float* z, float* xhat, cudaStream_
 // decoder forward (from zp) + backward; leaves g (n,128 padded) in pl->gpad.  The loss seed is the box loss of
 // boxes / target (brush gradients), or -- dxhat != NULL -- the caller's cotangent dL/dx_hat (n,3,64,64) over the whole
 // frame (ian_decode_vjp_*); only the seed kernel differs between the two.
+// param (IAN_simple, dxhat set): the parameter VJP's seed kernel, which also stores dec_out's seed image and dL/dh3.
 int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* target, int target_is_frame,
-                  const float* dxhat, cudaStream_t st) {
+                  const float* dxhat, cudaStream_t st, bool param = false) {
   int rc;
   if ((rc = run_decode_from_planes(h, pl, pl->xhat, st)) != IAN_OK) return rc;
   if (has_flow(h)) {
@@ -871,8 +888,12 @@ int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* ta
   }
   {
     ScopedTimer tm(h, T_BRUSH_SEED, st);
-    LAUNCH_TRY(h, launch_brush_seed_bwd(pl->xhat, boxes, target, target_is_frame, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale,
-                                        pl->h3.p, pl->d3.p, pl->d3.plane, pl->n, st));
+    if (param)
+      LAUNCH_TRY(h, launch_brush_param_seed_bwd(pl->xhat, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale, pl->h3.p, pl->d3.p,
+                                                pl->d3.plane, pl->pseed, pl->dh3.p, pl->n, st));
+    else
+      LAUNCH_TRY(h, launch_brush_seed_bwd(pl->xhat, boxes, target, target_is_frame, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale,
+                                          pl->h3.p, pl->d3.p, pl->d3.plane, pl->n, st));
   }
   for (int l : {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2})
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
@@ -901,8 +922,16 @@ int validate_boxes(ian_handle* h, const int32_t* bx, int n) {
 // ---- weight preparation --------------------------------------------------------------------------
 const HostParam& P(ian_handle* h, const char* name) { return h->params[name]; }
 
-int upload_gemm_weights(ian_handle* h, int l, const std::vector<float>& B, int ntiles, int Cout, int Cin,
-                        const std::vector<float>& scale, const std::vector<float>& shift) {
+// device buffer of `bytes`: allocated on first use (ian_finalize), overwritten in place afterwards (ian_update_param_host),
+// so plans, tensor maps and captured graphs that hold the pointer stay valid
+template <typename T>
+int put_dev(ian_handle* h, T*& dst, const void* src, size_t bytes) {
+  if (!dst) CUDA_TRY(h, cudaMalloc((void**)&dst, bytes));
+  CUDA_TRY(h, cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+  return IAN_OK;
+}
+
+int upload_tiles(ian_handle* h, int l, const std::vector<float>& B, int ntiles, int Cout, int Cin) {
   DevWeights& w = h->w[l];
   const long long elems = (long long)ntiles * Cout * Cin;
   std::vector<uint16_t> planes((size_t)elems * 2);
@@ -911,15 +940,19 @@ int upload_gemm_weights(ian_handle* h, int l, const std::vector<float>& B, int n
     planes[i] = hi;
     planes[elems + i] = f2bf(B[i] - bf2f(hi));
   }
-  CUDA_TRY(h, cudaMalloc((void**)&w.b, planes.size() * 2));
-  CUDA_TRY(h, cudaMemcpy(w.b, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice));
+  int rc = put_dev(h, w.b, planes.data(), planes.size() * 2);
+  if (rc != IAN_OK) return rc;
   w.plane = elems; w.ntiles = ntiles; w.Cout = Cout; w.Cin = Cin;
-  CUDA_TRY(h, cudaMalloc((void**)&w.scale, scale.size() * 4));
-  CUDA_TRY(h, cudaMemcpy(w.scale, scale.data(), scale.size() * 4, cudaMemcpyHostToDevice));
-  if (!shift.empty()) {
-    CUDA_TRY(h, cudaMalloc((void**)&w.shift, shift.size() * 4));
-    CUDA_TRY(h, cudaMemcpy(w.shift, shift.data(), shift.size() * 4, cudaMemcpyHostToDevice));
-  }
+  return IAN_OK;
+}
+
+int upload_gemm_weights(ian_handle* h, int l, const std::vector<float>& B, int ntiles, int Cout, int Cin,
+                        const std::vector<float>& scale, const std::vector<float>& shift) {
+  int rc = upload_tiles(h, l, B, ntiles, Cout, Cin);
+  if (rc != IAN_OK) return rc;
+  DevWeights& w = h->w[l];
+  if ((rc = put_dev(h, w.scale, scale.data(), scale.size() * 4)) != IAN_OK) return rc;
+  if (!shift.empty() && (rc = put_dev(h, w.shift, shift.data(), shift.size() * 4)) != IAN_OK) return rc;
   return IAN_OK;
 }
 
@@ -1044,83 +1077,101 @@ void transpose_tiles(const std::vector<float>& comp, int nt, int F, int C, std::
       for (int c = 0; c < C; ++c) out[((size_t)t * C + c) * F + f] = comp[((size_t)t * F + f) * C + c];
 }
 
-int prepare_simple_decoder(ian_handle* h) {
-  int rc;
-  std::vector<float> B, sc, sf;
-  // l_dec_fc2: reference column j = c*16 + hw -> our column hw*1024 + c; Cin 100 -> 128
-  std::vector<float> sc0, sf0;
-  {
-    const auto& W = P(h, "l_dec_fc2.W").data;
-    B.assign((size_t)16384 * 128, 0.f);
-    std::vector<float> s, f;
-    fold_bn(h, "bnorm_dec_fc2", 16384, s, f);
-    sc0.resize(16384);
-    sf0.resize(16384);
-    for (int c = 0; c < 1024; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 1024 + c;
-        sc0[col] = s[j];
-        sf0[col] = f[j];
-        for (int k = 0; k < 100; ++k) B[(size_t)col * 128 + k] = W[(size_t)k * 16384 + j];
+// ---- IAN_simple decoder: one derivation per parameter group, shared by ian_finalize and ian_update_param_host ----------
+// Each writes every device buffer derived from its group: allocated by the first call, overwritten in place by later ones.
+const char* kDecBn[4] = {"bnorm_dec_fc2", "bnorm_dc1", "bnorm_dc2", "bnorm_dc3"};
+const int kDecBnC[4] = {16384, 512, 256, 128};
+struct DecConv { int lf, lb; const char* w; int Cin, Cout; };
+const DecConv kDecConv[3] = {{L_DEC_CONV1, L_BWD_CONV1, "dec_conv1.W", 1024, 512},
+                             {L_DEC_CONV2, L_BWD_CONV2, "dec_conv2.W", 512, 256},
+                             {L_DEC_CONV3, L_BWD_CONV3, "dec_conv3.W", 256, 128}};
+
+// l_dec_fc2: reference column j = c*16 + hw -> our column hw*1024 + c; Cin 100 -> 128.  Forward tiles B[col][k]; backward
+// (dz[k] = sum_col d0[col] W[k][col]) tiles B[k][col], Cout 100 -> 128, unit scale.
+int simple_fc2_weights(ian_handle* h, const std::vector<float>& W) {
+  std::vector<float> B((size_t)16384 * 128, 0.f), Bt((size_t)128 * 16384, 0.f);
+  for (int c = 0; c < 1024; ++c)
+    for (int hw = 0; hw < 16; ++hw) {
+      const int j = c * 16 + hw, col = hw * 1024 + c;
+      for (int k = 0; k < 100; ++k) {
+        B[(size_t)col * 128 + k] = W[(size_t)k * 16384 + j];
+        Bt[(size_t)k * 16384 + col] = W[(size_t)k * 16384 + j];
       }
-    if ((rc = upload_gemm_weights(h, L_DEC_FC2, B, 1, 16384, 128, sc0, sf0)) != IAN_OK) return rc;
-    // backward: dz[k] = sum_col d0[col] * W[k][col]  -> B[k][col], Cout 100 -> 128
-    B.assign((size_t)128 * 16384, 0.f);
-    for (int c = 0; c < 1024; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 1024 + c;
-        for (int k = 0; k < 100; ++k) B[(size_t)k * 16384 + col] = W[(size_t)k * 16384 + j];
-      }
-    std::vector<float> ones(128, 1.f);
-    if ((rc = upload_gemm_weights(h, L_BWD_FC2, B, 1, 128, 16384, ones, {})) != IAN_OK) return rc;
-  }
-  // dec_conv1..3: W (Cin,Cout,5,5).  forward B[k][co][ci] = W[ci][co][k]; backward B[k][ci][co] = W[ci][co][k]
-  struct DS { int lf, lb; const char* w; const char* bn; int Cin, Cout; } decs[] = {
-      {L_DEC_CONV1, L_BWD_CONV1, "dec_conv1.W", "bnorm_dc1", 1024, 512},
-      {L_DEC_CONV2, L_BWD_CONV2, "dec_conv2.W", "bnorm_dc2", 512, 256},
-      {L_DEC_CONV3, L_BWD_CONV3, "dec_conv3.W", "bnorm_dc3", 256, 128}};
-  std::vector<float> prev_scale = sc0;   // scale applied in the backward epilogue = BN scale of the layer BELOW
-  std::vector<std::vector<float>> fwd_scales;
-  for (auto& d : decs) {
-    const auto& W = P(h, d.w).data;
-    B.assign((size_t)25 * d.Cout * d.Cin, 0.f);
-    for (int ci = 0; ci < d.Cin; ++ci)
-      for (int co = 0; co < d.Cout; ++co)
-        for (int t = 0; t < 25; ++t) B[((size_t)t * d.Cout + co) * d.Cin + ci] = W[((size_t)ci * d.Cout + co) * 25 + t];
-    fold_bn(h, d.bn, d.Cout, sc, sf);
-    if ((rc = upload_gemm_weights(h, d.lf, B, 25, d.Cout, d.Cin, sc, sf)) != IAN_OK) return rc;
-    for (int ci = 0; ci < d.Cin; ++ci)
-      for (int co = 0; co < d.Cout; ++co)
-        for (int t = 0; t < 25; ++t) B[((size_t)t * d.Cin + ci) * d.Cout + co] = W[((size_t)ci * d.Cout + co) * 25 + t];
-    // backward GEMM of this layer produces the gradient w.r.t. its INPUT activation, whose BN scale is prev_scale
-    if ((rc = upload_gemm_weights(h, d.lb, B, 25, d.Cin, d.Cout, prev_scale, {})) != IAN_OK) return rc;
-    prev_scale = sc;
-  }
-  // dec_out: wt[ki*5+kj][ci][co(4)] = W[ci][co][ki][kj]
-  {
-    const auto& W = P(h, "dec_out.W").data;
-    // tensor-core form (decout_tc.cu): rows j = tap*3+co (75, padded to 80), K-major over ci; bf16 hi|lo planes
-    {
-      std::vector<uint16_t> planes(2 * 80 * 128, 0);
-      for (int ci = 0; ci < 128; ++ci)
-        for (int co = 0; co < 3; ++co)
-          for (int t = 0; t < 25; ++t) {
-            const float w = W[(ci * 3 + co) * 25 + t];
-            const uint16_t hi = f2bf(w);
-            planes[(t * 3 + co) * 128 + ci] = hi;
-            planes[80 * 128 + (t * 3 + co) * 128 + ci] = f2bf(w - bf2f(hi));
-          }
-      CUDA_TRY(h, cudaMalloc((void**)&h->decout_tc_wt, planes.size() * 2));
-      CUDA_TRY(h, cudaMemcpy(h->decout_tc_wt, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice));
     }
-    std::vector<float> wt(25 * 128 * 4, 0.f);
-    for (int ci = 0; ci < 128; ++ci)
-      for (int co = 0; co < 3; ++co)
-        for (int t = 0; t < 25; ++t) wt[(t * 128 + ci) * 4 + co] = W[(ci * 3 + co) * 25 + t];
-    CUDA_TRY(h, cudaMalloc((void**)&h->decout_wt, wt.size() * 4));
-    CUDA_TRY(h, cudaMemcpy(h->decout_wt, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice));
+  int rc = upload_tiles(h, L_DEC_FC2, B, 1, 16384, 128);
+  if (rc != IAN_OK) return rc;
+  if ((rc = upload_tiles(h, L_BWD_FC2, Bt, 1, 128, 16384)) != IAN_OK) return rc;
+  const std::vector<float> ones(128, 1.f);
+  return put_dev(h, h->w[L_BWD_FC2].scale, ones.data(), ones.size() * 4);
+}
+
+// dec_conv k (W (Cin,Cout,5,5)): forward B[t][co][ci] = W[ci][co][t]; backward-data B[t][ci][co] = W[ci][co][t]
+int simple_conv_weights(ian_handle* h, int k, const std::vector<float>& W) {
+  const DecConv& d = kDecConv[k];
+  std::vector<float> B((size_t)25 * d.Cout * d.Cin), Bt((size_t)25 * d.Cout * d.Cin);
+  for (int ci = 0; ci < d.Cin; ++ci)
+    for (int co = 0; co < d.Cout; ++co)
+      for (int t = 0; t < 25; ++t) {
+        const float v = W[((size_t)ci * d.Cout + co) * 25 + t];
+        B[((size_t)t * d.Cout + co) * d.Cin + ci] = v;
+        Bt[((size_t)t * d.Cin + ci) * d.Cout + co] = v;
+      }
+  int rc = upload_tiles(h, d.lf, B, 25, d.Cout, d.Cin);
+  if (rc != IAN_OK) return rc;
+  return upload_tiles(h, d.lb, Bt, 25, d.Cin, d.Cout);
+}
+
+// dec_out W (128,3,5,5): tensor-core form (decout_tc.cu, rows tap*3+co padded to 80, K-major over ci, bf16 hi|lo planes)
+// and the FFMA form wt[tap][ci][co(4)] (SIMT forward, every seed kernel)
+int simple_dec_out_weights(ian_handle* h, const std::vector<float>& W) {
+  std::vector<uint16_t> planes(2 * 80 * 128, 0);
+  std::vector<float> wt(25 * 128 * 4, 0.f);
+  for (int ci = 0; ci < 128; ++ci)
+    for (int co = 0; co < 3; ++co)
+      for (int t = 0; t < 25; ++t) {
+        const float w = W[(ci * 3 + co) * 25 + t];
+        const uint16_t hi = f2bf(w);
+        planes[(t * 3 + co) * 128 + ci] = hi;
+        planes[80 * 128 + (t * 3 + co) * 128 + ci] = f2bf(w - bf2f(hi));
+        wt[(t * 128 + ci) * 4 + co] = w;
+      }
+  int rc = put_dev(h, h->decout_tc_wt, planes.data(), planes.size() * 2);
+  if (rc != IAN_OK) return rc;
+  return put_dev(h, h->decout_wt, wt.data(), wt.size() * 4);
+}
+
+// decoder BatchNorm k (0: bnorm_dec_fc2, 1..3: bnorm_dc1..3) from the host copy h->dec_bn[k]: the folded scale / shift of the
+// layer's forward epilogue, the same scale in the backward-data epilogue of the layer above (bnorm_dc3's is read by the
+// seed kernels from the forward buffer), and mean / inv_std on the device once the parameter VJP has used them
+int simple_bn(ian_handle* h, int k) {
+  const int C = kDecBnC[k];
+  const auto& f = h->dec_bn[k];      // beta, gamma, mean, inv_std
+  std::vector<float> sc(C), sf(C);
+  for (int j = 0; j < C; ++j) {
+    const int i = k == 0 ? (j % 1024) * 16 + j / 1024 : j;   // fc2: our column j = hw*1024 + c <- reference c*16 + hw
+    sc[j] = f[1][i] * f[3][i];
+    sf[j] = f[0][i] - f[2][i] * sc[j];
+  }
+  const int lf = k == 0 ? L_DEC_FC2 : kDecConv[k - 1].lf;
+  int rc = put_dev(h, h->w[lf].scale, sc.data(), C * 4);
+  if (rc != IAN_OK) return rc;
+  if ((rc = put_dev(h, h->w[lf].shift, sf.data(), C * 4)) != IAN_OK) return rc;
+  if (k < 3 && (rc = put_dev(h, h->w[kDecConv[k].lb].scale, sc.data(), C * 4)) != IAN_OK) return rc;
+  if (h->dec_bn_stats[k][0]) {
+    if ((rc = put_dev(h, h->dec_bn_stats[k][0], f[2].data(), C * 4)) != IAN_OK) return rc;
+    if ((rc = put_dev(h, h->dec_bn_stats[k][1], f[3].data(), C * 4)) != IAN_OK) return rc;
   }
   return IAN_OK;
+}
+
+int prepare_simple_decoder(ian_handle* h) {
+  for (int k = 0; k < 4; ++k)
+    for (int f = 0; f < 4; ++f) h->dec_bn[k][f] = P(h, (std::string(kDecBn[k]) + "." + kBnFields[f]).c_str()).data;
+  int rc = simple_fc2_weights(h, P(h, "l_dec_fc2.W").data);
+  for (int k = 0; k < 3 && rc == IAN_OK; ++k) rc = simple_conv_weights(h, k, P(h, kDecConv[k].w).data);
+  for (int k = 0; k < 4 && rc == IAN_OK; ++k) rc = simple_bn(h, k);
+  if (rc == IAN_OK) rc = simple_dec_out_weights(h, P(h, "dec_out.W").data);
+  return rc;
 }
 
 // composite MDC weights (reference layers.py:207-258): per distinct offset one [F][C] matrix
@@ -1638,6 +1689,136 @@ int run_encode_vjp(ian_handle* h, Plan* pl, const float* x, const float* eps, co
   return IAN_OK;
 }
 
+// ---- decoder parameter VJP (IAN_simple) ----------------------------------------------------------------
+// dL/dtheta for the 13 trainable decoder tensors of train_IAN_simple.py:353 (`decoder_params`) on the deterministic graph
+// of X_hat_fn (API.py:46): inference BatchNorm with mean / inv_std constant.  The chain is the decoder VJP's (run_grad_core
+// with the dense seed), so dz is bit for bit ian_decode_vjp_*'s; on top of it:
+//   * the forward layers keep their raw pre-BN sums x (out_raw) and the backward-data layers keep their accumulators before
+//     mask and scale, which are dL/dh of the layer below (out_raw in ACT_MASK mode); the seed kernel stores dL/dh3 and
+//     dec_out's seed image;
+//   * weight gradients: the transposes of the four forward tap-GEMMs (wgrad_tc.cu) with G = d0..d3 (dL/d raw output) and
+//     A = zp, h0, h1, h2, and dec_out's FFMA reduction (param_vjp.cu);
+//   * BatchNorm: d beta = sum dL/dy, d gamma = sum dL/dy * (x - mean) * inv_std, dL/dy = dL/dh * (h > 0) -- no division by
+//     gamma or by the folded scale, so a channel with gamma = 0 still gets its gradients.
+enum PvSlot { PV_FC2, PV_CONV1, PV_CONV2, PV_CONV3, PV_OUT, PV_BN0_B, PV_BN0_G, PV_BN1_B, PV_BN1_G, PV_BN2_B, PV_BN2_G,
+              PV_BN3_B, PV_BN3_G, PV_COUNT };
+const char* kPvNames[PV_COUNT] = {"l_dec_fc2.W", "dec_conv1.W", "dec_conv2.W", "dec_conv3.W", "dec_out.W",
+                                  "bnorm_dec_fc2.beta", "bnorm_dec_fc2.gamma", "bnorm_dc1.beta", "bnorm_dc1.gamma",
+                                  "bnorm_dc2.beta", "bnorm_dc2.gamma", "bnorm_dc3.beta", "bnorm_dc3.gamma"};
+const long long kPvSize[PV_COUNT] = {100LL * 16384, 1024LL * 512 * 25, 512LL * 256 * 25, 256LL * 128 * 25, 128LL * 3 * 25,
+                                     16384, 16384, 512, 512, 256, 256, 128, 128};
+// the split-K slabs of one weight gradient stay within 16 M floats (64 MB per plan: dec_conv1's unsplit slab is 13.1 M)
+constexpr long long kWgradMaxWsFloats = 16LL << 20;
+
+int ensure_param_vjp_plan(ian_handle* h, Plan* pl) {
+  for (int k = 0; k < 4; ++k)                             // the handle's BN statistics (first call on the handle)
+    if (!h->dec_bn_stats[k][0]) {
+      int rc = put_dev(h, h->dec_bn_stats[k][0], h->dec_bn[k][2].data(), h->dec_bn[k][2].size() * 4);
+      if (rc != IAN_OK) return rc;
+      if ((rc = put_dev(h, h->dec_bn_stats[k][1], h->dec_bn[k][3].data(), h->dec_bn[k][3].size() * 4)) != IAN_OK) return rc;
+    }
+  if (pl->pvjp) return IAN_OK;
+  const long long N = pl->n;
+  int rc;
+#define AP(t, e) if ((rc = alloc_planes(h, pl, pl->t, (e))) != IAN_OK) return rc;
+  AP(x0r, N * 16384) AP(x1r, N * 8 * 8 * 512) AP(x2r, N * 16 * 16 * 256) AP(x3r, N * 32 * 32 * 128)
+  AP(dh0, N * 16384) AP(dh1, N * 8 * 8 * 512) AP(dh2, N * 16 * 16 * 256) AP(dh3, N * 32 * 32 * 128)
+#undef AP
+  if ((rc = alloc_buf(h, pl, pl->pseed, N * 3 * 4096)) != IAN_OK) return rc;
+  const int fwd[4] = {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3};
+  const Planes* grd[4] = {&pl->d0, &pl->d1, &pl->d2, &pl->d3};
+  long long need = 0;
+  for (int k = 0; k < 4; ++k) {
+    WgradGemm& w = pl->wg[k];
+    memset(&w, 0, sizeof(w));
+    w.f = pl->g[fwd[k]];
+    w.gr = grd[k]->p;
+    w.gr_plane = grd[k]->plane;
+    w.ws_slab = (long long)h->w[fwd[k]].ntiles * w.f.Cout * w.f.Cin;
+    w.ksplit = h->splitk ? wgrad_choose_ksplit(w, kWgradMaxWsFloats) : 1;
+    need = std::max(need, w.ksplit * w.ws_slab);
+    char err[256] = {0};
+    pl->wmaps[k] = wgrad_build_maps(w, err, sizeof(err));
+    if (!pl->wmaps[k]) return fail(h, IAN_ERR_CUDA, "wgrad %s: %s", kLayerNames[fwd[k]], err);
+  }
+  if ((rc = alloc_buf(h, pl, pl->pws, need)) != IAN_OK) return rc;
+  for (auto& w : pl->wg) w.ws = pl->pws;
+  long long part = (long long)decout_wgrad_chunks(pl->n) * 25 * 384;
+  const int bnC[4] = {16384, 512, 256, 128};
+  const long long bnR[4] = {N, N * 64, N * 256, N * 1024};
+  for (int k = 0; k < 4; ++k) part = std::max(part, (long long)bn_param_chunks(bnC[k], bnR[k]) * 2 * bnC[k]);
+  if ((rc = alloc_buf(h, pl, pl->ppart, part)) != IAN_OK) return rc;
+  pl->pvjp = true;
+  return IAN_OK;
+}
+
+// zp holds the latent planes; out[PV_COUNT] device pointers (nullable); accumulate: add into out (a later batch chunk)
+int run_param_vjp(ian_handle* h, Plan* pl, const float* dxhat, float* const* out, int accumulate, cudaStream_t st) {
+  TapGemm* g = pl->g;
+  const int raw_l[7] = {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3, L_BWD_CONV1, L_BWD_CONV2, L_BWD_CONV3};
+  const Planes* raw_p[7] = {&pl->x0r, &pl->x1r, &pl->x2r, &pl->x3r, &pl->dh0, &pl->dh1, &pl->dh2};
+  for (int k = 0; k < 7; ++k) { g[raw_l[k]].out_raw = raw_p[k]->p; g[raw_l[k]].out_raw_plane = raw_p[k]->plane; }
+  int rc = run_grad_core(h, pl, nullptr, nullptr, 0, dxhat, st, true);
+  for (int k = 0; k < 7; ++k) { g[raw_l[k]].out_raw = nullptr; g[raw_l[k]].out_raw_plane = 0; }
+  if (rc != IAN_OK) return rc;
+  for (int k = 0; k < 4; ++k) {
+    if (!out[PV_FC2 + k]) continue;
+    {
+      ScopedTimer tm(h, T_WGRAD_FC2 + k, st);
+      if (h->path == IAN_PATH_TC) LAUNCH_TRY(h, launch_wgrad_tc(pl->wg[k], pl->wmaps[k], st));
+      else LAUNCH_TRY(h, launch_wgrad_simt(pl->wg[k], st));
+    }
+    LAUNCH_TRY(h, launch_wgrad_finalize(pl->wg[k], k == 0 ? WG_FC2 : WG_DECONV, out[PV_FC2 + k], accumulate, st));
+  }
+  if (out[PV_OUT]) {
+    ScopedTimer tm(h, T_WGRAD_DEC_OUT, st);
+    LAUNCH_TRY(h, launch_decout_wgrad(pl->pseed, pl->h3.p, pl->h3.plane, pl->n, pl->ppart, out[PV_OUT], accumulate, st));
+  }
+  const long long N = pl->n;
+  struct Bn { const Planes *dh, *hh, *x; int C; long long R; } bns[4] = {
+      {&pl->dh0, &pl->h0, &pl->x0r, 16384, N}, {&pl->dh1, &pl->h1, &pl->x1r, 512, N * 64},
+      {&pl->dh2, &pl->h2, &pl->x2r, 256, N * 256}, {&pl->dh3, &pl->h3, &pl->x3r, 128, N * 1024}};
+  for (int k = 0; k < 4; ++k) {
+    float* db = out[PV_BN0_B + 2 * k];
+    float* dg = out[PV_BN0_G + 2 * k];
+    if (!db && !dg) continue;
+    const Bn& b = bns[k];
+    LAUNCH_TRY(h, launch_bn_param_bwd(b.dh->p, b.dh->plane, b.hh->p, b.x->p, b.x->plane, h->dec_bn_stats[k][0],
+                                      h->dec_bn_stats[k][1], b.C, b.R, k == 0 ? 1 : 0, pl->ppart, db, dg, accumulate, st));
+  }
+  return IAN_OK;
+}
+
+// slot of parameter `index` of ian_model_param_spec, or -1 when the parameter VJP does not compute it
+int pv_slot(int model_kind, int index) {
+  if (model_kind != IAN_MODEL_SIMPLE) return -1;
+  static const std::vector<Spec> specs = spec_list(IAN_MODEL_SIMPLE);
+  if (index < 0 || index >= (int)specs.size()) return -1;
+  for (int k = 0; k < PV_COUNT; ++k)
+    if (specs[index].name == kPvNames[k]) return k;
+  return -1;
+}
+
+// common checks; fills out[PV_COUNT] from grads (spec-indexed)
+int check_param_vjp(ian_handle* h, const float* z, const float* dx_hat, int n, float* const* grads, float** out) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (h->model_kind != IAN_MODEL_SIMPLE)
+    return fail(h, IAN_ERR_UNSUPPORTED, "parameter gradients are implemented for IAN_simple only");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  if (n > 0 && (!z || !dx_hat)) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  for (int k = 0; k < PV_COUNT; ++k) out[k] = nullptr;
+  if (!grads) return IAN_OK;
+  static const std::vector<Spec> specs = spec_list(IAN_MODEL_SIMPLE);
+  for (int i = 0; i < (int)specs.size(); ++i) {
+    if (!grads[i]) continue;
+    const int k = pv_slot(h->model_kind, i);
+    if (k < 0) return fail(h, IAN_ERR_INVALID, "no gradient is computed for parameter %d ('%s')", i, specs[i].name.c_str());
+    out[k] = grads[i];
+  }
+  return IAN_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1783,6 +1964,8 @@ int ian_destroy(ian_handle* h) {
   for (auto& w : h->w) { cudaFree(w.b); cudaFree(w.scale); cudaFree(w.shift); }
   cudaFree(h->conv1_wt); cudaFree(h->conv1_b); cudaFree(h->decout_wt); cudaFree(h->decout_tc_wt); cudaFree(h->conv1_bwd_wt); cudaFree(h->conv1_bwd_tc_wt);
   cudaFree(h->sk_ws); cudaFree(h->sk_flags);
+  for (auto& s : h->dec_bn_stats) { cudaFree(s[0]); cudaFree(s[1]); }
+  for (float* p : h->pv_dev) cudaFree(p);
   cudaFree(h->conv1_tc_wt); if (h->conv1_maps) conv1_free_maps(h->conv1_maps);
   cudaFree(h->made_w); cudaFree(h->made_b); cudaFree(h->head_taps); cudaFree(h->head_wgb); cudaFree(h->head_wbb);
   cudaFree(h->head_tc_wt);
@@ -2030,6 +2213,93 @@ int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int 
   if (rc != IAN_OK) return rc;
   CUDA_TRY(h, cudaStreamSynchronize(st));
   return IAN_OK;
+}
+
+// ---- decoder parameter vector-Jacobian product (IAN_simple) -----------------------------------------------
+int ian_param_vjp_supported(int model_kind, int index) { return pv_slot(model_kind, index) >= 0 ? 1 : 0; }
+
+int ian_decode_param_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                             void* stream) {
+  float* out[PV_COUNT];
+  int rc = check_param_vjp(h, z, dx_hat, n, grads, out);
+  if (rc != IAN_OK || n == 0) return rc;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    int r = ensure_param_vjp_plan(h, pl);
+    if (r != IAN_OK) return r;
+    LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
+    if ((r = run_param_vjp(h, pl, dx_hat + (size_t)off * 12288, out, off > 0, st)) != IAN_OK) return r;
+    if (dz) CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToDevice, st));
+    return (int)IAN_OK;
+  });
+}
+
+// Every gradient is computed into the handle's device buffers (allocated on the first call), so a captured graph does not
+// depend on which ones the caller asked for; the requested ones are copied out.
+int ian_decode_param_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads) {
+  float* req[PV_COUNT];
+  int rc = check_param_vjp(h, z, dx_hat, n, grads, req);
+  if (rc != IAN_OK || n == 0) return rc;
+  DeviceGuard dg(h->device);
+  cudaStream_t st = h->stream;
+  for (int k = 0; k < PV_COUNT; ++k)
+    if (!h->pv_dev[k]) CUDA_TRY(h, cudaMalloc((void**)&h->pv_dev[k], (size_t)kPvSize[k] * 4));
+  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    int r = ensure_param_vjp_plan(h, pl);
+    if (r != IAN_OK) return r;
+    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(h, cudaMemcpyAsync(pl->target, dx_hat + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
+    r = run_graphed(h, pl, Plan::G_PARAM_VJP, off > 0 ? 1 : 0, st, [&] {
+      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
+      return run_param_vjp(h, pl, pl->target, h->pv_dev, off > 0, st);
+    });
+    if (r != IAN_OK) return r;
+    if (dz) CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToHost, st));
+    return (int)IAN_OK;
+  });
+  if (rc != IAN_OK) return rc;
+  for (int k = 0; k < PV_COUNT; ++k)
+    if (req[k]) CUDA_TRY(h, cudaMemcpyAsync(req[k], h->pv_dev[k], (size_t)kPvSize[k] * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+// Replace one IAN_simple decoder parameter of a finalized handle: re-derive what ian_finalize derives from its group and
+// write it into the same device buffers (tiles of both directions, dec_out's two weight forms, folded BatchNorm vectors).
+// The device is synchronised first, so the update is ordered after all work enqueued before the call.
+int ian_update_param_host(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim) {
+  if (!h || !name || !data || !shape) return fail(h, IAN_ERR_INVALID, "NULL argument");
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "the handle is not finalized: use ian_set_param");
+  if (h->model_kind != IAN_MODEL_SIMPLE) return fail(h, IAN_ERR_UNSUPPORTED, "in-place updates are implemented for IAN_simple only");
+  const std::string n(name);
+  int group = -1, bn = -1, field = -1;                 // group: 0 fc2, 1..3 dec_conv, 4 dec_out, 5 BatchNorm
+  if (n == "l_dec_fc2.W") group = 0;
+  for (int k = 0; k < 3; ++k) if (n == kDecConv[k].w) group = 1 + k;
+  if (n == "dec_out.W") group = 4;
+  for (int k = 0; k < 4; ++k)
+    for (int f = 0; f < 4; ++f)
+      if (n == std::string(kDecBn[k]) + "." + kBnFields[f]) { group = 5; bn = k; field = f; }
+  if (group < 0) return fail(h, IAN_ERR_INVALID, "'%s' is not an IAN_simple decoder parameter that can be updated", name);
+  const std::vector<Spec> specs = spec_list(h->model_kind);
+  const Spec* spec = nullptr;
+  for (const auto& sp : specs) if (sp.name == n) spec = &sp;
+  if (ndim != (int)spec->shape.size()) return fail(h, IAN_ERR_INVALID, "parameter %s: expected %d dims, got %d", name, (int)spec->shape.size(), ndim);
+  int64_t elems = 1;
+  for (int i = 0; i < ndim; ++i) {
+    if (shape[i] != spec->shape[i])
+      return fail(h, IAN_ERR_INVALID, "parameter %s: shape mismatch at dim %d (expected %lld, got %lld)", name, i,
+                  (long long)spec->shape[i], (long long)shape[i]);
+    elems *= shape[i];
+  }
+  DeviceGuard dg(h->device);
+  CUDA_TRY(h, cudaDeviceSynchronize());
+  const std::vector<float> v(data, data + elems);
+  if (group == 0) return simple_fc2_weights(h, v);
+  if (group <= 3) return simple_conv_weights(h, group - 1, v);
+  if (group == 4) return simple_dec_out_weights(h, v);
+  h->dec_bn[bn][field] = v;
+  return simple_bn(h, bn);
 }
 
 // ---- encoder vector-Jacobian product --------------------------------------------------------------

@@ -188,4 +188,30 @@ int tc_num_sms();
 size_t tc_sk_workspace_floats();   // per handle: one 128 x 256 fp32 slot per SM
 size_t tc_sk_flag_ints();
 
+// ---- weight gradient of a forward tap-GEMM (wgrad_tc.cu) -------------------------------------------
+//   dB[wtile_t][co][ci] = sum_{n,p,q} G[n, p*osh+oh0, q*osw+ow0, co] * A[n, (p+dh_t)*sh+vh_t, (q+dw_t)*sw+vw_t, ci]
+// One GEMM per tap: M = Cout, N = Cin, K = the forward M grid (n*Hg*Wg pixels of the tap's phase).  G is dL/d(raw output)
+// of the forward layer `f`; its A operand (taps, views, zero padding) is the forward's.  Every weight tile must belong to
+// exactly one (phase, tap), so no sum across taps is needed (taps_deconv_s2, taps_dense; wgrad_build_maps checks it).
+// K split s writes raw float32 sums to slab s of ws ([ksplit][ntiles][Cout][Cin]); launch_wgrad_finalize adds the slabs in
+// split order and scatters into the reference layout -- no atomics, bit-reproducible.
+struct WgradGemm {
+  TapGemm f;
+  const __nv_bfloat16* gr;      // split planes with the forward output's geometry (n, Hout, Wout, Cout)
+  long long gr_plane;
+  int ksplit;
+  float* ws;
+  long long ws_slab;            // ntiles * Cout * Cin
+};
+enum WgradLayout { WG_DECONV = 0,   // dW[ci][co][t] = dB[t][co][ci]  (DeconvLayer W (Cin, Cout, 5, 5))
+                   WG_FC2 = 1 };    // l_dec_fc2: dW[k][c*16 + hw] = dB[0][hw*1024 + c][k], k < 100
+struct WgradMaps;   // opaque: CUtensorMaps of G (one per phase) and A (one per view)
+WgradMaps* wgrad_build_maps(const WgradGemm& w, char* err, int errlen);
+void wgrad_free_maps(WgradMaps*);
+int wgrad_kboxes(const WgradGemm& w);   // 64-pixel K steps per tap on the tensor-core path
+int wgrad_choose_ksplit(const WgradGemm& w, long long max_ws_floats);
+int launch_wgrad_tc(const WgradGemm& w, const WgradMaps* maps, cudaStream_t st);
+int launch_wgrad_simt(const WgradGemm& w, cudaStream_t st);
+int launch_wgrad_finalize(const WgradGemm& w, int layout, float* out, int accumulate, cudaStream_t st);
+
 }  // namespace ian

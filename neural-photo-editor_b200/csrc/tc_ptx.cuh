@@ -149,6 +149,20 @@ template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint
       : "l"(a), "l"(b), "r"(accum));
 }
 
+// The same product with both operands MN-major (transpose immediates = 1, legal for bf16): A is stored as K rows of M
+// contiguous elements, B as K rows of N contiguous elements -- the layout of a channel-contiguous activation box when the
+// contraction runs over pixels (wgrad_tc.cu).  Descriptors from make_sw128_mn_desc.
+template <int N> __device__ __forceinline__ void wgmma_bf16_mn(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accum);
+template <> __device__ __forceinline__ void wgmma_bf16_mn<128>(float (&d)[64], uint64_t a, uint64_t b, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(accum));
+}
+
 // accumulator row / column of fragment element j for thread `tid` (0..127) of the warpgroup
 __device__ __forceinline__ int frag_row(int tid, int j) { return 16 * (tid >> 5) + ((tid & 31) >> 2) + 8 * ((j >> 1) & 1); }
 __device__ __forceinline__ int frag_col(int tid, int j) { return 8 * (j >> 2) + 2 * (tid & 3) + (j & 1); }
@@ -160,6 +174,19 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);        // start address, 16-byte units
   d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset between 8-row groups
+  d |= (uint64_t)1 << 62;                         // SWIZZLE_128B
+  return d;
+}
+
+// MN-major, 128B-swizzled operand descriptor.  The canonical layout is ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in
+// elements: a swizzle atom is 8 K-rows of 64 contiguous MN elements (1024 B), SBO steps between 8-row K groups (1024 B when
+// the rows are packed) and LBO between 64-wide MN blocks.  A K = 16 slice is two K groups, so the next slice starts
+// 2 * SBO further on; start addresses stay 1024-aligned and the base-offset field stays 0.
+__device__ __forceinline__ uint64_t make_sw128_mn_desc(uint32_t saddr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);        // start address, 16-byte units
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // leading byte offset: next 64-wide MN block
+  d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset: next 8-row K group
   d |= (uint64_t)1 << 62;                         // SWIZZLE_128B
   return d;
 }

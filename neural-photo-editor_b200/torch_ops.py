@@ -10,6 +10,12 @@
     encoder, and a differentiable decode(encode(x)).  eps is a constant input: it gets no gradient, and an eps that
     requires grad is refused.
 
+  * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
+    (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
+    (ian_decode_param_vjp_dev) that also returns dz.  Before each forward, every tensor whose in-place version moved since
+    its last upload is written back into the handle (ian_update_param_host), so a plain torch.optim loop over
+    params.values() fine-tunes the generator with no extra call.
+
 A backward costs one forward plus one backward of that half of the model: the library recomputes the forward from the
 saved input instead of keeping the activations of the forward call.  The op is once-differentiable (no double backward).  Inputs and outputs are
 torch CUDA float32 tensors on the model's device; torch only carries the device memory and the stream.
@@ -20,6 +26,7 @@ from .train_ops import _lib_stream
 
 _Decode = None
 _Encode = None
+_DecodeParams = None
 
 
 def _check_tensor(model, t, what):
@@ -128,7 +135,86 @@ def encode(model, x, eps=None):
     return _encode_function().apply(model, x, eps)
 
 
-def decode(model, z):
+def _params_function():
+    global _DecodeParams
+    if _DecodeParams is not None:
+        return _DecodeParams
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class DecodeParams(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, model, z, names, *tensors):
+            _check_tensor(model, z, "z")
+            if z.dim() != 2 or z.shape[1] != 100:
+                raise ValueError("z must be (n,100), got %r" % (tuple(z.shape),))
+            _sync_params(model, names, tensors)
+            z = z.contiguous()
+            n = int(z.shape[0])
+            x = torch.empty(n, 3, 64, 64, dtype=torch.float32, device=z.device)
+            if n:
+                with _lib_stream(model, z) as st:
+                    model.decode_dev(z.data_ptr(), n, x.data_ptr(), st)
+            ctx.model, ctx.names = model, names
+            ctx.save_for_backward(z, *tensors)
+            return x
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            z, *tensors = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, g, "grad_output")
+            g = g.contiguous()
+            n = int(z.shape[0])
+            want_z = ctx.needs_input_grad[1]
+            dz = torch.zeros_like(z) if want_z else None
+            grads = [torch.zeros_like(t) if ctx.needs_input_grad[3 + i] else None for i, t in enumerate(tensors)]
+            if n:
+                ptrs = {name: gr.data_ptr() for name, gr in zip(ctx.names, grads) if gr is not None}
+                with _lib_stream(model, z) as st:
+                    model.decode_param_vjp_dev(z.data_ptr(), g.data_ptr(), n, dz.data_ptr() if want_z else 0, ptrs, st)
+            return (None, dz, None) + tuple(grads)
+
+    _DecodeParams = DecodeParams
+    return DecodeParams
+
+
+def _sync_params(model, names, tensors):
+    """write every tensor whose identity or in-place version changed since its last upload back into the handle"""
+    seen = getattr(model, "_param_uploads", None)
+    if seen is None:
+        seen = model._param_uploads = {}
+    changed = {}
+    for name, t in zip(names, tensors):
+        _check_tensor(model, t, name)
+        key = (id(t), t._version)
+        if seen.get(name) != key:
+            changed[name] = t.detach().cpu().numpy()
+            seen[name] = key
+    if changed:
+        model.update_params(changed)
+
+
+def decoder_parameters(model, weights):
+    """{name: leaf float32 CUDA tensor with requires_grad} for the IAN_simple decoder's trainable tensors
+    (model.param_vjp_names()), built from the checkpoint mapping `weights` and uploaded into the handle once, so that the
+    handle provably holds their values."""
+    import torch
+    names = model.param_vjp_names()
+    if not names:
+        raise ValueError("this graph has no parameter gradients (IAN_simple only)")
+    params = {n: torch.tensor(weights[n], dtype=torch.float32, device="cuda:%d" % model.device).requires_grad_(True)
+              for n in names}
+    _sync_params(model, names, [params[n] for n in names])
+    return params
+
+
+def decode(model, z, params=None):
     """x_hat = decoder(z) for z (n,100) float32 CUDA on the model's device; differentiable w.r.t. z (one decoder forward +
-    one backward per backward call)."""
-    return _function().apply(model, z)
+    one backward per backward call).  With params (from decoder_parameters), also differentiable w.r.t. those tensors:
+    one ian_decode_param_vjp_dev returns dz and every gradient; tensors that do not require grad get None."""
+    if params is None:
+        return _function().apply(model, z)
+    names = list(params)
+    return _params_function().apply(model, z, tuple(names), *[params[n] for n in names])
