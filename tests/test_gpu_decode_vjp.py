@@ -17,6 +17,9 @@ ian_decode_vjp_*, API.IAN.decode_vjp, torch_ops.decode) on all three graphs and 
      batches, bf16 against float32.
   D. the torch autograd binding: bit-identical to decode_vjp on the default and a side stream, a torch-driven SGD loop
      against the float64 oracle, once-differentiable.
+These bounds are set by rectifier kinks of the synthetic weights.  The fidelity check is tests/test_gpu_well_conditioned.py:
+on weights with no rectifier near its kink, every sample on every graph to 1.7e-4 relative L2 and 1.1e-4 max-abs / max|ref|
+(measured on an H100 80GB HBM3 at 700 W: worst 8.1e-5 / 7.4e-5).
 Measured values go to vjp_parity.json when IAN_TEST_RECORD names a directory."""
 import json
 import os

@@ -26,6 +26,10 @@ API.IAN.encode_vjp, torch_ops.encode) on all three graphs and both CUDA paths.
      before and after an encoder VJP on it.
   D. the torch autograd binding: bit-identical to encode_vjp_dev on the default and a side stream, decode(encode(x))
      against float64 autograd of the composite, once-differentiable, eps.requires_grad refused.
+These bounds are set by rectifier kinks of the synthetic weights.  The fidelity check is tests/test_gpu_well_conditioned.py:
+on weights with no rectifier near its kink, every sample on every graph, with and without eps, to 5.2e-4 relative L2 and
+3.65e-4 max-abs / max|ref| (measured on an H100 80GB HBM3 at 700 W: worst 2.1e-4 / 3.0e-4 on IAN_simple, 1.0e-4 / 1.2e-4 on the
+flow graphs).
 Measured values go to encvjp_parity.json when IAN_TEST_RECORD names a directory."""
 import json
 import os

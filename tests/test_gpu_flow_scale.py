@@ -46,6 +46,8 @@ import pytest
 from oracle import ian_full_numpy as fn
 from oracle import weights as ow
 
+import scale_inputs
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 X_TOL, Z_K, EPS_K, BF16_MAX, BF16_MEAN = 2e-4, 3e-4, 1e-3, 0.1, 5e-3
@@ -109,31 +111,7 @@ def handles(npe, monkeypatch):
 
 
 # ---- inputs and probes ----------------------------------------------------------------------------------------------
-_INPUTS = {}
-
-
-def _inputs(n, seed):
-    if (n, seed) not in _INPUTS:
-        rng = np.random.default_rng(seed)
-        boxes = np.empty((n, 4), np.int32)
-        for k in range(n):
-            if k % 4 == 0:
-                boxes[k] = [3, 5, 20, 17]
-            elif k % 4 == 1:
-                boxes[k] = [40, 30, 41, 31]                  # one pixel
-            elif k % 4 == 2:
-                boxes[k] = [0, 47, 64, 64]                   # the full width
-            else:
-                c1, r1 = rng.integers(0, 48, 2)
-                boxes[k] = [c1, r1, c1 + rng.integers(2, 17), r1 + rng.integers(2, 17)]
-        _INPUTS[(n, seed)] = {
-            "x": rng.uniform(-1, 1, (n, 3, 64, 64)).astype(np.float32),
-            "z": rng.standard_normal((n, 100)).astype(np.float32),
-            "eps": rng.standard_normal((n, 100)).astype(np.float32),
-            "rgb": rng.uniform(-1, 1, (n, 3)).astype(np.float32),
-            "frame": rng.uniform(-1, 1, (n, 3, 64, 64)).astype(np.float32),
-            "boxes": boxes}
-    return _INPUTS[(n, seed)]
+_inputs = scale_inputs.inputs
 
 
 def _probes(n, sms):
