@@ -41,6 +41,11 @@ inline float bf2f(uint16_t h) {
   memcpy(&f, &u, 4);
   return f;
 }
+// float32 w as the bf16 pair hi + lo that the 3-pass tensor-core kernels multiply
+inline void split_hi_lo(float w, uint16_t& hi, uint16_t& lo) {
+  hi = f2bf(w);
+  lo = f2bf(w - bf2f(hi));
+}
 
 struct HostParam {
   std::vector<int64_t> shape;
@@ -127,6 +132,11 @@ std::vector<Spec> spec_list(int kind) {
   add_mdcl(v, "R", 2, 128, {2, 3, 4}); add_mdcl(v, "G_a", 2, 128, {2, 3, 4}); add_mdcl(v, "G_b", 2, 2, {2, 3, 4});
   add_mdcl(v, "B_a", 2, 128, {2, 3, 4}); add_mdcl(v, "B_b", 2, 4, {2, 3, 4});
   return v;
+}
+
+const std::vector<Spec>& cached_specs(int kind) {
+  static const std::vector<Spec> cache[3] = {spec_list(0), spec_list(1), spec_list(2)};
+  return cache[kind];
 }
 
 enum LayerId {
@@ -453,50 +463,68 @@ int choose_ksplit(const TapGemm& g) {
   return ks;
 }
 
-// Small batches (NPE runs batch 1): a layer with fewer tiles than SMs would stream its weights through a handful of
-// SMs.  Mark every such layer (ksplit = 0: "choose") so choose_ksplit() can spread K over the chip.
-void mark_splitk_candidates(Plan* pl, std::initializer_list<int> layers) {
-  for (int l : layers) {
-    TapGemm& g = pl->g[l];
-    if (g.out_f32_t) continue;
-    const int bn = (g.Cout % 256 == 0) ? 256 : (g.Cout % 128 == 0) ? 128 : 16;
-    const long long tiles = (long long)((g.n_img * g.Hg * g.Wg + 127) / 128) * (g.Cout / bn) * g.nphase;
-    if (tiles <= 74) g.ksplit = 0;
+// A fixed sequence of tap-GEMM layers, in run order
+struct LayerList {
+  int n = 0;
+  int l[32] = {};
+  const int* begin() const { return l; }
+  const int* end() const { return l + n; }
+  LayerList operator+(const LayerList& o) const {
+    LayerList r = *this;
+    for (int x : o) r.l[r.n++] = x;
+    return r;
   }
+};
+
+// The tap-GEMM layers of each graph, read by the run functions and by finish_maps.  The encoder (IAN_simple.py:84-126;
+// its enc_fc1 activation differs per graph, not its layers) and the encoder VJP are shared by all three graphs.
+const LayerList kEncoder = {5, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD}};
+const LayerList kEncoderBwd = {5, {E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2}};
+struct DecoderLayers { LayerList fwd, bwd; };   // the decoder forward, and its backward-data from the last layer down to z
+const DecoderLayers kSimpleDecoder = {{4, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3}},
+                                      {4, {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}}};
+const DecoderLayers kV1Decoder = {{5, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3, F_DEC_CONV4}},
+                                  {6, {F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}}};
+const DecoderLayers kFullDecoder = {{11, {F_DEC_FC2, F_DEC_CONV1, F_MD1A, F_MD1B, F_DEC_CONV2, F_MD2A, F_MD2B, F_DEC_CONV3,
+                                          F_MD3A, F_MD3B, F_DEC_CONV4}},
+                                    {12, {F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B,
+                                          F_BWD_MD2A, F_BWD_CONV2, F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1, F_BWD_FC2}}};
+const DecoderLayers& decoder_layers(const ian_handle* h) {
+  return h->model_kind == IAN_MODEL_FULL ? kFullDecoder : h->model_kind == IAN_MODEL_V1 ? kV1Decoder : kSimpleDecoder;
 }
 
-// One workspace per plan, shared by its split-K layers (they run back to back on one stream):
-// [ksplit][pixel][Cout] float32 slabs, sized for the largest user.
-int alloc_splitk_workspace(ian_handle* h, Plan* pl) {
+// Tensor maps of `layers`, their split-K factors, and one split-K workspace shared by them (they run back to back on one
+// stream): [ksplit][pixel][Cout] float32 slabs, sized for the largest user.
+// Small batches (NPE runs batch 1): a layer with fewer tiles than SMs would stream its weights through a handful of
+// SMs.  Every such layer is marked (ksplit = 0: "choose") so choose_ksplit() can spread K over the chip.
+int finish_maps(ian_handle* h, Plan* pl, const LayerList& layers) {
   long long need = 0;
-  for (int l = 0; l < L_COUNT; ++l) {
+  for (int l : layers) {
     TapGemm& g = pl->g[l];
-    if (g.ksplit <= 1) continue;
-    g.ws_slab = (long long)g.n_img * g.Hout * g.Wout * g.Cout;
-    need = std::max(need, g.ws_slab * g.ksplit);
+    const int bn = (g.Cout % 256 == 0) ? 256 : (g.Cout % 128 == 0) ? 128 : 16;
+    const long long tiles = (long long)((g.n_img * g.Hg * g.Wg + 127) / 128) * (g.Cout / bn) * g.nphase;
+    if (!g.out_f32_t && tiles <= 74) g.ksplit = 0;
+    char err[256] = {0};
+    pl->maps[l] = tc_build_maps(g, err, sizeof(err));
+    if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
+    if (g.ksplit == 0) g.ksplit = h->splitk ? choose_ksplit(g) : 1;
+    if (g.ksplit > 1) {
+      g.ws_slab = (long long)g.n_img * g.Hout * g.Wout * g.Cout;
+      need = std::max(need, g.ws_slab * g.ksplit);
+    }
   }
   if (need == 0) return IAN_OK;
   float* ws = nullptr;
   int rc = alloc_buf(h, pl, ws, need);
   if (rc != IAN_OK) return rc;
-  for (int l = 0; l < L_COUNT; ++l)
+  for (int l : layers)
     if (pl->g[l].ksplit > 1) pl->g[l].ws = ws;
   return IAN_OK;
 }
 
-int finish_maps(ian_handle* h, Plan* pl, std::initializer_list<int> layers) {
-  for (int l : layers) {
-    char err[256] = {0};
-    pl->maps[l] = tc_build_maps(pl->g[l], err, sizeof(err));
-    if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
-    if (pl->g[l].ksplit == 0) pl->g[l].ksplit = h->splitk ? choose_ksplit(pl->g[l]) : 1;
-  }
-  return alloc_splitk_workspace(h, pl);
-}
-
 // decoder of IANv1 (reference IANv1.py:125-201): dense (linear) -> 4 x [deconv, BN, relu] -> RGB-Beta head.  The last deconv
 // has 64 output channels; it is stored 128 wide (upper half zero weights) so the head GEMM keeps Cin % 64 == 0 tiles.
-int build_plan_v1(ian_handle* h, Plan* pl, Plan** out) {
+void wire_decoder_v1(ian_handle* h, Plan* pl) {
   TapGemm* g = pl->g;
   const int n = pl->n;
   auto outp = [](TapGemm& gg, const Planes& t) { gg.out = t.p; gg.out_plane = t.plane; };
@@ -525,22 +553,10 @@ int build_plan_v1(ian_handle* h, Plan* pl, Plan** out) {
   bwd(L_BWD_CONV1, pl->d1, 8, 512, pl->d0, nullptr, ACT_NONE);          // l_dec_fc2 is linear here (IANv1.py:125-130)
   set_io(g[L_BWD_FC2], pl->d0, n, 1, 1, 16384, 1, 1, h->w[L_BWD_FC2], 1, 1); taps_dense(g[L_BWD_FC2]);
   g[L_BWD_FC2].act = ACT_NONE; g[L_BWD_FC2].out_f32 = pl->gpad; g[L_BWD_FC2].ksplit = 0;
-  mark_splitk_candidates(pl, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD, L_DEC_FC2, L_DEC_CONV1,
-                              L_DEC_CONV2, L_DEC_CONV3, F_DEC_CONV4, F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1});
-  int rc = finish_maps(h, pl, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD, L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2,
-                           L_DEC_CONV3, F_DEC_CONV4, F_HEAD, F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2});
-  if (rc != IAN_OK) return rc;
-  {
-    char err[256] = {0};
-    pl->head_maps = head_build_maps(pl->fh4.p, pl->fh4.plane, n, h->head_tc_wt, 3 * 80 * 128, err, sizeof(err));
-    if (!pl->head_maps) return fail(h, IAN_ERR_CUDA, "rgb head: %s", err);
-  }
-  *out = pl;
-  return IAN_OK;
 }
 
 // decoder of the full IAN (reference IAN.py:129-207): dense -> 3 x (deconv, MDBLOCK) -> deconv -> RGB-Beta head
-int build_plan_full(ian_handle* h, Plan* pl, Plan** out) {
+void wire_decoder_full(ian_handle* h, Plan* pl) {
   TapGemm* g = pl->g;
   const int n = pl->n;
   auto outp = [](TapGemm& gg, const Planes& t) { gg.out = t.p; gg.out_plane = t.plane; };
@@ -593,22 +609,29 @@ int build_plan_full(ian_handle* h, Plan* pl, Plan** out) {
   g[F_BWD_CONV1].act = ACT_MASK; g[F_BWD_CONV1].mask = pl->fh0.p; g[F_BWD_CONV1].mask_slope = 0.2f; outp(g[F_BWD_CONV1], pl->dfh0);
   set_io(g[F_BWD_FC2], pl->dfh0, n, 1, 1, 8192, 1, 1, h->w[F_BWD_FC2], 1, 1); taps_dense(g[F_BWD_FC2]);
   g[F_BWD_FC2].act = ACT_NONE; g[F_BWD_FC2].out_f32 = pl->gpad; g[F_BWD_FC2].ksplit = 0;
-  mark_splitk_candidates(pl, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD, F_DEC_FC2, F_DEC_CONV1, F_MD1A,
-                              F_MD1B, F_DEC_CONV2, F_MD2A, F_MD2B, F_DEC_CONV3, F_MD3A, F_MD3B, F_DEC_CONV4,
-                              F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B, F_BWD_MD2A, F_BWD_CONV2,
-                              F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1});
-  int rc = finish_maps(h, pl, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD, F_DEC_FC2, F_DEC_CONV1, F_MD1A, F_MD1B,
-                               F_DEC_CONV2, F_MD2A, F_MD2B, F_DEC_CONV3, F_MD3A, F_MD3B, F_DEC_CONV4, F_HEAD,
-                               F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B, F_BWD_MD2A, F_BWD_CONV2,
-                               F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1, F_BWD_FC2});
-  if (rc != IAN_OK) return rc;
-  {
-    char err[256] = {0};
-    pl->head_maps = head_build_maps(pl->fh4.p, pl->fh4.plane, n, h->head_tc_wt, 3 * 80 * 128, err, sizeof(err));
-    if (!pl->head_maps) return fail(h, IAN_ERR_CUDA, "rgb head: %s", err);
-  }
-  *out = pl;
-  return IAN_OK;
+}
+
+// decoder of IAN_simple (IAN_simple.py:129-170) and its backward-data for the latent brush (T.grad at API.py:59,64)
+void wire_decoder_simple(ian_handle* h, Plan* pl) {
+  TapGemm* g = pl->g;
+  const int n = pl->n;
+  set_io(g[L_DEC_FC2], pl->zp, n, 1, 1, 128, 1, 1, h->w[L_DEC_FC2], 1, 1); taps_dense(g[L_DEC_FC2]);
+  g[L_DEC_FC2].act = ACT_RELU; g[L_DEC_FC2].out = pl->h0.p; g[L_DEC_FC2].out_plane = pl->h0.plane;
+  set_io(g[L_DEC_CONV1], pl->h0, n, 4, 4, 1024, 4, 4, h->w[L_DEC_CONV1], 8, 8); taps_deconv_s2(g[L_DEC_CONV1]);
+  g[L_DEC_CONV1].act = ACT_RELU; g[L_DEC_CONV1].out = pl->h1.p; g[L_DEC_CONV1].out_plane = pl->h1.plane;
+  set_io(g[L_DEC_CONV2], pl->h1, n, 8, 8, 512, 8, 8, h->w[L_DEC_CONV2], 16, 16); taps_deconv_s2(g[L_DEC_CONV2]);
+  g[L_DEC_CONV2].act = ACT_RELU; g[L_DEC_CONV2].out = pl->h2.p; g[L_DEC_CONV2].out_plane = pl->h2.plane;
+  set_io(g[L_DEC_CONV3], pl->h2, n, 16, 16, 256, 16, 16, h->w[L_DEC_CONV3], 32, 32); taps_deconv_s2(g[L_DEC_CONV3]);
+  g[L_DEC_CONV3].act = ACT_RELU; g[L_DEC_CONV3].out = pl->h3.p; g[L_DEC_CONV3].out_plane = pl->h3.plane;
+  set_io(g[L_BWD_CONV3], pl->d3, n, 32, 32, 128, 16, 16, h->w[L_BWD_CONV3], 16, 16); taps_deconv_bwd(g[L_BWD_CONV3]);
+  g[L_BWD_CONV3].act = ACT_MASK; g[L_BWD_CONV3].mask = pl->h2.p; g[L_BWD_CONV3].out = pl->d2.p; g[L_BWD_CONV3].out_plane = pl->d2.plane;
+  set_io(g[L_BWD_CONV2], pl->d2, n, 16, 16, 256, 8, 8, h->w[L_BWD_CONV2], 8, 8); taps_deconv_bwd(g[L_BWD_CONV2]);
+  g[L_BWD_CONV2].act = ACT_MASK; g[L_BWD_CONV2].mask = pl->h1.p; g[L_BWD_CONV2].out = pl->d1.p; g[L_BWD_CONV2].out_plane = pl->d1.plane;
+  set_io(g[L_BWD_CONV1], pl->d1, n, 8, 8, 512, 4, 4, h->w[L_BWD_CONV1], 4, 4); taps_deconv_bwd(g[L_BWD_CONV1]);
+  g[L_BWD_CONV1].act = ACT_MASK; g[L_BWD_CONV1].mask = pl->h0.p; g[L_BWD_CONV1].out = pl->d0.p; g[L_BWD_CONV1].out_plane = pl->d0.plane;
+  g[L_BWD_CONV1].scale_pix_stride = 1024;   // bnorm_dec_fc2 is per FEATURE (pixel, channel)
+  set_io(g[L_BWD_FC2], pl->d0, n, 1, 1, 16384, 1, 1, h->w[L_BWD_FC2], 1, 1); taps_dense(g[L_BWD_FC2]);
+  g[L_BWD_FC2].act = ACT_NONE; g[L_BWD_FC2].out_f32 = pl->gpad; g[L_BWD_FC2].ksplit = 0;
 }
 
 int build_plan(ian_handle* h, int n, Plan** out) {
@@ -670,39 +693,17 @@ int build_plan(ian_handle* h, int n, Plan** out) {
     pl->conv1_out = conv1_build_out_map(pl->a1.p, pl->a1.plane, n, err, sizeof(err));
     if (!pl->conv1_out) return fail(h, IAN_ERR_CUDA, "enc_conv1: %s", err);
   }
-  if (full) return build_plan_full(h, pl, out);
-  if (v1) return build_plan_v1(h, pl, out);
-  // ---- decoder (IAN_simple.py:129-170)
-  set_io(g[L_DEC_FC2], pl->zp, n, 1, 1, 128, 1, 1, h->w[L_DEC_FC2], 1, 1); taps_dense(g[L_DEC_FC2]);
-  g[L_DEC_FC2].act = ACT_RELU; g[L_DEC_FC2].out = pl->h0.p; g[L_DEC_FC2].out_plane = pl->h0.plane;
-  set_io(g[L_DEC_CONV1], pl->h0, n, 4, 4, 1024, 4, 4, h->w[L_DEC_CONV1], 8, 8); taps_deconv_s2(g[L_DEC_CONV1]);
-  g[L_DEC_CONV1].act = ACT_RELU; g[L_DEC_CONV1].out = pl->h1.p; g[L_DEC_CONV1].out_plane = pl->h1.plane;
-  set_io(g[L_DEC_CONV2], pl->h1, n, 8, 8, 512, 8, 8, h->w[L_DEC_CONV2], 16, 16); taps_deconv_s2(g[L_DEC_CONV2]);
-  g[L_DEC_CONV2].act = ACT_RELU; g[L_DEC_CONV2].out = pl->h2.p; g[L_DEC_CONV2].out_plane = pl->h2.plane;
-  set_io(g[L_DEC_CONV3], pl->h2, n, 16, 16, 256, 16, 16, h->w[L_DEC_CONV3], 32, 32); taps_deconv_s2(g[L_DEC_CONV3]);
-  g[L_DEC_CONV3].act = ACT_RELU; g[L_DEC_CONV3].out = pl->h3.p; g[L_DEC_CONV3].out_plane = pl->h3.plane;
-  // ---- decoder backward-data for the latent brush (T.grad at API.py:59,64)
-  set_io(g[L_BWD_CONV3], pl->d3, n, 32, 32, 128, 16, 16, h->w[L_BWD_CONV3], 16, 16); taps_deconv_bwd(g[L_BWD_CONV3]);
-  g[L_BWD_CONV3].act = ACT_MASK; g[L_BWD_CONV3].mask = pl->h2.p; g[L_BWD_CONV3].out = pl->d2.p; g[L_BWD_CONV3].out_plane = pl->d2.plane;
-  set_io(g[L_BWD_CONV2], pl->d2, n, 16, 16, 256, 8, 8, h->w[L_BWD_CONV2], 8, 8); taps_deconv_bwd(g[L_BWD_CONV2]);
-  g[L_BWD_CONV2].act = ACT_MASK; g[L_BWD_CONV2].mask = pl->h1.p; g[L_BWD_CONV2].out = pl->d1.p; g[L_BWD_CONV2].out_plane = pl->d1.plane;
-  set_io(g[L_BWD_CONV1], pl->d1, n, 8, 8, 512, 4, 4, h->w[L_BWD_CONV1], 4, 4); taps_deconv_bwd(g[L_BWD_CONV1]);
-  g[L_BWD_CONV1].act = ACT_MASK; g[L_BWD_CONV1].mask = pl->h0.p; g[L_BWD_CONV1].out = pl->d0.p; g[L_BWD_CONV1].out_plane = pl->d0.plane;
-  g[L_BWD_CONV1].scale_pix_stride = 1024;   // bnorm_dec_fc2 is per FEATURE (pixel, channel)
-  set_io(g[L_BWD_FC2], pl->d0, n, 1, 1, 16384, 1, 1, h->w[L_BWD_FC2], 1, 1); taps_dense(g[L_BWD_FC2]);
-  g[L_BWD_FC2].act = ACT_NONE; g[L_BWD_FC2].out_f32 = pl->gpad; g[L_BWD_FC2].ksplit = 0;
-
-  mark_splitk_candidates(pl, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD, L_DEC_FC2, L_DEC_CONV1,
-                              L_DEC_CONV2, L_DEC_CONV3, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1});
-  for (int l = 0; l < F_DEC_FC2; ++l) {
-    char err[256] = {0};
-    pl->maps[l] = tc_build_maps(g[l], err, sizeof(err));
-    if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
-    if (g[l].ksplit == 0) g[l].ksplit = h->splitk ? choose_ksplit(g[l]) : 1;
-  }
-  if ((rc = alloc_splitk_workspace(h, pl)) != IAN_OK) return rc;
-  {
-    char err[256] = {0};
+  if (full) wire_decoder_full(h, pl);
+  else if (v1) wire_decoder_v1(h, pl);
+  else wire_decoder_simple(h, pl);
+  const DecoderLayers& dec = decoder_layers(h);
+  const LayerList head = {has_flow(h) ? 1 : 0, {F_HEAD}};   // the head GEMM of the verification path (run_head)
+  if ((rc = finish_maps(h, pl, kEncoder + dec.fwd + head + dec.bwd)) != IAN_OK) return rc;
+  char err[256] = {0};
+  if (has_flow(h)) {
+    pl->head_maps = head_build_maps(pl->fh4.p, pl->fh4.plane, n, h->head_tc_wt, 3 * 80 * 128, err, sizeof(err));
+    if (!pl->head_maps) return fail(h, IAN_ERR_CUDA, "rgb head: %s", err);
+  } else {
     pl->decout_maps = decout_build_maps(pl->h3.p, pl->h3.plane, n, h->decout_tc_wt, 80 * 128, err, sizeof(err));
     if (!pl->decout_maps) return fail(h, IAN_ERR_CUDA, "dec_out: %s", err);
   }
@@ -798,7 +799,7 @@ int run_encode(ian_handle* h, Plan* pl, const float* x, const float* eps, float*
       LAUNCH_TRY(h, launch_conv1(x, h->conv1_wt, h->conv1_b, pl->a1.p, pl->a1.plane, n, st));
   }
   int rc;
-  for (int l : {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD})
+  for (int l : kEncoder)
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
   if (has_flow(h)) {
     // l_Z_IAF = mu (+ exp(ls) eps), then l_Z = IAF(l_Z_IAF; MADE_mu, MADE_ls)   (IAN.py:126-128)
@@ -833,18 +834,9 @@ int run_head(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
 // zp must already hold the latent planes
 int run_decode_from_planes(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
   int rc;
-  if (h->model_kind == IAN_MODEL_V1) {
-    for (int l : {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3, F_DEC_CONV4})
-      if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
-    return run_head(h, pl, xhat, st);
-  }
-  if (h->model_kind == IAN_MODEL_FULL) {
-    for (int l : {F_DEC_FC2, F_DEC_CONV1, F_MD1A, F_MD1B, F_DEC_CONV2, F_MD2A, F_MD2B, F_DEC_CONV3, F_MD3A, F_MD3B, F_DEC_CONV4})
-      if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
-    return run_head(h, pl, xhat, st);
-  }
-  for (int l : {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3})
+  for (int l : decoder_layers(h).fwd)
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+  if (has_flow(h)) return run_head(h, pl, xhat, st);
   ScopedTimer tm(h, T_DEC_OUT, st);
   if (h->path == IAN_PATH_TC) {
     float* one[1] = {xhat};
@@ -876,17 +868,7 @@ int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* ta
     }
     LAUNCH_TRY(h, launch_head_bwd(pl->rg, h->head_taps, h->head_wgb, h->head_wbb, h->head_ntaps, pl->dpre, pl->dha2.p,
                                   pl->dha2.plane, pl->n, st));
-    if (h->model_kind == IAN_MODEL_V1) {
-      for (int l : {F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2})
-        if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
-    } else {
-      for (int l : {F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B, F_BWD_MD2A, F_BWD_CONV2,
-                    F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1, F_BWD_FC2})
-        if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
-    }
-    return IAN_OK;
-  }
-  {
+  } else {
     ScopedTimer tm(h, T_BRUSH_SEED, st);
     if (param)
       LAUNCH_TRY(h, launch_brush_param_seed_bwd(pl->xhat, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale, pl->h3.p, pl->d3.p,
@@ -895,12 +877,10 @@ int run_grad_core(ian_handle* h, Plan* pl, const int32_t* boxes, const float* ta
       LAUNCH_TRY(h, launch_brush_seed_bwd(pl->xhat, boxes, target, target_is_frame, dxhat, h->decout_wt, h->w[L_DEC_CONV3].scale,
                                           pl->h3.p, pl->d3.p, pl->d3.plane, pl->n, st));
   }
-  for (int l : {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2})
+  for (int l : decoder_layers(h).bwd)
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
   return IAN_OK;
 }
-
-int check_brush_supported(ian_handle*) { return IAN_OK; }   // all three graphs have their decoder backward
 
 int check_ready(ian_handle* h, int n, const void* a, const void* b) {
   if (!h) return IAN_ERR_INVALID;
@@ -935,11 +915,7 @@ int upload_tiles(ian_handle* h, int l, const std::vector<float>& B, int ntiles, 
   DevWeights& w = h->w[l];
   const long long elems = (long long)ntiles * Cout * Cin;
   std::vector<uint16_t> planes((size_t)elems * 2);
-  for (long long i = 0; i < elems; ++i) {
-    const uint16_t hi = f2bf(B[i]);
-    planes[i] = hi;
-    planes[elems + i] = f2bf(B[i] - bf2f(hi));
-  }
+  for (long long i = 0; i < elems; ++i) split_hi_lo(B[i], planes[i], planes[elems + i]);
   int rc = put_dev(h, w.b, planes.data(), planes.size() * 2);
   if (rc != IAN_OK) return rc;
   w.plane = elems; w.ntiles = ntiles; w.Cout = Cout; w.Cin = Cin;
@@ -1034,15 +1010,10 @@ int prepare_encoder(ian_handle* h) {
     std::vector<uint16_t> planes(3 * 128 * 64, 0);
     for (int o = 0; o < 128; ++o)
       for (int k = 0; k < 75; ++k) {
-        const uint16_t hi = f2bf(W[o * 75 + k]);
-        const uint16_t lo = f2bf(W[o * 75 + k] - bf2f(hi));
-        if (k < 64) {
-          planes[o * 64 + k] = hi;
-          planes[128 * 64 + o * 64 + k] = lo;
-        } else {
-          planes[2 * 128 * 64 + o * 64 + (k - 64)] = hi;
-          planes[2 * 128 * 64 + o * 64 + 16 + (k - 64)] = lo;
-        }
+        if (k < 64)
+          split_hi_lo(W[o * 75 + k], planes[o * 64 + k], planes[128 * 64 + o * 64 + k]);
+        else
+          split_hi_lo(W[o * 75 + k], planes[2 * 128 * 64 + o * 64 + (k - 64)], planes[2 * 128 * 64 + o * 64 + 16 + (k - 64)]);
       }
     CUDA_TRY(h, cudaMalloc((void**)&h->conv1_tc_wt, planes.size() * 2));
     CUDA_TRY(h, cudaMemcpy(h->conv1_tc_wt, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice));
@@ -1053,12 +1024,13 @@ int prepare_encoder(ian_handle* h) {
   return IAN_OK;
 }
 
-// 5x5 stride-2 transposed conv weights W (Cin,Cout,5,5) -> forward tiles B[k][co][ci] = W[ci][co][k]
-void deconv_fwd_tiles(const std::vector<float>& W, int Cin, int Cout, std::vector<float>& B) {
-  B.assign((size_t)25 * Cout * Cin, 0.f);
+// 5x5 stride-2 transposed conv weights W (Cin,Cout,5,5) -> forward tiles B[k][co][ci] = W[ci][co][k] (GEMM Cout padded to
+// CoutPad with zero rows)
+void deconv_fwd_tiles(const std::vector<float>& W, int Cin, int Cout, int CoutPad, std::vector<float>& B) {
+  B.assign((size_t)25 * CoutPad * Cin, 0.f);
   for (int ci = 0; ci < Cin; ++ci)
     for (int co = 0; co < Cout; ++co)
-      for (int t = 0; t < 25; ++t) B[((size_t)t * Cout + co) * Cin + ci] = W[((size_t)ci * Cout + co) * 25 + t];
+      for (int t = 0; t < 25; ++t) B[((size_t)t * CoutPad + co) * Cin + ci] = W[((size_t)ci * Cout + co) * 25 + t];
 }
 
 // backward-data of the same layer: the gradient w.r.t. the deconv's INPUT is a stride-2 convolution of the output gradient
@@ -1077,6 +1049,20 @@ void transpose_tiles(const std::vector<float>& comp, int nt, int F, int C, std::
       for (int c = 0; c < C; ++c) out[((size_t)t * C + c) * F + f] = comp[((size_t)t * F + f) * C + c];
 }
 
+// l_dec_fc2 (W (100, 16C)): the reference's column j = c*16 + hw is our NHWC column hw*C + c; K 100 -> 128.  Forward tiles
+// B[col][k] (GEMM Cout 16C, Cin 128); backward (dz[k] = sum_col d[col] W[k][col]) tiles B[k][col] (GEMM Cout 128, Cin 16C).
+void fc2_tiles(const std::vector<float>& W, int C, bool bwd, std::vector<float>& B) {
+  const size_t cols = (size_t)16 * C;
+  B.assign(cols * 128, 0.f);
+  for (int c = 0; c < C; ++c)
+    for (int hw = 0; hw < 16; ++hw) {
+      const size_t j = (size_t)c * 16 + hw, col = hw * (size_t)C + c;
+      for (int k = 0; k < 100; ++k) (bwd ? B[k * cols + col] : B[col * 128 + k]) = W[k * cols + j];
+    }
+}
+// the reference's column of our column col (a per-feature vector of l_dec_fc2's output)
+inline int fc2_ref_col(int col, int C) { return (col % C) * 16 + col / C; }
+
 // ---- IAN_simple decoder: one derivation per parameter group, shared by ian_finalize and ian_update_param_host ----------
 // Each writes every device buffer derived from its group: allocated by the first call, overwritten in place by later ones.
 const char* kDecBn[4] = {"bnorm_dec_fc2", "bnorm_dc1", "bnorm_dc2", "bnorm_dc3"};
@@ -1086,39 +1072,27 @@ const DecConv kDecConv[3] = {{L_DEC_CONV1, L_BWD_CONV1, "dec_conv1.W", 1024, 512
                              {L_DEC_CONV2, L_BWD_CONV2, "dec_conv2.W", 512, 256},
                              {L_DEC_CONV3, L_BWD_CONV3, "dec_conv3.W", 256, 128}};
 
-// l_dec_fc2: reference column j = c*16 + hw -> our column hw*1024 + c; Cin 100 -> 128.  Forward tiles B[col][k]; backward
-// (dz[k] = sum_col d0[col] W[k][col]) tiles B[k][col], Cout 100 -> 128, unit scale.
+// l_dec_fc2: forward and backward tiles (fc2_tiles), the backward with unit scale
 int simple_fc2_weights(ian_handle* h, const std::vector<float>& W) {
-  std::vector<float> B((size_t)16384 * 128, 0.f), Bt((size_t)128 * 16384, 0.f);
-  for (int c = 0; c < 1024; ++c)
-    for (int hw = 0; hw < 16; ++hw) {
-      const int j = c * 16 + hw, col = hw * 1024 + c;
-      for (int k = 0; k < 100; ++k) {
-        B[(size_t)col * 128 + k] = W[(size_t)k * 16384 + j];
-        Bt[(size_t)k * 16384 + col] = W[(size_t)k * 16384 + j];
-      }
-    }
+  std::vector<float> B;
+  fc2_tiles(W, 1024, false, B);
   int rc = upload_tiles(h, L_DEC_FC2, B, 1, 16384, 128);
   if (rc != IAN_OK) return rc;
-  if ((rc = upload_tiles(h, L_BWD_FC2, Bt, 1, 128, 16384)) != IAN_OK) return rc;
+  fc2_tiles(W, 1024, true, B);
+  if ((rc = upload_tiles(h, L_BWD_FC2, B, 1, 128, 16384)) != IAN_OK) return rc;
   const std::vector<float> ones(128, 1.f);
   return put_dev(h, h->w[L_BWD_FC2].scale, ones.data(), ones.size() * 4);
 }
 
-// dec_conv k (W (Cin,Cout,5,5)): forward B[t][co][ci] = W[ci][co][t]; backward-data B[t][ci][co] = W[ci][co][t]
+// dec_conv k (W (Cin,Cout,5,5)): forward and backward-data tiles
 int simple_conv_weights(ian_handle* h, int k, const std::vector<float>& W) {
   const DecConv& d = kDecConv[k];
-  std::vector<float> B((size_t)25 * d.Cout * d.Cin), Bt((size_t)25 * d.Cout * d.Cin);
-  for (int ci = 0; ci < d.Cin; ++ci)
-    for (int co = 0; co < d.Cout; ++co)
-      for (int t = 0; t < 25; ++t) {
-        const float v = W[((size_t)ci * d.Cout + co) * 25 + t];
-        B[((size_t)t * d.Cout + co) * d.Cin + ci] = v;
-        Bt[((size_t)t * d.Cin + ci) * d.Cout + co] = v;
-      }
+  std::vector<float> B;
+  deconv_fwd_tiles(W, d.Cin, d.Cout, d.Cout, B);
   int rc = upload_tiles(h, d.lf, B, 25, d.Cout, d.Cin);
   if (rc != IAN_OK) return rc;
-  return upload_tiles(h, d.lb, Bt, 25, d.Cin, d.Cout);
+  deconv_bwd_tiles(W, d.Cin, d.Cout, d.Cout, B);
+  return upload_tiles(h, d.lb, B, 25, d.Cin, d.Cout);
 }
 
 // dec_out W (128,3,5,5): tensor-core form (decout_tc.cu, rows tap*3+co padded to 80, K-major over ci, bf16 hi|lo planes)
@@ -1130,9 +1104,7 @@ int simple_dec_out_weights(ian_handle* h, const std::vector<float>& W) {
     for (int co = 0; co < 3; ++co)
       for (int t = 0; t < 25; ++t) {
         const float w = W[(ci * 3 + co) * 25 + t];
-        const uint16_t hi = f2bf(w);
-        planes[(t * 3 + co) * 128 + ci] = hi;
-        planes[80 * 128 + (t * 3 + co) * 128 + ci] = f2bf(w - bf2f(hi));
+        split_hi_lo(w, planes[(t * 3 + co) * 128 + ci], planes[80 * 128 + (t * 3 + co) * 128 + ci]);
         wt[(t * 128 + ci) * 4 + co] = w;
       }
   int rc = put_dev(h, h->decout_tc_wt, planes.data(), planes.size() * 2);
@@ -1148,7 +1120,7 @@ int simple_bn(ian_handle* h, int k) {
   const auto& f = h->dec_bn[k];      // beta, gamma, mean, inv_std
   std::vector<float> sc(C), sf(C);
   for (int j = 0; j < C; ++j) {
-    const int i = k == 0 ? (j % 1024) * 16 + j / 1024 : j;   // fc2: our column j = hw*1024 + c <- reference c*16 + hw
+    const int i = k == 0 ? fc2_ref_col(j, 1024) : j;
     sc[j] = f[1][i] * f[3][i];
     sf[j] = f[0][i] - f[2][i] * sc[j];
   }
@@ -1304,11 +1276,8 @@ int prepare_head(ian_handle* h, int C, const std::vector<float>& scale_below /*B
         for (int j = 0; j < 33; ++j)
           for (int f = 0; f < 2; ++f)
             for (int c = 0; c < 128; ++c) {
-              const float w = B[((size_t)(order[j] * 6 + 2 * k + f)) * 128 + c];
-              const uint16_t hi = f2bf(w);
               const size_t row = (size_t)k * 80 + j * 2 + f;
-              planes[row * 128 + c] = hi;
-              planes[plane + row * 128 + c] = f2bf(w - bf2f(hi));
+              split_hi_lo(B[((size_t)(order[j] * 6 + 2 * k + f)) * 128 + c], planes[row * 128 + c], planes[plane + row * 128 + c]);
             }
       CUDA_TRY(h, cudaMalloc((void**)&h->head_tc_wt, planes.size() * 2));
       CUDA_TRY(h, cudaMemcpy(h->head_tc_wt, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice));
@@ -1328,34 +1297,24 @@ int prepare_v1_decoder(ian_handle* h) {
   int rc;
   std::vector<float> B, sc, sf;
   if ((rc = prepare_made(h)) != IAN_OK) return rc;
-  {   // l_dec_fc2: dense 100 -> 16384 + bias, NO nonlinearity; column j = c*16+hw -> hw*1024 + c
-    const auto& W = P(h, "l_dec_fc2.W").data;
+  {   // l_dec_fc2: dense 100 -> 16384 + bias, NO nonlinearity
     const auto& b = P(h, "l_dec_fc2.b").data;
-    B.assign((size_t)16384 * 128, 0.f);
+    fc2_tiles(P(h, "l_dec_fc2.W").data, 1024, false, B);
     sc.assign(16384, 1.f);
-    sf.assign(16384, 0.f);
-    for (int c = 0; c < 1024; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 1024 + c;
-        sf[col] = b[j];
-        for (int k = 0; k < 100; ++k) B[(size_t)col * 128 + k] = W[(size_t)k * 16384 + j];
-      }
+    sf.resize(16384);
+    for (int col = 0; col < 16384; ++col) sf[col] = b[fc2_ref_col(col, 1024)];
     if ((rc = upload_gemm_weights(h, L_DEC_FC2, B, 1, 16384, 128, sc, sf)) != IAN_OK) return rc;
   }
   struct St { int l; const char* w; const char* bn; int Cin, Cout; } sts[3] = {
       {L_DEC_CONV1, "dec_conv1.W", "bnorm_dc1", 1024, 512}, {L_DEC_CONV2, "dec_conv2.W", "bnorm_dc2", 512, 256},
       {L_DEC_CONV3, "dec_conv3.W", "bnorm_dc3", 256, 128}};
   for (const St& s : sts) {
-    deconv_fwd_tiles(P(h, s.w).data, s.Cin, s.Cout, B);
+    deconv_fwd_tiles(P(h, s.w).data, s.Cin, s.Cout, s.Cout, B);
     fold_bn(h, s.bn, s.Cout, sc, sf);
     if ((rc = upload_gemm_weights(h, s.l, B, 25, s.Cout, s.Cin, sc, sf)) != IAN_OK) return rc;
   }
   {   // dec_conv4: 128 -> 64 channels, stored 128 wide: channels 64..127 have zero weights, scale and shift (relu(0) = 0)
-    const auto& W = P(h, "dec_conv4.W").data;
-    B.assign((size_t)25 * 128 * 128, 0.f);
-    for (int ci = 0; ci < 128; ++ci)
-      for (int co = 0; co < 64; ++co)
-        for (int t = 0; t < 25; ++t) B[((size_t)t * 128 + co) * 128 + ci] = W[((size_t)ci * 64 + co) * 25 + t];
+    deconv_fwd_tiles(P(h, "dec_conv4.W").data, 128, 64, 128, B);
     fold_bn(h, "bnorm_dc4", 64, sc, sf);
     sc.resize(128, 0.f);
     sf.resize(128, 0.f);
@@ -1372,16 +1331,8 @@ int prepare_v1_decoder(ian_handle* h) {
   if ((rc = upload_gemm_weights(h, L_BWD_CONV2, B, 25, 512, 256, s1, {})) != IAN_OK) return rc;
   deconv_bwd_tiles(P(h, "dec_conv1.W").data, 1024, 512, 512, B);
   if ((rc = upload_gemm_weights(h, L_BWD_CONV1, B, 25, 1024, 512, std::vector<float>(1024, 1.f), {})) != IAN_OK) return rc;
-  {   // dz[k] = sum_col d0[col] * W[k][col]
-    const auto& W = P(h, "l_dec_fc2.W").data;
-    B.assign((size_t)128 * 16384, 0.f);
-    for (int c = 0; c < 1024; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 1024 + c;
-        for (int k = 0; k < 100; ++k) B[(size_t)k * 16384 + col] = W[(size_t)k * 16384 + j];
-      }
-    if ((rc = upload_gemm_weights(h, L_BWD_FC2, B, 1, 128, 16384, std::vector<float>(128, 1.f), {})) != IAN_OK) return rc;
-  }
+  fc2_tiles(P(h, "l_dec_fc2.W").data, 1024, true, B);
+  if ((rc = upload_gemm_weights(h, L_BWD_FC2, B, 1, 128, 16384, std::vector<float>(128, 1.f), {})) != IAN_OK) return rc;
   return prepare_head(h, 64, s4);
 }
 
@@ -1389,19 +1340,13 @@ int prepare_full_decoder(ian_handle* h) {
   int rc;
   std::vector<float> B, sc, sf, comp;
   if ((rc = prepare_made(h)) != IAN_OK) return rc;
-  // ---- l_dec_fc2: dense 100 -> 8192 + bias, lrelu (IAN.py:129-134); column j = c*16+hw -> hw*512 + c
+  // ---- l_dec_fc2: dense 100 -> 8192 + bias, lrelu (IAN.py:129-134)
   {
-    const auto& W = P(h, "l_dec_fc2.W").data;
     const auto& b = P(h, "l_dec_fc2.b").data;
-    B.assign((size_t)8192 * 128, 0.f);
+    fc2_tiles(P(h, "l_dec_fc2.W").data, 512, false, B);
     sc.assign(8192, 1.f);
-    sf.assign(8192, 0.f);
-    for (int c = 0; c < 512; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 512 + c;
-        sf[col] = b[j];
-        for (int k = 0; k < 100; ++k) B[(size_t)col * 128 + k] = W[(size_t)k * 8192 + j];
-      }
+    sf.resize(8192);
+    for (int col = 0; col < 8192; ++col) sf[col] = b[fc2_ref_col(col, 512)];
     if ((rc = upload_gemm_weights(h, F_DEC_FC2, B, 1, 8192, 128, sc, sf)) != IAN_OK) return rc;
   }
   // ---- deconvs + MDBLOCKs (IAN.py:139-171)
@@ -1410,7 +1355,7 @@ int prepare_full_decoder(ian_handle* h) {
                      {F_DEC_CONV2, F_MD2A, F_MD2B, "dec_conv2.W", "dec_conv3a", 512, 256, {0, 2, 3}},
                      {F_DEC_CONV3, F_MD3A, F_MD3B, "dec_conv3.W", "dec_conv4a", 256, 128, {0, 2, 3}}};
   for (const St& s : sts) {
-    deconv_fwd_tiles(P(h, s.w).data, s.Cin, s.Cout, B);
+    deconv_fwd_tiles(P(h, s.w).data, s.Cin, s.Cout, s.Cout, B);
     fold_bn(h, std::string(s.blk) + "bnorm0", s.Cout, sc, sf);
     if ((rc = upload_gemm_weights(h, s.dconv, B, 25, s.Cout, s.Cin, sc, sf)) != IAN_OK) return rc;
     const int nt = (int)mdc_offsets(s.scales).size();
@@ -1421,11 +1366,11 @@ int prepare_full_decoder(ian_handle* h) {
     fold_bn(h, std::string(s.blk) + "bnorm2", s.Cout, sc, sf);
     if ((rc = upload_gemm_weights(h, s.mdb, comp, nt, s.Cout, s.Cout, sc, sf)) != IAN_OK) return rc;
   }
-  deconv_fwd_tiles(P(h, "dec_conv4.W").data, 128, 128, B);
+  deconv_fwd_tiles(P(h, "dec_conv4.W").data, 128, 128, 128, B);
   fold_bn(h, "bnorm_dc4", 128, sc, sf);
   if ((rc = upload_gemm_weights(h, F_DEC_CONV4, B, 25, 128, 128, sc, sf)) != IAN_OK) return rc;
   if ((rc = prepare_head(h, 128, sc)) != IAN_OK) return rc;
-  // ---- brush backward (see build_plan_full): every backward GEMM's epilogue applies the BN scale of the activation it lands on
+  // ---- brush backward (see wire_decoder_full): every backward GEMM's epilogue applies the BN scale of the activation it lands on
   struct Bk { int dconv, mdb, mda; const char* w_above; int Cin_above, Cout_above; const char* blk; int C; std::vector<int> scales; };
   // dconv = backward-data of the deconv ABOVE block `blk` (w_above: (Cin_above = this block's C, Cout_above))
   const Bk bks[3] = {{F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, "dec_conv4.W", 128, 128, "dec_conv4a", 128, {0, 2, 3}},
@@ -1448,17 +1393,8 @@ int prepare_full_decoder(ian_handle* h) {
   }
   deconv_bwd_tiles(P(h, "dec_conv1.W").data, 512, 512, 512, B);
   if ((rc = upload_gemm_weights(h, F_BWD_CONV1, B, 25, 512, 512, std::vector<float>(512, 1.f), {})) != IAN_OK) return rc;
-  {   // dz[k] = sum_col dfh0[col] * W[k][col], col = hw*512 + c
-    const auto& W = P(h, "l_dec_fc2.W").data;
-    B.assign((size_t)128 * 8192, 0.f);
-    for (int c = 0; c < 512; ++c)
-      for (int hw = 0; hw < 16; ++hw) {
-        const int j = c * 16 + hw, col = hw * 512 + c;
-        for (int k = 0; k < 100; ++k) B[(size_t)k * 8192 + col] = W[(size_t)k * 8192 + j];
-      }
-    if ((rc = upload_gemm_weights(h, F_BWD_FC2, B, 1, 128, 8192, std::vector<float>(128, 1.f), {})) != IAN_OK) return rc;
-  }
-  return IAN_OK;
+  fc2_tiles(P(h, "l_dec_fc2.W").data, 512, true, B);
+  return upload_gemm_weights(h, F_BWD_FC2, B, 1, 128, 8192, std::vector<float>(128, 1.f), {});
 }
 
 // stream memory operations (driver API, fetched through the runtime): the free / pushed flag handshake of the pipelined
@@ -1590,12 +1526,8 @@ int ensure_enc_vjp_weights(ian_handle* h) {
   std::vector<uint16_t> planes(2 * 80 * 128, 0);
   for (int t = 0; t < 25; ++t)
     for (int c = 0; c < 3; ++c)
-      for (int o = 0; o < 128; ++o) {
-        const float w = wt[((size_t)t * 128 + o) * 4 + c];
-        const uint16_t hi = f2bf(w);
-        planes[(t * 3 + c) * 128 + o] = hi;
-        planes[80 * 128 + (t * 3 + c) * 128 + o] = f2bf(w - bf2f(hi));
-      }
+      for (int o = 0; o < 128; ++o)
+        split_hi_lo(wt[((size_t)t * 128 + o) * 4 + c], planes[(t * 3 + c) * 128 + o], planes[80 * 128 + (t * 3 + c) * 128 + o]);
   if (!h->conv1_bwd_tc_wt) {
     CUDA_TRY(h, cudaMalloc((void**)&h->conv1_bwd_tc_wt, planes.size() * 2));
     CUDA_TRY(h, cudaMemcpyAsync(h->conv1_bwd_tc_wt, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice, st));
@@ -1637,24 +1569,8 @@ int ensure_enc_vjp_plan(ian_handle* h, Plan* pl) {
   mask(E_BWD_CONV3, pl->a2, pl->e2);
   set_io(g[E_BWD_CONV2], pl->e2, n, 16, 16, 256, 16, 16, h->w[E_BWD_CONV2], 32, 32); taps_deconv_s2(g[E_BWD_CONV2]);
   mask(E_BWD_CONV2, pl->a1, pl->e1);
-  const std::initializer_list<int> layers = {E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2};
-  mark_splitk_candidates(pl, layers);
-  long long need = 0;
-  for (int l : layers) {
-    char err[256] = {0};
-    pl->maps[l] = tc_build_maps(g[l], err, sizeof(err));
-    if (!pl->maps[l]) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[l], err);
-    if (g[l].ksplit == 0) g[l].ksplit = h->splitk ? choose_ksplit(g[l]) : 1;
-    if (g[l].ksplit > 1) {
-      g[l].ws_slab = (long long)g[l].n_img * g[l].Hout * g[l].Wout * g[l].Cout;
-      need = std::max(need, g[l].ws_slab * g[l].ksplit);
-    }
-  }
-  if (need) {                                           // the chain's own split-K slabs: the plan's other layers keep theirs
-    float* ws = nullptr;
-    if ((rc = alloc_buf(h, pl, ws, need)) != IAN_OK) return rc;
-    for (int l : layers) if (g[l].ksplit > 1) g[l].ws = ws;
-  }
+  // the chain's own split-K slabs: the plan's other layers keep theirs
+  if ((rc = finish_maps(h, pl, kEncoderBwd)) != IAN_OK) return rc;
   {   // both paths: ian_set_path may switch a live handle
     char err[256] = {0};
     pl->conv1_bwd_maps = decout_build_maps(pl->e1.p, pl->e1.plane, n, h->conv1_bwd_tc_wt, 80 * 128, err, sizeof(err));
@@ -1676,11 +1592,12 @@ int run_encode_vjp(ian_handle* h, Plan* pl, const float* x, const float* eps, co
     dzi = pl->edzi;
   }
   LAUNCH_TRY(h, launch_enc_vjp_seed(pl->head, eps, dzi, h->w[L_ENC_HEAD].scale, pl->eh.p, pl->eh.plane, n, st));
-  if ((rc = run_gemm(h, pl, E_BWD_HEAD, st)) != IAN_OK) return rc;
-  LAUNCH_TRY(h, launch_enc_fc1_bwd(pl->eg, pl->f1.p, pl->f1.plane, h->w[L_ENC_FC1].scale, has_flow(h) ? 0 : 1, pl->ef1.p,
-                                   pl->ef1.plane, n, st));
-  for (int l : {E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2})
+  for (int l : kEncoderBwd) {
     if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+    if (l == E_BWD_HEAD)   // enc_fc1's ReLU / ELU derivative between the head's adjoint and enc_fc1's
+      LAUNCH_TRY(h, launch_enc_fc1_bwd(pl->eg, pl->f1.p, pl->f1.plane, h->w[L_ENC_FC1].scale, has_flow(h) ? 0 : 1, pl->ef1.p,
+                                       pl->ef1.plane, n, st));
+  }
   ScopedTimer tm(h, T_CONV1_BWD, st);
   if (h->path == IAN_PATH_TC)
     LAUNCH_TRY(h, launch_conv1_bwd_tc(pl->conv1_bwd_maps, dx, n, st));
@@ -1725,7 +1642,7 @@ int ensure_param_vjp_plan(ian_handle* h, Plan* pl) {
   AP(dh0, N * 16384) AP(dh1, N * 8 * 8 * 512) AP(dh2, N * 16 * 16 * 256) AP(dh3, N * 32 * 32 * 128)
 #undef AP
   if ((rc = alloc_buf(h, pl, pl->pseed, N * 3 * 4096)) != IAN_OK) return rc;
-  const int fwd[4] = {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3};
+  const int* fwd = kSimpleDecoder.fwd.l;
   const Planes* grd[4] = {&pl->d0, &pl->d1, &pl->d2, &pl->d3};
   long long need = 0;
   for (int k = 0; k < 4; ++k) {
@@ -1792,7 +1709,7 @@ int run_param_vjp(ian_handle* h, Plan* pl, const float* dxhat, float* const* out
 // slot of parameter `index` of ian_model_param_spec, or -1 when the parameter VJP does not compute it
 int pv_slot(int model_kind, int index) {
   if (model_kind != IAN_MODEL_SIMPLE) return -1;
-  static const std::vector<Spec> specs = spec_list(IAN_MODEL_SIMPLE);
+  const std::vector<Spec>& specs = cached_specs(IAN_MODEL_SIMPLE);
   if (index < 0 || index >= (int)specs.size()) return -1;
   for (int k = 0; k < PV_COUNT; ++k)
     if (specs[index].name == kPvNames[k]) return k;
@@ -1809,7 +1726,7 @@ int check_param_vjp(ian_handle* h, const float* z, const float* dx_hat, int n, f
   if (n > 0 && (!z || !dx_hat)) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
   for (int k = 0; k < PV_COUNT; ++k) out[k] = nullptr;
   if (!grads) return IAN_OK;
-  static const std::vector<Spec> specs = spec_list(IAN_MODEL_SIMPLE);
+  const std::vector<Spec>& specs = cached_specs(IAN_MODEL_SIMPLE);
   for (int i = 0; i < (int)specs.size(); ++i) {
     if (!grads[i]) continue;
     const int k = pv_slot(h->model_kind, i);
@@ -1817,6 +1734,240 @@ int check_param_vjp(ian_handle* h, const float* z, const float* dx_hat, int n, f
     out[k] = grads[i];
   }
   return IAN_OK;
+}
+
+// the host form's set-up of a plan: the handle's gradient buffers (first call), then the plan's
+int prepare_param_vjp_host(ian_handle* h, Plan* pl) {
+  for (int k = 0; k < PV_COUNT; ++k)
+    if (!h->pv_dev[k]) CUDA_TRY(h, cudaMalloc((void**)&h->pv_dev[k], (size_t)kPvSize[k] * 4));
+  return ensure_param_vjp_plan(h, pl);
+}
+
+// name and shape of a parameter against the model's list; *elems: its element count
+int check_param_shape(ian_handle* h, const char* name, const int64_t* shape, int ndim, int64_t* elems) {
+  const Spec* spec = nullptr;
+  for (const auto& sp : cached_specs(h->model_kind))
+    if (sp.name == name) spec = &sp;
+  if (!spec) return fail(h, IAN_ERR_INVALID, "unknown parameter name '%s'", name);
+  if (ndim != (int)spec->shape.size()) return fail(h, IAN_ERR_INVALID, "parameter %s: expected %d dims, got %d", name, (int)spec->shape.size(), ndim);
+  *elems = 1;
+  for (int i = 0; i < ndim; ++i) {
+    if (shape[i] != spec->shape[i])
+      return fail(h, IAN_ERR_INVALID, "parameter %s: shape mismatch at dim %d (expected %lld, got %lld)", name, i,
+                  (long long)spec->shape[i], (long long)shape[i]);
+    *elems *= shape[i];
+  }
+  return IAN_OK;
+}
+
+// ---- the two forms of an entry point --------------------------------------------------------------
+// Each batch entry point is one body over one chunk's device pointers, which run_entry runs in two forms:
+//   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
+//   host form (ian_*_host): per chunk, the caller's inputs are copied into plan buffers, the body runs on those, its kernel
+//   chain (Chunk::graphed) replayed as a CUDA graph on small plans, the outputs are copied back; then one synchronise.
+enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ };
+void* stage_buf(Plan* pl, int s) {
+  switch (s) {
+    case S_X: return pl->x;
+    case S_EPS: return pl->eps;
+    case S_Z: return pl->z;
+    case S_XHAT: return pl->xhat;
+    case S_BOXES: return pl->boxes;
+    case S_TARGET: return pl->target;
+    default: return pl->edz;
+  }
+}
+enum { IN = 1, OUT = 2, INOUT = 3 };
+struct Arg {              // one per-sample tensor of an entry point
+  const void* user;       // the caller's pointer; nullptr: an optional tensor left out
+  size_t bytes;           // per sample
+  int stage;              // StageBuf: its plan buffer in the host form
+  int dir;                // IN, OUT or INOUT
+};
+
+struct Chunk {
+  ian_handle* h;
+  Plan* pl;
+  int off, cn;
+  cudaStream_t st;
+  bool host;
+  void* p[4];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
+  float* f(int i) const { return (float*)p[i]; }
+  const int32_t* i32(int i) const { return (const int32_t*)p[i]; }
+  // a kernel chain: replayed from graph `slot` by the host form (run_graphed), launched as is by the device form
+  template <typename F>
+  int graphed(int slot, uint64_t key, F&& chain) const { return host ? run_graphed(h, pl, slot, key, st, chain) : chain(); }
+};
+
+// prepare (nullable): per-plan set-up, run before any staging copy because no allocation may happen during a capture
+template <typename Body>
+int run_entry(ian_handle* h, bool host, void* stream, int n, std::initializer_list<Arg> args, int (*prepare)(ian_handle*, Plan*),
+              Body&& body) {
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  const int rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    int r = prepare ? prepare(h, pl) : (int)IAN_OK;
+    if (r != IAN_OK) return r;
+    Chunk c{h, pl, off, cn, st, host, {}};
+    int i = 0;
+    for (const Arg& a : args) {
+      char* u = a.user ? (char*)a.user + (size_t)off * a.bytes : nullptr;
+      void* p = !host ? u : (u || a.dir != IN) ? stage_buf(pl, a.stage) : nullptr;
+      if (host && u && (a.dir & IN)) CUDA_TRY(h, cudaMemcpyAsync(p, u, (size_t)cn * a.bytes, cudaMemcpyHostToDevice, st));
+      c.p[i++] = p;
+    }
+    if ((r = body(c)) != IAN_OK) return r;
+    i = 0;
+    for (const Arg& a : args) {
+      void* p = c.p[i++];
+      if (host && a.user && (a.dir & OUT))
+        CUDA_TRY(h, cudaMemcpyAsync((char*)a.user + (size_t)off * a.bytes, p, (size_t)cn * a.bytes, cudaMemcpyDeviceToHost, st));
+    }
+    return (int)IAN_OK;
+  });
+  if (rc != IAN_OK || !host) return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+constexpr size_t kImageBytes = 12288 * 4, kLatentBytes = 400;
+
+// dz: columns 0..99 of gpad (n,128), a pitched copy (no box, so no empty-box NaN rule)
+int copy_dz(const Chunk& c, float* dz) {
+  if (dz)
+    CUDA_TRY(c.h, cudaMemcpy2DAsync(dz + (size_t)c.off * 100, 400, c.pl->gpad, 512, 400, c.cn,
+                                    c.host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c.st));
+  return IAN_OK;
+}
+
+int call_encode(ian_handle* h, bool host, const float* x, int n, const float* eps, float* z, void* stream) {
+  int rc = check_ready(h, n, x, z);
+  if (rc != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {eps, kLatentBytes, S_EPS, IN}, {z, kLatentBytes, S_Z, OUT}},
+                   nullptr, [&](const Chunk& c) {
+    return c.graphed(eps ? Plan::G_ENCODE_EPS : Plan::G_ENCODE, 0,
+                     [&] { return run_encode(h, c.pl, c.f(0), c.f(1), c.f(2), c.st); });
+  });
+}
+
+int call_decode(ian_handle* h, bool host, const float* z, int n, float* x, void* stream) {
+  int rc = check_ready(h, n, z, x);
+  if (rc != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_XHAT, OUT}}, nullptr,
+                   [&](const Chunk& c) {
+    return c.graphed(Plan::G_DECODE, 0, [&] { return run_decode(h, c.pl, c.f(0), c.f(1), c.st); });
+  });
+}
+
+int call_reconstruct(ian_handle* h, bool host, const float* x, int n, float* z_out, float* x_hat, void* stream) {
+  int rc = check_ready(h, n, x, x_hat);
+  if (rc != IAN_OK) return rc;
+  return run_entry(h, host, stream, n,
+                   {{x, kImageBytes, S_X, IN}, {z_out, kLatentBytes, S_Z, OUT}, {x_hat, kImageBytes, S_XHAT, OUT}}, nullptr,
+                   [&](const Chunk& c) {
+    return c.graphed(Plan::G_RECON, 0, [&] {
+      int q = run_encode(h, c.pl, c.f(0), nullptr, c.f(1), c.st);
+      return q != IAN_OK ? q : run_decode_from_planes(h, c.pl, c.f(2), c.st);
+    });
+  });
+}
+
+int call_grad(ian_handle* h, bool host, const float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
+              float* g, void* stream) {
+  int rc = check_ready(h, n, z, g);
+  if (rc != IAN_OK) return rc;
+  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
+  if (host && (rc = validate_boxes(h, boxes, n)) != IAN_OK) return rc;
+  const size_t tbytes = (target_is_frame ? 12288 : 3) * 4;
+  // the host form stages g in z's buffer
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {boxes, 16, S_BOXES, IN}, {target, tbytes, S_TARGET, IN},
+                                        {g, kLatentBytes, S_Z, OUT}}, nullptr, [&](const Chunk& c) {
+    return c.graphed(Plan::G_GRAD, (target ? 1 : 0) + (target_is_frame ? 2 : 0), [&] {
+      LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+      int q = run_grad_core(h, c.pl, c.i32(1), c.f(2), target_is_frame, nullptr, c.st);
+      if (q != IAN_OK) return q;
+      LAUNCH_TRY(h, launch_brush_update(c.pl->gpad, c.i32(1), 0.f, c.f(3), nullptr, nullptr, 0, c.cn, c.st));
+      return (int)IAN_OK;
+    });
+  });
+}
+
+// The brush gradient's kernels with the dense seed (run_grad_core, dxhat set); the host form stages the cotangent in the
+// plan's frame-target buffer (n,3,64,64).
+int call_decode_vjp(ian_handle* h, bool host, const float* z, const float* dx_hat, int n, float* dz, void* stream) {
+  int rc = check_ready(h, n, z, dz);
+  if (rc != IAN_OK) return rc;
+  if (!dx_hat) return fail(h, IAN_ERR_INVALID, "dx_hat is NULL");
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {dx_hat, kImageBytes, S_TARGET, IN}}, nullptr,
+                   [&](const Chunk& c) {
+    int r = c.graphed(Plan::G_VJP, 0, [&] {
+      LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+      return run_grad_core(h, c.pl, nullptr, nullptr, 0, c.f(1), c.st);
+    });
+    return r != IAN_OK ? r : copy_dz(c, dz);
+  });
+}
+
+// The host form computes every gradient into the handle's device buffers (allocated on the first call), so a captured graph
+// does not depend on which ones the caller asked for; the requested ones are copied out after the last chunk.
+int call_param_vjp(ian_handle* h, bool host, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                   void* stream) {
+  float* req[PV_COUNT];
+  int rc = check_param_vjp(h, z, dx_hat, n, grads, req);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {dx_hat, kImageBytes, S_TARGET, IN}},
+                   host ? prepare_param_vjp_host : ensure_param_vjp_plan, [&](const Chunk& c) {
+    const int accumulate = c.off > 0;
+    int r = c.graphed(Plan::G_PARAM_VJP, accumulate, [&] {
+      LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+      return run_param_vjp(h, c.pl, c.f(1), host ? h->pv_dev : req, accumulate, c.st);
+    });
+    if (r == IAN_OK) r = copy_dz(c, dz);
+    if (r != IAN_OK || !host || c.off + c.cn < n) return r;
+    for (int k = 0; k < PV_COUNT; ++k)
+      if (req[k]) CUDA_TRY(h, cudaMemcpyAsync(req[k], h->pv_dev[k], (size_t)kPvSize[k] * 4, cudaMemcpyDeviceToHost, c.st));
+    return (int)IAN_OK;
+  });
+}
+
+// The first call on a handle permutes the backward weight tiles; the first call on a plan allocates its gradient planes
+// and tensor maps (about 1 MB per image).  Both happen before any graph capture; handles and plans that never call these
+// keep their memory as it was.  The host form stages dz in the plan's edz buffer and dx in its x_hat buffer.
+int call_encode_vjp(ian_handle* h, bool host, const float* x, int n, const float* eps, const float* dz, float* dx, void* stream) {
+  int rc = check_ready(h, n, x, dx);
+  if (rc != IAN_OK) return rc;
+  if (!dz) return fail(h, IAN_ERR_INVALID, "dz is NULL");
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {eps, kLatentBytes, S_EPS, IN}, {dz, kLatentBytes, S_EDZ, IN},
+                                        {dx, kImageBytes, S_XHAT, OUT}}, ensure_enc_vjp_plan, [&](const Chunk& c) {
+    return c.graphed(Plan::G_ENC_VJP, eps ? 1 : 0,
+                     [&] { return run_encode_vjp(h, c.pl, c.f(0), c.f(1), c.f(2), c.f(3), c.st); });
+  });
+}
+
+// The host form captures one paint step and replays it n_steps times; its key holds the weight's bits.
+int call_edit_loop(ian_handle* h, bool host, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
+                   int n_steps, float weight, void* stream) {
+  int rc = check_ready(h, n, z, z);
+  if (rc != IAN_OK) return rc;
+  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
+  if (!host && n_steps < 0) return fail(h, IAN_ERR_INVALID, "n_steps < 0");
+  if (host && (rc = validate_boxes(h, boxes, n)) != IAN_OK) return rc;
+  const size_t tbytes = (target_is_frame ? 12288 : 3) * 4;
+  const uint64_t key = float_bits(weight) * 4 + (target ? 1 : 0) + (target_is_frame ? 2 : 0);
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, INOUT}, {boxes, 16, S_BOXES, IN}, {target, tbytes, S_TARGET, IN}},
+                   nullptr, [&](const Chunk& c) {
+    LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+    for (int s = 0; s < n_steps; ++s) {
+      int r = c.graphed(Plan::G_EDIT_STEP, key, [&] {
+        int q = run_grad_core(h, c.pl, c.i32(1), c.f(2), target_is_frame, nullptr, c.st);
+        if (q != IAN_OK) return q;
+        LAUNCH_TRY(h, launch_brush_update(c.pl->gpad, c.i32(1), weight, nullptr, c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+        return (int)IAN_OK;
+      });
+      if (r != IAN_OK) return r;
+    }
+    return (int)IAN_OK;
+  });
 }
 
 }  // namespace
@@ -1863,19 +2014,9 @@ int ian_create(int model_kind, int device, ian_handle** out) {
 int ian_set_param(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim) {
   if (!h || !name || !data || !shape) return fail(h, IAN_ERR_INVALID, "NULL argument");
   if (h->finalized) return fail(h, IAN_ERR_STATE, "model already finalized");
-  const std::vector<Spec> specs = spec_list(h->model_kind);
-  const Spec* spec = nullptr;
-  for (const auto& sp : specs)
-    if (sp.name == name) spec = &sp;
-  if (!spec) return fail(h, IAN_ERR_INVALID, "unknown parameter name '%s'", name);
-  if (ndim != (int)spec->shape.size()) return fail(h, IAN_ERR_INVALID, "parameter %s: expected %d dims, got %d", name, (int)spec->shape.size(), ndim);
-  int64_t elems = 1;
-  for (int i = 0; i < ndim; ++i) {
-    if (shape[i] != spec->shape[i])
-      return fail(h, IAN_ERR_INVALID, "parameter %s: shape mismatch at dim %d (expected %lld, got %lld)", name, i,
-                  (long long)spec->shape[i], (long long)shape[i]);
-    elems *= shape[i];
-  }
+  int64_t elems = 0;
+  int rc = check_param_shape(h, name, shape, ndim, &elems);
+  if (rc != IAN_OK) return rc;
   HostParam& p = h->params[name];
   p.shape.assign(shape, shape + ndim);
   p.data.assign(data, data + elems);
@@ -1898,13 +2039,6 @@ int ian_set_made_ordering(ian_handle* h, const int32_t* ordering, int n) {
 // The model's OWN parameter list: what `lasagne.layers.get_all_params(...)` hands GANcheckpoints.load_weights in the
 // reference (API.py:23-30).  A loader iterates these names and looks each one up in the checkpoint, so that extra keys
 // of the file (log_sigma_theta, discriminator weights, metadata ...) are ignored exactly as the reference does.
-static const std::vector<Spec>& cached_specs(int kind) {
-  static std::vector<Spec> cache[3];
-  static bool built[3] = {false, false, false};
-  if (!built[kind]) { cache[kind] = spec_list(kind); built[kind] = true; }
-  return cache[kind];
-}
-
 int ian_model_param_count(int model_kind) {
   if (model_kind < 0 || model_kind > 2) return IAN_ERR_INVALID;
   return (int)cached_specs(model_kind).size();
@@ -1938,7 +2072,7 @@ int ian_debug_made_weights(ian_handle* h, float* out /*[2][3][100][100]*/) {
 int ian_finalize(ian_handle* h) {
   if (!h) return IAN_ERR_INVALID;
   if (h->finalized) return IAN_OK;
-  for (const auto& sp : spec_list(h->model_kind))
+  for (const auto& sp : cached_specs(h->model_kind))
     if (!h->params.count(sp.name)) return fail(h, IAN_ERR_STATE, "missing parameter '%s'", sp.name.c_str());
   DeviceGuard dg(h->device);
   int rc = prepare_encoder(h);
@@ -2031,240 +2165,6 @@ double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset) {
   return -1.0;
 }
 
-// ---- encode ---------------------------------------------------------------------------------------
-int ian_encode_dev(ian_handle* h, const float* x, int n, const float* eps, float* z, void* stream) {
-  int rc = check_ready(h, n, x, z);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int) {
-    return run_encode(h, pl, x + (size_t)off * 12288, eps ? eps + (size_t)off * 100 : nullptr, z + (size_t)off * 100, st);
-  });
-}
-
-int ian_encode_host(ian_handle* h, const float* x, int n, const float* eps, float* z) {
-  int rc = check_ready(h, n, x, z);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->x, x + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    if (eps) CUDA_TRY(h, cudaMemcpyAsync(pl->eps, eps + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    int r = run_graphed(h, pl, eps ? Plan::G_ENCODE_EPS : Plan::G_ENCODE, 0, st,
-                        [&] { return run_encode(h, pl, pl->x, eps ? pl->eps : nullptr, pl->z, st); });
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(z + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
-// ---- decode ---------------------------------------------------------------------------------------
-int ian_decode_dev(ian_handle* h, const float* z, int n, float* x, void* stream) {
-  int rc = check_ready(h, n, z, x);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int) {
-    return run_decode(h, pl, z + (size_t)off * 100, x + (size_t)off * 12288, st);
-  });
-}
-
-int ian_decode_host(ian_handle* h, const float* z, int n, float* x) {
-  int rc = check_ready(h, n, z, x);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    int r = run_graphed(h, pl, Plan::G_DECODE, 0, st, [&] { return run_decode(h, pl, pl->z, pl->xhat, st); });
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(x + (size_t)off * 12288, pl->xhat, (size_t)cn * 12288 * 4, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
-// ---- encode -> decode -----------------------------------------------------------------------------
-int ian_reconstruct_dev(ian_handle* h, const float* x, int n, float* z_out, float* x_hat, void* stream) {
-  int rc = check_ready(h, n, x, x_hat);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int) {
-    int r = run_encode(h, pl, x + (size_t)off * 12288, nullptr, z_out ? z_out + (size_t)off * 100 : nullptr, st);
-    if (r != IAN_OK) return r;
-    return run_decode_from_planes(h, pl, x_hat + (size_t)off * 12288, st);
-  });
-}
-
-int ian_reconstruct_host(ian_handle* h, const float* x, int n, float* z_out, float* x_hat) {
-  int rc = check_ready(h, n, x, x_hat);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->x, x + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    int r = run_graphed(h, pl, Plan::G_RECON, 0, st, [&] {
-      int q = run_encode(h, pl, pl->x, nullptr, pl->z, st);
-      return q != IAN_OK ? q : run_decode_from_planes(h, pl, pl->xhat, st);
-    });
-    if (r != IAN_OK) return r;
-    if (z_out) CUDA_TRY(h, cudaMemcpyAsync(z_out + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(h, cudaMemcpyAsync(x_hat + (size_t)off * 12288, pl->xhat, (size_t)cn * 12288 * 4, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
-// ---- brush gradient -------------------------------------------------------------------------------
-int ian_grad_dev(ian_handle* h, const float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
-                 float* g, void* stream) {
-  int rc = check_ready(h, n, z, g);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  const size_t tstride = target_is_frame ? 12288 : 3;
-  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
-    int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, nullptr, st);
-    if (r != IAN_OK) return r;
-    LAUNCH_TRY(h, launch_brush_update(pl->gpad, boxes + (size_t)off * 4, 0.f, g + (size_t)off * 100, nullptr, nullptr, 0, cn, st));
-    return (int)IAN_OK;
-  });
-}
-
-int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
-                  float* g) {
-  int rc = check_ready(h, n, z, g);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
-  if ((rc = validate_boxes(h, boxes, n)) != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  const size_t tstride = target_is_frame ? 12288 : 3;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(h, cudaMemcpyAsync(pl->boxes, boxes + (size_t)off * 4, (size_t)cn * 16, cudaMemcpyHostToDevice, st));
-    if (target) CUDA_TRY(h, cudaMemcpyAsync(pl->target, target + off * tstride, cn * tstride * 4, cudaMemcpyHostToDevice, st));
-    int r = run_graphed(h, pl, Plan::G_GRAD, (target ? 1 : 0) + (target_is_frame ? 2 : 0), st, [&] {
-      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-      int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, nullptr, st);
-      if (q != IAN_OK) return q;
-      LAUNCH_TRY(h, launch_brush_update(pl->gpad, pl->boxes, 0.f, pl->z /*reuse as g staging*/, nullptr, nullptr, 0, cn, st));
-      return (int)IAN_OK;
-    });
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(g + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
-// ---- decoder vector-Jacobian product --------------------------------------------------------------
-// The brush gradient's kernels with the dense seed (run_grad_core, dxhat set); dz is columns 0..99 of gpad (n,128), a
-// strided copy (no box, so no empty-box NaN rule).
-int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream) {
-  int rc = check_ready(h, n, z, dz);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!dx_hat) return fail(h, IAN_ERR_INVALID, "dx_hat is NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
-    int r = run_grad_core(h, pl, nullptr, nullptr, 0, dx_hat + (size_t)off * 12288, st);
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToDevice, st));
-    return (int)IAN_OK;
-  });
-}
-
-int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz) {
-  int rc = check_ready(h, n, z, dz);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!dx_hat) return fail(h, IAN_ERR_INVALID, "dx_hat is NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    // the plan's frame-target buffer (n,3,64,64) stages the cotangent
-    CUDA_TRY(h, cudaMemcpyAsync(pl->target, dx_hat + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    int r = run_graphed(h, pl, Plan::G_VJP, 0, st, [&] {
-      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-      return run_grad_core(h, pl, nullptr, nullptr, 0, pl->target, st);
-    });
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
-// ---- decoder parameter vector-Jacobian product (IAN_simple) -----------------------------------------------
-int ian_param_vjp_supported(int model_kind, int index) { return pv_slot(model_kind, index) >= 0 ? 1 : 0; }
-
-int ian_decode_param_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
-                             void* stream) {
-  float* out[PV_COUNT];
-  int rc = check_param_vjp(h, z, dx_hat, n, grads, out);
-  if (rc != IAN_OK || n == 0) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    int r = ensure_param_vjp_plan(h, pl);
-    if (r != IAN_OK) return r;
-    LAUNCH_TRY(h, launch_z_to_planes(z + (size_t)off * 100, pl->zp.p, pl->zp.plane, cn, st));
-    if ((r = run_param_vjp(h, pl, dx_hat + (size_t)off * 12288, out, off > 0, st)) != IAN_OK) return r;
-    if (dz) CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToDevice, st));
-    return (int)IAN_OK;
-  });
-}
-
-// Every gradient is computed into the handle's device buffers (allocated on the first call), so a captured graph does not
-// depend on which ones the caller asked for; the requested ones are copied out.
-int ian_decode_param_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads) {
-  float* req[PV_COUNT];
-  int rc = check_param_vjp(h, z, dx_hat, n, grads, req);
-  if (rc != IAN_OK || n == 0) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  for (int k = 0; k < PV_COUNT; ++k)
-    if (!h->pv_dev[k]) CUDA_TRY(h, cudaMalloc((void**)&h->pv_dev[k], (size_t)kPvSize[k] * 4));
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    int r = ensure_param_vjp_plan(h, pl);
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(h, cudaMemcpyAsync(pl->target, dx_hat + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    r = run_graphed(h, pl, Plan::G_PARAM_VJP, off > 0 ? 1 : 0, st, [&] {
-      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-      return run_param_vjp(h, pl, pl->target, h->pv_dev, off > 0, st);
-    });
-    if (r != IAN_OK) return r;
-    if (dz) CUDA_TRY(h, cudaMemcpy2DAsync(dz + (size_t)off * 100, 400, pl->gpad, 512, 400, cn, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  for (int k = 0; k < PV_COUNT; ++k)
-    if (req[k]) CUDA_TRY(h, cudaMemcpyAsync(req[k], h->pv_dev[k], (size_t)kPvSize[k] * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
-}
-
 // Replace one IAN_simple decoder parameter of a finalized handle: re-derive what ian_finalize derives from its group and
 // write it into the same device buffers (tiles of both directions, dec_out's two weight forms, folded BatchNorm vectors).
 // The device is synchronised first, so the update is ordered after all work enqueued before the call.
@@ -2281,17 +2181,9 @@ int ian_update_param_host(ian_handle* h, const char* name, const float* data, co
     for (int f = 0; f < 4; ++f)
       if (n == std::string(kDecBn[k]) + "." + kBnFields[f]) { group = 5; bn = k; field = f; }
   if (group < 0) return fail(h, IAN_ERR_INVALID, "'%s' is not an IAN_simple decoder parameter that can be updated", name);
-  const std::vector<Spec> specs = spec_list(h->model_kind);
-  const Spec* spec = nullptr;
-  for (const auto& sp : specs) if (sp.name == n) spec = &sp;
-  if (ndim != (int)spec->shape.size()) return fail(h, IAN_ERR_INVALID, "parameter %s: expected %d dims, got %d", name, (int)spec->shape.size(), ndim);
-  int64_t elems = 1;
-  for (int i = 0; i < ndim; ++i) {
-    if (shape[i] != spec->shape[i])
-      return fail(h, IAN_ERR_INVALID, "parameter %s: shape mismatch at dim %d (expected %lld, got %lld)", name, i,
-                  (long long)spec->shape[i], (long long)shape[i]);
-    elems *= shape[i];
-  }
+  int64_t elems = 0;
+  int rc = check_param_shape(h, name, shape, ndim, &elems);
+  if (rc != IAN_OK) return rc;
   DeviceGuard dg(h->device);
   CUDA_TRY(h, cudaDeviceSynchronize());
   const std::vector<float> v(data, data + elems);
@@ -2302,104 +2194,64 @@ int ian_update_param_host(ian_handle* h, const char* name, const float* data, co
   return simple_bn(h, bn);
 }
 
-// ---- encoder vector-Jacobian product --------------------------------------------------------------
-// The first call on a handle permutes the backward weight tiles; the first call on a plan allocates its gradient planes
-// and tensor maps (about 1 MB per image).  Both happen before any graph capture; handles and plans that never call these
-// keep their memory as it was.
+// ---- batch entry points: one body each (call_*), in the device and the host form ---------------------------------
+int ian_encode_dev(ian_handle* h, const float* x, int n, const float* eps, float* z, void* stream) {
+  return call_encode(h, false, x, n, eps, z, stream);
+}
+int ian_encode_host(ian_handle* h, const float* x, int n, const float* eps, float* z) {
+  return call_encode(h, true, x, n, eps, z, nullptr);
+}
+
+int ian_decode_dev(ian_handle* h, const float* z, int n, float* x, void* stream) { return call_decode(h, false, z, n, x, stream); }
+int ian_decode_host(ian_handle* h, const float* z, int n, float* x) { return call_decode(h, true, z, n, x, nullptr); }
+
+int ian_reconstruct_dev(ian_handle* h, const float* x, int n, float* z_out, float* x_hat, void* stream) {
+  return call_reconstruct(h, false, x, n, z_out, x_hat, stream);
+}
+int ian_reconstruct_host(ian_handle* h, const float* x, int n, float* z_out, float* x_hat) {
+  return call_reconstruct(h, true, x, n, z_out, x_hat, nullptr);
+}
+
+int ian_grad_dev(ian_handle* h, const float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
+                 float* g, void* stream) {
+  return call_grad(h, false, z, boxes, target, target_is_frame, n, g, stream);
+}
+int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
+                  float* g) {
+  return call_grad(h, true, z, boxes, target, target_is_frame, n, g, nullptr);
+}
+
+int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream) {
+  return call_decode_vjp(h, false, z, dx_hat, n, dz, stream);
+}
+int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz) {
+  return call_decode_vjp(h, true, z, dx_hat, n, dz, nullptr);
+}
+
+int ian_param_vjp_supported(int model_kind, int index) { return pv_slot(model_kind, index) >= 0 ? 1 : 0; }
+int ian_decode_param_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                             void* stream) {
+  return call_param_vjp(h, false, z, dx_hat, n, dz, grads, stream);
+}
+int ian_decode_param_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads) {
+  return call_param_vjp(h, true, z, dx_hat, n, dz, grads, nullptr);
+}
+
 int ian_encode_vjp_dev(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx, void* stream) {
-  int rc = check_ready(h, n, x, dx);
-  if (rc != IAN_OK) return rc;
-  if (!dz) return fail(h, IAN_ERR_INVALID, "dz is NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  return for_chunks(h, n, [&](Plan* pl, int off, int) {
-    int r = ensure_enc_vjp_plan(h, pl);
-    if (r != IAN_OK) return r;
-    return run_encode_vjp(h, pl, x + (size_t)off * 12288, eps ? eps + (size_t)off * 100 : nullptr, dz + (size_t)off * 100,
-                          dx + (size_t)off * 12288, st);
-  });
+  return call_encode_vjp(h, false, x, n, eps, dz, dx, stream);
 }
-
 int ian_encode_vjp_host(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx) {
-  int rc = check_ready(h, n, x, dx);
-  if (rc != IAN_OK) return rc;
-  if (!dz) return fail(h, IAN_ERR_INVALID, "dz is NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    int r = ensure_enc_vjp_plan(h, pl);
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(pl->x, x + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    if (eps) CUDA_TRY(h, cudaMemcpyAsync(pl->eps, eps + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(h, cudaMemcpyAsync(pl->edz, dz + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    // the plan's x_hat buffer (n,3,64,64) stages dx
-    r = run_graphed(h, pl, Plan::G_ENC_VJP, eps ? 1 : 0, st,
-                    [&] { return run_encode_vjp(h, pl, pl->x, eps ? pl->eps : nullptr, pl->edz, pl->xhat, st); });
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(dx + (size_t)off * 12288, pl->xhat, (size_t)cn * 12288 * 4, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
+  return call_encode_vjp(h, true, x, n, eps, dz, dx, nullptr);
 }
 
-// ---- edit loop ------------------------------------------------------------------------------------
 int ian_edit_loop_dev(ian_handle* h, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
                       int n_steps, float weight, void* stream) {
-  int rc = check_ready(h, n, z, z);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
-  if (n_steps < 0) return fail(h, IAN_ERR_INVALID, "n_steps < 0");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  const size_t tstride = target_is_frame ? 12288 : 3;
-  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    float* zc = z + (size_t)off * 100;
-    LAUNCH_TRY(h, launch_z_to_planes(zc, pl->zp.p, pl->zp.plane, cn, st));
-    for (int s = 0; s < n_steps; ++s) {
-      int r = run_grad_core(h, pl, boxes + (size_t)off * 4, target ? target + off * tstride : nullptr, target_is_frame, nullptr, st);
-      if (r != IAN_OK) return r;
-      LAUNCH_TRY(h, launch_brush_update(pl->gpad, boxes + (size_t)off * 4, weight, nullptr, zc, pl->zp.p, pl->zp.plane, cn, st));
-    }
-    return (int)IAN_OK;
-  });
+  return call_edit_loop(h, false, z, boxes, target, target_is_frame, n, n_steps, weight, stream);
 }
-
 int ian_edit_loop_host(ian_handle* h, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
                        int n_steps, float weight) {
-  int rc = check_ready(h, n, z, z);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
-  if (!boxes) return fail(h, IAN_ERR_INVALID, "boxes is NULL");
-  if ((rc = validate_boxes(h, boxes, n)) != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  const size_t tstride = target_is_frame ? 12288 : 3;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->z, z + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(h, cudaMemcpyAsync(pl->boxes, boxes + (size_t)off * 4, (size_t)cn * 16, cudaMemcpyHostToDevice, st));
-    if (target) CUDA_TRY(h, cudaMemcpyAsync(pl->target, target + off * tstride, cn * tstride * 4, cudaMemcpyHostToDevice, st));
-    LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-    const uint64_t key = float_bits(weight) * 4 + (target ? 1 : 0) + (target_is_frame ? 2 : 0);
-    for (int s = 0; s < n_steps; ++s) {                    // one graph = one paint step, replayed n_steps times
-      int r = run_graphed(h, pl, Plan::G_EDIT_STEP, key, st, [&] {
-        int q = run_grad_core(h, pl, pl->boxes, target ? pl->target : nullptr, target_is_frame, nullptr, st);
-        if (q != IAN_OK) return q;
-        LAUNCH_TRY(h, launch_brush_update(pl->gpad, pl->boxes, weight, nullptr, pl->z, pl->zp.p, pl->zp.plane, cn, st));
-        return (int)IAN_OK;
-      });
-      if (r != IAN_OK) return r;
-    }
-    CUDA_TRY(h, cudaMemcpyAsync(z + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
+  return call_edit_loop(h, true, z, boxes, target, target_is_frame, n, n_steps, weight, nullptr);
 }
-
 
 // ---- pipelined host API -----------------------------------------------------------------------------
 int ian_host_alloc(ian_handle* h, size_t bytes, void** out) {
@@ -2741,7 +2593,6 @@ int ian_paint_stroke_host(ian_handle* h, float* z, const int32_t* box, const flo
                           const uint8_t* recon_u8, const float* error, uint8_t* im_u8, uint8_t* display_u8) {
   int rc = check_ready(h, 1, z, rgb_frame);
   if (rc != IAN_OK) return rc;
-  if ((rc = check_brush_supported(h)) != IAN_OK) return rc;
   if (!box || !recon_u8 || !error || !im_u8) return fail(h, IAN_ERR_INVALID, "NULL argument");
   if ((rc = validate_boxes(h, box, 1)) != IAN_OK) return rc;
   DeviceGuard dg(h->device);

@@ -9,8 +9,14 @@
         secondary blocks, with the card name, power limit and sampled SM clock of every run, and compares the
         --dump-outputs arrays (z.npy, xhat.npy of the last timed step) of every build with "base" bit for bit.
         Raw result lines go to DIR/ab_<steps>.jsonl (default DIR: build/ab/results).
+    python tools/ab_builds.py outputs REV
+        runs every batch entry point in its host and its device form (the calls of tests/test_gpu_launch_forms.py) on
+        seeded inputs and synthetic oracle.weights, in one child process per build, and prints per array whether
+        build/ab/<REV> ("base") and the in-tree build ("head") give the same bits: the three graphs; the tensor-core path
+        by default and with IAN_STREAMK=0, IAN_STREAMK=2 and IAN_GRAPHS=0; the SIMT path; batches 1, 3, 47, 130 and 513.
 """
 import argparse
+import hashlib
 import json
 import os
 import shutil
@@ -119,11 +125,67 @@ def cmd_run(args):
             print("outputs %s vs base %s: %s (max abs diff %.3g)" % (name, f, "bit-identical" if same else "DIFFER", diff))
 
 
+OUTPUT_CONFIGS = [("tc", {}), ("tc", {"IAN_STREAMK": "0"}), ("tc", {"IAN_STREAMK": "2"}), ("tc", {"IAN_GRAPHS": "0"}),
+                  ("simt", {})]
+OUTPUT_BATCHES = (1, 3, 47, 130, 513)
+
+
+def cmd_dump(out):
+    """child of `outputs`: sha256 and sum of |a| of every array, for the build IAN_B200_LIB names"""
+    import importlib
+    import numpy as np
+    sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+    import test_gpu_launch_forms as lf
+    npe = importlib.import_module("neural-photo-editor_b200")
+    res = {}
+    for graph in ("simple", "full", "v1"):
+        for path, env in OUTPUT_CONFIGS:
+            for k in lf.ENV:
+                os.environ.pop(k, None)
+            os.environ.update(env)
+            m = npe.IAN(lf.CONFIG[graph], True, weights=lf._weights(graph), path=path)
+            cfg = "%s-%s%s" % (graph, path, "".join("-%s=%s" % kv for kv in env.items()))
+            for n in OUTPUT_BATCHES:
+                for name, host, dev in lf._pairs(m, npe, lf._inputs(n, 7000 + n)):
+                    for form, a in (("host", host), ("dev", dev)):
+                        a = np.ascontiguousarray(a)
+                        res["%s n=%d %s %s" % (cfg, n, name, form)] = [hashlib.sha256(a.tobytes()).hexdigest(), list(a.shape),
+                                                                       float(np.abs(a.astype(np.float64)).sum())]
+            m.close()
+    with open(out, "w") as f:
+        json.dump(res, f)
+
+
+def cmd_outputs(rev):
+    libs = [("base", os.path.join(ab_dir(rev), "libian_b200.so")), ("head", HEAD_LIB)]
+    res = {}
+    with tempfile.TemporaryDirectory(prefix="ian_ab_out_") as tmp:
+        for name, lib in libs:
+            if not os.path.exists(lib):
+                raise SystemExit("missing %s (python tools/ab_builds.py build %s)" % (lib, rev))
+            out = os.path.join(tmp, name + ".json")
+            subprocess.run([sys.executable, os.path.abspath(__file__), "_dump", out], check=True, cwd=ROOT, stdout=subprocess.DEVNULL,
+                           env=dict(os.environ, IAN_B200_LIB=lib))
+            res[name] = json.load(open(out))
+    base, head = res["base"], res["head"]
+    ndiff = 0
+    for key in sorted(set(base) | set(head)):
+        same = key in base and key in head and base[key][:2] == head[key][:2]
+        ndiff += not same
+        print("%-70s %s" % (key, "bit-identical" if same else "DIFFER (sum|a| base %s, head %s)" % (
+            base.get(key, [None] * 3)[2], head.get(key, [None] * 3)[2])))
+    print("\n%d arrays, %d DIFFER (base %s, head in-tree)" % (len(set(base) | set(head)), ndiff, rev))
+    if ndiff:
+        raise SystemExit(1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     sub = ap.add_subparsers(dest="cmd", required=True)
     b = sub.add_parser("build")
     b.add_argument("rev")
+    sub.add_parser("outputs").add_argument("rev")
+    sub.add_parser("_dump").add_argument("out")
     r = sub.add_parser("run")
     r.add_argument("rev")
     r.add_argument("--rounds", type=int, default=3)
@@ -134,6 +196,10 @@ def main():
     a = ap.parse_args()
     if a.cmd == "build":
         cmd_build(a.rev)
+    elif a.cmd == "outputs":
+        cmd_outputs(a.rev)
+    elif a.cmd == "_dump":
+        cmd_dump(a.out)
     else:
         cmd_run(a)
 
