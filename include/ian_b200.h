@@ -211,6 +211,22 @@ int ian_grad_host(ian_handle* h, const float* z, const int32_t* boxes, const flo
 int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, void* stream);
 int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz);
 
+/* ---- decoder Jacobian-vector product: forward mode through the decoder from l_Z (reference API.py:46) ----------------
+ *   dx_hat = (d x_hat / d z) . v
+ * z, v (n,100); dx_hat (n,3,64,64) float32 NCHW; x_hat (n,3,64,64) nullable: receives ian_decode_*(z) bit for bit.  On
+ * IAN.py / IANv1.py z is the decoder's input l_Z, as for ian_decode_* and ian_decode_vjp_* (no MADE/IAF).  One batch-100 call
+ * with the identity as v gives the 100 columns of the decoder's Jacobian at one latent.  Recomputes the forward; the tangent
+ * chain runs the forward's tap-GEMMs on tangent planes.  The derivative conventions are the decoder VJP's (rectify: h > 0;
+ * LeakyRectify: the sign of the stored activation, slope 0.2; tanh: 1 - x_hat^2 from the float32 x_hat; the RGB-Beta head's
+ * sigmoid and Beta-layer expressions), so <u, JVP(v)> = <ian_decode_vjp_*(u), v> up to float32 summation, also on samples
+ * at a rectifier kink.  All three graphs, both paths; bf16 precision on the flow graphs as for ian_decode_vjp_*.
+ * n == 0 does nothing; n < 0 or a NULL z, v or dx_hat -> IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE.  Deterministic
+ * (a repeated call is bit-identical).  The first call per batch size allocates that plan's tangent planes, maps and
+ * split-K slabs: about 1.0 MB per image on IAN_simple, 3.2 MB on IANv1.py and 5.9 MB on IAN.py; plans that never call
+ * it keep their memory. */
+int ian_decode_jvp_dev(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat, void* stream);
+int ian_decode_jvp_host(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -288,8 +304,10 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * `layer_name` ("enc_conv2", "dec_conv1", ...; the encoder VJP's "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4",
  * "bwd_enc_conv3", "bwd_enc_conv2"; "enc_conv1", "dec_out", "brush_seed" -- the loss-seed kernel of the brush gradients
  * and of ian_decode_vjp_* -- "enc_conv1_bwd" -- enc_conv1's adjoint in ian_encode_vjp_* -- for the edge kernels; "wgrad_l_dec_fc2", "wgrad_dec_conv1",
- * "wgrad_dec_conv2", "wgrad_dec_conv3" and "wgrad_dec_out" for the weight gradients of ian_decode_param_vjp_*) over
- * the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * "wgrad_dec_conv2", "wgrad_dec_conv3" and "wgrad_dec_out" for the weight gradients of ian_decode_param_vjp_*; in
+ * ian_decode_jvp_* "jvp_<layer>" for the tangent tap-GEMM of each decoder forward layer -- "jvp_l_dec_fc2", "jvp_dec_conv1",
+ * "jvp_full_dec_conv1", "jvp_dec_conv2a2", ... -- plus "dec_out_jvp" (IAN_simple) and "rgb_head_jvp" (the head's three
+ * convolutions on the tangent of its feature map, IAN.py / IANv1.py)) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

@@ -9,7 +9,8 @@ no CPU fallback.
 
 Extensions beyond the reference surface (SURVEY.md section 8b): `reconstruct`, `encode(..., eps)`,
 batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space loss (torch autograd binding:
-`torch_ops.decode`), the encoder VJP `encode_vjp` for any loss on the latent (torch autograd binding:
+`torch_ops.decode`), the decoder JVP `decode_jvp` and the Jacobian `decoder_jacobian` (torch forward-mode binding:
+`torch_ops.decode` under `torch.autograd.forward_ad`), the encoder VJP `encode_vjp` for any loss on the latent (torch autograd binding:
 `torch_ops.encode`), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
@@ -402,6 +403,36 @@ class IAN:
             self._check(self._lib.ian_decode_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz)))
         return dz
 
+    def decode_jvp(self, z, v, return_x_hat=False):
+        """Jacobian-vector product of the decoder, dx_hat = (d x_hat / d z) . v -- how the image moves when z moves along v:
+        z, v float32 (n,100) -> dx_hat float32 (n,3,64,64), and x_hat = sample_at(z) bit for bit when return_x_hat
+        (returned as (x_hat, dx_hat)).  Forward mode: one decoder forward and one tangent pass.  Its derivative conventions
+        are decode_vjp's, so <u, decode_jvp(z, v)> = <decode_vjp(z, u), v> up to float32 summation."""
+        z = _z(z)
+        v = _z(v, 'v')
+        n = z.shape[0]
+        if v.shape[0] != n:
+            raise ValueError("v must be (%d,100), got %r" % (n, v.shape))
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        xh = np.empty((n, 3, 64, 64), np.float32) if return_x_hat else None
+        if n:
+            self._check(self._lib.ian_decode_jvp_host(self._h, _fp(z), _fp(v), n, _fp(xh) if xh is not None else None, _fp(dx)))
+        return (xh, dx) if return_x_hat else dx
+
+    def decoder_jacobian(self, z):
+        """The decoder's Jacobian at each latent: z float32 (n,100) -> J float32 (n,100,3,64,64) with J[k, i] = d x_hat /
+        d z_i at z[k], i.e. J's 100 columns as images (NPE's latent canvas shows what each coordinate does to the picture;
+        J^T J is the pull-back metric, and Gauss-Newton steps fitting z to a photo need J).  One batch-100 decode_jvp with
+        the identity as tangents per row of z."""
+        z = _z(z)
+        n = z.shape[0]
+        J = np.empty((n, 100, 3, 64, 64), np.float32)
+        eye = np.eye(100, dtype=np.float32)
+        for k in range(n):
+            zk = np.ascontiguousarray(np.broadcast_to(z[k], (100, 100)))
+            self._check(self._lib.ian_decode_jvp_host(self._h, _fp(zk), _fp(eye), 100, None, _fp(J[k])))
+        return J
+
     def param_vjp_names(self):
         """names of the parameters decode_param_vjp returns gradients for, in ian_model_param_spec order: on IAN_simple
         the 13 tensors of train_IAN_simple.py:353 (`decoder_params`); empty on IAN.py / IANv1.py."""
@@ -575,6 +606,10 @@ class IAN:
 
     def decode_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, stream=0):
         self._check(self._lib.ian_decode_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr, stream or None))
+
+    def decode_jvp_dev(self, z_ptr, v_ptr, n, dx_ptr, xhat_ptr=0, stream=0):
+        """device-pointer form of decode_jvp; xhat_ptr may be 0"""
+        self._check(self._lib.ian_decode_jvp_dev(self._h, z_ptr, v_ptr, int(n), xhat_ptr or None, dx_ptr, stream or None))
 
     def decode_param_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, grad_ptrs, stream=0):
         """device-pointer form of decode_param_vjp: grad_ptrs {name: device pointer} (any subset of param_vjp_names()),

@@ -52,8 +52,11 @@ constexpr int kItemsPerImage = 16;           // 32 input rows / 2 interior rows 
 
 // kTanh = false (conv1_bwd_tc_kernel): the same GEMM + col2im with an identity epilogue.  enc_conv1's adjoint (3 <- 128
 // channels, 64x64 <- 32x32, stride 2, pad 2) is this transposed convolution on the tap-flipped conv1 weights.
-template <bool kTanh>
-__device__ __forceinline__ void decout_tc_body(const DecOutMaps& maps, const DecOutDst& dst, const int n_img) {
+// kJvp (decout_jvp_tc_kernel, the decoder JVP): the GEMM + col2im on the tangent planes of h3, then the tanh derivative
+// from the primal x_hat (xprim, dst's layout): dx_hat = y * (1 - x_hat^2).
+template <bool kTanh, bool kJvp = false>
+__device__ __forceinline__ void decout_tc_body(const DecOutMaps& maps, const DecOutDst& dst, const int n_img,
+                                               const float* __restrict__ xprim = nullptr) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -108,6 +111,11 @@ __device__ __forceinline__ void decout_tc_body(const DecOutMaps& maps, const Dec
   uint32_t i = 0;
   for (int w = blockIdx.x; w < total; w += gridDim.x) {
     const int n = w / kItemsPerImage, p0 = (w % kItemsPerImage) * 2;
+    float xp[3] = {0.f, 0.f, 0.f};                       // kJvp: the primal x_hat, loaded while the MMAs run
+    if (kJvp) {
+      const float* x = xprim + ((long long)n * 3 * 64 + (2 * p0 + ur)) * 64 + v;
+      xp[0] = x[0]; xp[1] = x[4096]; xp[2] = x[8192];
+    }
     float am[BN / 2], ac[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) { am[j] = 0.f; ac[j] = 0.f; }
@@ -159,6 +167,11 @@ __device__ __forceinline__ void decout_tc_body(const DecOutMaps& maps, const Dec
       }
     }
     const long long off = ((long long)n * 3 * 64 + (2 * p0 + ur)) * 64 + v;
+    if (kJvp) {
+      a0 *= 1.f - xp[0] * xp[0];
+      a1 *= 1.f - xp[1] * xp[1];
+      a2 *= 1.f - xp[2] * xp[2];
+    }
     const float y0 = kTanh ? tanhf(a0) : a0, y1 = kTanh ? tanhf(a1) : a1, y2 = kTanh ? tanhf(a2) : a2;
     for (int d = 0; d < dst.n; ++d) {                  // d > 0: peer GPUs' gather buffers (st.global over NVLink)
       float* o = dst.base[d] + off;
@@ -180,6 +193,13 @@ decout_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant_
 __global__ void __launch_bounds__(kThreads, 1)
 conv1_bwd_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant__ DecOutDst dst, const int n_img) {
   decout_tc_body<false>(maps, dst, n_img);
+}
+
+// decoder JVP: maps.a = the tangent planes of h3, maps.b = dec_out's weights; xhat = the primal output (n,3,64,64)
+__global__ void __launch_bounds__(kThreads, 1)
+decout_jvp_tc_kernel(const __grid_constant__ DecOutMaps maps, const __grid_constant__ DecOutDst dst, const int n_img,
+                     const float* __restrict__ xhat) {
+  decout_tc_body<false, true>(maps, dst, n_img, xhat);
 }
 
 // ---- cross-GPU barrier over peer memory: every rank owns flags[kMaxPeers]; rank r writes its epoch into slot r of
@@ -363,6 +383,24 @@ int launch_conv1_bwd_tc(const DecOutMaps* maps, float* dx, int n, cudaStream_t s
   dst.n = 1;
   dst.base[0] = dx;
   if (launch_pdl(conv1_bwd_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, dst, n) != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_dec_out_jvp_tc(const DecOutMaps* maps, const float* xhat, float* dxhat, int n, cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(decout_jvp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess) return -1;
+    attr_set.set_done(dev);
+  }
+  const int num_sms = tc_num_sms();
+  const int total = n * kItemsPerImage;
+  const int grid = total < num_sms ? total : num_sms;
+  DecOutDst dst;
+  memset(&dst, 0, sizeof(dst));
+  dst.n = 1;
+  dst.base[0] = dxhat;
+  if (launch_pdl(decout_jvp_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, dst, n, xhat) != cudaSuccess) return -1;
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -56,6 +56,13 @@ int launch_head_bwd_seed(const float* xhat, const float* rg, const float* bsave,
                          int target_is_frame, const float* dxhat, float* dpre, int n, cudaStream_t st);
 int launch_head_bwd(const float* rg, const int* taps, const float* wgb, const float* wbb, int ntaps, float* dpre,
                     __nv_bfloat16* a2, long long a2_plane, int n, cudaStream_t st);
+// decoder JVP (ian_decode_jvp_*).  Through the RGB-Beta head: tha = the three MDC convolutions of h4's tangent (ha's
+// layouts), rg / bsave the primal sigmoids of the forward -> tangent sigmoids trg (n,64,64,4) and dx_hat (n,3,64,64).
+// Through IAN_simple's dec_out (SIMT): the tangent planes t3 of h3 and the primal x_hat -> dx_hat = conv(t3) * (1 - x_hat^2).
+int launch_rgb_beta_head_jvp(const float* tha, int tha_planar, const float* rg, const float* bsave, float* trg, const int* taps,
+                             const float* wgb, const float* wbb, int ntaps, float* dxhat, int n, cudaStream_t st);
+int launch_dec_out_jvp(const __nv_bfloat16* t3, long long plane, const float* wt, const float* xhat, float* dxhat, int n,
+                       cudaStream_t st);
 // RGB-Beta head on the tensor-core path (head_tc.cu): dense GEMM per (image, conv) + on-chip tap gather -> ha [n][6][4096]
 // (the autoregressive sigmoid / Beta part stays the three per-pixel kernels of edge_kernels.cu)
 struct HeadMaps;
@@ -83,6 +90,9 @@ int launch_dec_out_tc(const DecOutMaps* maps, float* const* dsts, int ndst, int 
 // enc_conv1's adjoint on the tensor-core path: decout_tc's kernel body with an identity epilogue; maps built by
 // decout_build_maps on the conv1 gradient planes e1 and the [2][80][128] planes of rows tap*3 + c = W1[o][c][24 - tap]
 int launch_conv1_bwd_tc(const DecOutMaps* maps, float* dx, int n, cudaStream_t st);
+// decoder JVP on the tensor-core path: decout_tc's GEMM + col2im on the tangent planes of h3 (maps built by decout_build_maps
+// on them, with dec_out's weights), epilogue dx_hat = y * (1 - x_hat^2) from the primal x_hat
+int launch_dec_out_jvp_tc(const DecOutMaps* maps, const float* xhat, float* dxhat, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

@@ -96,9 +96,12 @@ constexpr int DO_T = 8, DO_P = DO_T + 2, DO_LD = 132;
 
 // kTanh = false (conv1_bwd_kernel): the same transposed convolution with an identity epilogue.  enc_conv1's adjoint
 // (3 <- 128 channels, 64x64 <- 32x32, stride 2, pad 2) is exactly this geometry with the tap-flipped conv1 weights.
-template <bool kTanh>
+// kJvp (dec_out_jvp_kernel, the decoder JVP): the same convolution of the tangent planes t3, and the tanh derivative taken
+// from the stored primal x_hat: dx_hat = y * (1 - x_hat^2), the factor the VJP's seed kernels multiply by.
+template <bool kTanh, bool kJvp = false>
 __device__ __forceinline__ void dec_out_body(const __nv_bfloat16* __restrict__ h3, long long plane,
-                                             const float* __restrict__ wt, float* __restrict__ xhat) {
+                                             const float* __restrict__ wt, float* __restrict__ xhat,
+                                             const float* __restrict__ xprim = nullptr) {
   extern __shared__ __align__(16) float smem[];
   float* Xs = smem;                          // [100][132]
   float* Ws = smem + DO_P * DO_P * DO_LD;    // [25*128*4]
@@ -157,6 +160,14 @@ __device__ __forceinline__ void dec_out_body(const __nv_bfloat16* __restrict__ h
   }
   const int oy = 2 * (py0 + p) + r, ox = 2 * (px0 + q) + s;
   float* o = xhat + (long long)img * 3 * 4096 + oy * 64 + ox;
+  if (kJvp) {
+    const float* xp = xprim + (long long)img * 3 * 4096 + oy * 64 + ox;
+    const float x0 = xp[0], x1 = xp[4096], x2 = xp[8192];
+    o[0] = a0 * (1.f - x0 * x0);
+    o[4096] = a1 * (1.f - x1 * x1);
+    o[8192] = a2 * (1.f - x2 * x2);
+    return;
+  }
   o[0] = kTanh ? tanhf(a0) : a0;
   o[4096] = kTanh ? tanhf(a1) : a1;
   o[8192] = kTanh ? tanhf(a2) : a2;
@@ -176,6 +187,15 @@ __global__ void __launch_bounds__(256) conv1_bwd_kernel(const __nv_bfloat16* __r
   pdl_trigger();
   pdl_wait();                                           // tapgemm.h: PDL
   dec_out_body<false>(e1, plane, wt, dx);
+}
+
+// decoder JVP: t3 (n,32,32,128) split planes = tangent of h3, xhat the primal dec_out output -> dx_hat (n,3,64,64) float32
+__global__ void __launch_bounds__(256) dec_out_jvp_kernel(const __nv_bfloat16* __restrict__ t3, long long plane,
+                                                          const float* __restrict__ wt /*[25][128][4]*/,
+                                                          const float* __restrict__ xhat, float* __restrict__ dxhat, int n_img) {
+  pdl_trigger();
+  pdl_wait();                                           // tapgemm.h: PDL
+  dec_out_body<false, true>(t3, plane, wt, dxhat, xhat);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -612,6 +632,88 @@ __global__ void head_b_out_kernel(const float* __restrict__ ha, int planar, cons
 }
 
 // ------------------------------------------------------------------------------------------------
+// Decoder JVP through the RGB-Beta head.  tha holds the three linear 128->2 MDC convolutions of the tangent of h4 (same
+// layouts as ha); rg / bsave are the primal sigmoids the forward stored.  Three passes mirror the forward (R, G, then B
+// and the output), with the derivative expressions of the head's backward (head_bwd_seed_body, head_bwd_g/r_kernel):
+//   tR = R(1-R) T_R;   tG = G(1-G) (T_Ga + MDC_Gb(tR));   tB = B(1-B) (T_Ba + MDC_Bb([tR, tG]))
+//   d out = 2 (b+1e-8)/(a+b+1e-8)^2 ta - 2 a/(a+b+1e-8)^2 tb    per Beta output (a, b: its two sigmoid channels)
+// trg (n,64,64,4) = [tR0 tR1 tG0 tG1] is the JVP's own buffer.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) head_jvp_r_kernel(const float* __restrict__ tha, int planar, const float* __restrict__ rg,
+                                                         float* __restrict__ trg, long long npix) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npix) return;
+  const float2 t = ha_pair(tha, i, 0, planar);
+  const float2 r = *reinterpret_cast<const float2*>(rg + i * 4);
+  *reinterpret_cast<float4*>(trg + i * 4) = make_float4(r.x * (1.f - r.x) * t.x, r.y * (1.f - r.y) * t.y, 0.f, 0.f);
+}
+
+__global__ void __launch_bounds__(256) head_jvp_g_kernel(const float* __restrict__ tha, int planar, const float* __restrict__ rg,
+                                                         float* __restrict__ trg, const int* __restrict__ taps,
+                                                         const float* __restrict__ wgb, int ntaps, int n) {
+  __shared__ int s_taps[2 * kHeadMaxTaps];
+  __shared__ __align__(16) float s_w[4 * kHeadMaxTaps];
+  for (int j = threadIdx.x; j < 2 * ntaps; j += blockDim.x) s_taps[j] = taps[j];
+  for (int j = threadIdx.x; j < 4 * ntaps; j += blockDim.x) s_w[j] = wgb[j];
+  __syncthreads();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * 4096) return;
+  const int q = (int)(i & 63), p = (int)((i >> 6) & 63);
+  const long long img = i >> 12;
+  const float2 gin = ha_pair(tha, i, 2, planar);
+  float g0 = gin.x, g1 = gin.y;
+  for (int t = 0; t < ntaps; ++t) {
+    const int pp = p + s_taps[2 * t], qq = q + s_taps[2 * t + 1];
+    if (pp < 0 || pp > 63 || qq < 0 || qq > 63) continue;
+    const float2 r = *reinterpret_cast<const float2*>(trg + ((img * 64 + pp) * 64 + qq) * 4);
+    const float4 w = *reinterpret_cast<const float4*>(s_w + t * 4);     // [out0: in0,in1 | out1: in0,in1]
+    g0 = fmaf(r.x, w.x, fmaf(r.y, w.y, g0));
+    g1 = fmaf(r.x, w.z, fmaf(r.y, w.w, g1));
+  }
+  const float2 G = *reinterpret_cast<const float2*>(rg + i * 4 + 2);
+  *reinterpret_cast<float2*>(trg + i * 4 + 2) = make_float2(G.x * (1.f - G.x) * g0, G.y * (1.f - G.y) * g1);
+}
+
+__device__ __forceinline__ float beta_jvp(float a, float b, float ta, float tb) {
+  const float s = a + b + 1e-8f;
+  return 2.f * (b + 1e-8f) / (s * s) * ta + (-2.f * a / (s * s)) * tb;
+}
+
+__global__ void __launch_bounds__(256) head_jvp_b_out_kernel(const float* __restrict__ tha, int planar, const float* __restrict__ rg,
+                                                             const float* __restrict__ bsave, const float* __restrict__ trg,
+                                                             const int* __restrict__ taps, const float* __restrict__ wbb, int ntaps,
+                                                             float* __restrict__ dxhat, int n) {
+  __shared__ int s_taps[2 * kHeadMaxTaps];
+  __shared__ __align__(16) float s_w[8 * kHeadMaxTaps];
+  for (int j = threadIdx.x; j < 2 * ntaps; j += blockDim.x) s_taps[j] = taps[j];
+  for (int j = threadIdx.x; j < 8 * ntaps; j += blockDim.x) s_w[j] = wbb[j];
+  __syncthreads();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * 4096) return;
+  const int q = (int)(i & 63), p = (int)((i >> 6) & 63);
+  const long long img = i >> 12;
+  const float2 bin = ha_pair(tha, i, 4, planar);
+  float b0 = bin.x, b1 = bin.y;
+  for (int t = 0; t < ntaps; ++t) {
+    const int pp = p + s_taps[2 * t], qq = q + s_taps[2 * t + 1];
+    if (pp < 0 || pp > 63 || qq < 0 || qq > 63) continue;
+    const float4 v = *reinterpret_cast<const float4*>(trg + ((img * 64 + pp) * 64 + qq) * 4);
+    const float4 w0 = *reinterpret_cast<const float4*>(s_w + t * 8);
+    const float4 w1 = *reinterpret_cast<const float4*>(s_w + t * 8 + 4);
+    b0 = fmaf(v.x, w0.x, fmaf(v.y, w0.y, fmaf(v.z, w0.z, fmaf(v.w, w0.w, b0))));
+    b1 = fmaf(v.x, w1.x, fmaf(v.y, w1.y, fmaf(v.z, w1.z, fmaf(v.w, w1.w, b1))));
+  }
+  const float4 me = *reinterpret_cast<const float4*>(rg + i * 4);
+  const float4 tme = *reinterpret_cast<const float4*>(trg + i * 4);
+  const float2 B = *reinterpret_cast<const float2*>(bsave + i * 2);
+  const float tB0 = B.x * (1.f - B.x) * b0, tB1 = B.y * (1.f - B.y) * b1;
+  float* o = dxhat + img * 3 * 4096 + p * 64 + q;
+  o[0] = beta_jvp(me.x, me.y, tme.x, tme.y);
+  o[4096] = beta_jvp(me.z, me.w, tme.z, tme.w);
+  o[8192] = beta_jvp(B.x, B.y, tB0, tB1);
+}
+
+// ------------------------------------------------------------------------------------------------
 // NPE photo-mode blend after a paint stroke (reference NPE.py:218-231), one 64x64 image, one block:
 //   DELTA = x_hat - to_tanh(RECON);  M = min(mean_c |DELTA|, 1);  MASK = gaussian_filter(M, sigma=0.7)
 //   D = MASK*DELTA + (1-MASK)*ERROR;  IM = uint8(from_tanh(to_tanh(RECON) + D))
@@ -775,6 +877,31 @@ int launch_rgb_beta_head(const float* ha, int ha_planar, float* rg, const int* t
   if (launch_pdl(head_g_kernel, dim3(blocks), dim3(256), 0, st, ha, ha_planar, rg, taps, wgb, ntaps, n) != cudaSuccess) return -1;
   if (launch_pdl(head_b_out_kernel, dim3(blocks), dim3(256), 0, st, ha, ha_planar, rg, taps, wbb, ntaps, xhat, bsave, n) != cudaSuccess) return -1;
   return cudaGetLastError() == cudaSuccess ? 3 : -1;
+}
+
+int launch_rgb_beta_head_jvp(const float* tha, int tha_planar, const float* rg, const float* bsave, float* trg, const int* taps,
+                             const float* wgb, const float* wbb, int ntaps, float* dxhat, int n, cudaStream_t st) {
+  const long long npix = (long long)n * 4096;
+  const unsigned blocks = (unsigned)((npix + 255) / 256);
+  if (ntaps > kHeadMaxTaps) return -1;
+  head_jvp_r_kernel<<<blocks, 256, 0, st>>>(tha, tha_planar, rg, trg, npix);
+  head_jvp_g_kernel<<<blocks, 256, 0, st>>>(tha, tha_planar, rg, trg, taps, wgb, ntaps, n);
+  head_jvp_b_out_kernel<<<blocks, 256, 0, st>>>(tha, tha_planar, rg, bsave, trg, taps, wbb, ntaps, dxhat, n);
+  return cudaGetLastError() == cudaSuccess ? 3 : -1;
+}
+
+int launch_dec_out_jvp(const __nv_bfloat16* t3, long long plane, const float* wt, const float* xhat, float* dxhat, int n,
+                       cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(dec_out_jvp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dec_out_smem_bytes()) != cudaSuccess) return -1;
+    attr_set.set_done(dev);
+  }
+  if (launch_pdl(dec_out_jvp_kernel, dim3((unsigned)n * 16u), dim3(256), (size_t)dec_out_smem_bytes(), st, t3, plane, wt, xhat, dxhat, n) !=
+      cudaSuccess)
+    return -1;
+  return CHECK_LAUNCH();
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -149,11 +149,17 @@ enum LayerId {
   F_BWD_CONV1, F_BWD_FC2,
   // encoder VJP (ian_encode_vjp_*): adjoints of the encoder head, enc_fc1 and enc_conv4..2, built on first use
   E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2,
+  // decoder Jacobian-vector product (ian_decode_jvp_*): the tangent twin of every decoder forward tap-GEMM (DecoderLayers::jvp) and of the head
+  // GEMM of the verification path; built on first use
+  J_DEC_FC2, J_DEC_CONV1, J_DEC_CONV2, J_DEC_CONV3,
+  JF_DEC_FC2, JF_DEC_CONV1, JF_MD1A, JF_MD1B, JF_DEC_CONV2, JF_MD2A, JF_MD2B, JF_DEC_CONV3, JF_MD3A, JF_MD3B, JF_DEC_CONV4,
+  J_HEAD,
   L_COUNT,
   T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
                                                         // enc_conv1_bwd: enc_conv1's adjoint, the encoder VJP's last kernel)
   T_WGRAD_FC2, T_WGRAD_CONV1, T_WGRAD_CONV2, T_WGRAD_CONV3, T_WGRAD_DEC_OUT,   // weight gradients of the parameter VJP
+  T_DEC_OUT_JVP,                                        // IAN_simple's dec_out in the decoder JVP
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -164,8 +170,13 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "bwd_dec_conv3a2", "bwd_dec_conv3a", "bwd_full_dec_conv2", "bwd_dec_conv2a2", "bwd_dec_conv2a",
                                     "bwd_full_dec_conv1", "bwd_full_dec_fc2",
                                     "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4", "bwd_enc_conv3", "bwd_enc_conv2",
+                                    "jvp_l_dec_fc2", "jvp_dec_conv1", "jvp_dec_conv2", "jvp_dec_conv3",
+                                    "jvp_full_dec_fc2", "jvp_full_dec_conv1", "jvp_dec_conv2a", "jvp_dec_conv2a2", "jvp_full_dec_conv2",
+                                    "jvp_dec_conv3a", "jvp_dec_conv3a2", "jvp_full_dec_conv3", "jvp_dec_conv4a", "jvp_dec_conv4a2",
+                                    "jvp_full_dec_conv4", "rgb_head_jvp",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
-                                    "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out"};
+                                    "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
+                                    "dec_out_jvp"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -322,7 +333,16 @@ struct Plan {
   float *pseed = nullptr, *pws = nullptr, *ppart = nullptr;
   WgradGemm wg[4];
   WgradMaps* wmaps[4] = {nullptr};
-  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_COUNT };
+  // decoder JVP (allocated on the plan's first ian_decode_jvp_* call): the tangent of the latent planes, and per decoder
+  // forward layer k the tangent of its output (jt[k]) and of its raw pre-BN sum where the forward keeps one (jr[k], IAN.py's
+  // block residuals); the tangent sigmoids of the RGB-Beta head, and the head's and dec_out's maps on the tangent planes.
+  // The head's tap table tt and ha are reused: the primal head has consumed them when the tangent head runs.
+  bool jvp = false;
+  Planes jzp, jt[11], jr[11];
+  float* jrg = nullptr;
+  DecOutMaps* jdecout_maps = nullptr;
+  HeadMaps* jhead_maps = nullptr;
+  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -480,15 +500,20 @@ struct LayerList {
 // its enc_fc1 activation differs per graph, not its layers) and the encoder VJP are shared by all three graphs.
 const LayerList kEncoder = {5, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD}};
 const LayerList kEncoderBwd = {5, {E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2}};
-struct DecoderLayers { LayerList fwd, bwd; };   // the decoder forward, and its backward-data from the last layer down to z
+// the decoder forward, its backward-data from the last layer down to z, and its tangent (JVP) chain: jvp[k] = jvp_twin(fwd[k])
+struct DecoderLayers { LayerList fwd, bwd, jvp; };
 const DecoderLayers kSimpleDecoder = {{4, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3}},
-                                      {4, {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}}};
+                                      {4, {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}},
+                                      {4, {J_DEC_FC2, J_DEC_CONV1, J_DEC_CONV2, J_DEC_CONV3}}};
 const DecoderLayers kV1Decoder = {{5, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3, F_DEC_CONV4}},
-                                  {6, {F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}}};
+                                  {6, {F_BWD_HEAD, F_BWD_CONV4, L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1, L_BWD_FC2}},
+                                  {5, {J_DEC_FC2, J_DEC_CONV1, J_DEC_CONV2, J_DEC_CONV3, JF_DEC_CONV4}}};
 const DecoderLayers kFullDecoder = {{11, {F_DEC_FC2, F_DEC_CONV1, F_MD1A, F_MD1B, F_DEC_CONV2, F_MD2A, F_MD2B, F_DEC_CONV3,
                                           F_MD3A, F_MD3B, F_DEC_CONV4}},
                                     {12, {F_BWD_HEAD, F_BWD_CONV4, F_BWD_MD3B, F_BWD_MD3A, F_BWD_CONV3, F_BWD_MD2B,
-                                          F_BWD_MD2A, F_BWD_CONV2, F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1, F_BWD_FC2}}};
+                                          F_BWD_MD2A, F_BWD_CONV2, F_BWD_MD1B, F_BWD_MD1A, F_BWD_CONV1, F_BWD_FC2}},
+                                    {11, {JF_DEC_FC2, JF_DEC_CONV1, JF_MD1A, JF_MD1B, JF_DEC_CONV2, JF_MD2A, JF_MD2B, JF_DEC_CONV3,
+                                          JF_MD3A, JF_MD3B, JF_DEC_CONV4}}};
 const DecoderLayers& decoder_layers(const ian_handle* h) {
   return h->model_kind == IAN_MODEL_FULL ? kFullDecoder : h->model_kind == IAN_MODEL_V1 ? kV1Decoder : kSimpleDecoder;
 }
@@ -724,6 +749,8 @@ void free_plan(Plan* pl) {
   if (pl->conv1_bwd_maps) decout_free_maps(pl->conv1_bwd_maps);
   if (pl->conv1_out) conv1_free_out_map(pl->conv1_out);
   if (pl->head_maps) head_free_maps(pl->head_maps);
+  if (pl->jdecout_maps) decout_free_maps(pl->jdecout_maps);
+  if (pl->jhead_maps) head_free_maps(pl->jhead_maps);
   for (auto& gs : pl->graph) if (gs.exec) cudaGraphExecDestroy(gs.exec);
   delete pl;
 }
@@ -1760,6 +1787,94 @@ int check_param_shape(ian_handle* h, const char* name, const int64_t* shape, int
   return IAN_OK;
 }
 
+// ---- decoder Jacobian-vector product ----------------------------------------------------------------
+// dx_hat = (d x_hat / d z) . v, forward mode through the decoder from l_Z.  A forward layer out = act(BN(conv(in) [+ res]))
+// has the tangent t_out = conv(t_in) [+ t_res]) * scale * act'(stored out): the same tap-GEMM (B tiles, taps, geometry, folded
+// BatchNorm scale, no shift) on the tangent planes, in ACT_MASK mode with the forward activation as the mask -- the masks and
+// scales the decoder VJP applies, so the JVP is the exact transpose of its linear map.  A layer with no activation (IANv1's
+// l_dec_fc2) stays ACT_NONE with no shift.  IAN.py's MDBLOCK: the deconv's tangent keeps its raw sum (out_raw), which joins
+// MDCL 2's tangent before scale and mask (res, res_after = 0), as in the forward.
+// The first call on a plan allocates the tangent planes (the decoder's activations once more) and builds their maps and
+// split-K slabs, before any graph capture; plans that never call it keep their memory.
+int ensure_jvp_plan(ian_handle* h, Plan* pl) {
+  if (pl->jvp) return IAN_OK;
+  const DecoderLayers& dec = decoder_layers(h);
+  TapGemm* g = pl->g;
+  int rc;
+  if ((rc = alloc_planes(h, pl, pl->jzp, pl->zp.plane)) != IAN_OK) return rc;
+  // forward plane -> its tangent (the forward's input, residual and mask pointers are looked up here)
+  std::map<const void*, const Planes*> tan = {{pl->zp.p, &pl->jzp}};
+  for (int k = 0; k < dec.fwd.n; ++k) {
+    const TapGemm& f = g[dec.fwd.l[k]];
+    TapGemm& t = g[dec.jvp.l[k]];
+    if ((rc = alloc_planes(h, pl, pl->jt[k], f.out_plane)) != IAN_OK) return rc;
+    if (f.out_raw && (rc = alloc_planes(h, pl, pl->jr[k], f.out_raw_plane)) != IAN_OK) return rc;
+    if (!tan.count(f.a) || (f.res && !tan.count(f.res)) || (f.act != ACT_NONE && f.act != ACT_RELU && f.act != ACT_LRELU))
+      return fail(h, IAN_ERR_STATE, "layer %s: no tangent rule", kLayerNames[dec.fwd.l[k]]);
+    t = f;
+    t.a = tan[f.a]->p; t.a_plane = tan[f.a]->plane;
+    t.shift = nullptr;
+    if (f.act != ACT_NONE) { t.act = ACT_MASK; t.mask = f.out; t.mask_slope = f.act == ACT_LRELU ? 0.2f : 0.f; }
+    t.out = pl->jt[k].p; t.out_plane = pl->jt[k].plane;
+    t.out_raw = f.out_raw ? pl->jr[k].p : nullptr; t.out_raw_plane = f.out_raw ? pl->jr[k].plane : 0;
+    if (f.res) { t.res = tan[f.res]->p; t.res_plane = tan[f.res]->plane; t.res_after = 0; }
+    t.ksplit = 1; t.ws = nullptr;                         // finish_maps decides again, as it did for the forward
+    tan[f.out] = &pl->jt[k];
+    if (f.out_raw) tan[f.out_raw] = &pl->jr[k];
+  }
+  const Planes* t4 = tan[has_flow(h) ? (const void*)pl->fh4.p : (const void*)pl->h3.p];
+  LayerList head = {0, {}};
+  if (has_flow(h)) {
+    g[J_HEAD] = g[F_HEAD];
+    g[J_HEAD].a = t4->p; g[J_HEAD].a_plane = t4->plane;   // writes the tap table tt, as the primal head does
+    g[J_HEAD].ksplit = 1; g[J_HEAD].ws = nullptr;
+    head = {1, {J_HEAD}};
+    if ((rc = alloc_buf(h, pl, pl->jrg, (long long)pl->n * 4096 * 4)) != IAN_OK) return rc;
+  }
+  if ((rc = finish_maps(h, pl, dec.jvp + head)) != IAN_OK) return rc;
+  char err[256] = {0};                                    // both paths: ian_set_path may switch a live handle
+  if (has_flow(h)) {
+    pl->jhead_maps = head_build_maps(t4->p, t4->plane, pl->n, h->head_tc_wt, 3 * 80 * 128, err, sizeof(err));
+    if (!pl->jhead_maps) return fail(h, IAN_ERR_CUDA, "rgb head (jvp): %s", err);
+  } else {
+    pl->jdecout_maps = decout_build_maps(t4->p, t4->plane, pl->n, h->decout_tc_wt, 80 * 128, err, sizeof(err));
+    if (!pl->jdecout_maps) return fail(h, IAN_ERR_CUDA, "dec_out (jvp): %s", err);
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  pl->jvp = true;
+  return IAN_OK;
+}
+
+// the primal (run_decode: the same kernels, so the same x_hat bits and stored activations), then the tangent chain from v
+int run_decode_jvp(ian_handle* h, Plan* pl, const float* z, const float* v, float* xhat, float* dxhat, cudaStream_t st) {
+  const int n = pl->n;
+  int rc;
+  if ((rc = run_decode(h, pl, z, xhat, st)) != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_z_to_planes(v, pl->jzp.p, pl->jzp.plane, n, st));
+  const DecoderLayers& dec = decoder_layers(h);
+  for (int l : dec.jvp)
+    if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+  const Planes& t4 = pl->jt[dec.jvp.n - 1];
+  if (has_flow(h)) {
+    if (h->path == IAN_PATH_TC) {
+      ScopedTimer tm(h, J_HEAD, st);
+      LAUNCH_TRY(h, launch_head_tc(pl->jhead_maps, h->passes, pl->ha, n, st));
+    } else {
+      if ((rc = run_gemm(h, pl, J_HEAD, st)) != IAN_OK) return rc;
+      LAUNCH_TRY(h, launch_head_gather(pl->tt, h->passes == 1 ? 1 : 0, h->head_taps, h->head_ntaps, pl->ha, n, st));
+    }
+    LAUNCH_TRY(h, launch_rgb_beta_head_jvp(pl->ha, h->path == IAN_PATH_TC ? 1 : 0, pl->rg, pl->bsave, pl->jrg, h->head_taps,
+                                           h->head_wgb, h->head_wbb, h->head_ntaps, dxhat, n, st));
+    return IAN_OK;
+  }
+  ScopedTimer tm(h, T_DEC_OUT_JVP, st);
+  if (h->path == IAN_PATH_TC)
+    LAUNCH_TRY(h, launch_dec_out_jvp_tc(pl->jdecout_maps, xhat, dxhat, n, st));
+  else
+    LAUNCH_TRY(h, launch_dec_out_jvp(t4.p, t4.plane, h->decout_wt, xhat, dxhat, n, st));
+  return IAN_OK;
+}
+
 // ---- the two forms of an entry point --------------------------------------------------------------
 // Each batch entry point is one body over one chunk's device pointers, which run_entry runs in two forms:
 //   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
@@ -1941,6 +2056,22 @@ int call_encode_vjp(ian_handle* h, bool host, const float* x, int n, const float
                                         {dx, kImageBytes, S_XHAT, OUT}}, ensure_enc_vjp_plan, [&](const Chunk& c) {
     return c.graphed(Plan::G_ENC_VJP, eps ? 1 : 0,
                      [&] { return run_encode_vjp(h, c.pl, c.f(0), c.f(1), c.f(2), c.f(3), c.st); });
+  });
+}
+
+// x_hat is nullable: the primal then goes to the plan's x_hat buffer.  The host form stages v in the plan's eps buffer,
+// x_hat in its x_hat buffer and dx_hat in its image buffer.
+int call_decode_jvp(ian_handle* h, bool host, const float* z, const float* v, int n, float* x_hat, float* dx_hat, void* stream) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  if (n == 0) return IAN_OK;
+  if (!z || !v || !dx_hat) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {v, kLatentBytes, S_EPS, IN}, {x_hat, kImageBytes, S_XHAT, OUT},
+                                        {dx_hat, kImageBytes, S_X, OUT}}, ensure_jvp_plan, [&](const Chunk& c) {
+    return c.graphed(Plan::G_JVP, 0, [&] {
+      return run_decode_jvp(h, c.pl, c.f(0), c.f(1), c.f(2) ? c.f(2) : c.pl->xhat, c.f(3), c.st);
+    });
   });
 }
 
@@ -2226,6 +2357,12 @@ int ian_decode_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n
 }
 int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz) {
   return call_decode_vjp(h, true, z, dx_hat, n, dz, nullptr);
+}
+int ian_decode_jvp_dev(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat, void* stream) {
+  return call_decode_jvp(h, false, z, v, n, x_hat, dx_hat, stream);
+}
+int ian_decode_jvp_host(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat) {
+  return call_decode_jvp(h, true, z, v, n, x_hat, dx_hat, nullptr);
 }
 
 int ian_param_vjp_supported(int model_kind, int index) { return pv_slot(model_kind, index) >= 0 ? 1 : 0; }

@@ -3,7 +3,8 @@
   * decode(model, z) = X_hat of the reference (API.py:46, sample_at) as a differentiable torch op.  Its backward is the
     decoder's vector-Jacobian product (ian_decode_vjp_dev), so any loss torch can write on the decoded images -- soft or
     per-pixel weighted brushes, L1, losses on the whole frame, refining a latent against a photo -- drives the latent
-    through torch.autograd, as any loss on X_hat was one T.grad away in the reference.
+    through torch.autograd, as any loss on X_hat was one T.grad away in the reference.  Its jvp is the decoder's
+    Jacobian-vector product (ian_decode_jvp_dev), so torch.autograd.forward_ad's make_dual / unpack_dual work through it.
   * encode(model, x, eps=None) = Z_hat of the reference (API.py:50) -- on IAN.py / IANv1.py after the MADE/IAF flow -- as a
     differentiable torch op.  Its backward is the encoder's vector-Jacobian product (ian_encode_vjp_dev): latent-consistency
     losses such as |E(G(z)) - z| or |E(x_hat) - E(x)|, saliency of a latent coordinate, optimising a photo against the
@@ -58,6 +59,7 @@ def _function():
                     model.decode_dev(z.data_ptr(), n, x.data_ptr(), st)
             ctx.model = model
             ctx.save_for_backward(z)
+            ctx.save_for_forward(z)
             return x
 
         @staticmethod
@@ -73,6 +75,19 @@ def _function():
                 with _lib_stream(model, z) as st:
                     model.decode_vjp_dev(z.data_ptr(), g.data_ptr(), n, dz.data_ptr(), st)
             return None, dz
+
+        @staticmethod
+        def jvp(ctx, _model_t, v):
+            (z,) = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, v, "tangent")
+            v = v.contiguous()
+            n = int(z.shape[0])
+            dx = torch.empty(n, 3, 64, 64, dtype=torch.float32, device=z.device)
+            if n:
+                with _lib_stream(model, z) as st:
+                    model.decode_jvp_dev(z.data_ptr(), v.data_ptr(), n, dx.data_ptr(), 0, st)
+            return dx
 
     _Decode = Decode
     return Decode
@@ -212,8 +227,10 @@ def decoder_parameters(model, weights):
 
 def decode(model, z, params=None):
     """x_hat = decoder(z) for z (n,100) float32 CUDA on the model's device; differentiable w.r.t. z (one decoder forward +
-    one backward per backward call).  With params (from decoder_parameters), also differentiable w.r.t. those tensors:
-    one ian_decode_param_vjp_dev returns dz and every gradient; tensors that do not require grad get None."""
+    one backward per backward call).  Without params it also supports forward mode: under torch.autograd.forward_ad a
+    dual z (make_dual(z, v)) gives x_hat with the tangent (d x_hat / d z) . v, from one ian_decode_jvp_dev call.
+    With params (from decoder_parameters), also differentiable w.r.t. those tensors: one ian_decode_param_vjp_dev returns
+    dz and every gradient; tensors that do not require grad get None.  That form is reverse mode only."""
     if params is None:
         return _function().apply(model, z)
     names = list(params)
