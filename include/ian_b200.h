@@ -227,6 +227,22 @@ int ian_decode_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int 
 int ian_decode_jvp_dev(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat, void* stream);
 int ian_decode_jvp_host(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat);
 
+/* ---- encoder Jacobian-vector product: forward mode through the encoder (reference API.py:50) ----------------------------
+ *   dz = (d z / d x) . v
+ * x, v (n,3,64,64) float32 NCHW in the units the graph sees; eps (n,100) nullable; dz (n,100); z (n,100) nullable: receives
+ * ian_encode_*(x, eps) bit for bit.  z is what ian_encode_* returns: mu (+ exp(logsigma) eps) on IAN_simple, and the
+ * MADE/IAF flow of that on IAN.py / IANv1.py.  eps is a constant input: there is no tangent with respect to it.  Recomputes
+ * the forward; the tangent chain runs the forward's tap-GEMMs on tangent planes.  The derivative conventions are the encoder
+ * VJP's (LeakyRectify: the sign of the stored activation, slope 0.2; enc_fc1: rectify 1 where f1 > 0 or elu f1 + 1; the
+ * flow's rectify 1/2 at exactly 0), so <u, JVP(v)> = <ian_encode_vjp_*(u), v> up to float32 summation.  All three graphs,
+ * both paths; bf16 precision on the flow graphs as for ian_encode_vjp_* (enc_conv1 and its tangent stay float32).
+ * n == 0 does nothing; n < 0 or a NULL x, v or dz -> IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE.  Deterministic
+ * (a repeated call is bit-identical).  The first call per batch size allocates that plan's tangent planes, maps and
+ * split-K slabs: the encoder's activations once more, about 1 MB per image (computed from the shapes); plans that never
+ * call it keep their memory. */
+int ian_encode_jvp_dev(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz, void* stream);
+int ian_encode_jvp_host(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -307,7 +323,8 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * "wgrad_dec_conv2", "wgrad_dec_conv3" and "wgrad_dec_out" for the weight gradients of ian_decode_param_vjp_*; in
  * ian_decode_jvp_* "jvp_<layer>" for the tangent tap-GEMM of each decoder forward layer -- "jvp_l_dec_fc2", "jvp_dec_conv1",
  * "jvp_full_dec_conv1", "jvp_dec_conv2a2", ... -- plus "dec_out_jvp" (IAN_simple) and "rgb_head_jvp" (the head's three
- * convolutions on the tangent of its feature map, IAN.py / IANv1.py)) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * convolutions on the tangent of its feature map, IAN.py / IANv1.py); in ian_encode_jvp_* "jvp_enc_conv1" (enc_conv1's
+ * tangent) and "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

@@ -11,7 +11,8 @@ Extensions beyond the reference surface (SURVEY.md section 8b): `reconstruct`, `
 batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space loss (torch autograd binding:
 `torch_ops.decode`), the decoder JVP `decode_jvp` and the Jacobian `decoder_jacobian` (torch forward-mode binding:
 `torch_ops.decode` under `torch.autograd.forward_ad`), the encoder VJP `encode_vjp` for any loss on the latent (torch autograd binding:
-`torch_ops.encode`), and `*_dev` variants taking device pointers.
+`torch_ops.encode`), the encoder JVP `encode_jvp` (torch forward-mode binding: `torch_ops.encode` under
+`torch.autograd.forward_ad`), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -495,6 +496,27 @@ class IAN:
             self._check(self._lib.ian_encode_vjp_host(self._h, _fp(x), n, _fp(e) if e is not None else None, _fp(d), _fp(dx)))
         return dx
 
+    def encode_jvp(self, images, v, eps=None, return_z=False):
+        """Jacobian-vector product of the encoder, dz = (d z / d x) . v -- how the latent moves when the image moves along
+        v: images and v float32 (n,3,64,64), eps as for encode() -> dz float32 (n,100), and z = encode(images, eps) bit for
+        bit when return_z (returned as (z, dz)).  z is what encode() returns (on IAN.py / IANv1.py after the MADE/IAF
+        flow); eps is a constant, with no tangent.  Forward mode: one encoder forward and one tangent pass.  Its derivative
+        conventions are encode_vjp's, so <u, encode_jvp(x, v)> = <encode_vjp(x, u), v> up to float32 summation."""
+        x = _img(images)
+        t = _img(v, 'v')
+        n = x.shape[0]
+        if t.shape[0] != n:
+            raise ValueError("v must be (%d,3,64,64), got %r" % (n, t.shape))
+        dz = np.empty((n, 100), np.float32)
+        z = np.empty((n, 100), np.float32) if return_z else None
+        if n:
+            e = None if eps is None else _z(eps, 'eps')
+            if e is not None and e.shape[0] != n:
+                raise ValueError("eps must be (%d,100), got %r" % (n, e.shape))
+            self._check(self._lib.ian_encode_jvp_host(self._h, _fp(x), _fp(t), n, _fp(e) if e is not None else None,
+                                                      _fp(z) if z is not None else None, _fp(dz)))
+        return (z, dz) if return_z else dz
+
     def edit_steps(self, z, boxes, rgb=None, n_steps=32, weight=0.05):
         """n_steps of the NPE paint rule per sample: Z <- Z - weight*g*(1+(x2-x1)) (reference NPE.py:199-209)."""
         z = _z(z).copy()
@@ -622,6 +644,11 @@ class IAN:
 
     def encode_vjp_dev(self, x_ptr, dz_ptr, n, dx_ptr, eps_ptr=0, stream=0):
         self._check(self._lib.ian_encode_vjp_dev(self._h, x_ptr, int(n), eps_ptr or None, dz_ptr, dx_ptr, stream or None))
+
+    def encode_jvp_dev(self, x_ptr, v_ptr, n, dz_ptr, z_ptr=0, eps_ptr=0, stream=0):
+        """device-pointer form of encode_jvp; z_ptr and eps_ptr may be 0"""
+        self._check(self._lib.ian_encode_jvp_dev(self._h, x_ptr, v_ptr, int(n), eps_ptr or None, z_ptr or None, dz_ptr,
+                                                 stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

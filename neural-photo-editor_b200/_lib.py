@@ -57,6 +57,8 @@ SIGNATURES = {
     "ian_decode_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F]),
     "ian_decode_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_jvp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, _F]),
+    "ian_encode_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_encode_jvp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, _F, _F]),
     "ian_param_vjp_supported": (C.c_int, [C.c_int, C.c_int]),
     "ian_decode_param_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_param_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),

@@ -50,6 +50,9 @@ constexpr int kPatchBytes = (kPatchFloats * 4 + 15) / 16 * 16;
 constexpr int kSmemBytes = 2 * kAStage + kBBytes + kOutBytes + 2 * kPatchBytes + 128 + 512;   // + barriers + staged bias
 static_assert(kSmemBytes <= 232448 - 1024, "conv1_tc: shared memory budget");
 constexpr int kTilesPerImage = 8;                  // 32 output rows / 4
+// conv1_tangent_tc_kernel: a1 signs of this many of a thread's 32 outputs per channel half are loaded while the MMAs run,
+// the rest in the epilogue; 16 or more spill at the 128-register cap of a 512-thread CTA
+constexpr int kPre = 8;
 
 // one 16-byte unit (8 consecutive k) of row m: values -> bf16 hi|lo -> swizzled position in both planes
 template <int K0>
@@ -98,9 +101,14 @@ __device__ __forceinline__ void build_quarter(int quarter, uint8_t* stage, const
   }
 }
 
-__global__ void __launch_bounds__(kThreads, 1)
-conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ Conv1OutMap omap, const float* __restrict__ x,
-                const float* __restrict__ bias, const int n_img) {
+// kTangent (conv1_tangent_tc_kernel, the encoder JVP): the same GEMM on the tangent image v, no bias, and the LeakyRectify
+// derivative read from the sign of the stored forward activation a1 (hi plane, mask > 0 ? 1 : 0.2, TapGemm's ACT_MASK
+// rule).  Shared memory is full, so the mask comes from global memory: kPre of a thread's 32 signs per channel half load
+// while the MMAs run, the rest in the epilogue.
+template <bool kTangent>
+__device__ __forceinline__ void conv1_tc_body(const Conv1Maps& maps, const Conv1OutMap& omap, const float* __restrict__ x,
+                                              const float* __restrict__ bias, const int n_img,
+                                              const __nv_bfloat16* __restrict__ mask) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = smem_u32(smem_raw);
   if (smem_base & 1023u) __trap();                     // the 128B-swizzled tiles need 1024-byte alignment (see kSmemBytes)
@@ -111,7 +119,7 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
   auto empty_bar = [&](int s) { return bar_base + 8u * (2 + s); };
   const uint32_t b_bar = bar_base + 64u;
   float* bias_s = reinterpret_cast<float*>(smem_al + (bar_base + 128u - smem_base));   // 128 floats, 16-byte aligned
-  if (threadIdx.x < 128) bias_s[threadIdx.x] = __ldg(bias + threadIdx.x);   // the epilogue reads it for every tile
+  if (!kTangent && threadIdx.x < 128) bias_s[threadIdx.x] = __ldg(bias + threadIdx.x);   // the epilogue reads it for every tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total = n_img * kTilesPerImage;
@@ -166,6 +174,14 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
           wgmma_bf16<64>(ac, a_hi, b_lo, 1u);
         }
         wgmma_commit();
+        // kTangent: the a1 signs of this thread's first kPre outputs are loaded while the MMAs run
+        const __nv_bfloat16* mrow = kTangent ? mask + (long long)((n * 32 + p0) * 32 + wg * 64) * 128 + h * 64 : nullptr;
+        __nv_bfloat162 mk[kTangent ? kPre / 2 : 1];
+        if (kTangent) {
+#pragma unroll
+          for (int j = 0; j < kPre; j += 2)
+            mk[kTangent ? j / 2 : 0] = *reinterpret_cast<const __nv_bfloat162*>(mrow + frag_row(wtid, j) * 128 + frag_col(wtid, j));
+        }
         wgmma_wait<0>();
         wgmma_fence_regs(am);
         wgmma_fence_regs(ac);
@@ -178,10 +194,20 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
 #pragma unroll
         for (int j = 0; j < 32; j += 2) {
           const int row = wg * 64 + frag_row(wtid, j), col = frag_col(wtid, j);
-          float v0 = am[j] + ac[j] + bias_s[h * 64 + col];
-          float v1 = am[j + 1] + ac[j + 1] + bias_s[h * 64 + col + 1];
-          v0 = fmaf(0.4f, fabsf(v0), 0.6f * v0);
-          v1 = fmaf(0.4f, fabsf(v1), 0.6f * v1);
+          float v0, v1;
+          if (kTangent) {
+            const float2 m = __bfloat1622float2(j < kPre ? mk[kTangent && j < kPre ? j / 2 : 0]
+                                                         : *reinterpret_cast<const __nv_bfloat162*>(mrow + row % 64 * 128 + col));
+            v0 = am[j] + ac[j];
+            v1 = am[j + 1] + ac[j + 1];
+            v0 = m.x > 0.f ? v0 : v0 * 0.2f;
+            v1 = m.y > 0.f ? v1 : v1 * 0.2f;
+          } else {
+            v0 = am[j] + ac[j] + bias_s[h * 64 + col];
+            v1 = am[j + 1] + ac[j + 1] + bias_s[h * 64 + col + 1];
+            v0 = fmaf(0.4f, fabsf(v0), 0.6f * v0);
+            v1 = fmaf(0.4f, fabsf(v1), 0.6f * v1);
+          }
           const __nv_bfloat162 hi = __floats2bfloat162_rn(v0, v1);
           const float2 hf = __bfloat1622float2(hi);
           const __nv_bfloat162 lo = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
@@ -249,6 +275,19 @@ conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ 
   }
 }
 
+__global__ void __launch_bounds__(kThreads, 1)
+conv1_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ Conv1OutMap omap, const float* __restrict__ x,
+                const float* __restrict__ bias, const int n_img) {
+  conv1_tc_body<false>(maps, omap, x, bias, n_img, nullptr);
+}
+
+// encoder JVP: v = the tangent image (n,3,64,64), omap = the tangent planes of a1, a1 = the forward activation's planes
+__global__ void __launch_bounds__(kThreads, 1)
+conv1_tangent_tc_kernel(const __grid_constant__ Conv1Maps maps, const __grid_constant__ Conv1OutMap omap,
+                        const float* __restrict__ v, const __nv_bfloat16* __restrict__ a1, const int n_img) {
+  conv1_tc_body<true>(maps, omap, v, nullptr, n_img, a1);
+}
+
 }  // namespace
 
 Conv1Maps* conv1_build_maps(const __nv_bfloat16* wt, char* err, int errlen) {
@@ -299,6 +338,21 @@ int launch_conv1_tc(const Conv1Maps* maps, const Conv1OutMap* omap, const float*
   const int total = n * kTilesPerImage;
   const int grid = total < num_sms ? total : num_sms;
   if (launch_pdl(conv1_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, *omap, x, bias, n) != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_conv1_tangent_tc(const Conv1Maps* maps, const Conv1OutMap* omap, const float* v, const __nv_bfloat16* a1, int n,
+                            cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(conv1_tangent_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess) return -1;
+    attr_set.set_done(dev);
+  }
+  const int num_sms = tc_num_sms();
+  const int total = n * kTilesPerImage;
+  const int grid = total < num_sms ? total : num_sms;
+  if (launch_pdl(conv1_tangent_tc_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, *maps, *omap, v, a1, n) != cudaSuccess) return -1;
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

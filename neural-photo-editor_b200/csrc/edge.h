@@ -18,6 +18,14 @@ int launch_enc_fc1_bwd(const float* g, const __nv_bfloat16* f1, long long f1_pla
                        __nv_bfloat16* out, long long plane, int n, cudaStream_t st);
 int launch_permute_tiles(const __nv_bfloat16* in, long long in_plane, __nv_bfloat16* out, int ntiles, int R, int C, int flip,
                          cudaStream_t st);
+// encoder JVP (ian_encode_jvp_*).  enc_conv1's tangent on the SIMT path: conv1_kernel's body on the tangent image v, no bias,
+// times LeakyRectify' from the sign of the stored a1 planes -> the tangent planes of a1 (edge_kernels.cu).  Then (enc_vjp.cu)
+// the sample tangent th (n,256) [t_mu | t_ls] -> t_z_iaf (n,100), and forward mode through the MADE/IAF flow from the
+// forward's z0 and the tangent tz0 -> tz (n,100).
+int launch_conv1_tangent(const float* v, const float* wt, const __nv_bfloat16* a1, __nv_bfloat16* out, long long plane, int n,
+                         cudaStream_t st);
+int launch_sample_tangent(const float* head, const float* eps, const float* th, float* tz, int n, cudaStream_t st);
+int launch_made_iaf_tangent(const float* z0, const float* tz0, const float* mw, const float* mb, float* tz, int n, cudaStream_t st);
 int launch_sample(const float* head, const float* eps, float* z, __nv_bfloat16* zp, long long zplane, int n,
                   cudaStream_t st);
 int launch_z_to_planes(const float* z, __nv_bfloat16* zp, long long zplane, int n, cudaStream_t st);
@@ -80,6 +88,10 @@ void conv1_free_maps(Conv1Maps*);
 Conv1OutMap* conv1_build_out_map(__nv_bfloat16* out, long long plane, int n, char* err, int errlen);
 void conv1_free_out_map(Conv1OutMap*);
 int launch_conv1_tc(const Conv1Maps* maps, const Conv1OutMap* omap, const float* x, const float* bias, int n, cudaStream_t st);
+// encoder JVP: enc_conv1's tangent on the tensor cores -- conv1_tc's GEMM on the tangent image v, no bias, LeakyRectify' from
+// the sign of the stored a1 (hi plane) -> the planes omap was built on
+int launch_conv1_tangent_tc(const Conv1Maps* maps, const Conv1OutMap* omap, const float* v, const __nv_bfloat16* a1, int n,
+                            cudaStream_t st);
 // dec_out on the tensor-core path (decout_tc.cu)
 struct DecOutMaps;
 DecOutMaps* decout_build_maps(const __nv_bfloat16* h3, long long h3_plane, int n_img, const __nv_bfloat16* wt,

@@ -22,9 +22,12 @@ __device__ __forceinline__ float lrelu02(float v) { return 0.6f * v + 0.4f * fab
 constexpr int C1_TILE = 8;
 constexpr int C1_PATCH = 2 * C1_TILE + 3;   // 19
 
-__global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ x, const float* __restrict__ wt /*[75][128]*/,
-                                                    const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
-                                                    long long out_plane, int n_img) {
+// kTangent (conv1_tangent_kernel, the encoder JVP): the same convolution of the tangent image, no bias, and the LeakyRectify
+// derivative from the sign of the stored forward activation a1 (mask, hi plane): mask > 0 ? 1 : 0.2.
+template <bool kTangent>
+__device__ __forceinline__ void conv1_body(const float* __restrict__ x, const float* __restrict__ wt, const float* __restrict__ bias,
+                                           __nv_bfloat16* __restrict__ out, long long out_plane,
+                                           const __nv_bfloat16* __restrict__ mask) {
   __shared__ __align__(16) float Ws[75 * 128];
   __shared__ float Xs[3][C1_PATCH][C1_PATCH + 1];
   const int tid = threadIdx.x;
@@ -72,6 +75,19 @@ __global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ x,
       }
     }
   }
+  if (kTangent) {
+#pragma unroll
+    for (int p = 0; p < C1_TILE; ++p) {
+      const long long pix = (long long)(img * 32 + oy0 + py) * 32 + ox0 + p;
+      __align__(8) __nv_bfloat16 mk[4], hi4[4], lo4[4];
+      *reinterpret_cast<uint2*>(mk) = *reinterpret_cast<const uint2*>(mask + pix * 128 + cg * 4);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) split_bf16(__bfloat162float(mk[j]) > 0.f ? acc[p][j] : acc[p][j] * 0.2f, hi4[j], lo4[j]);
+      *reinterpret_cast<uint2*>(out + pix * 128 + cg * 4) = *reinterpret_cast<uint2*>(hi4);
+      *reinterpret_cast<uint2*>(out + out_plane + pix * 128 + cg * 4) = *reinterpret_cast<uint2*>(lo4);
+    }
+    return;
+  }
   const float4 b4 = *reinterpret_cast<const float4*>(bias + cg * 4);
   const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
 #pragma unroll
@@ -83,6 +99,19 @@ __global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ x,
     *reinterpret_cast<uint2*>(out + pix * 128 + cg * 4) = *reinterpret_cast<uint2*>(hi4);
     *reinterpret_cast<uint2*>(out + out_plane + pix * 128 + cg * 4) = *reinterpret_cast<uint2*>(lo4);
   }
+}
+
+__global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ x, const float* __restrict__ wt /*[75][128]*/,
+                                                    const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
+                                                    long long out_plane, int n_img) {
+  conv1_body<false>(x, wt, bias, out, out_plane, nullptr);
+}
+
+// encoder JVP: v (n,3,64,64) the tangent image, a1 the forward activation's planes -> the tangent planes of a1
+__global__ void __launch_bounds__(256) conv1_tangent_kernel(const float* __restrict__ v, const float* __restrict__ wt /*[75][128]*/,
+                                                            const __nv_bfloat16* __restrict__ a1, __nv_bfloat16* __restrict__ out,
+                                                            long long out_plane, int n_img) {
+  conv1_body<true>(v, wt, nullptr, out, out_plane, a1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -781,6 +810,12 @@ __global__ void __launch_bounds__(1024) npe_blend_kernel(const float* __restrict
 int launch_conv1(const float* x, const float* wt, const float* bias, __nv_bfloat16* out, long long plane, int n,
                  cudaStream_t st) {
   conv1_kernel<<<n * 16, 256, 0, st>>>(x, wt, bias, out, plane, n);
+  return CHECK_LAUNCH();
+}
+
+int launch_conv1_tangent(const float* v, const float* wt, const __nv_bfloat16* a1, __nv_bfloat16* out, long long plane, int n,
+                         cudaStream_t st) {
+  conv1_tangent_kernel<<<n * 16, 256, 0, st>>>(v, wt, a1, out, plane, n);
   return CHECK_LAUNCH();
 }
 

@@ -4,6 +4,9 @@
 //   seed         : dz_iaf -> gradient of the encoder head's pre-BatchNorm GEMM output (mu | logsigma columns)
 //   fc1_bwd      : float32 gradient of enc_fc1's output -> ReLU / ELU derivative * bnorm_enc_fc1 scale, split planes
 //   permute      : forward weight tiles [t][R][C] -> backward tiles [t'][C][R] (t' = t or 24 - t), both bf16 planes
+// and the two of the encoder Jacobian-vector product dz = (dz/dx) v (ian_encode_jvp_*) after its tangent tap-GEMMs:
+//   sample_tangent   : tangent of the encoder head [t_mu | t_ls] -> tangent of z_iaf = mu (+ exp(logsigma) eps)
+//   made_iaf_tangent : forward mode through the MADE/IAF latent flow, one block per sample
 #include "edge.h"
 
 namespace ian {
@@ -112,6 +115,88 @@ __global__ void __launch_bounds__(128) made_iaf_bwd_kernel(const float* __restri
   }
 }
 
+// Forward mode of the same flow: with the forward recomputed as above (made_iaf_kernel's fmaf order),
+//   t_u = rect'(pu) (t_z0 W0);  t_h = rect'(ph) (t_u W0);  t_o = t_h W1 + t_u Wd   per net
+//   t_z = (t_z0 - t_o_mu) / exp(o_ls) - z t_o_ls
+// with the backward's rect' (1/2 at exactly 0), so this is the exact transpose of made_iaf_bwd_kernel's linear map.
+__global__ void __launch_bounds__(128) made_iaf_tangent_kernel(const float* __restrict__ z0, const float* __restrict__ tz0,
+                                                               const float* __restrict__ mw, const float* __restrict__ mb,
+                                                               float* __restrict__ tz, int n) {
+  pdl_trigger();
+  pdl_wait();                                           // tapgemm.h: PDL
+  __shared__ float zs[100], tzs[100];
+  __shared__ float us[2][100], hs[2][100], tus[2][100], ths[2][100];
+  const int k = blockIdx.x, j = threadIdx.x;
+  if (j < 100) {
+    zs[j] = z0[k * 100 + j];
+    tzs[j] = tz0[k * 100 + j];
+  }
+  __syncthreads();
+  if (j < 100) {
+#pragma unroll
+    for (int net = 0; net < 2; ++net) {
+      const float* W0 = mw + (net * 3 + 0) * 10000;
+      float a = mb[(net * 3 + 0) * 100 + j], t = 0.f;
+      for (int i = 0; i < 100; ++i) {
+        a = fmaf(zs[i], W0[i * 100 + j], a);
+        t = fmaf(tzs[i], W0[i * 100 + j], t);
+      }
+      us[net][j] = 0.5f * (a + fabsf(a));
+      tus[net][j] = t * rect_grad(a);
+    }
+  }
+  __syncthreads();
+  if (j < 100) {
+#pragma unroll
+    for (int net = 0; net < 2; ++net) {
+      const float* W0 = mw + (net * 3 + 0) * 10000;
+      float a = mb[(net * 3 + 0) * 100 + j], t = 0.f;
+      for (int i = 0; i < 100; ++i) {
+        a = fmaf(us[net][i], W0[i * 100 + j], a);
+        t = fmaf(tus[net][i], W0[i * 100 + j], t);
+      }
+      hs[net][j] = 0.5f * (a + fabsf(a));
+      ths[net][j] = t * rect_grad(a);
+    }
+  }
+  __syncthreads();
+  if (j < 100) {
+    float o[2], to[2];
+#pragma unroll
+    for (int net = 0; net < 2; ++net) {
+      const float* W1 = mw + (net * 3 + 1) * 10000;
+      const float* Wd = mw + (net * 3 + 2) * 10000;
+      float a = mb[(net * 3 + 1) * 100 + j] + mb[(net * 3 + 2) * 100 + j];
+      float a1 = 0.f, a2 = 0.f, t1 = 0.f, t2 = 0.f;
+      for (int i = 0; i < 100; ++i) {
+        a1 = fmaf(hs[net][i], W1[i * 100 + j], a1);
+        a2 = fmaf(us[net][i], Wd[i * 100 + j], a2);
+        t1 = fmaf(ths[net][i], W1[i * 100 + j], t1);
+        t2 = fmaf(tus[net][i], Wd[i * 100 + j], t2);
+      }
+      o[net] = a + a1 + a2;
+      to[net] = t1 + t2;
+    }
+    const float e = expf(o[1]);
+    const float z = (zs[j] - o[0]) / e;
+    tz[k * 100 + j] = (tzs[j] - to[0]) / e - z * to[1];
+  }
+}
+
+// th (n,256) float32 = the tangent [t_mu | t_ls | 0] of the encoder head (BatchNorm scale applied, no shift), head the
+// forward's: t_z_iaf = t_mu (+ exp(logsigma) eps t_ls) -- the transpose of enc_vjp_seed_kernel's map; eps is a constant.
+__global__ void sample_tangent_kernel(const float* __restrict__ head, const float* __restrict__ eps, const float* __restrict__ th,
+                                      float* __restrict__ tz, int n) {
+  pdl_trigger();
+  pdl_wait();                                           // tapgemm.h: PDL
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * 100) return;
+  const int k = i / 100, j = i % 100;
+  float v = th[k * 256 + j];
+  if (eps) v = fmaf(expf(head[k * 256 + 100 + j]) * eps[i], th[k * 256 + 100 + j], v);
+  tz[i] = v;
+}
+
 // head (n,256) float32 = [mu | logsigma | 0] after BatchNorm; z_iaf = mu (+ exp(logsigma) eps) (sample_kernel).
 // out (n,256) split planes: d(pre-BN head) = [dz scale_mu | dz exp(logsigma) eps scale_ls | 0].
 __global__ void enc_vjp_seed_kernel(const float* __restrict__ head, const float* __restrict__ eps, const float* __restrict__ dz,
@@ -166,6 +251,17 @@ __global__ void permute_tiles_kernel(const __nv_bfloat16* __restrict__ in, long 
 
 int launch_made_iaf_bwd(const float* z0, const float* mw, const float* mb, const float* dz, float* dzi, int n, cudaStream_t st) {
   if (launch_pdl(made_iaf_bwd_kernel, dim3(n), dim3(128), 0, st, z0, mw, mb, dz, dzi, n) != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_made_iaf_tangent(const float* z0, const float* tz0, const float* mw, const float* mb, float* tz, int n, cudaStream_t st) {
+  if (launch_pdl(made_iaf_tangent_kernel, dim3(n), dim3(128), 0, st, z0, tz0, mw, mb, tz, n) != cudaSuccess) return -1;
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_sample_tangent(const float* head, const float* eps, const float* th, float* tz, int n, cudaStream_t st) {
+  if (launch_pdl(sample_tangent_kernel, dim3((n * 100 + 255) / 256), dim3(256), 0, st, head, eps, th, tz, n) != cudaSuccess)
+    return -1;
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

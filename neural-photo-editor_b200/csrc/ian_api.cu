@@ -154,12 +154,16 @@ enum LayerId {
   J_DEC_FC2, J_DEC_CONV1, J_DEC_CONV2, J_DEC_CONV3,
   JF_DEC_FC2, JF_DEC_CONV1, JF_MD1A, JF_MD1B, JF_DEC_CONV2, JF_MD2A, JF_MD2B, JF_DEC_CONV3, JF_MD3A, JF_MD3B, JF_DEC_CONV4,
   J_HEAD,
+  // encoder Jacobian-vector product (ian_encode_jvp_*): the tangent twins of enc_conv2..4, enc_fc1 and the encoder head
+  // (kEncoderJvp); built on first use
+  JE_ENC_CONV2, JE_ENC_CONV3, JE_ENC_CONV4, JE_ENC_FC1, JE_ENC_HEAD,
   L_COUNT,
   T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
                                                         // enc_conv1_bwd: enc_conv1's adjoint, the encoder VJP's last kernel)
   T_WGRAD_FC2, T_WGRAD_CONV1, T_WGRAD_CONV2, T_WGRAD_CONV3, T_WGRAD_DEC_OUT,   // weight gradients of the parameter VJP
   T_DEC_OUT_JVP,                                        // IAN_simple's dec_out in the decoder JVP
+  T_CONV1_TANGENT,                                      // enc_conv1's tangent in the encoder JVP
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -174,9 +178,10 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_full_dec_fc2", "jvp_full_dec_conv1", "jvp_dec_conv2a", "jvp_dec_conv2a2", "jvp_full_dec_conv2",
                                     "jvp_dec_conv3a", "jvp_dec_conv3a2", "jvp_full_dec_conv3", "jvp_dec_conv4a", "jvp_dec_conv4a2",
                                     "jvp_full_dec_conv4", "rgb_head_jvp",
+                                    "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
-                                    "dec_out_jvp"};
+                                    "dec_out_jvp", "jvp_enc_conv1"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -342,7 +347,15 @@ struct Plan {
   float* jrg = nullptr;
   DecOutMaps* jdecout_maps = nullptr;
   HeadMaps* jhead_maps = nullptr;
-  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_COUNT };
+  // encoder JVP (allocated on the plan's first ian_encode_jvp_* call): the tangents of a1..a4 and of enc_fc1's output (split
+  // planes), enc_fc1's tangent before its activation derivative, the head's tangent [t_mu | t_ls] and t_z_iaf (float32), and
+  // the TMA-store view of a1's tangent
+  bool ejvp = false;
+  Planes jea[4], jef1;
+  float *jeg = nullptr, *jeh = nullptr, *jez0 = nullptr;
+  Conv1OutMap* jconv1_out = nullptr;
+  enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
+         G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -500,6 +513,8 @@ struct LayerList {
 // its enc_fc1 activation differs per graph, not its layers) and the encoder VJP are shared by all three graphs.
 const LayerList kEncoder = {5, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4, L_ENC_FC1, L_ENC_HEAD}};
 const LayerList kEncoderBwd = {5, {E_BWD_HEAD, E_BWD_FC1, E_BWD_CONV4, E_BWD_CONV3, E_BWD_CONV2}};
+// the encoder's tangent (JVP) chain: kEncoderJvp.l[k] is the tangent twin of kEncoder.l[k]
+const LayerList kEncoderJvp = {5, {JE_ENC_CONV2, JE_ENC_CONV3, JE_ENC_CONV4, JE_ENC_FC1, JE_ENC_HEAD}};
 // the decoder forward, its backward-data from the last layer down to z, and its tangent (JVP) chain: jvp[k] = jvp_twin(fwd[k])
 struct DecoderLayers { LayerList fwd, bwd, jvp; };
 const DecoderLayers kSimpleDecoder = {{4, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3}},
@@ -751,6 +766,7 @@ void free_plan(Plan* pl) {
   if (pl->head_maps) head_free_maps(pl->head_maps);
   if (pl->jdecout_maps) decout_free_maps(pl->jdecout_maps);
   if (pl->jhead_maps) head_free_maps(pl->jhead_maps);
+  if (pl->jconv1_out) conv1_free_out_map(pl->jconv1_out);
   for (auto& gs : pl->graph) if (gs.exec) cudaGraphExecDestroy(gs.exec);
   delete pl;
 }
@@ -1794,6 +1810,33 @@ int check_param_shape(ian_handle* h, const char* name, const int64_t* shape, int
 // scales the decoder VJP applies, so the JVP is the exact transpose of its linear map.  A layer with no activation (IANv1's
 // l_dec_fc2) stays ACT_NONE with no shift.  IAN.py's MDBLOCK: the deconv's tangent keeps its raw sum (out_raw), which joins
 // MDCL 2's tangent before scale and mask (res, res_after = 0), as in the forward.
+
+// forward plane -> its tangent (a twin's input, residual and mask pointers are looked up here)
+using TangentMap = std::map<const void*, const Planes*>;
+
+// Slot lt becomes the tangent twin of forward layer lf (rule above, shared by the decoder and the encoder JVP).  Allocates
+// the twin's output planes `out` (and `raw` where the forward keeps its raw sum) and records them in `tan`.
+int tangent_twin(ian_handle* h, Plan* pl, int lf, int lt, TangentMap& tan, Planes& out, Planes& raw) {
+  const TapGemm& f = pl->g[lf];
+  TapGemm& t = pl->g[lt];
+  int rc;
+  if ((rc = alloc_planes(h, pl, out, f.out_plane)) != IAN_OK) return rc;
+  if (f.out_raw && (rc = alloc_planes(h, pl, raw, f.out_raw_plane)) != IAN_OK) return rc;
+  if (!tan.count(f.a) || (f.res && !tan.count(f.res)) || (f.act != ACT_NONE && f.act != ACT_RELU && f.act != ACT_LRELU))
+    return fail(h, IAN_ERR_STATE, "layer %s: no tangent rule", kLayerNames[lf]);
+  t = f;
+  t.a = tan[f.a]->p; t.a_plane = tan[f.a]->plane;
+  t.shift = nullptr;
+  if (f.act != ACT_NONE) { t.act = ACT_MASK; t.mask = f.out; t.mask_slope = f.act == ACT_LRELU ? 0.2f : 0.f; }
+  t.out = out.p; t.out_plane = out.plane;
+  t.out_raw = f.out_raw ? raw.p : nullptr; t.out_raw_plane = f.out_raw ? raw.plane : 0;
+  if (f.res) { t.res = tan[f.res]->p; t.res_plane = tan[f.res]->plane; t.res_after = 0; }
+  t.ksplit = 1; t.ws = nullptr;                           // finish_maps decides again, as it did for the forward
+  tan[f.out] = &out;
+  if (f.out_raw) tan[f.out_raw] = &raw;
+  return IAN_OK;
+}
+
 // The first call on a plan allocates the tangent planes (the decoder's activations once more) and builds their maps and
 // split-K slabs, before any graph capture; plans that never call it keep their memory.
 int ensure_jvp_plan(ian_handle* h, Plan* pl) {
@@ -1802,26 +1845,9 @@ int ensure_jvp_plan(ian_handle* h, Plan* pl) {
   TapGemm* g = pl->g;
   int rc;
   if ((rc = alloc_planes(h, pl, pl->jzp, pl->zp.plane)) != IAN_OK) return rc;
-  // forward plane -> its tangent (the forward's input, residual and mask pointers are looked up here)
-  std::map<const void*, const Planes*> tan = {{pl->zp.p, &pl->jzp}};
-  for (int k = 0; k < dec.fwd.n; ++k) {
-    const TapGemm& f = g[dec.fwd.l[k]];
-    TapGemm& t = g[dec.jvp.l[k]];
-    if ((rc = alloc_planes(h, pl, pl->jt[k], f.out_plane)) != IAN_OK) return rc;
-    if (f.out_raw && (rc = alloc_planes(h, pl, pl->jr[k], f.out_raw_plane)) != IAN_OK) return rc;
-    if (!tan.count(f.a) || (f.res && !tan.count(f.res)) || (f.act != ACT_NONE && f.act != ACT_RELU && f.act != ACT_LRELU))
-      return fail(h, IAN_ERR_STATE, "layer %s: no tangent rule", kLayerNames[dec.fwd.l[k]]);
-    t = f;
-    t.a = tan[f.a]->p; t.a_plane = tan[f.a]->plane;
-    t.shift = nullptr;
-    if (f.act != ACT_NONE) { t.act = ACT_MASK; t.mask = f.out; t.mask_slope = f.act == ACT_LRELU ? 0.2f : 0.f; }
-    t.out = pl->jt[k].p; t.out_plane = pl->jt[k].plane;
-    t.out_raw = f.out_raw ? pl->jr[k].p : nullptr; t.out_raw_plane = f.out_raw ? pl->jr[k].plane : 0;
-    if (f.res) { t.res = tan[f.res]->p; t.res_plane = tan[f.res]->plane; t.res_after = 0; }
-    t.ksplit = 1; t.ws = nullptr;                         // finish_maps decides again, as it did for the forward
-    tan[f.out] = &pl->jt[k];
-    if (f.out_raw) tan[f.out_raw] = &pl->jr[k];
-  }
+  TangentMap tan = {{pl->zp.p, &pl->jzp}};
+  for (int k = 0; k < dec.fwd.n; ++k)
+    if ((rc = tangent_twin(h, pl, dec.fwd.l[k], dec.jvp.l[k], tan, pl->jt[k], pl->jr[k])) != IAN_OK) return rc;
   const Planes* t4 = tan[has_flow(h) ? (const void*)pl->fh4.p : (const void*)pl->h3.p];
   LayerList head = {0, {}};
   if (has_flow(h)) {
@@ -1875,6 +1901,83 @@ int run_decode_jvp(ian_handle* h, Plan* pl, const float* z, const float* v, floa
   return IAN_OK;
 }
 
+// ---- encoder Jacobian-vector product ----------------------------------------------------------------
+// dz = (dz/dx) . v, forward mode through the encoder and, on IAN.py / IANv1.py, the MADE/IAF flow.  With the encoder VJP's
+// derivative conventions, so it is the exact transpose of that linear map:
+//   enc_conv1: t_a1 = conv1(v) (no bias) * lrelu'(a1), conv1_tc's GEMM (or conv1_kernel's FFMA body) with a mask epilogue;
+//   enc_conv2..4: tangent twins (tangent_twin) against a2..a4;
+//   enc_fc1: its twin writes float32 with no scale and no activation, then enc_fc1_bwd_kernel -- the encoder VJP's
+//            element-wise step -- applies scale * act'(f1) (rectify on the flow graphs, elu' = f1 + 1 on IAN_simple);
+//   enc_head: its twin with scale and no shift, float32 [t_mu | t_ls];
+//   sample: t_z_iaf = t_mu (+ exp(logsigma) eps t_ls); eps is a constant input;
+//   flow: made_iaf_tangent_kernel from the forward's z0.
+// enc_conv1 and its tangent run in float32 in either precision, as in the forward.  The first call on a plan allocates the
+// tangent planes (the encoder's activations once more, about 1 MB per image) and builds their maps and split-K slabs, before
+// any graph capture; plans that never call it keep their memory.
+int ensure_enc_jvp_plan(ian_handle* h, Plan* pl) {
+  if (pl->ejvp) return IAN_OK;
+  const long long N = pl->n;
+  TapGemm* g = pl->g;
+  int rc;
+  if ((rc = alloc_planes(h, pl, pl->jea[0], pl->a1.plane)) != IAN_OK) return rc;
+  TangentMap tan = {{pl->a1.p, &pl->jea[0]}};
+  Planes raw;                                             // the encoder keeps no raw sums
+  for (int k = 0; k < 3; ++k)
+    if ((rc = tangent_twin(h, pl, kEncoder.l[k], kEncoderJvp.l[k], tan, pl->jea[k + 1], raw)) != IAN_OK) return rc;
+  if ((rc = alloc_planes(h, pl, pl->jef1, pl->f1.plane)) != IAN_OK) return rc;
+  if ((rc = alloc_buf(h, pl, pl->jeg, N * 1024)) != IAN_OK) return rc;
+  if ((rc = alloc_buf(h, pl, pl->jeh, N * 256)) != IAN_OK) return rc;
+  if (has_flow(h) && (rc = alloc_buf(h, pl, pl->jez0, N * 100)) != IAN_OK) return rc;
+  TapGemm& fc1 = g[JE_ENC_FC1];
+  fc1 = g[L_ENC_FC1];
+  fc1.a = pl->jea[3].p; fc1.a_plane = pl->jea[3].plane;
+  fc1.act = ACT_NONE; fc1.scale = nullptr; fc1.shift = nullptr;
+  fc1.out = nullptr; fc1.out_plane = 0; fc1.out_f32 = pl->jeg;
+  fc1.ksplit = 0; fc1.ws = nullptr;                       // as wired for the forward: finish_maps chooses
+  TapGemm& head = g[JE_ENC_HEAD];
+  head = g[L_ENC_HEAD];
+  head.a = pl->jef1.p; head.a_plane = pl->jef1.plane;
+  head.shift = nullptr; head.out_f32 = pl->jeh;
+  head.ksplit = 1; head.ws = nullptr;
+  // the chain's own split-K slabs: the plan's other layers keep theirs
+  if ((rc = finish_maps(h, pl, kEncoderJvp)) != IAN_OK) return rc;
+  {   // both paths: ian_set_path may switch a live handle
+    char err[256] = {0};
+    pl->jconv1_out = conv1_build_out_map(pl->jea[0].p, pl->jea[0].plane, pl->n, err, sizeof(err));
+    if (!pl->jconv1_out) return fail(h, IAN_ERR_CUDA, "enc_conv1 (jvp): %s", err);
+  }
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  pl->ejvp = true;
+  return IAN_OK;
+}
+
+// the primal (run_encode: the same kernels, so z and the stored activations carry ian_encode_*'s bits), then the tangent chain
+int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, const float* eps, float* z, float* dz, cudaStream_t st) {
+  const int n = pl->n;
+  int rc;
+  if ((rc = run_encode(h, pl, x, eps, z, st)) != IAN_OK) return rc;
+  {
+    ScopedTimer tm(h, T_CONV1_TANGENT, st);
+    if (h->path == IAN_PATH_TC)
+      LAUNCH_TRY(h, launch_conv1_tangent_tc(h->conv1_maps, pl->jconv1_out, v, pl->a1.p, n, st));
+    else
+      LAUNCH_TRY(h, launch_conv1_tangent(v, h->conv1_wt, pl->a1.p, pl->jea[0].p, pl->jea[0].plane, n, st));
+  }
+  for (int l : kEncoderJvp) {
+    if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+    if (l == JE_ENC_FC1)   // enc_fc1's BatchNorm scale and ReLU / ELU derivative between its twin and the head's
+      LAUNCH_TRY(h, launch_enc_fc1_bwd(pl->jeg, pl->f1.p, pl->f1.plane, h->w[L_ENC_FC1].scale, has_flow(h) ? 0 : 1, pl->jef1.p,
+                                       pl->jef1.plane, n, st));
+  }
+  if (!has_flow(h)) {
+    LAUNCH_TRY(h, launch_sample_tangent(pl->head, eps, pl->jeh, dz, n, st));
+    return IAN_OK;
+  }
+  LAUNCH_TRY(h, launch_sample_tangent(pl->head, eps, pl->jeh, pl->jez0, n, st));
+  LAUNCH_TRY(h, launch_made_iaf_tangent(pl->z0, pl->jez0, h->made_w, h->made_b, dz, n, st));
+  return IAN_OK;
+}
+
 // ---- the two forms of an entry point --------------------------------------------------------------
 // Each batch entry point is one body over one chunk's device pointers, which run_entry runs in two forms:
 //   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
@@ -1906,7 +2009,7 @@ struct Chunk {
   int off, cn;
   cudaStream_t st;
   bool host;
-  void* p[4];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
+  void* p[5];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
   float* f(int i) const { return (float*)p[i]; }
   const int32_t* i32(int i) const { return (const int32_t*)p[i]; }
   // a kernel chain: replayed from graph `slot` by the host form (run_graphed), launched as is by the device form
@@ -2071,6 +2174,24 @@ int call_decode_jvp(ian_handle* h, bool host, const float* z, const float* v, in
                                         {dx_hat, kImageBytes, S_X, OUT}}, ensure_jvp_plan, [&](const Chunk& c) {
     return c.graphed(Plan::G_JVP, 0, [&] {
       return run_decode_jvp(h, c.pl, c.f(0), c.f(1), c.f(2) ? c.f(2) : c.pl->xhat, c.f(3), c.st);
+    });
+  });
+}
+
+// z is nullable: the primal then goes to the plan's z buffer.  The host form stages v in the plan's frame-target buffer,
+// z in its z buffer and dz in its x_hat buffer.
+int call_encode_jvp(ian_handle* h, bool host, const float* x, const float* v, int n, const float* eps, float* z, float* dz,
+                    void* stream) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  if (n == 0) return IAN_OK;
+  if (!x || !v || !dz) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {v, kImageBytes, S_TARGET, IN}, {eps, kLatentBytes, S_EPS, IN},
+                                        {z, kLatentBytes, S_Z, OUT}, {dz, kLatentBytes, S_XHAT, OUT}}, ensure_enc_jvp_plan,
+                   [&](const Chunk& c) {
+    return c.graphed(Plan::G_ENC_JVP, eps ? 1 : 0, [&] {
+      return run_encode_jvp(h, c.pl, c.f(0), c.f(1), c.f(2), c.f(3) ? c.f(3) : c.pl->z, c.f(4), c.st);
     });
   });
 }
@@ -2363,6 +2484,12 @@ int ian_decode_jvp_dev(ian_handle* h, const float* z, const float* v, int n, flo
 }
 int ian_decode_jvp_host(ian_handle* h, const float* z, const float* v, int n, float* x_hat, float* dx_hat) {
   return call_decode_jvp(h, true, z, v, n, x_hat, dx_hat, nullptr);
+}
+int ian_encode_jvp_dev(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz, void* stream) {
+  return call_encode_jvp(h, false, x, v, n, eps, z, dz, stream);
+}
+int ian_encode_jvp_host(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz) {
+  return call_encode_jvp(h, true, x, v, n, eps, z, dz, nullptr);
 }
 
 int ian_param_vjp_supported(int model_kind, int index) { return pv_slot(model_kind, index) >= 0 ? 1 : 0; }

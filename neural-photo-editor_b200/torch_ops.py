@@ -8,8 +8,9 @@
   * encode(model, x, eps=None) = Z_hat of the reference (API.py:50) -- on IAN.py / IANv1.py after the MADE/IAF flow -- as a
     differentiable torch op.  Its backward is the encoder's vector-Jacobian product (ian_encode_vjp_dev): latent-consistency
     losses such as |E(G(z)) - z| or |E(x_hat) - E(x)|, saliency of a latent coordinate, optimising a photo against the
-    encoder, and a differentiable decode(encode(x)).  eps is a constant input: it gets no gradient, and an eps that
-    requires grad is refused.
+    encoder, and a differentiable decode(encode(x)).  Its jvp is the encoder's Jacobian-vector product (ian_encode_jvp_dev),
+    so forward mode works through encode and through decode(encode(x)).  eps is a constant input: it gets no gradient or
+    tangent, and an eps that requires grad or carries a tangent is refused.
 
   * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
@@ -119,7 +120,9 @@ def _encode_function():
                     model.encode_dev(x.data_ptr(), n, z.data_ptr(), eps.data_ptr() if eps is not None else 0, st)
             ctx.model = model
             ctx.has_eps = eps is not None
-            ctx.save_for_backward(x, eps if eps is not None else x.new_empty(0))
+            saved = (x, eps if eps is not None else x.new_empty(0))
+            ctx.save_for_backward(*saved)
+            ctx.save_for_forward(*saved)
             return z
 
         @staticmethod
@@ -137,16 +140,39 @@ def _encode_function():
                                          eps.data_ptr() if ctx.has_eps else 0, st)
             return None, dx, None
 
+        @staticmethod
+        def jvp(ctx, _model_t, v, _eps_t):
+            x, eps = ctx.saved_tensors
+            model = ctx.model
+            n = int(x.shape[0])
+            dz = torch.zeros(n, 100, dtype=torch.float32, device=x.device)
+            if v is None:
+                return dz
+            _check_tensor(model, v, "tangent")
+            v = v.contiguous()
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.encode_jvp_dev(x.data_ptr(), v.data_ptr(), n, dz.data_ptr(), 0,
+                                         eps.data_ptr() if ctx.has_eps else 0, st)
+            return dz
+
     _Encode = Encode
     return Encode
 
 
 def encode(model, x, eps=None):
     """z = encoder(x) (what model.encode returns) for x (n,3,64,64) float32 CUDA on the model's device, eps (n,100) or None;
-    differentiable w.r.t. x (one encoder forward + one backward per backward call).  eps is not differentiated: pass a
-    tensor that does not require grad."""
+    differentiable w.r.t. x (one encoder forward + one backward per backward call).  It also supports forward mode: under
+    torch.autograd.forward_ad a dual x (make_dual(x, v)) gives z with the tangent (d z / d x) . v, from one
+    ian_encode_jvp_dev call, so forward mode runs through decode(encode(x)) too.  eps is not differentiated: pass a
+    tensor that neither requires grad nor carries a forward-mode tangent."""
     if eps is not None and getattr(eps, "requires_grad", False):
         raise ValueError("torch_ops.encode does not differentiate w.r.t. eps; pass eps.detach() (eps.requires_grad is set)")
+    if eps is not None:
+        import torch.autograd.forward_ad as fwAD
+        if fwAD.unpack_dual(eps).tangent is not None:
+            raise ValueError("torch_ops.encode does not differentiate w.r.t. eps; pass its primal (eps carries a forward-mode "
+                             "tangent)")
     return _encode_function().apply(model, x, eps)
 
 
