@@ -79,7 +79,10 @@ static int symbols(void) {
       (anyfn)ian_bn_train_normalize_dev, (anyfn)ian_minibatch_discrim_dev, (anyfn)ian_decode_vjp_dev,
       (anyfn)ian_decode_vjp_host, (anyfn)ian_encode_vjp_dev, (anyfn)ian_encode_vjp_host,
       (anyfn)ian_param_vjp_supported, (anyfn)ian_decode_param_vjp_dev, (anyfn)ian_decode_param_vjp_host, (anyfn)ian_update_param_host,
-      (anyfn)ian_decode_jvp_dev, (anyfn)ian_decode_jvp_host, (anyfn)ian_encode_jvp_dev, (anyfn)ian_encode_jvp_host};
+      (anyfn)ian_decode_jvp_dev, (anyfn)ian_decode_jvp_host, (anyfn)ian_encode_jvp_dev, (anyfn)ian_encode_jvp_host,
+      (anyfn)ian_encode_pre_dev, (anyfn)ian_flow_dev, (anyfn)ian_flow_vjp_dev, (anyfn)ian_flow_vjp_host, (anyfn)ian_flow_jvp_dev,
+      (anyfn)ian_flow_jvp_host, (anyfn)ian_encode_pre_vjp_dev, (anyfn)ian_encode_pre_vjp_host, (anyfn)ian_encode_pre_jvp_dev,
+      (anyfn)ian_encode_pre_jvp_host};
   size_t i, n = sizeof(fn) / sizeof(fn[0]);
   for (i = 0; i < n; ++i)
     if (!fn[i]) return 1;

@@ -185,9 +185,41 @@ int ian_gather_wait_dev(ian_handle* h, float** gathered_out, void* stream);
  *   Z_IAF_fn : l_Z_IAF -> l_Z = (z - MADE_mu(z)) / exp(MADE_ls(z))                 -> ian_flow_host(z_out)
  *   sample   : l_Z_IAF -> X (flow, then decoder)                                   -> ian_flow_host(x_out)
  *   sampleZ  : l_Z -> X                                                            -> ian_decode_host
- * For IAN_MODEL_SIMPLE there is no flow: Zfn == encode and Z_IAF_fn is the identity. */
+ * For IAN_MODEL_SIMPLE there is no flow: Zfn == encode and Z_IAF_fn is the identity.  The _dev forms run the same kernels
+ * as the _host forms (bit-identical results); as for ian_encode_*, n must be positive. */
+int ian_encode_pre_dev(ian_handle* h, const float* x, int n, float* z_iaf, void* stream);
 int ian_encode_pre_host(ian_handle* h, const float* x, int n, float* z_iaf);
+int ian_flow_dev(ian_handle* h, const float* z_iaf, int n, float* z_out /*nullable*/, float* x_out /*nullable*/, void* stream);
 int ian_flow_host(ian_handle* h, const float* z_iaf, int n, float* z_out /*nullable*/, float* x_out /*nullable*/);
+
+/* ---- derivatives of the sampling script's functions: the prior space l_Z_IAF --------------------------------------------
+ * On IAN.py / IANv1.py the generative prior lives in l_Z_IAF, the input of the MADE/IAF flow (sample_IAN.py feeds N(0,1)
+ * noise there and interpolates there).  These split the encoder's derivatives at that boundary:
+ *   flow (Z_IAF_fn):   dz_iaf = (d l_Z / d l_Z_IAF)^T . dz          dz = (d l_Z / d l_Z_IAF) . v
+ *   Zfn:               dx = (d l_Z_IAF / d x)^T . dz_iaf            dz_iaf = (d l_Z_IAF / d x) . v
+ * Zfn is deterministic (l_Z_IAF = mu, no eps).  z_iaf, dz, v (flow), dz_iaf (n,100); x, v (Zfn), dx (n,3,64,64).
+ * ian_flow_jvp_*'s z (nullable) receives Z_IAF_fn(z_iaf) and ian_encode_pre_jvp_*'s z_iaf (nullable) Zfn(x), bit for bit.
+ * ian_encode_vjp_*(x, dz) equals ian_encode_pre_vjp_*(x, ian_flow_vjp_*(Zfn(x), dz)) and ian_encode_jvp_*(x, v) equals
+ * ian_flow_jvp_*(Zfn(x), ian_encode_pre_jvp_*(x, v)) bit for bit, eps absent.  `sample` (l_Z_IAF -> X) has no entry of its
+ * own; its derivatives are the compositions
+ *   VJP: ian_flow_vjp_*(z_iaf, ian_decode_vjp_*(Z_IAF_fn(z_iaf), dx))      JVP: ian_decode_jvp_*(Z_IAF_fn(z_iaf), ian_flow_jvp_*(z_iaf, v))
+ * The flow runs in float32 FFMA in either precision (made_iaf_kernel's summation order, recomputed); its rectify' is 1/2 at
+ * exactly 0, as in the encoder VJP and JVP, so ian_flow_vjp_* is the exact transpose of ian_flow_jvp_*'s linear map.  On
+ * IAN_MODEL_SIMPLE the flow is the identity: ian_flow_vjp_* returns dz, ian_flow_jvp_* returns v (and z_iaf as z), and the
+ * ian_encode_pre_* derivatives return what ian_encode_vjp_* / ian_encode_jvp_* return with eps = NULL.  All three graphs,
+ * both paths; bf16 precision on the flow graphs as for ian_encode_vjp_* / ian_encode_jvp_*.  n == 0 does nothing; n < 0 or a
+ * NULL required pointer -> IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE.  Deterministic (a repeated call is
+ * bit-identical).  The flow entries need no memory beyond a plan's (n,100) buffers; the Zfn entries allocate what
+ * ian_encode_vjp_* / ian_encode_jvp_* allocate on their first call per batch size, and share it with them. */
+int ian_flow_vjp_dev(ian_handle* h, const float* z_iaf, const float* dz, int n, float* dz_iaf, void* stream);
+int ian_flow_vjp_host(ian_handle* h, const float* z_iaf, const float* dz, int n, float* dz_iaf);
+int ian_flow_jvp_dev(ian_handle* h, const float* z_iaf, const float* v, int n, float* z /*nullable*/, float* dz, void* stream);
+int ian_flow_jvp_host(ian_handle* h, const float* z_iaf, const float* v, int n, float* z /*nullable*/, float* dz);
+int ian_encode_pre_vjp_dev(ian_handle* h, const float* x, int n, const float* dz_iaf, float* dx, void* stream);
+int ian_encode_pre_vjp_host(ian_handle* h, const float* x, int n, const float* dz_iaf, float* dx);
+int ian_encode_pre_jvp_dev(ian_handle* h, const float* x, const float* v, int n, float* z_iaf /*nullable*/, float* dz_iaf,
+                           void* stream);
+int ian_encode_pre_jvp_host(ian_handle* h, const float* x, const float* v, int n, float* z_iaf /*nullable*/, float* dz_iaf);
 
 /* ---- latent-brush gradients: replace calculate_RGB_gradient / calculate_lighten_gradient
  * (reference API.py:59, 64; IAN.imgrad / IAN.imgradRGB API.py:66-76), batched per sample -------- */

@@ -12,7 +12,9 @@ batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space 
 `torch_ops.decode`), the decoder JVP `decode_jvp` and the Jacobian `decoder_jacobian` (torch forward-mode binding:
 `torch_ops.decode` under `torch.autograd.forward_ad`), the encoder VJP `encode_vjp` for any loss on the latent (torch autograd binding:
 `torch_ops.encode`), the encoder JVP `encode_jvp` (torch forward-mode binding: `torch_ops.encode` under
-`torch.autograd.forward_ad`), and `*_dev` variants taking device pointers.
+`torch.autograd.forward_ad`), the encoder Jacobian `encoder_jacobian`, the derivatives of the sampling script's
+functions in the prior space l_Z_IAF -- `flow_vjp` / `flow_jvp` (Z_IAF_fn) and `encode_pre_vjp` / `encode_pre_jvp` (Zfn),
+torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -517,6 +519,85 @@ class IAN:
                                                       _fp(z) if z is not None else None, _fp(dz)))
         return (z, dz) if return_z else dz
 
+    def encoder_jacobian(self, images, eps=None):
+        """The encoder's Jacobian at each image: images float32 (n,3,64,64), eps as for encode() -> J float32
+        (n,100,3,64,64) with J[k, i] = d z_i / d x at x[k], z as encode() returns it (on IAN.py / IANv1.py after the MADE/IAF
+        flow): J's 100 rows as images, the saliency map of every latent coordinate.  One batch-100 encode_vjp with the
+        identity as cotangents per image."""
+        x = _img(images)
+        n = x.shape[0]
+        e = None if eps is None else _z(eps, 'eps')
+        if e is not None and e.shape[0] != n:
+            raise ValueError("eps must be (%d,100), got %r" % (n, e.shape))
+        J = np.empty((n, 100, 3, 64, 64), np.float32)
+        eye = np.eye(100, dtype=np.float32)
+        for k in range(n):
+            xk = np.ascontiguousarray(np.broadcast_to(x[k], (100, 3, 64, 64)))
+            ek = None if e is None else np.ascontiguousarray(np.broadcast_to(e[k], (100, 100)))
+            self._check(self._lib.ian_encode_vjp_host(self._h, _fp(xk), 100, _fp(ek) if ek is not None else None, _fp(eye),
+                                                      _fp(J[k])))
+        return J
+
+    # ---- derivatives in the prior space l_Z_IAF (the sampling script's Zfn / Z_IAF_fn / sample) ------------------------
+    def encode_pre_vjp(self, images, dz_iaf):
+        """Vector-Jacobian product of Zfn (X -> l_Z_IAF, deterministic), dx = (d z_iaf / d x)^T . dz_iaf: images
+        (n,3,64,64), dz_iaf float32 (n,100) -> dx float32 (n,3,64,64).  encode_vjp(x, dz) equals
+        encode_pre_vjp(x, flow_vjp(Zfn(x), dz)) bit for bit; on IAN_simple it is encode_vjp with eps absent."""
+        x = _img(images)
+        n = x.shape[0]
+        d = _z(dz_iaf, 'dz_iaf')
+        if d.shape[0] != n:
+            raise ValueError("dz_iaf must be (%d,100), got %r" % (n, d.shape))
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        if n:
+            self._check(self._lib.ian_encode_pre_vjp_host(self._h, _fp(x), n, _fp(d), _fp(dx)))
+        return dx
+
+    def encode_pre_jvp(self, images, v, return_z=False):
+        """Jacobian-vector product of Zfn, dz_iaf = (d z_iaf / d x) . v: images and v float32 (n,3,64,64) -> dz_iaf float32
+        (n,100), and z_iaf = Zfn(images) bit for bit when return_z (returned as (z_iaf, dz_iaf)).  encode_jvp(x, v) equals
+        flow_jvp(Zfn(x), encode_pre_jvp(x, v)) bit for bit."""
+        x = _img(images)
+        t = _img(v, 'v')
+        n = x.shape[0]
+        if t.shape[0] != n:
+            raise ValueError("v must be (%d,3,64,64), got %r" % (n, t.shape))
+        dz = np.empty((n, 100), np.float32)
+        z = np.empty((n, 100), np.float32) if return_z else None
+        if n:
+            self._check(self._lib.ian_encode_pre_jvp_host(self._h, _fp(x), _fp(t), n, _fp(z) if z is not None else None,
+                                                          _fp(dz)))
+        return (z, dz) if return_z else dz
+
+    def flow_vjp(self, z_iaf, dz):
+        """Vector-Jacobian product of the MADE/IAF flow (Z_IAF_fn: l_Z_IAF -> l_Z), dz_iaf = (d z / d z_iaf)^T . dz: z_iaf,
+        dz float32 (n,100) -> dz_iaf float32 (n,100).  The gradient in the prior space: for a loss on sample(z_iaf)'s image,
+        flow_vjp(z_iaf, decode_vjp(Z_IAF_fn(z_iaf), dL/dx)).  dz itself on IAN_simple (no flow)."""
+        z0 = _z(z_iaf, 'z_iaf')
+        d = _z(dz, 'dz')
+        n = z0.shape[0]
+        if d.shape[0] != n:
+            raise ValueError("dz must be (%d,100), got %r" % (n, d.shape))
+        out = np.empty_like(z0)
+        if n:
+            self._check(self._lib.ian_flow_vjp_host(self._h, _fp(z0), _fp(d), n, _fp(out)))
+        return out
+
+    def flow_jvp(self, z_iaf, v, return_z=False):
+        """Jacobian-vector product of the MADE/IAF flow, dz = (d z / d z_iaf) . v: z_iaf, v float32 (n,100) -> dz float32
+        (n,100), and z = Z_IAF_fn(z_iaf) bit for bit when return_z (returned as (z, dz)).  How a prior sample's image moves
+        along v: decode_jvp(Z_IAF_fn(z_iaf), flow_jvp(z_iaf, v)).  v itself on IAN_simple (no flow)."""
+        z0 = _z(z_iaf, 'z_iaf')
+        t = _z(v, 'v')
+        n = z0.shape[0]
+        if t.shape[0] != n:
+            raise ValueError("v must be (%d,100), got %r" % (n, t.shape))
+        dz = np.empty_like(z0)
+        z = np.empty_like(z0) if return_z else None
+        if n:
+            self._check(self._lib.ian_flow_jvp_host(self._h, _fp(z0), _fp(t), n, _fp(z) if z is not None else None, _fp(dz)))
+        return (z, dz) if return_z else dz
+
     def edit_steps(self, z, boxes, rgb=None, n_steps=32, weight=0.05):
         """n_steps of the NPE paint rule per sample: Z <- Z - weight*g*(1+(x2-x1)) (reference NPE.py:199-209)."""
         z = _z(z).copy()
@@ -649,6 +730,29 @@ class IAN:
         """device-pointer form of encode_jvp; z_ptr and eps_ptr may be 0"""
         self._check(self._lib.ian_encode_jvp_dev(self._h, x_ptr, v_ptr, int(n), eps_ptr or None, z_ptr or None, dz_ptr,
                                                  stream or None))
+
+    def Zfn_dev(self, x_ptr, n, z_iaf_ptr, stream=0):
+        """device-pointer form of Zfn"""
+        self._check(self._lib.ian_encode_pre_dev(self._h, x_ptr, int(n), z_iaf_ptr, stream or None))
+
+    def flow_dev(self, z_iaf_ptr, n, z_ptr=0, x_ptr=0, stream=0):
+        """device-pointer form of Z_IAF_fn (z_ptr) and sample (x_ptr); either may be 0, not both"""
+        self._check(self._lib.ian_flow_dev(self._h, z_iaf_ptr, int(n), z_ptr or None, x_ptr or None, stream or None))
+
+    def flow_vjp_dev(self, z_iaf_ptr, dz_ptr, n, dz_iaf_ptr, stream=0):
+        self._check(self._lib.ian_flow_vjp_dev(self._h, z_iaf_ptr, dz_ptr, int(n), dz_iaf_ptr, stream or None))
+
+    def flow_jvp_dev(self, z_iaf_ptr, v_ptr, n, dz_ptr, z_ptr=0, stream=0):
+        """device-pointer form of flow_jvp; z_ptr may be 0"""
+        self._check(self._lib.ian_flow_jvp_dev(self._h, z_iaf_ptr, v_ptr, int(n), z_ptr or None, dz_ptr, stream or None))
+
+    def encode_pre_vjp_dev(self, x_ptr, dz_iaf_ptr, n, dx_ptr, stream=0):
+        self._check(self._lib.ian_encode_pre_vjp_dev(self._h, x_ptr, int(n), dz_iaf_ptr, dx_ptr, stream or None))
+
+    def encode_pre_jvp_dev(self, x_ptr, v_ptr, n, dz_iaf_ptr, z_iaf_ptr=0, stream=0):
+        """device-pointer form of encode_pre_jvp; z_iaf_ptr may be 0"""
+        self._check(self._lib.ian_encode_pre_jvp_dev(self._h, x_ptr, v_ptr, int(n), z_iaf_ptr or None, dz_iaf_ptr,
+                                                     stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

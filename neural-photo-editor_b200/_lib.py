@@ -51,6 +51,16 @@ SIGNATURES = {
     "ian_gather_wait_dev": (C.c_int, [_H, C.POINTER(C.c_void_p), C.c_void_p]),
     "ian_encode_pre_host": (C.c_int, [_H, _F, C.c_int, _F]),
     "ian_flow_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
+    "ian_encode_pre_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ian_flow_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_flow_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ian_flow_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F]),
+    "ian_flow_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_flow_jvp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, _F]),
+    "ian_encode_pre_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_encode_pre_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
+    "ian_encode_pre_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_encode_pre_jvp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, _F]),
     "ian_grad_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ian_grad_host": (C.c_int, [_H, _F, _I, _F, C.c_int, C.c_int, _F]),
     "ian_decode_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -355,7 +355,7 @@ struct Plan {
   float *jeg = nullptr, *jeh = nullptr, *jez0 = nullptr;
   Conv1OutMap* jconv1_out = nullptr;
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
-         G_COUNT };
+         G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
   std::vector<void*> allocs;
 };
@@ -1624,13 +1624,16 @@ int ensure_enc_vjp_plan(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
-// the forward (run_encode) on x, then the backward chain; dz (n,100) is the cotangent of what ian_encode_* returns
-int run_encode_vjp(ian_handle* h, Plan* pl, const float* x, const float* eps, const float* dz, float* dx, cudaStream_t st) {
+// the forward (run_encode) on x, then the backward chain.  dz (n,100) is the cotangent of what ian_encode_* returns, taken
+// through the MADE/IAF flow's adjoint first; with pre, it is the cotangent of l_Z_IAF (ian_encode_pre_vjp_*) and the chain
+// starts at the encoder's sample step.
+int run_encode_vjp(ian_handle* h, Plan* pl, const float* x, const float* eps, const float* dz, float* dx, cudaStream_t st,
+                   bool pre = false) {
   const int n = pl->n;
   int rc;
   if ((rc = run_encode(h, pl, x, eps, nullptr, st)) != IAN_OK) return rc;
   const float* dzi = dz;
-  if (has_flow(h)) {
+  if (has_flow(h) && !pre) {
     LAUNCH_TRY(h, launch_made_iaf_bwd(pl->z0, h->made_w, h->made_b, dz, pl->edzi, n, st));
     dzi = pl->edzi;
   }
@@ -1951,11 +1954,14 @@ int ensure_enc_jvp_plan(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
-// the primal (run_encode: the same kernels, so z and the stored activations carry ian_encode_*'s bits), then the tangent chain
-int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, const float* eps, float* z, float* dz, cudaStream_t st) {
+// the primal (run_encode: the same kernels, so z and the stored activations carry ian_encode_*'s bits), then the tangent chain.
+// With pre the chain stops at l_Z_IAF (ian_encode_pre_jvp_*): z (nullable) receives l_Z_IAF as ian_encode_pre_* computes it,
+// and dz its tangent, without the flow's.
+int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, const float* eps, float* z, float* dz, cudaStream_t st,
+                   bool pre = false) {
   const int n = pl->n;
   int rc;
-  if ((rc = run_encode(h, pl, x, eps, z, st)) != IAN_OK) return rc;
+  if ((rc = pre ? run_encode(h, pl, x, eps, pl->z, st, z) : run_encode(h, pl, x, eps, z, st)) != IAN_OK) return rc;
   {
     ScopedTimer tm(h, T_CONV1_TANGENT, st);
     if (h->path == IAN_PATH_TC)
@@ -1969,7 +1975,7 @@ int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, cons
       LAUNCH_TRY(h, launch_enc_fc1_bwd(pl->jeg, pl->f1.p, pl->f1.plane, h->w[L_ENC_FC1].scale, has_flow(h) ? 0 : 1, pl->jef1.p,
                                        pl->jef1.plane, n, st));
   }
-  if (!has_flow(h)) {
+  if (!has_flow(h) || pre) {
     LAUNCH_TRY(h, launch_sample_tangent(pl->head, eps, pl->jeh, dz, n, st));
     return IAN_OK;
   }
@@ -2193,6 +2199,118 @@ int call_encode_jvp(ian_handle* h, bool host, const float* x, const float* v, in
     return c.graphed(Plan::G_ENC_JVP, eps ? 1 : 0, [&] {
       return run_encode_jvp(h, c.pl, c.f(0), c.f(1), c.f(2), c.f(3) ? c.f(3) : c.pl->z, c.f(4), c.st);
     });
+  });
+}
+
+// ---- the sampling script's function set and its derivatives (sample_IAN.py:86-94) ----------------------------------------
+// Zfn: X -> l_Z_IAF (deterministic: mu).  The encoder's kernels with l_Z_IAF kept (run_encode's z_pre); the host form stages
+// it in the plan's eps buffer.
+int call_encode_pre(ian_handle* h, bool host, const float* x, int n, float* z_iaf, void* stream) {
+  int rc = check_ready(h, n, x, z_iaf);
+  if (rc != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z_iaf, kLatentBytes, S_EPS, OUT}}, nullptr,
+                   [&](const Chunk& c) {
+    return c.graphed(Plan::G_ENCODE_PRE, 0, [&] { return run_encode(h, c.pl, c.f(0), nullptr, c.pl->z, c.st, c.f(1)); });
+  });
+}
+
+// l_Z_IAF -> l_Z (Z_IAF_fn) into z_out or the plan's z buffer, and the latent planes; x_out != NULL also decodes them
+// (`sample`).  The host form stages z_iaf in the plan's eps buffer; it decides on the caller's pointers, because it stages
+// every output whether asked for or not.
+int run_flow(ian_handle* h, Plan* pl, const float* z_iaf, float* z, cudaStream_t st) {
+  if (has_flow(h)) {
+    LAUNCH_TRY(h, launch_made_iaf(z_iaf, h->made_w, h->made_b, z, pl->zp.p, pl->zp.plane, pl->n, st));
+    return IAN_OK;
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(z, z_iaf, (size_t)pl->n * 400, cudaMemcpyDeviceToDevice, st));
+  LAUNCH_TRY(h, launch_z_to_planes(z, pl->zp.p, pl->zp.plane, pl->n, st));
+  return IAN_OK;
+}
+
+int call_flow(ian_handle* h, bool host, const float* z_iaf, int n, float* z_out, float* x_out, void* stream) {
+  int rc = check_ready(h, n, z_iaf, z_iaf);
+  if (rc != IAN_OK) return rc;
+  if (!z_out && !x_out) return fail(h, IAN_ERR_INVALID, "both outputs are NULL");
+  return run_entry(h, host, stream, n, {{z_iaf, kLatentBytes, S_EPS, IN}, {z_out, kLatentBytes, S_Z, OUT},
+                                        {x_out, kImageBytes, S_XHAT, OUT}}, nullptr, [&](const Chunk& c) {
+    return c.graphed(Plan::G_FLOW, x_out ? 1 : 0, [&] {
+      int q = run_flow(h, c.pl, c.f(0), z_out ? c.f(1) : c.pl->z, c.st);
+      return q != IAN_OK || !x_out ? q : run_decode_from_planes(h, c.pl, c.f(2), c.st);
+    });
+  });
+}
+
+int check_flow_grad(ian_handle* h, int n, const void* a, const void* b, const void* c) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  if (n > 0 && (!a || !b || !c)) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return IAN_OK;
+}
+
+// dz_iaf = (d l_Z / d l_Z_IAF)^T dz: made_iaf_bwd_kernel on the caller's z_iaf (a copy of dz on IAN_simple).  Needs only the
+// plan's (n,100) buffers: the host form stages z_iaf in its eps buffer, dz in its frame-target buffer and dz_iaf in its z buffer.
+int call_flow_vjp(ian_handle* h, bool host, const float* z_iaf, const float* dz, int n, float* dz_iaf, void* stream) {
+  int rc = check_flow_grad(h, n, z_iaf, dz, dz_iaf);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{z_iaf, kLatentBytes, S_EPS, IN}, {dz, kLatentBytes, S_TARGET, IN},
+                                        {dz_iaf, kLatentBytes, S_Z, OUT}}, nullptr, [&](const Chunk& c) {
+    return c.graphed(Plan::G_FLOW_VJP, 0, [&] {
+      if (has_flow(h))
+        LAUNCH_TRY(h, launch_made_iaf_bwd(c.f(0), h->made_w, h->made_b, c.f(1), c.f(2), c.cn, c.st));
+      else if (c.f(2) != c.f(1))
+        CUDA_TRY(h, cudaMemcpyAsync(c.f(2), c.f(1), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
+      return (int)IAN_OK;
+    });
+  });
+}
+
+// dz = (d l_Z / d l_Z_IAF) . v: made_iaf_tangent_kernel on the caller's z_iaf, after made_iaf_kernel for the primal when z is
+// wanted (v and z_iaf copied on IAN_simple).  The host form stages z_iaf in the eps buffer, v in the frame-target buffer, z in
+// the z buffer and dz in the x_hat buffer.
+int call_flow_jvp(ian_handle* h, bool host, const float* z_iaf, const float* v, int n, float* z, float* dz, void* stream) {
+  int rc = check_flow_grad(h, n, z_iaf, v, dz);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{z_iaf, kLatentBytes, S_EPS, IN}, {v, kLatentBytes, S_TARGET, IN},
+                                        {z, kLatentBytes, S_Z, OUT}, {dz, kLatentBytes, S_XHAT, OUT}}, nullptr,
+                   [&](const Chunk& c) {
+    return c.graphed(Plan::G_FLOW_JVP, z ? 1 : 0, [&] {
+      const size_t bytes = (size_t)c.cn * 400;
+      if (has_flow(h)) {
+        if (z) LAUNCH_TRY(h, launch_made_iaf(c.f(0), h->made_w, h->made_b, c.f(2), nullptr, 0, c.cn, c.st));
+        LAUNCH_TRY(h, launch_made_iaf_tangent(c.f(0), c.f(1), h->made_w, h->made_b, c.f(3), c.cn, c.st));
+        return (int)IAN_OK;
+      }
+      if (z && c.f(2) != c.f(0)) CUDA_TRY(h, cudaMemcpyAsync(c.f(2), c.f(0), bytes, cudaMemcpyDeviceToDevice, c.st));
+      if (c.f(3) != c.f(1)) CUDA_TRY(h, cudaMemcpyAsync(c.f(3), c.f(1), bytes, cudaMemcpyDeviceToDevice, c.st));
+      return (int)IAN_OK;
+    });
+  });
+}
+
+// Zfn's VJP: the encoder VJP's chain seeded with dz_iaf at the sample step, eps absent.  The host form stages dz_iaf in the
+// plan's edz buffer and dx in its x_hat buffer.
+int call_encode_pre_vjp(ian_handle* h, bool host, const float* x, int n, const float* dz_iaf, float* dx, void* stream) {
+  int rc = check_flow_grad(h, n, x, dz_iaf, dx);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {dz_iaf, kLatentBytes, S_EDZ, IN},
+                                        {dx, kImageBytes, S_XHAT, OUT}}, ensure_enc_vjp_plan, [&](const Chunk& c) {
+    return c.graphed(Plan::G_ENC_PRE_VJP, 0,
+                     [&] { return run_encode_vjp(h, c.pl, c.f(0), nullptr, c.f(1), c.f(2), c.st, true); });
+  });
+}
+
+// Zfn's JVP: the encoder JVP's chain up to the tangent of l_Z_IAF, eps absent.  z_iaf is nullable.  The host form stages v in
+// the plan's frame-target buffer, z_iaf in its eps buffer and dz_iaf in its x_hat buffer.
+int call_encode_pre_jvp(ian_handle* h, bool host, const float* x, const float* v, int n, float* z_iaf, float* dz_iaf,
+                        void* stream) {
+  int rc = check_flow_grad(h, n, x, v, dz_iaf);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {v, kImageBytes, S_TARGET, IN},
+                                        {z_iaf, kLatentBytes, S_EPS, OUT}, {dz_iaf, kLatentBytes, S_XHAT, OUT}},
+                   ensure_enc_jvp_plan, [&](const Chunk& c) {
+    return c.graphed(Plan::G_ENC_PRE_JVP, 0,
+                     [&] { return run_encode_jvp(h, c.pl, c.f(0), c.f(1), nullptr, c.f(2), c.f(3), c.st, true); });
   });
 }
 
@@ -2594,52 +2712,42 @@ int ian_reconstruct_wait(ian_handle* h, int ticket) {
   return IAN_OK;
 }
 
-// ---- sample_IAN.py function set (reference sample_IAN.py:86-94) ----------------------------------------
-// Zfn: X -> l_Z_IAF (deterministic: mu).  For IAN_simple there is no flow and this equals ian_encode_host.
-int ian_encode_pre_host(ian_handle* h, const float* x, int n, float* z_iaf) {
-  int rc = check_ready(h, n, x, z_iaf);
-  if (rc != IAN_OK) return rc;
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->x, x + (size_t)off * 12288, (size_t)cn * 12288 * 4, cudaMemcpyHostToDevice, st));
-    int r = run_encode(h, pl, pl->x, nullptr, pl->z, st, pl->eps /*staging for l_Z_IAF*/);
-    if (r != IAN_OK) return r;
-    CUDA_TRY(h, cudaMemcpyAsync(z_iaf + (size_t)off * 100, pl->eps, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
+// ---- sample_IAN.py function set (reference sample_IAN.py:86-94) and its derivatives ---------------------------------------
+int ian_encode_pre_dev(ian_handle* h, const float* x, int n, float* z_iaf, void* stream) {
+  return call_encode_pre(h, false, x, n, z_iaf, stream);
 }
-
-// Z_IAF_fn: l_Z_IAF -> l_Z = (z - MADE_mu(z)) / exp(MADE_ls(z)); identity for IAN_simple.
-// x_out != NULL additionally decodes: `sample` of sample_IAN.py:86 (l_Z_IAF -> X).
-int ian_flow_host(ian_handle* h, const float* z_iaf, int n, float* z_out /*nullable*/, float* x_out /*nullable*/) {
-  int rc = check_ready(h, n, z_iaf, z_iaf);
-  if (rc != IAN_OK) return rc;
-  if (!z_out && !x_out) return fail(h, IAN_ERR_INVALID, "both outputs are NULL");
-  DeviceGuard dg(h->device);
-  cudaStream_t st = h->stream;
-  rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    CUDA_TRY(h, cudaMemcpyAsync(pl->eps, z_iaf + (size_t)off * 100, (size_t)cn * 400, cudaMemcpyHostToDevice, st));
-    if (has_flow(h))
-      LAUNCH_TRY(h, launch_made_iaf(pl->eps, h->made_w, h->made_b, pl->z, pl->zp.p, pl->zp.plane, cn, st));
-    else {
-      CUDA_TRY(h, cudaMemcpyAsync(pl->z, pl->eps, (size_t)cn * 400, cudaMemcpyDeviceToDevice, st));
-      LAUNCH_TRY(h, launch_z_to_planes(pl->z, pl->zp.p, pl->zp.plane, cn, st));
-    }
-    if (z_out) CUDA_TRY(h, cudaMemcpyAsync(z_out + (size_t)off * 100, pl->z, (size_t)cn * 400, cudaMemcpyDeviceToHost, st));
-    if (x_out) {
-      int r = run_decode_from_planes(h, pl, pl->xhat, st);
-      if (r != IAN_OK) return r;
-      CUDA_TRY(h, cudaMemcpyAsync(x_out + (size_t)off * 12288, pl->xhat, (size_t)cn * 12288 * 4, cudaMemcpyDeviceToHost, st));
-    }
-    return (int)IAN_OK;
-  });
-  if (rc != IAN_OK) return rc;
-  CUDA_TRY(h, cudaStreamSynchronize(st));
-  return IAN_OK;
+int ian_encode_pre_host(ian_handle* h, const float* x, int n, float* z_iaf) {
+  return call_encode_pre(h, true, x, n, z_iaf, nullptr);
+}
+int ian_flow_dev(ian_handle* h, const float* z_iaf, int n, float* z_out, float* x_out, void* stream) {
+  return call_flow(h, false, z_iaf, n, z_out, x_out, stream);
+}
+int ian_flow_host(ian_handle* h, const float* z_iaf, int n, float* z_out, float* x_out) {
+  return call_flow(h, true, z_iaf, n, z_out, x_out, nullptr);
+}
+int ian_flow_vjp_dev(ian_handle* h, const float* z_iaf, const float* dz, int n, float* dz_iaf, void* stream) {
+  return call_flow_vjp(h, false, z_iaf, dz, n, dz_iaf, stream);
+}
+int ian_flow_vjp_host(ian_handle* h, const float* z_iaf, const float* dz, int n, float* dz_iaf) {
+  return call_flow_vjp(h, true, z_iaf, dz, n, dz_iaf, nullptr);
+}
+int ian_flow_jvp_dev(ian_handle* h, const float* z_iaf, const float* v, int n, float* z, float* dz, void* stream) {
+  return call_flow_jvp(h, false, z_iaf, v, n, z, dz, stream);
+}
+int ian_flow_jvp_host(ian_handle* h, const float* z_iaf, const float* v, int n, float* z, float* dz) {
+  return call_flow_jvp(h, true, z_iaf, v, n, z, dz, nullptr);
+}
+int ian_encode_pre_vjp_dev(ian_handle* h, const float* x, int n, const float* dz_iaf, float* dx, void* stream) {
+  return call_encode_pre_vjp(h, false, x, n, dz_iaf, dx, stream);
+}
+int ian_encode_pre_vjp_host(ian_handle* h, const float* x, int n, const float* dz_iaf, float* dx) {
+  return call_encode_pre_vjp(h, true, x, n, dz_iaf, dx, nullptr);
+}
+int ian_encode_pre_jvp_dev(ian_handle* h, const float* x, const float* v, int n, float* z_iaf, float* dz_iaf, void* stream) {
+  return call_encode_pre_jvp(h, false, x, v, n, z_iaf, dz_iaf, stream);
+}
+int ian_encode_pre_jvp_host(ian_handle* h, const float* x, const float* v, int n, float* z_iaf, float* dz_iaf) {
+  return call_encode_pre_jvp(h, true, x, v, n, z_iaf, dz_iaf, nullptr);
 }
 
 // ---- fused all-gather of decoded images over NVLink peer memory ---------------------------------------------

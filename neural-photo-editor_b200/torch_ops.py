@@ -11,6 +11,10 @@
     encoder, and a differentiable decode(encode(x)).  Its jvp is the encoder's Jacobian-vector product (ian_encode_jvp_dev),
     so forward mode works through encode and through decode(encode(x)).  eps is a constant input: it gets no gradient or
     tangent, and an eps that requires grad or carries a tangent is refused.
+  * encode_pre(model, x) = Zfn and flow(model, z_iaf) = Z_IAF_fn of the reference's sampling script (sample_IAN.py:91-94):
+    the encoder split at l_Z_IAF, the input of the MADE/IAF flow where the generative prior lives.  Both are differentiable
+    in reverse and forward mode, so decode(model, flow(model, z_iaf)) -- the script's `sample` -- optimises in prior space,
+    and flow(model, encode_pre(model, x)) is encode(model, x) with eps absent.
 
   * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
@@ -174,6 +178,93 @@ def encode(model, x, eps=None):
             raise ValueError("torch_ops.encode does not differentiate w.r.t. eps; pass its primal (eps carries a forward-mode "
                              "tangent)")
     return _encode_function().apply(model, x, eps)
+
+
+_Prior = {}
+
+
+def _prior_function(kind):
+    """the Function of encode_pre (x (n,3,64,64) -> z_iaf) or flow (z_iaf -> z): forward, backward and jvp are one library
+    call each"""
+    if kind in _Prior:
+        return _Prior[kind]
+    import torch
+    from torch.autograd.function import once_differentiable
+    pre = kind == "encode_pre"
+    in_shape, what = ((3, 64, 64), "x") if pre else ((100,), "z_iaf")
+
+    class Prior(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, model, a):
+            _check_tensor(model, a, what)
+            if tuple(a.shape[1:]) != in_shape or a.dim() != 1 + len(in_shape):
+                raise ValueError("%s must be (n,%s), got %r" % (what, ",".join(map(str, in_shape)), tuple(a.shape)))
+            a = a.contiguous()
+            n = int(a.shape[0])
+            z = torch.empty(n, 100, dtype=torch.float32, device=a.device)
+            if n:
+                with _lib_stream(model, a) as st:
+                    if pre:
+                        model.Zfn_dev(a.data_ptr(), n, z.data_ptr(), st)
+                    else:
+                        model.flow_dev(a.data_ptr(), n, z.data_ptr(), 0, st)
+            ctx.model = model
+            ctx.save_for_backward(a)
+            ctx.save_for_forward(a)
+            return z
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            (a,) = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, g, "grad_output")
+            g = g.contiguous()
+            n = int(a.shape[0])
+            da = torch.empty_like(a)
+            if n:
+                with _lib_stream(model, a) as st:
+                    if pre:
+                        model.encode_pre_vjp_dev(a.data_ptr(), g.data_ptr(), n, da.data_ptr(), st)
+                    else:
+                        model.flow_vjp_dev(a.data_ptr(), g.data_ptr(), n, da.data_ptr(), st)
+            return None, da
+
+        @staticmethod
+        def jvp(ctx, _model_t, v):
+            (a,) = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, v, "tangent")
+            v = v.contiguous()
+            n = int(a.shape[0])
+            dz = torch.empty(n, 100, dtype=torch.float32, device=a.device)
+            if n:
+                with _lib_stream(model, a) as st:
+                    if pre:
+                        model.encode_pre_jvp_dev(a.data_ptr(), v.data_ptr(), n, dz.data_ptr(), 0, st)
+                    else:
+                        model.flow_jvp_dev(a.data_ptr(), v.data_ptr(), n, dz.data_ptr(), 0, st)
+            return dz
+
+    _Prior[kind] = Prior
+    return Prior
+
+
+def encode_pre(model, x):
+    """z_iaf = Zfn(x) (model.Zfn: X -> l_Z_IAF, deterministic, before the MADE/IAF flow; encode itself on IAN_simple) for x
+    (n,3,64,64) float32 CUDA on the model's device.  Differentiable w.r.t. x in reverse mode (one ian_encode_pre_vjp_dev call
+    per backward) and forward mode (one ian_encode_pre_jvp_dev call).  flow(model, encode_pre(model, x)) is encode(model, x)
+    with eps absent, in both modes."""
+    return _prior_function("encode_pre").apply(model, x)
+
+
+def flow(model, z_iaf):
+    """z = Z_IAF_fn(z_iaf) (model.Z_IAF_fn: the MADE/IAF flow l_Z_IAF -> l_Z; the identity on IAN_simple) for z_iaf (n,100)
+    float32 CUDA on the model's device.  Differentiable in reverse mode (one ian_flow_vjp_dev call per backward) and forward
+    mode (one ian_flow_jvp_dev call).  decode(model, flow(model, z_iaf)) is the sampling script's `sample` (sample_IAN.py:86),
+    so losses on a prior sample's image -- fitting z_iaf to a photo, a brush loss plus a |z_iaf|^2 prior term -- drive z_iaf
+    through torch.autograd."""
+    return _prior_function("flow").apply(model, z_iaf)
 
 
 def _params_function():

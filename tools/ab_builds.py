@@ -14,6 +14,7 @@
         seeded inputs and synthetic oracle.weights, in one child process per build, and prints per array whether
         build/ab/<REV> ("base") and the in-tree build ("head") give the same bits: the three graphs; the tensor-core path
         by default and with IAN_STREAMK=0, IAN_STREAMK=2 and IAN_GRAPHS=0; the SIMT path; batches 1, 3, 47, 130 and 513.
+        Also the host forms of the sampling script's Zfn, Z_IAF_fn and sample on seeded images and N(0,1) latents.
 """
 import argparse
 import hashlib
@@ -135,7 +136,13 @@ def cmd_dump(out):
     import importlib
     import numpy as np
     sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+    import ctypes
     import test_gpu_launch_forms as lf
+    lib = importlib.import_module("neural-photo-editor_b200._lib")
+    so = ctypes.CDLL(lib.LIB_PATH)
+    for name in list(lib.SIGNATURES):      # an older build lacks the entry points added after it; none of them is called here
+        if not hasattr(so, name):
+            del lib.SIGNATURES[name]
     npe = importlib.import_module("neural-photo-editor_b200")
     res = {}
     for graph in ("simple", "full", "v1"):
@@ -146,11 +153,17 @@ def cmd_dump(out):
             m = npe.IAN(lf.CONFIG[graph], True, weights=lf._weights(graph), path=path)
             cfg = "%s-%s%s" % (graph, path, "".join("-%s=%s" % kv for kv in env.items()))
             for n in OUTPUT_BATCHES:
-                for name, host, dev in lf._pairs(m, npe, lf._inputs(n, 7000 + n)):
-                    for form, a in (("host", host), ("dev", dev)):
-                        a = np.ascontiguousarray(a)
-                        res["%s n=%d %s %s" % (cfg, n, name, form)] = [hashlib.sha256(a.tobytes()).hexdigest(), list(a.shape),
-                                                                       float(np.abs(a.astype(np.float64)).sum())]
+                arrays = [("%s %s" % (name, form), a) for name, host, dev in lf._pairs(m, npe, lf._inputs(n, 7000 + n))
+                          for form, a in (("host", host), ("dev", dev))]
+                # the sampling script's function set (host forms: the only ones older builds have)
+                rng = np.random.default_rng(7100 + n)
+                x = np.tanh(rng.standard_normal((n, 3, 64, 64))).astype(np.float32)
+                zi = rng.standard_normal((n, 100)).astype(np.float32)
+                arrays += [("Zfn host", m.Zfn(x)), ("Z_IAF_fn host", m.Z_IAF_fn(zi)), ("sample host", m.sample(zi))]
+                for name, a in arrays:
+                    a = np.ascontiguousarray(a)
+                    res["%s n=%d %s" % (cfg, n, name)] = [hashlib.sha256(a.tobytes()).hexdigest(), list(a.shape),
+                                                          float(np.abs(a.astype(np.float64)).sum())]
             m.close()
     with open(out, "w") as f:
         json.dump(res, f)
