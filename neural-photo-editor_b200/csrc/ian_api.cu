@@ -208,6 +208,7 @@ struct ian_handle {
   bool coop_finalize = true;   // deep split-K layers: cooperative finalize kernel (IAN_FINALIZE8=0: one thread per output everywhere)
   bool pdl = true;             // programmatic dependent launch along the kernel chains (tapgemm.h; IAN_PDL=0 turns it off)
   bool graphs = true;          // replay small-batch host calls as CUDA graphs (IAN_GRAPHS=0 turns it off)
+  bool epi_tma = true;         // plain tap-GEMM tiles leave through TMA stores (tapgemm.h; IAN_EPI_TMA=0: thread stores)
   bool capturing = false;
   bool finalized = false;
   cudaStream_t stream = nullptr;
@@ -810,6 +811,7 @@ int run_gemm(ian_handle* h, Plan* pl, int l, cudaStream_t st) {
   g.sk_force = h->streamk == 2 ? 1 : 0;
   g.sk_flags = h->sk_flags;
   g.sk_epoch = ++h->sk_epoch;
+  g.epi_tma = h->epi_tma ? 1 : 0;
   ian_handle::Timed tm{};
   if (h->timing) {
     CUDA_TRY(h, cudaEventCreate(&tm.e0));
@@ -2377,6 +2379,7 @@ int ian_create(int model_kind, int device, ian_handle** out) {
   if (const char* c = getenv("IAN_PDL")) h->pdl = atoi(c) != 0;
   if (const char* c = getenv("IAN_FINALIZE8")) h->coop_finalize = atoi(c) != 0;
   if (const char* c = getenv("IAN_GRAPHS")) h->graphs = atoi(c) != 0;
+  if (const char* c = getenv("IAN_EPI_TMA")) h->epi_tma = atoi(c) != 0;
   *out = h;
   return IAN_OK;
 }

@@ -151,6 +151,10 @@ struct TapGemm {
   int* sk_flags;
   int sk_epoch;
   int sk_force;                 // 1: stream-K on every eligible launch, skipping the makespan test (tests use it)
+  // 1: whole tiles of a plain epilogue (scale/shift + none/LReLU/ReLU/ELU into `out` only) leave through TMA stores
+  // straight from the accumulators (tensor-core path, float32 mode).  The caller sets the wish (IAN_EPI_TMA=0 clears
+  // it); launch_tapgemm_tc keeps it only where the layer qualifies.  Both forms compute the same bits.
+  int epi_tma;
 };
 
 // 128-row M tiles are boxes {Nt images, Ht rows, Wt cols} of the (n, p, q) output grid
@@ -178,7 +182,7 @@ __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bflo
 int launch_tapgemm_simt(const TapGemm& g, cudaStream_t st);
 // tensor-core path; maps are built by tc_build_maps() once per plan.  Its K steps run chunk-major: step `it` of a phase
 // is channel chunk it / ntaps of tap it % ntaps (split-K and stream-K ranges are cut on that index).
-struct TcMaps;   // opaque: CUtensorMaps for A views and B
+struct TcMaps;   // opaque: CUtensorMaps for A views, B and (where a map can describe it) the output planes
 TcMaps* tc_build_maps(const TapGemm& g, char* err, int errlen);
 void tc_free_maps(TcMaps*);
 int launch_tapgemm_tc(const TapGemm& g, const TcMaps* maps, cudaStream_t st);

@@ -16,7 +16,9 @@
 //                (in float32 mode 32 columns at a time, in four rounds), and the same eight warps run the epilogue
 //                one pixel row per thread: BatchNorm scale/shift + activation (or backward scale * ReLU-mask),
 //                re-split to bf16 hi/lo planes and store NHWC at the phase's output stride; or store raw sums to
-//                this K split's workspace slab.
+//                this K split's workspace slab.  Plain whole tiles in float32 mode (g.epi_tma) skip the float32
+//                staging: the epilogue runs on the accumulator fragments and each round leaves through TMA stores
+//                that drain while the next tile's MMAs run.
 // Pipeline: STAGES-deep smem ring with full/empty mbarriers (TMA -> wgmma -> release after wgmma.wait_group); the
 // producer runs ahead across work items, so the next tile's operands load while the epilogue of this one runs.
 #include <cuda.h>
@@ -35,6 +37,11 @@ struct TcMaps {
   CUtensorMap b;        // weights, box = {64 ch, BN, 2 planes}
   CUtensorMap a1[4];    // same tensors, hi plane only (single-pass bf16 mode)
   CUtensorMap b1;
+  // the output's hi and lo planes as 5-D views {C, pw, Wq, ph, N*Hq} (the TMA-store epilogue), box {32 ch, 1, Wt, 1, Ht*Nt};
+  // built for o_out / o_plane only, so a launch whose `out` differs keeps the thread-store epilogue
+  CUtensorMap o[2];
+  const __nv_bfloat16* o_out;
+  long long o_plane;
   int Wt, Ht, Nt, BN;
   mutable int sk_choice;   // cached stream-K decision of launch_tapgemm_tc: -1 unknown, 0 whole tiles, 1 stream-K
 };
@@ -63,15 +70,25 @@ template <int BN, int PASSES> struct TcCfg {
   static constexpr int kRound = (PASSES == 3 && BN > 32) ? 32 : BN;
   static constexpr int kRounds = BN / kRound;
   static constexpr int kLd = kRound + 8;                       // staging row pitch in floats (conflict-free fragment stores)
-  static constexpr int kStagingBytes = BM * kLd * 4;
-  static constexpr int kStageSmem = kEpiWarps * 1024;          // per-warp scale|shift staging
-  static constexpr int kStagesFit = (220 * 1024 - kStagingBytes - kStageSmem) / kStageBytes;
+  // float32 mode at BN = 128 may write plain tiles with TMA stores straight from the accumulators (g.epi_tma): one
+  // round's 32 columns as bf16 hi|lo tiles of BM rows x 64 B (64B-swizzled), double-buffered so that a round's
+  // stores drain while the next round (or the next tile's K loop) runs.  The float32 staging tile of the other
+  // epilogues aliases the two buffers.
+  static constexpr bool kTmaEpi = PASSES == 3 && BN == 128;
+  static constexpr int kOutPlaneBytes = BM * kRound * 2;
+  static constexpr int kOutRoundBytes = 2 * kOutPlaneBytes;
+  static constexpr int kStagingBytes = kTmaEpi && 2 * kOutRoundBytes > BM * kLd * 4 ? 2 * kOutRoundBytes : BM * kLd * 4;
+  // scale|shift of the tile's columns: one copy per CTA where the TMA-store buffers need the room, else one per warp
+  static constexpr int kStageSmem = kTmaEpi ? 1024 : kEpiWarps * 1024;
+  static constexpr int kStagesFit = (232448 - 1024 - 256 - kStagingBytes - kStageSmem) / kStageBytes;
   static constexpr int kStages = kStagesFit > 6 ? 6 : kStagesFit;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kStageSmem + kStagingBytes;
   static_assert(kStages >= 2 && kSmemBytes <= 232448, "tapgemm_tc: shared memory budget");
 };
-// float32 mode at BN = 128 runs the heavy layers: one K step's 64 KB load must not be the only one in flight
-static_assert(TcCfg<128, 3>::kStages == 3 && TcCfg<128, 3>::kSmemBytes == 226560, "tapgemm_tc: three float32-mode stages");
+// float32 mode at BN = 128 runs the heavy layers: one K step's 64 KB load must not be the only one in flight, and the
+// TMA-store buffers take their own 32 KB next to the three stages: 3 * 65536 + 32768 + 1024 + 1024 + 256
+static_assert(TcCfg<128, 3>::kStages == 3 && TcCfg<128, 3>::kSmemBytes == 231680, "tapgemm_tc: three float32-mode stages");
+static_assert(TcCfg<128, 3>::kRound == 32 && TcCfg<128, 3>::kOutRoundBytes == 16384, "tapgemm_tc: 32-column TMA-store rounds");
 
 // ---------------------------------------------------------------- kernel
 // Persistent, warp-specialised.  Work items w = blockIdx.x + i*gridDim.x over
@@ -194,13 +211,14 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + S * Cfg::kStageBytes;
+  const uint32_t stg_base = smem_base + S * Cfg::kStageBytes;   // epilogue staging, 1024-aligned (swizzled TMA-store tiles)
+  const uint32_t bar_base = stg_base + Cfg::kStagingBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  const uint32_t stage_smem = bar_base + 256u;       // per-epilogue-warp scale|shift staging: 8 x (128 + 128) floats
+  const uint32_t stage_smem = bar_base + 256u;       // scale|shift of the tile's columns: (1 or 8) x (128 + 128) floats
   uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
   float* stage_ptr = reinterpret_cast<float*>(smem_al + (stage_smem - smem_base));
-  float* acc_tile = stage_ptr + kEpiWarps * 256;     // [BM][kLd] float32: the finished accumulators of one tile
+  float* acc_tile = reinterpret_cast<float*>(smem_al + (stg_base - smem_base));   // [BM][kLd] float32 round staging
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -256,14 +274,14 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
   const int lg = warp & 3;                              // 32-row group of the tile this warp's epilogue handles
   const int half = ew >> 2;                           // which half of a round's columns
   const bool has_cols = RW >= 32 || half == 0;
-  float* my_stage = stage_ptr + ew * 256;             // [0,128): scale, [128,256): shift of the tile's columns
+  float* my_stage = stage_ptr + (Cfg::kTmaEpi ? 0 : ew * 256);   // [0,128): scale, [128,256): shift of the tile's columns
   // activation as a branch-free a*t + b*|t| (none / LeakyRectify(0.2) / rectify; lasagne forms, SURVEY C.5)
   const float act_a = g.act == ACT_LRELU ? 0.6f : g.act == ACT_RELU ? 0.5f : 1.f;
   const float act_b = g.act == ACT_LRELU ? 0.4f : g.act == ACT_RELU ? 0.5f : 0.f;
   const int ml = lg * 32 + lane;                        // tile row of this thread's epilogue
-  const int wl = ml % maps.Wt;
-  const int hl = (ml / maps.Wt) % maps.Ht;
-  const int nl = ml / (maps.Wt * maps.Ht);
+  const int wl0 = ml % maps.Wt;
+  const int hl0 = (ml / maps.Wt) % maps.Ht;
+  const int nl0 = ml / (maps.Wt * maps.Ht);
   uint32_t i = 0;
   WorkIter<BN, SK> iter;
   iter.init(g, maps, total_work);
@@ -271,13 +289,23 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
   while (iter.next(g, maps, wi)) {
     const Phase ph = g.phase[wi.phase];
     if (wi.it1 <= wi.it0) continue;                     // (uniform over the CTA)
-    if (has_cols && g.scale_pix_stride == 0) {          // stage this tile's per-channel scale/shift while the MMAs run
-      __syncwarp();
-      for (int c = lane; c < BN; c += 32) {
-        my_stage[c] = g.scale ? __ldg(g.scale + wi.co0 + c) : 1.f;
-        my_stage[128 + c] = g.shift ? __ldg(g.shift + wi.co0 + c) : 0.f;
+    if (g.scale_pix_stride == 0) {                      // stage this tile's per-channel scale/shift while the MMAs run
+      if constexpr (Cfg::kTmaEpi) {
+        // one copy per CTA: every consumer warp has finished the previous tile's epilogue, which reads it; the first
+        // barrier of this tile's epilogue publishes the new values
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        for (int c = threadIdx.x; c < BN; c += 32 * kEpiWarps) {
+          my_stage[c] = g.scale ? __ldg(g.scale + wi.co0 + c) : 1.f;
+          my_stage[128 + c] = g.shift ? __ldg(g.shift + wi.co0 + c) : 0.f;
+        }
+      } else if (has_cols) {
+        __syncwarp();
+        for (int c = lane; c < BN; c += 32) {
+          my_stage[c] = g.scale ? __ldg(g.scale + wi.co0 + c) : 1.f;
+          my_stage[128 + c] = g.shift ? __ldg(g.shift + wi.co0 + c) : 0.f;
+        }
+        __syncwarp();
       }
-      __syncwarp();
     }
     // ---- main loop: this warpgroup's 64 rows x BN columns (declared per tile: dead during the epilogue)
     float acc_m[R], acc_c[PASSES == 3 ? R : 1];
@@ -317,6 +345,60 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
 #pragma unroll
       for (int j = 0; j < R; ++j) acc_m[j] += acc_c[j];   // main + cross: the one float32 add of every output
     }
+    // ===================== TMA-store epilogue (plain whole tiles, float32 mode) =====================
+    // The same float operations per element as the thread-store epilogue below, run on the accumulator fragments; each
+    // 32-column round is written as bf16 hi|lo into a swizzled staging buffer and leaves through two TMA stores issued by
+    // thread 0.  Nothing waits for those stores here: the warps go on to the next tile and its K loop hides them.
+    // Hazards: (1) a buffer is rewritten only after thread 0's cp.async.bulk.wait_group.read has seen the stores that
+    // read it (round r-2, possibly of the previous tile) and a barrier has passed that on; (2) the generic epilogue's
+    // float32 staging aliases the buffers and waits for every outstanding store first; (3) thread 0 waits for all its
+    // stores to complete before the CTA exits (shared memory must outlive them, and the next kernel's
+    // griddepcontrol.wait relies on this grid's writes being done); (4) the choice is uniform over the CTA.
+    if constexpr (Cfg::kTmaEpi) {
+      if (g.epi_tma && wi.sk_role == 0) {
+#pragma unroll
+        for (int r = 0; r < Cfg::kRounds; ++r) {
+          const uint32_t buf = stg_base + (uint32_t)(r & 1) * Cfg::kOutRoundBytes;
+          if (threadIdx.x == 0) bulk_wait_group_read1();   // (1): every group but the newest (round r-1) has been read
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+          for (int j = 0; j < RW / 2; j += 2) {         // registers [r*RW/2, (r+1)*RW/2) hold this round's columns
+            const float2 a = make_float2(acc_m[r * RW / 2 + j], acc_m[r * RW / 2 + j + 1]);
+            const int row = wg * 64 + frag_row(wtid, j);
+            const int c = frag_col(wtid, j);            // column inside the round (even)
+            const float2 sc = *reinterpret_cast<const float2*>(my_stage + r * RW + c);
+            const float2 sf = *reinterpret_cast<const float2*>(my_stage + 128 + r * RW + c);
+            float v0 = fmaf(a.x, sc.x, sf.x), v1 = fmaf(a.y, sc.y, sf.y);
+            if (g.act == ACT_ELU) {
+              v0 = v0 > 0.f ? v0 : expm1f(v0);
+              v1 = v1 > 0.f ? v1 : expm1f(v1);
+            } else if (g.act != ACT_NONE) {
+              v0 = fmaf(act_b, fabsf(v0), act_a * v0);
+              v1 = fmaf(act_b, fabsf(v1), act_a * v1);
+            }
+            const __nv_bfloat162 hi = __floats2bfloat162_rn(v0, v1);
+            const float2 hf = __bfloat1622float2(hi);
+            const __nv_bfloat162 lo = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
+            // 64-byte rows, 64B swizzle: 16-byte unit c/8 of row `row` sits at unit (c/8) ^ ((row/2) % 4)
+            const uint32_t off = (uint32_t)row * 64u + ((((uint32_t)c >> 3) ^ (((uint32_t)row >> 1) & 3u)) << 4) + ((uint32_t)c & 7u) * 2u;
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + off), "r"(*reinterpret_cast<const uint32_t*>(&hi)) : "memory");
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + Cfg::kOutPlaneBytes + off), "r"(*reinterpret_cast<const uint32_t*>(&lo))
+                         : "memory");
+          }
+          fence_proxy_async_smem();                     // generic-proxy writes -> visible to the TMA store
+          asm volatile("bar.sync 1, 256;" ::: "memory");
+          if (threadIdx.x == 0) {
+            // rows of an image n >= n_img fall outside the map's N*Hq extent and are not written
+            const int c4 = wi.n0 * g.Hg + wi.p0;
+            tma_store_5d(&maps.o[0], buf, wi.co0 + r * RW, ph.ow0, wi.q0, ph.oh0, c4);
+            tma_store_5d(&maps.o[1], buf + Cfg::kOutPlaneBytes, wi.co0 + r * RW, ph.ow0, wi.q0, ph.oh0, c4);
+            bulk_commit_group();
+          }
+        }
+        continue;
+      }
+      if (threadIdx.x == 0) bulk_wait_group_read0();   // (2): the float32 staging below overwrites the store buffers
+    }
     // ===================== epilogue =====================
     if (SK && wi.sk_role == 2 && has_cols) {          // finisher: the later parts were computed first; wait for them
       for (int k = (int)blockIdx.x + 1 + lane; k <= wi.sk_last; k += 32) {
@@ -330,6 +412,17 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
         } while (fv != g.sk_epoch);
       }
       __syncwarp();
+    }
+    // the row's (n, p, q) offsets in the tile; the stream-K float32 form derives them here from a fresh %tid.x rather
+    // than keeping them live across the main loop, whose 128 accumulator registers leave no room for them there
+    int nl = nl0, hl = hl0, wl = wl0;
+    if constexpr (SK && Cfg::kTmaEpi) {
+      uint32_t tid;
+      asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+      const int row = (int)((tid >> 5) & 3u) * 32 + (int)(tid & 31u);
+      wl = row % maps.Wt;
+      hl = (row / maps.Wt) % maps.Ht;
+      nl = row / (maps.Wt * maps.Ht);
     }
     const int n = wi.n0 + nl, p = wi.p0 + hl, q = wi.q0 + wl;
     const bool valid = n < g.n_img;
@@ -488,6 +581,9 @@ tapgemm_tc_kernel(const __grid_constant__ TapGemm g, const __grid_constant__ TcM
       }
     }
   }
+  if constexpr (Cfg::kTmaEpi) {
+    if (threadIdx.x == 0) bulk_wait_group0();          // (3): every TMA-stored byte has landed before the CTA retires
+  }
 }
 
 }  // namespace
@@ -547,6 +643,25 @@ TcMaps* tc_build_maps(const TapGemm& g, char* err, int errlen) {
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { snprintf(err, errlen, "cuTensorMapEncodeTiled(B1) failed: %d", (int)r); delete m; return nullptr; }
   }
+  // Output planes for the TMA-store epilogue, where a map can describe the output: output pixel
+  // (n, p*os_h + oh0, q*os_w + ow0) of NHWC [n][Hout][Wout][C] is element (c, ow0, q, oh0, n*Hg + p) of the view
+  // {C, os_w, Wg, os_h, N*Hg}.  H and N merge because stride(N) = Hg * stride(Hg); a tile's box {32, 1, Wt, 1, Ht*Nt} then
+  // covers its rows in tile order, since Nt > 1 only when Ht = Hg.  One map per plane, so the rows n >= n_img of a
+  // partial last m-tile are clipped at the N*Hg extent instead of landing in the other plane.
+  if (g.out && m->BN == 128 && g.Hout == g.osh * g.Hg && g.Wout == g.osw * g.Wg && (g.out_plane * 2) % 16 == 0 &&
+      (uintptr_t)g.out % 16 == 0) {
+    const cuuint64_t C = (cuuint64_t)g.Cout;
+    cuuint64_t dims[5] = {C, (cuuint64_t)g.osw, (cuuint64_t)g.Wg, (cuuint64_t)g.osh, (cuuint64_t)g.n_img * g.Hg};
+    cuuint64_t strides[4] = {C * 2, C * 2 * g.osw, C * 2 * g.Wout, C * 2 * g.Wout * g.osh};
+    cuuint32_t box[5] = {32, 1, (cuuint32_t)m->Wt, 1, (cuuint32_t)(m->Ht * m->Nt)};
+    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    bool ok = true;
+    for (int pl = 0; pl < 2 && ok; ++pl)
+      ok = enc(&m->o[pl], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)(g.out + pl * g.out_plane), dims, strides, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    if (ok) { m->o_out = g.out; m->o_plane = g.out_plane; }   // otherwise this layer keeps the thread-store epilogue
+  }
   return m;
 }
 
@@ -592,7 +707,15 @@ static int launch_one(const TapGemm& g, const TcMaps* maps, int tiles_m, int num
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
-int launch_tapgemm_tc(const TapGemm& g, const TcMaps* maps, cudaStream_t st) {
+int launch_tapgemm_tc(const TapGemm& g_in, const TcMaps* maps, cudaStream_t st) {
+  // TMA-store epilogue only for plain outputs: float32 mode, whole K, scale/shift + none/LReLU/ReLU/ELU into `out` and
+  // nothing else, into the planes the output maps were built for.  Stream-K tiles cut by a CTA boundary, split-K slabs,
+  // MDBLOCK, the backward mask and the head's tables keep the thread-store epilogue.
+  TapGemm g = g_in;
+  g.epi_tma = g_in.epi_tma && g.passes == 3 && maps->BN == 128 && g.ksplit == 1 && g.out && g.out == maps->o_out &&
+              g.out_plane == maps->o_plane && g.scale_pix_stride == 0 &&
+              (g.act == ACT_NONE || g.act == ACT_LRELU || g.act == ACT_RELU || g.act == ACT_ELU) && !g.out_raw && !g.res &&
+              !g.mask && !g.out_f32 && !g.out_f32_t;
   const int num_sms = tc_num_sms();
   const int tiles_m = (g.Wg / maps->Wt) * (g.Hg / maps->Ht) * ((g.n_img + maps->Nt - 1) / maps->Nt);
   const long long tiles = (long long)tiles_m * (g.Cout / maps->BN) * g.nphase;
