@@ -275,6 +275,36 @@ int ian_decode_jvp_host(ian_handle* h, const float* z, const float* v, int n, fl
 int ian_encode_jvp_dev(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz, void* stream);
 int ian_encode_jvp_host(ian_handle* h, const float* x, const float* v, int n, const float* eps, float* z, float* dz);
 
+/* ---- latent fit: Gauss-Newton normal equations of the decoder and a batched Levenberg-Marquardt fit to images -----------
+ * Per sample: z (100) is the decoder's input l_Z, as for ian_decode_* and ian_decode_jvp_* (on IAN.py / IANv1.py after the
+ * MADE/IAF flow); x (3,64,64) float32 NCHW is the target in [-1,1]; x_hat = ian_decode_*(z) at the call's batch size,
+ * r = x_hat - x (12288 values) and J = d x_hat / d z (12288 x 100), with ian_decode_jvp_*'s derivative conventions.
+ *
+ * ian_decode_gauss_newton_*: A = J^T J (n,100,100; the decoder's pull-back metric, both triangles), g = J^T r (n,100) and
+ *   e = r^T r (n, nullable), float64.  J comes from one batch-100 decoder JVP per sample with the identity as tangents (the
+ *   bits of ian_decode_jvp_* on a 100-row batch, what API.IAN.decoder_jacobian returns); A, g and e are float64 sums of
+ *   exact float64 products of the float32 J and of r formed in float64, added in a fixed order.
+ * ian_fit_latent_*: `iters` Levenberg-Marquardt steps per sample, in place on z (in: the start, out: the fit); loss
+ *   (n, iters+1) float32, nullable, receives e / 12288 (the mean squared error) of the start and after every step.  Each
+ *   step solves (A + lambda D) delta = -g by a float64 Cholesky factorisation, D = diag(max(A_ii, 1e-9 max_j A_jj)), and
+ *   decodes z_trial = float32(z + delta).  If e(z_trial) < e(z) the step is accepted: z <- z_trial, lambda <- max(lambda/10,
+ *   1e-7); otherwise (also when a pivot is not positive) z is unchanged and lambda <- min(10 lambda, 1e10).  lambda starts
+ *   at 1e-3.  These constants are fixed.  e(z) is the float64 sum of (x_hat - x)^2 in one fixed order, so the loss history
+ *   is non-increasing and a step that repeats the previous entry leaves z bit-unchanged.  No host round trip: every
+ *   decision is made on the device, per sample.
+ * Both: all three graphs, both paths; bf16 precision on the flow graphs as for ian_decode_jvp_* (the normal equations and
+ * the solve are float64 in either precision).  n == 0 does nothing; n < 0, iters < 0 or a NULL z, x, A or g ->
+ * IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE.  Deterministic (a repeated call is bit-identical; the device form
+ * computes the host form's bits).  The first call on a handle allocates 5.0 MB (the identity tangents, J and the Gram's
+ * partial sums) and the batch-100 plan with its decoder-JVP tangent planes (what ian_decode_jvp_* allocates at n = 100);
+ * the first call per batch size allocates that plan's normal equations and fit state, about 180 KB per image. */
+int ian_decode_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double* A, double* g,
+                                double* e /*nullable*/, void* stream);
+int ian_decode_gauss_newton_host(ian_handle* h, const float* z, const float* x, int n, double* A, double* g,
+                                 double* e /*nullable*/);
+int ian_fit_latent_dev(ian_handle* h, const float* x, int n, float* z, int iters, float* loss /*nullable*/, void* stream);
+int ian_fit_latent_host(ian_handle* h, const float* x, int n, float* z, int iters, float* loss /*nullable*/);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -356,7 +386,9 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * ian_decode_jvp_* "jvp_<layer>" for the tangent tap-GEMM of each decoder forward layer -- "jvp_l_dec_fc2", "jvp_dec_conv1",
  * "jvp_full_dec_conv1", "jvp_dec_conv2a2", ... -- plus "dec_out_jvp" (IAN_simple) and "rgb_head_jvp" (the head's three
  * convolutions on the tangent of its feature map, IAN.py / IANv1.py); in ian_encode_jvp_* "jvp_enc_conv1" (enc_conv1's
- * tangent) and "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * tangent) and "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head"; in the latent fit "gn_gram"
+ * (the normal equations' Gram of one sample, with its chunk reduction) and "gn_solve" (the Levenberg-Marquardt solve of
+ * the batch)) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

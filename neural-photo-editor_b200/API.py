@@ -14,7 +14,8 @@ batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space 
 `torch_ops.encode`), the encoder JVP `encode_jvp` (torch forward-mode binding: `torch_ops.encode` under
 `torch.autograd.forward_ad`), the encoder Jacobian `encoder_jacobian`, the derivatives of the sampling script's
 functions in the prior space l_Z_IAF -- `flow_vjp` / `flow_jvp` (Z_IAF_fn) and `encode_pre_vjp` / `encode_pre_jvp` (Zfn),
-torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, and `*_dev` variants taking device pointers.
+torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, the decoder's Gauss-Newton normal equations `gauss_newton` and
+the batched Levenberg-Marquardt latent fit `fit_latent`, and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -436,6 +437,43 @@ class IAN:
             self._check(self._lib.ian_decode_jvp_host(self._h, _fp(zk), _fp(eye), 100, None, _fp(J[k])))
         return J
 
+    def gauss_newton(self, z, images):
+        """The decoder's Gauss-Newton normal equations at each latent for the target images: z float32 (n,100), images
+        float32 (n,3,64,64) in [-1,1] -> (A (n,100,100), g (n,100), e (n,)) float64 with r = sample_at(z) - images,
+        A = J^T J (the pull-back metric), g = J^T r and e = r^T r, J = decoder_jacobian(z)'s bits.  z is l_Z, as for
+        sample_at.  Costs one batch-100 decode_jvp per sample."""
+        z = _z(z)
+        x = _img(images)
+        n = z.shape[0]
+        if x.shape[0] != n:
+            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        A = np.empty((n, 100, 100), np.float64)
+        g = np.empty((n, 100), np.float64)
+        e = np.empty((n,), np.float64)
+        if n:
+            d = C.POINTER(C.c_double)
+            self._check(self._lib.ian_decode_gauss_newton_host(self._h, _fp(z), _fp(x), n, A.ctypes.data_as(d),
+                                                               g.ctypes.data_as(d), e.ctypes.data_as(d)))
+        return A, g, e
+
+    def fit_latent(self, images, z0=None, iters=10, return_loss=False):
+        """Fit a latent to each image: `iters` Levenberg-Marquardt steps on |sample_at(z) - images|^2, every decision on the
+        GPU.  images float32 (n,3,64,64) in [-1,1]; z0 float32 (n,100) the start (default: encode_images(images)) -> z
+        float32 (n,100), and with return_loss the per-sample mean squared error of the start and after every step, float32
+        (n, iters+1), non-increasing.  z is l_Z, as for sample_at (on IAN.py / IANv1.py after the MADE/IAF flow)."""
+        x = _img(images)
+        n = x.shape[0]
+        iters = _int_scalar(iters, 'iters')
+        if iters < 0:
+            raise ValueError("iters must not be negative (got %d)" % iters)
+        z = self.encode_images(x) if z0 is None else _z(z0, 'z0').copy()
+        if z.shape[0] != n:
+            raise ValueError("z0 must be (%d,100), got %r" % (n, z.shape))
+        loss = np.empty((n, iters + 1), np.float32)
+        if n:
+            self._check(self._lib.ian_fit_latent_host(self._h, _fp(x), n, _fp(z), iters, _fp(loss)))
+        return (z, loss) if return_loss else z
+
     def param_vjp_names(self):
         """names of the parameters decode_param_vjp returns gradients for, in ian_model_param_spec order: on IAN_simple
         the 13 tensors of train_IAN_simple.py:353 (`decoder_params`); empty on IAN.py / IANv1.py."""
@@ -753,6 +791,15 @@ class IAN:
         """device-pointer form of encode_pre_jvp; z_iaf_ptr may be 0"""
         self._check(self._lib.ian_encode_pre_jvp_dev(self._h, x_ptr, v_ptr, int(n), z_iaf_ptr or None, dz_iaf_ptr,
                                                      stream or None))
+
+    def gauss_newton_dev(self, z_ptr, x_ptr, n, A_ptr, g_ptr, e_ptr=0, stream=0):
+        """device-pointer form of gauss_newton: A (n,100,100), g (n,100), e (n) float64; e_ptr may be 0"""
+        self._check(self._lib.ian_decode_gauss_newton_dev(self._h, z_ptr, x_ptr, int(n), A_ptr, g_ptr, e_ptr or None,
+                                                          stream or None))
+
+    def fit_latent_dev(self, x_ptr, n, z_ptr, iters, loss_ptr=0, stream=0):
+        """device-pointer form of fit_latent: z (n,100) in place (in: the start), loss (n, iters+1) float32; loss_ptr may be 0"""
+        self._check(self._lib.ian_fit_latent_dev(self._h, x_ptr, int(n), z_ptr, int(iters), loss_ptr or None, stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

@@ -105,6 +105,23 @@ int launch_conv1_bwd_tc(const DecOutMaps* maps, float* dx, int n, cudaStream_t s
 // decoder JVP on the tensor-core path: decout_tc's GEMM + col2im on the tangent planes of h3 (maps built by decout_build_maps
 // on them, with dec_out's weights), epilogue dx_hat = y * (1 - x_hat^2) from the primal x_hat
 int launch_dec_out_jvp_tc(const DecOutMaps* maps, const float* xhat, float* dxhat, int n, cudaStream_t st);
+// latent fit (gn_kernels.cu, ian_decode_gauss_newton_* / ian_fit_latent_*).  The Levenberg-Marquardt constants, fixed:
+// lambda starts at 1e-3, is divided by 10 on an accepted step (not below 1e-7) and multiplied by 10 on a rejected one (not
+// above 1e10); the damping is lambda * diag(max(A_ii, 1e-9 * max_j A_jj)).
+constexpr double kGnLambda0 = 1e-3, kGnLambdaMin = 1e-7, kGnLambdaMax = 1e10, kGnLambdaFactor = 10.0, kGnDampFloor = 1e-9;
+size_t gn_part_doubles();                              // the Gram's chunk partials, per JVP pass
+// z (100) -> zrep (100,100), every row z
+int launch_gn_replicate(const float* z, float* zrep, cudaStream_t st);
+// J (100,12288) float32, x_hat and x (12288) -> A (100,100), g (100), e (nullable) float64, via part (gn_part_doubles())
+int launch_gn_gram(const float* J, const float* xh, const float* x, double* part, double* A, double* g, double* e,
+                   cudaStream_t st);
+// per sample k < n: A (n,100,100), g (n,100), lambda (n) float64, z (n,100) -> z_trial (n,100), ok (n): 0 = rejected step
+int launch_gn_solve(const double* A, const double* g, const double* lam, const float* z, float* zt, int* ok, int n,
+                    cudaStream_t st);
+// per sample: e_trial from x_hat_trial and x (n,12288), then accept or reject (init: set e, lambda from the start) and
+// loss[k * ldl + col] (nullable) = e / 12288
+int launch_gn_accept(int init, const float* xht, const float* x, float* xh, double* e, double* lam, float* z, const float* zt,
+                     const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

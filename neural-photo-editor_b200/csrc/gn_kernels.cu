@@ -1,0 +1,262 @@
+// gn_kernels.cu -- the kernels of the latent fit (ian_decode_gauss_newton_*, ian_fit_latent_*; DESIGN section 5.6i).
+// Per sample, with J the decoder's Jacobian at z as 100 rows of 12288 pixels (decode_jvp's output with the identity as
+// tangents) and r = x_hat - x:
+//   gn_replicate     : z -> the 100 x 100 batch of the Jacobian's JVP pass (every row z)
+//   gn_gram          : partial sums of the upper triangle of [J | r]^T [J | r] over 16 pixel chunks, float64
+//   gn_gram_reduce   : the chunk partials added in chunk order -> A = J^T J (both triangles), g = J^T r, e = r^T r
+//   gn_solve         : Levenberg-Marquardt step: Cholesky of A + lambda D in float64, delta = -(A + lambda D)^-1 g,
+//                      z_trial = float32(z + delta), or a rejected step when a pivot is not positive
+//   gn_accept        : e_trial = |x_hat(z_trial) - x|^2 in a fixed order; accept / reject, lambda, the loss history
+// Operands are float32; every product is formed in float64, where a product of two float32 values is exact, so A, g and e
+// differ from a float64 Gram of the same J and r only by summation order.
+#include "edge.h"
+
+namespace ian {
+
+namespace {
+
+constexpr int kPix = 12288;             // 3 x 64 x 64
+constexpr int kLat = 100;
+constexpr int kBlk = 32;                // the Gram's output blocks are 32 x 32
+constexpr int kNBlk = 4;                // ceil(101 / 32): rows 0..99 are J, row 100 is r, the rest zero
+constexpr int kPairs = kNBlk * (kNBlk + 1) / 2;   // blocks (bi <= bj) of the upper triangle
+constexpr int kChunks = 16;             // pixel chunks per sample: kPairs x kChunks = 160 CTAs
+constexpr int kChunkPix = kPix / kChunks;
+constexpr int kSub = 64;                // pixels staged in shared memory per step
+constexpr int kLd = kLat + 1;           // row stride of the solver's matrix in shared memory
+
+__device__ __forceinline__ double gram_row(const float* __restrict__ J, const float* __restrict__ xh,
+                                           const float* __restrict__ x, int row, int p) {
+  if (row < kLat) return (double)J[(size_t)row * kPix + p];
+  if (row == kLat) return (double)xh[p] - (double)x[p];
+  return 0.0;
+}
+
+__global__ void __launch_bounds__(256) gn_replicate_kernel(const float* __restrict__ z, float* __restrict__ zrep) {
+  pdl_trigger();
+  pdl_wait();                                           // tapgemm.h: PDL
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < kLat * kLat) zrep[i] = z[i % kLat];
+}
+
+// grid (kPairs, kChunks), 256 threads, each a 2 x 2 tile of the 32 x 32 output block; part[chunk][pair][32][32]
+__global__ void __launch_bounds__(256) gn_gram_kernel(const float* __restrict__ J, const float* __restrict__ xh,
+                                                      const float* __restrict__ x, double* __restrict__ part) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ double sa[kSub][kBlk + 1], sb[kSub][kBlk + 1];
+  int q = blockIdx.x, bi = 0;
+  while (q >= kNBlk - bi) { q -= kNBlk - bi; ++bi; }
+  const int bj = bi + q, chunk = blockIdx.y, t = threadIdx.x;
+  const int ti = (t >> 4) * 2, tj = (t & 15) * 2;
+  double acc00 = 0.0, acc01 = 0.0, acc10 = 0.0, acc11 = 0.0;
+  for (int p0 = chunk * kChunkPix; p0 < (chunk + 1) * kChunkPix; p0 += kSub) {
+    for (int e = t; e < kBlk * kSub; e += 256) {
+      const int r = e / kSub, p = e % kSub;
+      sa[p][r] = gram_row(J, xh, x, bi * kBlk + r, p0 + p);
+      sb[p][r] = gram_row(J, xh, x, bj * kBlk + r, p0 + p);
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int p = 0; p < kSub; ++p) {
+      const double a0 = sa[p][ti], a1 = sa[p][ti + 1], b0 = sb[p][tj], b1 = sb[p][tj + 1];
+      acc00 = fma(a0, b0, acc00);
+      acc01 = fma(a0, b1, acc01);
+      acc10 = fma(a1, b0, acc10);
+      acc11 = fma(a1, b1, acc11);
+    }
+    __syncthreads();
+  }
+  double* o = part + ((size_t)(chunk * kPairs + blockIdx.x) * kBlk + ti) * kBlk + tj;
+  o[0] = acc00;
+  o[1] = acc01;
+  o[kBlk] = acc10;
+  o[kBlk + 1] = acc11;
+}
+
+// one thread per (i, j) of the 101 x 101 Gram: (i, j) and (j, i) add the same partials in the same order, so A is exactly
+// symmetric
+__global__ void __launch_bounds__(256) gn_gram_reduce_kernel(const double* __restrict__ part, double* __restrict__ A,
+                                                             double* __restrict__ g, double* __restrict__ e) {
+  pdl_trigger();
+  pdl_wait();
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (kLat + 1) * (kLat + 1)) return;
+  const int i = idx / (kLat + 1), j = idx % (kLat + 1);
+  const int lo = min(i, j), hi = max(i, j), bi = lo / kBlk, bj = hi / kBlk;
+  const int pair = bi * kNBlk - bi * (bi - 1) / 2 + (bj - bi);
+  const double* p = part + ((size_t)pair * kBlk + lo % kBlk) * kBlk + hi % kBlk;
+  double s = 0.0;
+  for (int c = 0; c < kChunks; ++c) s += p[(size_t)c * kPairs * kBlk * kBlk];
+  if (i < kLat && j < kLat) A[i * kLat + j] = s;
+  else if (i < kLat) g[i] = s;
+  else if (i == kLat && j == kLat && e) *e = s;
+}
+
+// one CTA per sample; dynamic shared memory: the 100 x kLd float64 matrix
+__global__ void __launch_bounds__(256) gn_solve_kernel(const double* __restrict__ A, const double* __restrict__ g,
+                                                       const double* __restrict__ lam, const float* __restrict__ z,
+                                                       float* __restrict__ zt, int* __restrict__ ok) {
+  pdl_trigger();
+  pdl_wait();
+  extern __shared__ double M[];
+  __shared__ double b[kLat];
+  __shared__ double dmax;
+  __shared__ int bad;
+  const int k = blockIdx.x, t = threadIdx.x;
+  const double* Ak = A + (size_t)k * kLat * kLat;
+  if (t == 0) {
+    double m = 0.0;
+    for (int i = 0; i < kLat; ++i) m = fmax(m, Ak[i * (kLat + 1)]);
+    dmax = m;
+    bad = 0;
+  }
+  __syncthreads();
+  const double l = lam[k], dfloor = kGnDampFloor * dmax;
+  for (int e = t; e < kLat * kLat; e += 256) {
+    const int i = e / kLat, j = e % kLat;
+    double v = Ak[e];
+    if (i == j) v += l * fmax(v, dfloor);
+    M[i * kLd + j] = v;
+  }
+  for (int i = t; i < kLat; i += 256) b[i] = -g[(size_t)k * kLat + i];
+  __syncthreads();
+  // Cholesky M = L L^T, right-looking, L in the lower triangle; every element is updated by one thread in column order
+  for (int c = 0; c < kLat; ++c) {
+    if (t == 0) {
+      const double d = M[c * kLd + c];
+      if (!(d > 0.0)) bad = 1;                            // also NaN
+      M[c * kLd + c] = sqrt(d);
+    }
+    __syncthreads();
+    if (bad) break;
+    const double dc = M[c * kLd + c];
+    for (int i = c + 1 + t; i < kLat; i += 256) M[i * kLd + c] /= dc;
+    __syncthreads();
+    const int m = kLat - 1 - c;
+    for (int e = t; e < m * m; e += 256) {
+      const int i = c + 1 + e / m, j = c + 1 + e % m;
+      if (j <= i) M[i * kLd + j] = fma(-M[i * kLd + c], M[j * kLd + c], M[i * kLd + j]);
+    }
+    __syncthreads();
+  }
+  if (!bad) {
+    for (int c = 0; c < kLat; ++c) {                      // L y = -g
+      if (t == 0) b[c] /= M[c * kLd + c];
+      __syncthreads();
+      for (int i = c + 1 + t; i < kLat; i += 256) b[i] = fma(-M[i * kLd + c], b[c], b[i]);
+      __syncthreads();
+    }
+    for (int c = kLat - 1; c >= 0; --c) {                 // L^T delta = y
+      if (t == 0) b[c] /= M[c * kLd + c];
+      __syncthreads();
+      for (int i = t; i < c; i += 256) b[i] = fma(-M[c * kLd + i], b[c], b[i]);
+      __syncthreads();
+    }
+  }
+  float v = 0.f;
+  int fin = 1;
+  if (t < kLat) {
+    v = z[(size_t)k * kLat + t];
+    if (!bad) {
+      const float w = (float)((double)v + b[t]);
+      fin = isfinite(w);
+      v = w;
+    }
+  }
+  const int good = !bad && __syncthreads_and(fin);
+  if (t < kLat) zt[(size_t)k * kLat + t] = good ? v : z[(size_t)k * kLat + t];
+  if (t == 0) ok[k] = good;
+}
+
+// one CTA per sample.  init: x_hat_trial is the start's decode (x_hat itself): e, lambda and loss column 0 are set.
+// Otherwise accept when the step was solved and e_trial < e: z <- z_trial, x_hat <- x_hat_trial, e <- e_trial,
+// lambda <- max(lambda / 10, min); else lambda <- min(10 lambda, max).  loss[k * ldl + col] = e / 12288 after the decision.
+__global__ void __launch_bounds__(256) gn_accept_kernel(int init, const float* __restrict__ xht, const float* __restrict__ x,
+                                                        float* xh, double* __restrict__ e, double* __restrict__ lam,
+                                                        float* __restrict__ z, const float* __restrict__ zt,
+                                                        const int* __restrict__ ok, float* __restrict__ loss, long long ldl,
+                                                        int col) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ double red[256];
+  __shared__ int acc;
+  const int k = blockIdx.x, t = threadIdx.x;
+  const float* a = xht + (size_t)k * kPix;
+  const float* b = x + (size_t)k * kPix;
+  double s = 0.0;
+  for (int p = t; p < kPix; p += 256) {
+    const double d = (double)a[p] - (double)b[p];
+    s = fma(d, d, s);
+  }
+  red[t] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (t < w) red[t] += red[t + w];
+    __syncthreads();
+  }
+  if (t == 0) {
+    const double et = red[0];
+    int take = 0;
+    if (init) {
+      e[k] = et;
+      lam[k] = kGnLambda0;
+    } else {
+      take = ok[k] && et < e[k];
+      if (take) {
+        e[k] = et;
+        lam[k] = fmax(lam[k] / kGnLambdaFactor, kGnLambdaMin);
+      } else {
+        lam[k] = fmin(lam[k] * kGnLambdaFactor, kGnLambdaMax);
+      }
+    }
+    if (loss) loss[(size_t)k * ldl + col] = (float)(e[k] / (double)kPix);
+    acc = take;
+  }
+  __syncthreads();
+  if (!acc) return;
+  for (int p = t; p < kPix; p += 256) xh[(size_t)k * kPix + p] = a[p];
+  if (t < kLat) z[(size_t)k * kLat + t] = zt[(size_t)k * kLat + t];
+}
+
+constexpr size_t kSolveSmem = (size_t)kLat * kLd * sizeof(double);
+
+}  // namespace
+
+size_t gn_part_doubles() { return (size_t)kChunks * kPairs * kBlk * kBlk; }
+
+int launch_gn_replicate(const float* z, float* zrep, cudaStream_t st) {
+  if (launch_pdl(gn_replicate_kernel, dim3((kLat * kLat + 255) / 256), dim3(256), 0, st, z, zrep) != cudaSuccess) return -1;
+  return 1;
+}
+
+int launch_gn_gram(const float* J, const float* xh, const float* x, double* part, double* A, double* g, double* e,
+                   cudaStream_t st) {
+  if (launch_pdl(gn_gram_kernel, dim3(kPairs, kChunks), dim3(256), 0, st, J, xh, x, part) != cudaSuccess) return -1;
+  if (launch_pdl(gn_gram_reduce_kernel, dim3(((kLat + 1) * (kLat + 1) + 255) / 256), dim3(256), 0, st, (const double*)part, A,
+                 g, e) != cudaSuccess)
+    return -1;
+  return 2;
+}
+
+int launch_gn_solve(const double* A, const double* g, const double* lam, const float* z, float* zt, int* ok, int n,
+                    cudaStream_t st) {
+  static DeviceOnce attr_set;
+  const int dev = cur_device();
+  if (!attr_set.is_done(dev)) {
+    if (cudaFuncSetAttribute(gn_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveSmem) != cudaSuccess)
+      return -1;
+    attr_set.set_done(dev);
+  }
+  if (launch_pdl(gn_solve_kernel, dim3(n), dim3(256), kSolveSmem, st, A, g, lam, z, zt, ok) != cudaSuccess) return -1;
+  return 1;
+}
+
+int launch_gn_accept(int init, const float* xht, const float* x, float* xh, double* e, double* lam, float* z, const float* zt,
+                     const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st) {
+  if (launch_pdl(gn_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, xh, e, lam, z, zt, ok, loss, ldl, col) != cudaSuccess)
+    return -1;
+  return 1;
+}
+
+}  // namespace ian

@@ -164,6 +164,7 @@ enum LayerId {
   T_WGRAD_FC2, T_WGRAD_CONV1, T_WGRAD_CONV2, T_WGRAD_CONV3, T_WGRAD_DEC_OUT,   // weight gradients of the parameter VJP
   T_DEC_OUT_JVP,                                        // IAN_simple's dec_out in the decoder JVP
   T_CONV1_TANGENT,                                      // enc_conv1's tangent in the encoder JVP
+  T_GN_GRAM, T_GN_SOLVE,                                // the latent fit's Gram (with its chunk reduction) and LM solve
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -181,7 +182,7 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
-                                    "dec_out_jvp", "jvp_enc_conv1"};
+                                    "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -260,6 +261,10 @@ struct ian_handle {
   int head_dy_start[10] = {0};              // taps sorted by row offset: taps with dy = -4 + i are [dy_start[i], dy_start[i+1])
   int head_dx[33] = {0};
   std::map<int, Plan*> plans;
+  // latent fit (ian_decode_gauss_newton_*, ian_fit_latent_*; allocated on the first call): the JVP pass's identity tangents
+  // and replicated latent (100,100), the Jacobian J (100,3,64,64) it writes, and the Gram's chunk partials
+  float *gn_eye = nullptr, *gn_zrep = nullptr, *gn_J = nullptr;
+  double* gn_part = nullptr;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -355,6 +360,14 @@ struct Plan {
   Planes jea[4], jef1;
   float *jeg = nullptr, *jeh = nullptr, *jez0 = nullptr;
   Conv1OutMap* jconv1_out = nullptr;
+  // latent fit (allocated on the plan's first ian_decode_gauss_newton_* / ian_fit_latent_* call): the normal equations A, g
+  // and the Gram's e; per sample the fit's state -- e, lambda, x_hat at z -- and its trial z, x_hat and solve flag; the host
+  // form's loss history (grown to the largest iteration count asked for)
+  bool gn = false;
+  double *gnA = nullptr, *gng = nullptr, *gne = nullptr, *fe = nullptr, *flam = nullptr;
+  float *fxh = nullptr, *fxt = nullptr, *fzt = nullptr, *floss = nullptr;
+  int* fok = nullptr;
+  long long floss_cap = 0;
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -768,6 +781,7 @@ void free_plan(Plan* pl) {
   if (pl->jdecout_maps) decout_free_maps(pl->jdecout_maps);
   if (pl->jhead_maps) head_free_maps(pl->jhead_maps);
   if (pl->jconv1_out) conv1_free_out_map(pl->jconv1_out);
+  cudaFree(pl->floss);
   for (auto& gs : pl->graph) if (gs.exec) cudaGraphExecDestroy(gs.exec);
   delete pl;
 }
@@ -1991,7 +2005,7 @@ int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, cons
 //   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
 //   host form (ian_*_host): per chunk, the caller's inputs are copied into plan buffers, the body runs on those, its kernel
 //   chain (Chunk::graphed) replayed as a CUDA graph on small plans, the outputs are copied back; then one synchronise.
-enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ };
+enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ, S_GN_A, S_GN_G, S_GN_E };
 void* stage_buf(Plan* pl, int s) {
   switch (s) {
     case S_X: return pl->x;
@@ -2000,6 +2014,9 @@ void* stage_buf(Plan* pl, int s) {
     case S_XHAT: return pl->xhat;
     case S_BOXES: return pl->boxes;
     case S_TARGET: return pl->target;
+    case S_GN_A: return pl->gnA;
+    case S_GN_G: return pl->gng;
+    case S_GN_E: return pl->gne;
     default: return pl->edz;
   }
 }
@@ -2342,6 +2359,127 @@ int call_edit_loop(ian_handle* h, bool host, float* z, const int32_t* boxes, con
   });
 }
 
+// ---- latent fit: Levenberg-Marquardt on the decoder's Gauss-Newton normal equations (DESIGN section 5.6i) ----------------
+// r = x_hat - x comes from run_decode on the caller's batch plan, so x_hat has ian_decode_*'s bits at that batch size.  J
+// comes from run_decode_jvp on the 100-row plan that decoder_jacobian uses -- the latent replicated 100 times, the identity
+// as tangents -- one sample per pass, so the JVP's memory stays what a batch-100 ian_decode_jvp_* call allocates, plus the
+// 4.9 MB J buffer on the handle.  The first call on a handle allocates the handle's buffers and the 100-row plan's tangent
+// planes; the first call on a plan its normal equations and fit state (about 180 KB per image); all before any launch.
+int ensure_gn_plan(ian_handle* h, Plan* pl) {
+  int rc;
+  if (!h->gn_part) {
+    std::vector<float> eye(10000, 0.f);
+    for (int i = 0; i < 100; ++i) eye[i * 101] = 1.f;
+    if ((rc = put_dev(h, h->gn_eye, eye.data(), eye.size() * sizeof(float))) != IAN_OK) return rc;
+    if (!h->gn_zrep) CUDA_TRY(h, cudaMalloc((void**)&h->gn_zrep, 10000 * sizeof(float)));
+    if (!h->gn_J) CUDA_TRY(h, cudaMalloc((void**)&h->gn_J, (size_t)100 * 12288 * sizeof(float)));
+    CUDA_TRY(h, cudaMalloc((void**)&h->gn_part, gn_part_doubles() * sizeof(double)));
+  }
+  Plan* jp = nullptr;
+  if ((rc = get_plan(h, 100, &jp)) != IAN_OK || (rc = ensure_jvp_plan(h, jp)) != IAN_OK) return rc;
+  if (pl->gn) return IAN_OK;
+  const long long N = pl->n;
+  if ((rc = alloc_buf(h, pl, pl->gnA, N * 10000)) != IAN_OK || (rc = alloc_buf(h, pl, pl->gng, N * 100)) != IAN_OK ||
+      (rc = alloc_buf(h, pl, pl->gne, N)) != IAN_OK || (rc = alloc_buf(h, pl, pl->fe, N)) != IAN_OK ||
+      (rc = alloc_buf(h, pl, pl->flam, N)) != IAN_OK || (rc = alloc_buf(h, pl, pl->fxh, N * 12288)) != IAN_OK ||
+      (rc = alloc_buf(h, pl, pl->fxt, N * 12288)) != IAN_OK || (rc = alloc_buf(h, pl, pl->fzt, N * 100)) != IAN_OK ||
+      (rc = alloc_buf(h, pl, pl->fok, N)) != IAN_OK)
+    return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  pl->gn = true;
+  return IAN_OK;
+}
+
+// A (n,100,100), g (n,100) and e (n, nullable) of n samples at z, with x_hat = decode(z) already in xh
+int run_normal_eqs(ian_handle* h, int n, const float* z, const float* x, const float* xh, double* A, double* g, double* e,
+                   cudaStream_t st) {
+  Plan* jp = nullptr;
+  int rc = get_plan(h, 100, &jp);
+  if (rc != IAN_OK) return rc;
+  for (int k = 0; k < n; ++k) {
+    LAUNCH_TRY(h, launch_gn_replicate(z + (size_t)k * 100, h->gn_zrep, st));
+    if ((rc = run_decode_jvp(h, jp, h->gn_zrep, h->gn_eye, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+    ScopedTimer tm(h, T_GN_GRAM, st);
+    LAUNCH_TRY(h, launch_gn_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, h->gn_part, A + (size_t)k * 10000,
+                                 g + (size_t)k * 100, e ? e + k : nullptr, st));
+  }
+  return IAN_OK;
+}
+
+// iters Levenberg-Marquardt steps in place on z (pl->n samples); loss (nullable) row k receives e / 12288 of the start and
+// after every step, row stride iters + 1.  The fit's e is only ever set from gn_accept_kernel's reduction, so the history
+// cannot increase.
+int run_fit(ian_handle* h, Plan* pl, const float* x, float* z, int iters, float* loss, cudaStream_t st) {
+  const int n = pl->n;
+  const long long ldl = (long long)iters + 1;
+  int rc;
+  if ((rc = run_decode(h, pl, z, pl->fxh, st)) != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_gn_accept(1, pl->fxh, x, pl->fxh, pl->fe, pl->flam, z, nullptr, nullptr, loss, ldl, 0, n, st));
+  for (int it = 0; it < iters; ++it) {
+    if ((rc = run_normal_eqs(h, n, z, x, pl->fxh, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
+    {
+      ScopedTimer tm(h, T_GN_SOLVE, st);
+      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, z, pl->fzt, pl->fok, n, st));
+    }
+    if ((rc = run_decode(h, pl, pl->fzt, pl->fxt, st)) != IAN_OK) return rc;
+    LAUNCH_TRY(h, launch_gn_accept(0, pl->fxt, x, pl->fxh, pl->fe, pl->flam, z, pl->fzt, pl->fok, loss, ldl, it + 1, n, st));
+  }
+  return IAN_OK;
+}
+
+int check_fit_args(ian_handle* h, int n) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  return IAN_OK;
+}
+
+// No CUDA graphs: the JVP passes run on the 100-row plan, whose schedule (stream-K) a capture would change, so both forms
+// launch the same kernels.  The host form stages z in the plan's z buffer, x in its image buffer and A, g, e in the plan's
+// own normal-equation buffers.
+int call_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, int n, double* A, double* g, double* e,
+                      void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!z || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {A, 80000, S_GN_A, OUT},
+                                        {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_gn_plan, [&](const Chunk& c) {
+    const int r = run_decode(h, c.pl, c.f(0), c.pl->fxh, c.st);
+    return r != IAN_OK ? r : run_normal_eqs(h, c.cn, c.f(0), c.f(1), c.pl->fxh, (double*)c.p[2], (double*)c.p[3],
+                                            c.p[4] ? (double*)c.p[4] : c.pl->gne, c.st);
+  });
+}
+
+// The host form stages x in the plan's image buffer and z in its z buffer; the loss history in a plan buffer grown to the
+// largest (chunk, iters) asked for.
+int call_fit_latent(ian_handle* h, bool host, const float* x, int n, float* z, int iters, float* loss, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
+  if (n == 0) return IAN_OK;
+  if (!x || !z) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  const size_t ldl = (size_t)iters + 1;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z, kLatentBytes, S_Z, INOUT}}, ensure_gn_plan,
+                   [&](const Chunk& c) {
+    float* l = loss && !host ? loss + (size_t)c.off * ldl : nullptr;
+    const long long need = (long long)(c.cn * ldl);
+    if (loss && host) {
+      if (c.pl->floss_cap < need) {
+        CUDA_TRY(h, cudaFree(c.pl->floss));
+        c.pl->floss = nullptr;
+        c.pl->floss_cap = 0;
+        CUDA_TRY(h, cudaMalloc((void**)&c.pl->floss, (size_t)need * sizeof(float)));
+        c.pl->floss_cap = need;
+      }
+      l = c.pl->floss;
+    }
+    const int r = run_fit(h, c.pl, c.f(0), c.f(1), iters, l, c.st);
+    if (r == IAN_OK && loss && host)
+      CUDA_TRY(h, cudaMemcpyAsync(loss + (size_t)c.off * ldl, l, (size_t)need * sizeof(float), cudaMemcpyDeviceToHost, c.st));
+    return r;
+  });
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -2477,6 +2615,7 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->made_w); cudaFree(h->made_b); cudaFree(h->head_taps); cudaFree(h->head_wgb); cudaFree(h->head_wbb);
   cudaFree(h->head_tc_wt);
   cudaFree(h->train_ws);
+  cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -2627,6 +2766,20 @@ int ian_encode_vjp_dev(ian_handle* h, const float* x, int n, const float* eps, c
 }
 int ian_encode_vjp_host(ian_handle* h, const float* x, int n, const float* eps, const float* dz, float* dx) {
   return call_encode_vjp(h, true, x, n, eps, dz, dx, nullptr);
+}
+
+int ian_decode_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double* A, double* g, double* e,
+                                void* stream) {
+  return call_gauss_newton(h, false, z, x, n, A, g, e, stream);
+}
+int ian_decode_gauss_newton_host(ian_handle* h, const float* z, const float* x, int n, double* A, double* g, double* e) {
+  return call_gauss_newton(h, true, z, x, n, A, g, e, nullptr);
+}
+int ian_fit_latent_dev(ian_handle* h, const float* x, int n, float* z, int iters, float* loss, void* stream) {
+  return call_fit_latent(h, false, x, n, z, iters, loss, stream);
+}
+int ian_fit_latent_host(ian_handle* h, const float* x, int n, float* z, int iters, float* loss) {
+  return call_fit_latent(h, true, x, n, z, iters, loss, nullptr);
 }
 
 int ian_edit_loop_dev(ian_handle* h, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
