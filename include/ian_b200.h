@@ -361,12 +361,17 @@ int ian_paint_stroke_host(ian_handle* h, float* z, const int32_t* box, const flo
  *
  * BatchNorm with BATCH statistics = lasagne BatchNormLayer.get_output_for(deterministic=False), i.e. every BN(...) of
  * reference IAN_simple.py:84-170 / layers.py:411-416 in training.  x is (n, c, hw) (NCHW with hw = H*W; dense layers: hw = 1).
- *   ian_bn_batch_stats_dev      per-channel sum and sum of squares (float64 [c] each) over (n, hw): warp-shuffle reductions,
- *                               fixed order, bit-reproducible.  Data-parallel ranks all-reduce the two arrays here
+ *   ian_bn_batch_stats_dev      per-channel sum and sum of squares (float64 [c] each) over (n, hw), accumulated in float64
+ *                               from the first term (every partial, per thread included): warp-shuffle reductions, fixed
+ *                               order, bit-reproducible.  Data-parallel ranks all-reduce the two arrays here
  *                               (cross-GPU synchronised BN) and pass the GLOBAL element count to the second call.
  *   ian_bn_train_normalize_dev  mean = sum/count, inv_std = 1/sqrt(sumsq/count - mean^2 + eps)  (biased variance);
  *                               y = (x - mean) * (gamma * inv_std) + beta;  running_mean / running_inv_std (nullable) are
  *                               updated in place: r <- (1 - alpha) r + alpha * batch value.  lasagne: eps 1e-4, alpha 0.1.
+ *                               Accuracy: the variance's float64 cancellation, relative ~1e-16 (|mean|/std)^2; then the
+ *                               float32 roundings of mean, gamma * inv_std and x - mean, which the reference also performs.
+ *                               A constant channel gives y = beta exactly.
+ * The three calls share one workspace per handle, so, like every other entry point, a handle serves one stream at a time.
  * ian_minibatch_discrim_dev     MinibatchLayer.get_output_for(init=False) of reference layers.py:486-524:
  *                               x (n,d), theta (d,K,P), log_weight_scale (K,P), b (K) -> out (n, d+K) = [x | f]. */
 int ian_bn_batch_stats_dev(ian_handle* h, const float* x, int n, int c, int hw, double* sum, double* sumsq, void* stream);

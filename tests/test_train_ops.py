@@ -1,7 +1,9 @@
 """Training-mode pieces (SURVEY 8f rank 4): BatchNorm with batch statistics and the MinibatchLayer forward.
 
 CPU part: the float64 oracle (oracle/train_numpy.py) against tests/golden/ref_exec_train.npz -- the reference's own
-MinibatchLayer class executed from the original project, and lasagne's training-mode batch_norm through the stand-in.
+MinibatchLayer class executed from the original project, and lasagne's training-mode batch_norm through the stand-in --
+and against tests/golden/ref_exec_train_edges.npz, the same at the kernels' shape and data edges.  The GPU edges and
+tight bounds are in tests/test_gpu_train_ops.py.
 GPU part: the CUDA ops through the C-ABI against the same fixture and against the oracle at training-size shapes
 (batch 128 conv activations; the 16384 -> 100x5 minibatch discrimination of IAN_simple.py:225-231).
 Tolerance: 2e-5 relative to the output scale (float32 data, float64-accumulated statistics)."""
@@ -15,6 +17,7 @@ from oracle import train_numpy as tn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = np.load(os.path.join(ROOT, "tests", "golden", "ref_exec_train.npz"))
+EDGES = np.load(os.path.join(ROOT, "tests", "golden", "ref_exec_train_edges.npz"))
 
 
 def test_oracle_matches_the_executed_reference_minibatch_layer():
@@ -34,6 +37,22 @@ def test_oracle_matches_training_mode_batch_norm():
         assert np.allclose(rm, 0.1 * x.astype(np.float64).mean(axes)) and np.allclose(ris, 0.9 + 0.1 * inv_std)
         yn = (y - REF["bn_%s_beta" % tag].reshape([1, -1] + [1] * (x.ndim - 2))) / REF["bn_%s_gamma" % tag].reshape([1, -1] + [1] * (x.ndim - 2))
         assert np.abs(yn.mean(axes)).max() <= 1e-9 and np.abs(yn.var(axes) - 1).max() <= 1e-3   # eps = 1e-4 inside the sqrt
+
+
+def test_oracle_matches_the_executed_reference_at_the_kernel_edges():
+    """tests/golden/ref_exec_train_edges.npz: the reference's MinibatchLayer at n = 1, K = P = 1 and K = 13, P = 5 with
+    d = 33, and training-mode batch_norm on an offset (mean 1000, std 1) and a constant (1000.1) channel."""
+    for tag in ("n1", "k1p1", "k13p5"):
+        g = lambda k: EDGES["mb_%s_%s" % (tag, k)]
+        out = tn.minibatch_layer(g("x"), g("theta"), g("lws"), g("b"))
+        assert out.shape == g("out").shape == (len(g("x")), 33 + len(g("b"))), tag
+        assert np.abs(out - g("out")).max() <= 1e-12, tag
+    assert np.array_equal(EDGES["mb_n1_out"][0, 33:], EDGES["mb_n1_b"].astype(np.float64))      # no pair but the self-pair
+    x = EDGES["bn_x"]
+    y, _, _, mean, inv_std = tn.batch_norm_train(x, EDGES["bn_gamma"], EDGES["bn_beta"], np.zeros(2), np.ones(2))
+    assert np.abs(y - EDGES["bn_y"]).max() <= 1e-12
+    assert abs(mean[0] - 1000) < 0.1 and mean[1] == np.float64(np.float32(1000.1)) and inv_std[1] == 1 / np.sqrt(1e-4)
+    assert np.all(EDGES["bn_y"][:, 1] == np.float64(EDGES["bn_beta"][1]))                           # constant channel: y = beta
 
 
 @pytest.mark.gpu
