@@ -305,6 +305,41 @@ int ian_decode_gauss_newton_host(ian_handle* h, const float* z, const float* x, 
 int ian_fit_latent_dev(ian_handle* h, const float* x, int n, float* z, int iters, float* loss /*nullable*/, void* stream);
 int ian_fit_latent_host(ian_handle* h, const float* x, int n, float* z, int iters, float* loss /*nullable*/);
 
+/* ---- masked latent fit under the prior: pixel-weighted Levenberg-Marquardt with a Gaussian prior in the sampling space --
+ * Per sample the fit runs in the fit space u (100): l_Z on IAN_simple, l_Z_IAF on IAN.py / IANv1.py (where the sampling
+ * script draws N(0, I)), with z = F(u) the MADE/IAF flow of ian_flow_* (the identity on IAN_simple).  With x_hat =
+ * decode(F(u)) (the bits of ian_flow_* with x_out at the call's batch size), r = x_hat - x, w (3,64,64) float32 per-pixel
+ * weights (NULL: all ones) and prior = beta >= 0 (a double; the pixel-noise variance of a Gaussian likelihood, so the
+ * minimiser is the MAP latent under N(0, I)):
+ *   E(u) = sum_p w_p r_p^2 + beta |u|^2,   J_u = d x_hat / d u = J_dec(F(u)) J_F(u)   (12288 x 100)
+ * Pixels with w_p == 0 contribute exactly nothing: they are skipped, so x may hold anything there, NaN included.
+ * ian_map_gauss_newton_*: A = J_u^T W J_u + beta I (n,100,100, both triangles), g = J_u^T W r + beta u (n,100) and e = E(u)
+ *   (n, nullable), float64.  J_u comes from one batch-100 pass per sample: u replicated 100 times, the flow's JVP with the
+ *   identity as tangents (ian_flow_jvp_*'s kernels), then the decoder JVP with those columns as tangents; on IAN_simple
+ *   exactly ian_decode_gauss_newton_*'s pass.  w multiplies one factor of every product (exact in float64), A, g and e are
+ *   summed in a fixed order and the prior terms are added once, after the pixel sums.
+ * ian_fit_latent_map_*: `iters` Levenberg-Marquardt steps per sample in place on u (in: the start, out: the fit), with
+ *   ian_fit_latent_*'s solve, damping, constants and accept / reject rule applied to this A, g and E; trial steps decode
+ *   F(u_trial).  z_out (n,100, nullable) receives F(u) of the final u with the bits of ian_flow_* (the l_Z that
+ *   ian_decode_*, the brush gradients and the paint stroke take); loss (n, iters+1, nullable) receives E / 12288, prior
+ *   term included, of the start and after every step: non-increasing, and a flat entry leaves u bit-unchanged.
+ * With w = NULL and prior = 0 on IAN_simple both compute ian_decode_gauss_newton_* / ian_fit_latent_*'s bits; w of all ones
+ * computes w = NULL's bits on every graph.
+ * Both: all three graphs, both paths; bf16 precision on the flow graphs.  n == 0 does nothing; n < 0, iters < 0, a negative
+ * or non-finite prior, or a NULL u, x, A or g -> IAN_ERR_INVALID; the host forms also reject a negative or non-finite
+ * weight with IAN_ERR_INVALID (the device forms take w as given); not finalized -> IAN_ERR_STATE.  Deterministic (a
+ * repeated call is bit-identical; the device form computes the host form's bits).  Memory: what ian_fit_latent_*
+ * allocates, shared with it -- the first call on a handle 5.0 MB and the batch-100 plan with its decoder-JVP tangent planes,
+ * plus 80 KB of flow rows on IAN.py / IANv1.py; the first call per batch size about 180 KB per image. */
+int ian_map_gauss_newton_dev(ian_handle* h, const float* u, const float* x, const float* w /*nullable*/, double prior, int n,
+                             double* A, double* g, double* e /*nullable*/, void* stream);
+int ian_map_gauss_newton_host(ian_handle* h, const float* u, const float* x, const float* w /*nullable*/, double prior, int n,
+                              double* A, double* g, double* e /*nullable*/);
+int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int n, float* u,
+                           float* z_out /*nullable*/, int iters, float* loss /*nullable*/, void* stream);
+int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int n, float* u,
+                            float* z_out /*nullable*/, int iters, float* loss /*nullable*/);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -393,7 +428,8 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * convolutions on the tangent of its feature map, IAN.py / IANv1.py); in ian_encode_jvp_* "jvp_enc_conv1" (enc_conv1's
  * tangent) and "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head"; in the latent fit "gn_gram"
  * (the normal equations' Gram of one sample, with its chunk reduction) and "gn_solve" (the Levenberg-Marquardt solve of
- * the batch)) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * the batch); in the masked fit "map_gram" (the weighted Gram of one sample, with its reduction and the prior terms) and
+ * "gn_solve") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

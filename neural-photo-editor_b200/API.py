@@ -15,7 +15,8 @@ batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space 
 `torch.autograd.forward_ad`), the encoder Jacobian `encoder_jacobian`, the derivatives of the sampling script's
 functions in the prior space l_Z_IAF -- `flow_vjp` / `flow_jvp` (Z_IAF_fn) and `encode_pre_vjp` / `encode_pre_jvp` (Zfn),
 torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, the decoder's Gauss-Newton normal equations `gauss_newton` and
-the batched Levenberg-Marquardt latent fit `fit_latent`, and `*_dev` variants taking device pointers.
+the batched Levenberg-Marquardt latent fit `fit_latent`, their pixel-weighted forms under the N(0, I) prior in the sampling
+space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -474,6 +475,62 @@ class IAN:
             self._check(self._lib.ian_fit_latent_host(self._h, _fp(x), n, _fp(z), iters, _fp(loss)))
         return (z, loss) if return_loss else z
 
+    def _map_args(self, images, weights, prior):
+        x = _img(images)
+        w = None if weights is None else _img(weights, 'weights')
+        if w is not None and w.shape != x.shape:
+            raise ValueError("weights must be %r, got %r" % (x.shape, w.shape))
+        prior = float(prior)
+        if not (np.isfinite(prior) and prior >= 0):
+            raise ValueError("prior must be finite and >= 0 (got %r)" % prior)
+        return x, w, prior
+
+    def gauss_newton_map(self, u, images, weights=None, prior=0.0):
+        """The normal equations of the masked fit under the prior at each fit-space point u: u float32 (n,100) (l_Z on
+        IAN_simple, l_Z_IAF on IAN.py / IANv1.py, as `sample` takes it), images float32 (n,3,64,64), weights float32
+        (n,3,64,64) finite and >= 0 (None: all ones; pixels of weight 0 are ignored, whatever the image holds there), prior
+        beta >= 0 -> (A (n,100,100), g (n,100), e (n,)) float64 with r = sample(u) - images, J_u = d sample / d u,
+        A = J_u^T W J_u + beta I, g = J_u^T W r + beta u and e = r^T W r + beta |u|^2."""
+        u = _z(u, 'u')
+        x, w, prior = self._map_args(images, weights, prior)
+        n = u.shape[0]
+        if x.shape[0] != n:
+            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        A = np.empty((n, 100, 100), np.float64)
+        g = np.empty((n, 100), np.float64)
+        e = np.empty((n,), np.float64)
+        if n:
+            d = C.POINTER(C.c_double)
+            self._check(self._lib.ian_map_gauss_newton_host(self._h, _fp(u), _fp(x), _fp(w) if w is not None else None, prior,
+                                                            n, A.ctypes.data_as(d), g.ctypes.data_as(d), e.ctypes.data_as(d)))
+        return A, g, e
+
+    def fit_latent_map(self, images, weights=None, prior=0.0, u0=None, iters=10, return_loss=False):
+        """Fit the sampling-space latent to each image under pixel weights and the N(0, I) prior: `iters`
+        Levenberg-Marquardt steps on sum_p w_p (sample(u) - images)_p^2 + prior |u|^2, every decision on the GPU.  Zero
+        weights mask pixels out (inpainting: the masked region is filled by the decoder).  u0 float32 (n,100) the start
+        (default: Zfn of the images with every zero-weight element set to 0, so masked content never reaches it) ->
+        (u float32 (n,100), z = Z_IAF_fn(u) float32 (n,100), the l_Z that sample_at / grad / paint_stroke take), and with
+        return_loss the per-sample objective / 12288 of the start and after every step, float32 (n, iters+1),
+        non-increasing."""
+        x, w, prior = self._map_args(images, weights, prior)
+        n = x.shape[0]
+        iters = _int_scalar(iters, 'iters')
+        if iters < 0:
+            raise ValueError("iters must not be negative (got %d)" % iters)
+        if u0 is None:
+            u = self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x))
+        else:
+            u = _z(u0, 'u0').copy()
+        if u.shape[0] != n:
+            raise ValueError("u0 must be (%d,100), got %r" % (n, u.shape))
+        z = np.empty((n, 100), np.float32)
+        loss = np.empty((n, iters + 1), np.float32)
+        if n:
+            self._check(self._lib.ian_fit_latent_map_host(self._h, _fp(x), _fp(w) if w is not None else None, prior, n, _fp(u),
+                                                          _fp(z), iters, _fp(loss)))
+        return (u, z, loss) if return_loss else (u, z)
+
     def param_vjp_names(self):
         """names of the parameters decode_param_vjp returns gradients for, in ian_model_param_spec order: on IAN_simple
         the 13 tensors of train_IAN_simple.py:353 (`decoder_params`); empty on IAN.py / IANv1.py."""
@@ -800,6 +857,17 @@ class IAN:
     def fit_latent_dev(self, x_ptr, n, z_ptr, iters, loss_ptr=0, stream=0):
         """device-pointer form of fit_latent: z (n,100) in place (in: the start), loss (n, iters+1) float32; loss_ptr may be 0"""
         self._check(self._lib.ian_fit_latent_dev(self._h, x_ptr, int(n), z_ptr, int(iters), loss_ptr or None, stream or None))
+
+    def gauss_newton_map_dev(self, u_ptr, x_ptr, w_ptr, prior, n, A_ptr, g_ptr, e_ptr=0, stream=0):
+        """device-pointer form of gauss_newton_map: A (n,100,100), g (n,100), e (n) float64; w_ptr and e_ptr may be 0"""
+        self._check(self._lib.ian_map_gauss_newton_dev(self._h, u_ptr, x_ptr, w_ptr or None, float(prior), int(n), A_ptr, g_ptr,
+                                                       e_ptr or None, stream or None))
+
+    def fit_latent_map_dev(self, x_ptr, w_ptr, prior, n, u_ptr, iters, z_ptr=0, loss_ptr=0, stream=0):
+        """device-pointer form of fit_latent_map: u (n,100) in place (in: the start), z (n,100) = F(u), loss (n, iters+1)
+        float32; w_ptr, z_ptr and loss_ptr may be 0"""
+        self._check(self._lib.ian_fit_latent_map_dev(self._h, x_ptr, w_ptr or None, float(prior), int(n), u_ptr, z_ptr or None,
+                                                     int(iters), loss_ptr or None, stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

@@ -122,6 +122,13 @@ int launch_gn_solve(const double* A, const double* g, const double* lam, const f
 // loss[k * ldl + col] (nullable) = e / 12288
 int launch_gn_accept(int init, const float* xht, const float* x, float* xh, double* e, double* lam, float* z, const float* zt,
                      const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st);
+// the masked fit under the prior (ian_map_gauss_newton_* / ian_fit_latent_map_*): launch_gn_gram and launch_gn_accept with
+// the pixel weight w (nullable: all ones; w == 0 pixels skipped) and the prior weight beta on the fit-space point u (100):
+// A = J^T W J + beta I, g = J^T W r + beta u, e = r^T W r + beta |u|^2
+int launch_map_gram(const float* J, const float* xh, const float* x, const float* w, double beta, const float* u, double* part,
+                    double* A, double* g, double* e, cudaStream_t st);
+int launch_map_accept(int init, const float* xht, const float* x, const float* w, double beta, float* xh, double* e, double* lam,
+                      float* u, const float* ut, const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

@@ -9,6 +9,11 @@
 //   gn_accept        : e_trial = |x_hat(z_trial) - x|^2 in a fixed order; accept / reject, lambda, the loss history
 // Operands are float32; every product is formed in float64, where a product of two float32 values is exact, so A, g and e
 // differ from a float64 Gram of the same J and r only by summation order.
+// The masked fit under the prior (ian_map_gauss_newton_*, ian_fit_latent_map_*; DESIGN section 5.6j) runs the same bodies
+// with a pixel weight w and a prior weight beta: map_gram weights one factor of every product by w (exact in float64),
+// map_gram_reduce adds beta I, beta u and beta |u|^2 after the chunk sums, and map_accept reduces
+// sum_p w_p (x_hat_p - x_p)^2 + beta |u|^2.  Pixels with w_p == 0 are staged or summed as nothing at all, so x there may
+// hold anything, NaN included.  The unweighted kernels instantiate the bodies without a weight.
 #include "edge.h"
 
 namespace ian {
@@ -39,9 +44,11 @@ __global__ void __launch_bounds__(256) gn_replicate_kernel(const float* __restri
   if (i < kLat * kLat) zrep[i] = z[i % kLat];
 }
 
-// grid (kPairs, kChunks), 256 threads, each a 2 x 2 tile of the 32 x 32 output block; part[chunk][pair][32][32]
-__global__ void __launch_bounds__(256) gn_gram_kernel(const float* __restrict__ J, const float* __restrict__ xh,
-                                                      const float* __restrict__ x, double* __restrict__ part) {
+// grid (kPairs, kChunks), 256 threads, each a 2 x 2 tile of the 32 x 32 output block; part[chunk][pair][32][32].
+// kMap: w (nullable: all ones) multiplies the first factor of every product; a pixel with w == 0 stages zeros in both.
+template <bool kMap>
+__device__ __forceinline__ void gram_body(const float* __restrict__ J, const float* __restrict__ xh,
+                                          const float* __restrict__ x, const float* __restrict__ w, double* __restrict__ part) {
   pdl_trigger();
   pdl_wait();
   __shared__ double sa[kSub][kBlk + 1], sb[kSub][kBlk + 1];
@@ -53,8 +60,14 @@ __global__ void __launch_bounds__(256) gn_gram_kernel(const float* __restrict__ 
   for (int p0 = chunk * kChunkPix; p0 < (chunk + 1) * kChunkPix; p0 += kSub) {
     for (int e = t; e < kBlk * kSub; e += 256) {
       const int r = e / kSub, p = e % kSub;
-      sa[p][r] = gram_row(J, xh, x, bi * kBlk + r, p0 + p);
-      sb[p][r] = gram_row(J, xh, x, bj * kBlk + r, p0 + p);
+      if (kMap && w) {
+        const double wp = (double)w[p0 + p];
+        sa[p][r] = wp == 0.0 ? 0.0 : wp * gram_row(J, xh, x, bi * kBlk + r, p0 + p);
+        sb[p][r] = wp == 0.0 ? 0.0 : gram_row(J, xh, x, bj * kBlk + r, p0 + p);
+      } else {
+        sa[p][r] = gram_row(J, xh, x, bi * kBlk + r, p0 + p);
+        sb[p][r] = gram_row(J, xh, x, bj * kBlk + r, p0 + p);
+      }
     }
     __syncthreads();
 #pragma unroll 8
@@ -74,10 +87,29 @@ __global__ void __launch_bounds__(256) gn_gram_kernel(const float* __restrict__ 
   o[kBlk + 1] = acc11;
 }
 
+__global__ void __launch_bounds__(256) gn_gram_kernel(const float* __restrict__ J, const float* __restrict__ xh,
+                                                      const float* __restrict__ x, double* __restrict__ part) {
+  gram_body<false>(J, xh, x, nullptr, part);
+}
+
+__global__ void __launch_bounds__(256) map_gram_kernel(const float* __restrict__ J, const float* __restrict__ xh,
+                                                       const float* __restrict__ x, const float* __restrict__ w,
+                                                       double* __restrict__ part) {
+  gram_body<true>(J, xh, x, w, part);
+}
+
+// beta |u|^2 of one sample's float32 u (100), in one fixed order
+__device__ __forceinline__ double prior_sq(const float* __restrict__ u) {
+  double s = 0.0;
+  for (int i = 0; i < kLat; ++i) s = fma((double)u[i], (double)u[i], s);
+  return s;
+}
+
 // one thread per (i, j) of the 101 x 101 Gram: (i, j) and (j, i) add the same partials in the same order, so A is exactly
-// symmetric
-__global__ void __launch_bounds__(256) gn_gram_reduce_kernel(const double* __restrict__ part, double* __restrict__ A,
-                                                             double* __restrict__ g, double* __restrict__ e) {
+// symmetric.  kMap: then A_ii += beta, g_i += beta u_i, e += beta |u|^2, each added once.
+template <bool kMap>
+__device__ __forceinline__ void gram_reduce_body(const double* __restrict__ part, double beta, const float* __restrict__ u,
+                                                 double* __restrict__ A, double* __restrict__ g, double* __restrict__ e) {
   pdl_trigger();
   pdl_wait();
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -88,9 +120,20 @@ __global__ void __launch_bounds__(256) gn_gram_reduce_kernel(const double* __res
   const double* p = part + ((size_t)pair * kBlk + lo % kBlk) * kBlk + hi % kBlk;
   double s = 0.0;
   for (int c = 0; c < kChunks; ++c) s += p[(size_t)c * kPairs * kBlk * kBlk];
-  if (i < kLat && j < kLat) A[i * kLat + j] = s;
-  else if (i < kLat) g[i] = s;
-  else if (i == kLat && j == kLat && e) *e = s;
+  if (i < kLat && j < kLat) A[i * kLat + j] = kMap && i == j ? s + beta : s;
+  else if (i < kLat) g[i] = kMap ? fma(beta, (double)u[i], s) : s;
+  else if (i == kLat && j == kLat && e) *e = kMap ? fma(beta, prior_sq(u), s) : s;
+}
+
+__global__ void __launch_bounds__(256) gn_gram_reduce_kernel(const double* __restrict__ part, double* __restrict__ A,
+                                                             double* __restrict__ g, double* __restrict__ e) {
+  gram_reduce_body<false>(part, 0.0, nullptr, A, g, e);
+}
+
+__global__ void __launch_bounds__(256) map_gram_reduce_kernel(const double* __restrict__ part, double beta,
+                                                              const float* __restrict__ u, double* __restrict__ A,
+                                                              double* __restrict__ g, double* __restrict__ e) {
+  gram_reduce_body<true>(part, beta, u, A, g, e);
 }
 
 // one CTA per sample; dynamic shared memory: the 100 x kLd float64 matrix
@@ -172,11 +215,12 @@ __global__ void __launch_bounds__(256) gn_solve_kernel(const double* __restrict_
 // one CTA per sample.  init: x_hat_trial is the start's decode (x_hat itself): e, lambda and loss column 0 are set.
 // Otherwise accept when the step was solved and e_trial < e: z <- z_trial, x_hat <- x_hat_trial, e <- e_trial,
 // lambda <- max(lambda / 10, min); else lambda <- min(10 lambda, max).  loss[k * ldl + col] = e / 12288 after the decision.
-__global__ void __launch_bounds__(256) gn_accept_kernel(int init, const float* __restrict__ xht, const float* __restrict__ x,
-                                                        float* xh, double* __restrict__ e, double* __restrict__ lam,
-                                                        float* __restrict__ z, const float* __restrict__ zt,
-                                                        const int* __restrict__ ok, float* __restrict__ loss, long long ldl,
-                                                        int col) {
+// kMap: e_trial = sum over w != 0 of w (x_hat_trial - x)^2 (w nullable: all ones) + beta |z_trial|^2 (init: |z|^2).
+template <bool kMap>
+__device__ __forceinline__ void accept_body(int init, const float* __restrict__ xht, const float* __restrict__ x,
+                                            const float* __restrict__ w, double beta, float* xh, double* __restrict__ e,
+                                            double* __restrict__ lam, float* __restrict__ z, const float* __restrict__ zt,
+                                            const int* __restrict__ ok, float* __restrict__ loss, long long ldl, int col) {
   pdl_trigger();
   pdl_wait();
   __shared__ double red[256];
@@ -184,19 +228,28 @@ __global__ void __launch_bounds__(256) gn_accept_kernel(int init, const float* _
   const int k = blockIdx.x, t = threadIdx.x;
   const float* a = xht + (size_t)k * kPix;
   const float* b = x + (size_t)k * kPix;
+  const float* wk = kMap && w ? w + (size_t)k * kPix : nullptr;
   double s = 0.0;
   for (int p = t; p < kPix; p += 256) {
-    const double d = (double)a[p] - (double)b[p];
-    s = fma(d, d, s);
+    if (kMap && wk) {
+      const double wp = (double)wk[p];
+      if (wp == 0.0) continue;
+      const double d = (double)a[p] - (double)b[p];
+      s = fma(wp * d, d, s);
+    } else {
+      const double d = (double)a[p] - (double)b[p];
+      s = fma(d, d, s);
+    }
   }
   red[t] = s;
   __syncthreads();
-  for (int w = 128; w > 0; w >>= 1) {
-    if (t < w) red[t] += red[t + w];
+  for (int half = 128; half > 0; half >>= 1) {
+    if (t < half) red[t] += red[t + half];
     __syncthreads();
   }
   if (t == 0) {
-    const double et = red[0];
+    double et = red[0];
+    if (kMap) et = fma(beta, prior_sq((init ? z : zt) + (size_t)k * kLat), et);
     int take = 0;
     if (init) {
       e[k] = et;
@@ -219,6 +272,23 @@ __global__ void __launch_bounds__(256) gn_accept_kernel(int init, const float* _
   if (t < kLat) z[(size_t)k * kLat + t] = zt[(size_t)k * kLat + t];
 }
 
+__global__ void __launch_bounds__(256) gn_accept_kernel(int init, const float* __restrict__ xht, const float* __restrict__ x,
+                                                        float* xh, double* __restrict__ e, double* __restrict__ lam,
+                                                        float* __restrict__ z, const float* __restrict__ zt,
+                                                        const int* __restrict__ ok, float* __restrict__ loss, long long ldl,
+                                                        int col) {
+  accept_body<false>(init, xht, x, nullptr, 0.0, xh, e, lam, z, zt, ok, loss, ldl, col);
+}
+
+__global__ void __launch_bounds__(256) map_accept_kernel(int init, const float* __restrict__ xht, const float* __restrict__ x,
+                                                         const float* __restrict__ w, double beta, float* xh,
+                                                         double* __restrict__ e, double* __restrict__ lam,
+                                                         float* __restrict__ z, const float* __restrict__ zt,
+                                                         const int* __restrict__ ok, float* __restrict__ loss, long long ldl,
+                                                         int col) {
+  accept_body<true>(init, xht, x, w, beta, xh, e, lam, z, zt, ok, loss, ldl, col);
+}
+
 constexpr size_t kSolveSmem = (size_t)kLat * kLd * sizeof(double);
 
 }  // namespace
@@ -239,6 +309,15 @@ int launch_gn_gram(const float* J, const float* xh, const float* x, double* part
   return 2;
 }
 
+int launch_map_gram(const float* J, const float* xh, const float* x, const float* w, double beta, const float* u, double* part,
+                    double* A, double* g, double* e, cudaStream_t st) {
+  if (launch_pdl(map_gram_kernel, dim3(kPairs, kChunks), dim3(256), 0, st, J, xh, x, w, part) != cudaSuccess) return -1;
+  if (launch_pdl(map_gram_reduce_kernel, dim3(((kLat + 1) * (kLat + 1) + 255) / 256), dim3(256), 0, st, (const double*)part,
+                 beta, u, A, g, e) != cudaSuccess)
+    return -1;
+  return 2;
+}
+
 int launch_gn_solve(const double* A, const double* g, const double* lam, const float* z, float* zt, int* ok, int n,
                     cudaStream_t st) {
   static DeviceOnce attr_set;
@@ -255,6 +334,14 @@ int launch_gn_solve(const double* A, const double* g, const double* lam, const f
 int launch_gn_accept(int init, const float* xht, const float* x, float* xh, double* e, double* lam, float* z, const float* zt,
                      const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st) {
   if (launch_pdl(gn_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, xh, e, lam, z, zt, ok, loss, ldl, col) != cudaSuccess)
+    return -1;
+  return 1;
+}
+
+int launch_map_accept(int init, const float* xht, const float* x, const float* w, double beta, float* xh, double* e, double* lam,
+                      float* u, const float* ut, const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st) {
+  if (launch_pdl(map_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, w, beta, xh, e, lam, u, ut, ok, loss, ldl, col) !=
+      cudaSuccess)
     return -1;
   return 1;
 }

@@ -165,6 +165,7 @@ enum LayerId {
   T_DEC_OUT_JVP,                                        // IAN_simple's dec_out in the decoder JVP
   T_CONV1_TANGENT,                                      // enc_conv1's tangent in the encoder JVP
   T_GN_GRAM, T_GN_SOLVE,                                // the latent fit's Gram (with its chunk reduction) and LM solve
+  T_MAP_GRAM,                                           // the masked fit's weighted Gram (with its reduction and the prior)
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -182,7 +183,7 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
-                                    "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve"};
+                                    "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -265,6 +266,8 @@ struct ian_handle {
   // and replicated latent (100,100), the Jacobian J (100,3,64,64) it writes, and the Gram's chunk partials
   float *gn_eye = nullptr, *gn_zrep = nullptr, *gn_J = nullptr;
   double* gn_part = nullptr;
+  // the masked fit on IAN.py / IANv1.py: the flow's outputs on the replicated u -- z = F(u) rows, then J_F's columns (2 x 100 x 100)
+  float* map_flow = nullptr;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -2034,7 +2037,7 @@ struct Chunk {
   int off, cn;
   cudaStream_t st;
   bool host;
-  void* p[5];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
+  void* p[6];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
   float* f(int i) const { return (float*)p[i]; }
   const int32_t* i32(int i) const { return (const int32_t*)p[i]; }
   // a kernel chain: replayed from graph `slot` by the host form (run_graphed), launched as is by the device form
@@ -2450,8 +2453,31 @@ int call_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, 
   });
 }
 
-// The host form stages x in the plan's image buffer and z in its z buffer; the loss history in a plan buffer grown to the
-// largest (chunk, iters) asked for.
+// The fit's loss history (nullable) of one chunk, row stride ldl: the caller's rows in the device form; in the host form a
+// plan buffer grown to the largest (chunk, iters) asked for, copied out by fit_loss_out.
+int fit_loss_buf(const Chunk& c, float* loss, size_t ldl, float** l) {
+  *l = loss && !c.host ? loss + (size_t)c.off * ldl : nullptr;
+  const long long need = (long long)(c.cn * ldl);
+  if (loss && c.host) {
+    if (c.pl->floss_cap < need) {
+      CUDA_TRY(c.h, cudaFree(c.pl->floss));
+      c.pl->floss = nullptr;
+      c.pl->floss_cap = 0;
+      CUDA_TRY(c.h, cudaMalloc((void**)&c.pl->floss, (size_t)need * sizeof(float)));
+      c.pl->floss_cap = need;
+    }
+    *l = c.pl->floss;
+  }
+  return IAN_OK;
+}
+
+int fit_loss_out(const Chunk& c, float* loss, size_t ldl, const float* l) {
+  if (loss && c.host)
+    CUDA_TRY(c.h, cudaMemcpyAsync(loss + (size_t)c.off * ldl, l, c.cn * ldl * sizeof(float), cudaMemcpyDeviceToHost, c.st));
+  return IAN_OK;
+}
+
+// The host form stages x in the plan's image buffer and z in its z buffer.
 int call_fit_latent(ian_handle* h, bool host, const float* x, int n, float* z, int iters, float* loss, void* stream) {
   int rc = check_fit_args(h, n);
   if (rc != IAN_OK) return rc;
@@ -2461,22 +2487,129 @@ int call_fit_latent(ian_handle* h, bool host, const float* x, int n, float* z, i
   const size_t ldl = (size_t)iters + 1;
   return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z, kLatentBytes, S_Z, INOUT}}, ensure_gn_plan,
                    [&](const Chunk& c) {
-    float* l = loss && !host ? loss + (size_t)c.off * ldl : nullptr;
-    const long long need = (long long)(c.cn * ldl);
-    if (loss && host) {
-      if (c.pl->floss_cap < need) {
-        CUDA_TRY(h, cudaFree(c.pl->floss));
-        c.pl->floss = nullptr;
-        c.pl->floss_cap = 0;
-        CUDA_TRY(h, cudaMalloc((void**)&c.pl->floss, (size_t)need * sizeof(float)));
-        c.pl->floss_cap = need;
-      }
-      l = c.pl->floss;
+    float* l = nullptr;
+    int r = fit_loss_buf(c, loss, ldl, &l);
+    if (r == IAN_OK) r = run_fit(h, c.pl, c.f(0), c.f(1), iters, l, c.st);
+    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
+  });
+}
+
+// ---- masked latent fit under the prior: pixel-weighted Levenberg-Marquardt in the fit space u (DESIGN section 5.6j) -------
+// u is l_Z on IAN_simple and l_Z_IAF on IAN.py / IANv1.py, and z = F(u) the MADE/IAF flow (the identity on IAN_simple).
+// x_hat = decode(F(u)) on the caller's batch plan: made_iaf_kernel writes the latent planes as `sample` does, so x_hat has
+// ian_flow_*'s bits with x_out at that batch size (on IAN_simple run_decode, the fit's own).  J_u = J_dec(F(u)) J_F(u)
+// comes from one batch-100 pass per sample on the plan the fit uses: u replicated 100 times, the flow's z rows and its
+// JVP with the identity as tangents (the kernels of ian_flow_jvp_*), then run_decode_jvp with those rows as tangents.  On
+// IAN_simple the pass is the fit's own.  The first call on a handle also allocates the flow's 80 KB of rows (flow graphs).
+int ensure_map_plan(ian_handle* h, Plan* pl) {
+  int rc = ensure_gn_plan(h, pl);
+  if (rc != IAN_OK) return rc;
+  if (has_flow(h) && !h->map_flow) CUDA_TRY(h, cudaMalloc((void**)&h->map_flow, 20000 * sizeof(float)));
+  return IAN_OK;
+}
+
+// x_hat = decode(F(u)) of the plan's n samples
+int run_map_decode(ian_handle* h, Plan* pl, const float* u, float* xh, cudaStream_t st) {
+  if (!has_flow(h)) return run_decode(h, pl, u, xh, st);
+  LAUNCH_TRY(h, launch_made_iaf(u, h->made_w, h->made_b, nullptr, pl->zp.p, pl->zp.plane, pl->n, st));
+  return run_decode_from_planes(h, pl, xh, st);
+}
+
+// A (n,100,100), g (n,100) and e (n, nullable) of n samples at u, with x_hat = decode(F(u)) already in xh; w nullable
+int run_map_normal_eqs(ian_handle* h, int n, const float* u, const float* x, const float* w, double beta, const float* xh,
+                       double* A, double* g, double* e, cudaStream_t st) {
+  Plan* jp = nullptr;
+  int rc = get_plan(h, 100, &jp);
+  if (rc != IAN_OK) return rc;
+  for (int k = 0; k < n; ++k) {
+    const float* uk = u + (size_t)k * 100;
+    const float *zr = h->gn_zrep, *tan = h->gn_eye;
+    LAUNCH_TRY(h, launch_gn_replicate(uk, h->gn_zrep, st));
+    if (has_flow(h)) {
+      zr = h->map_flow;
+      tan = h->map_flow + 10000;
+      LAUNCH_TRY(h, launch_made_iaf(h->gn_zrep, h->made_w, h->made_b, h->map_flow, nullptr, 0, 100, st));
+      LAUNCH_TRY(h, launch_made_iaf_tangent(h->gn_zrep, h->gn_eye, h->made_w, h->made_b, h->map_flow + 10000, 100, st));
     }
-    const int r = run_fit(h, c.pl, c.f(0), c.f(1), iters, l, c.st);
-    if (r == IAN_OK && loss && host)
-      CUDA_TRY(h, cudaMemcpyAsync(loss + (size_t)c.off * ldl, l, (size_t)need * sizeof(float), cudaMemcpyDeviceToHost, c.st));
-    return r;
+    if ((rc = run_decode_jvp(h, jp, zr, tan, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+    ScopedTimer tm(h, T_MAP_GRAM, st);
+    LAUNCH_TRY(h, launch_map_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, w ? w + (size_t)k * 12288 : nullptr,
+                                  beta, uk, h->gn_part, A + (size_t)k * 10000, g + (size_t)k * 100, e ? e + k : nullptr, st));
+  }
+  return IAN_OK;
+}
+
+// run_fit on E(u) = sum_p w_p r_p^2 + beta |u|^2: the same solve and rule, trial steps decoded from F(u_trial)
+int run_fit_map(ian_handle* h, Plan* pl, const float* x, const float* w, double beta, float* u, int iters, float* loss,
+                cudaStream_t st) {
+  const int n = pl->n;
+  const long long ldl = (long long)iters + 1;
+  int rc;
+  if ((rc = run_map_decode(h, pl, u, pl->fxh, st)) != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_map_accept(1, pl->fxh, x, w, beta, pl->fxh, pl->fe, pl->flam, u, nullptr, nullptr, loss, ldl, 0, n, st));
+  for (int it = 0; it < iters; ++it) {
+    if ((rc = run_map_normal_eqs(h, n, u, x, w, beta, pl->fxh, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
+    {
+      ScopedTimer tm(h, T_GN_SOLVE, st);
+      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, u, pl->fzt, pl->fok, n, st));
+    }
+    if ((rc = run_map_decode(h, pl, pl->fzt, pl->fxt, st)) != IAN_OK) return rc;
+    LAUNCH_TRY(h, launch_map_accept(0, pl->fxt, x, w, beta, pl->fxh, pl->fe, pl->flam, u, pl->fzt, pl->fok, loss, ldl, it + 1, n,
+                                    st));
+  }
+  return IAN_OK;
+}
+
+// the prior weight; in the host form also every pixel weight (the device form cannot read them)
+int check_map_args(ian_handle* h, bool host, int n, const float* w, double prior) {
+  if (!(prior >= 0.0) || !std::isfinite(prior)) return fail(h, IAN_ERR_INVALID, "prior must be finite and >= 0 (got %g)", prior);
+  if (host && w)
+    for (size_t i = 0; i < (size_t)n * 12288; ++i)
+      if (!(w[i] >= 0.f) || !std::isfinite(w[i]))
+        return fail(h, IAN_ERR_INVALID, "weight %zu (sample %zu) is %g: weights must be finite and >= 0", i, i / 12288, (double)w[i]);
+  return IAN_OK;
+}
+
+// As call_gauss_newton; the host form stages w in the plan's frame-target buffer.
+int call_map_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int n,
+                          double* A, double* g, double* e, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!u || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{u, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
+                                        {A, 80000, S_GN_A, OUT}, {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_map_plan,
+                   [&](const Chunk& c) {
+    const int r = run_map_decode(h, c.pl, c.f(0), c.pl->fxh, c.st);
+    return r != IAN_OK ? r : run_map_normal_eqs(h, c.cn, c.f(0), c.f(1), c.f(2), prior, c.pl->fxh, (double*)c.p[3],
+                                                (double*)c.p[4], c.p[5] ? (double*)c.p[5] : c.pl->gne, c.st);
+  });
+}
+
+// As call_fit_latent; the host form stages w in the plan's frame-target buffer and z_out in its eps buffer.  z_out = F(u)
+// comes from made_iaf_kernel on the final u, as ian_flow_* computes it (a copy of u on IAN_simple).
+int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w, double prior, int n, float* u, float* z_out,
+                        int iters, float* loss, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
+  if (n == 0) return IAN_OK;
+  if (!x || !u) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
+  const size_t ldl = (size_t)iters + 1;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
+                                        {u, kLatentBytes, S_Z, INOUT}, {z_out, kLatentBytes, S_EPS, OUT}}, ensure_map_plan,
+                   [&](const Chunk& c) {
+    float* l = nullptr;
+    int r = fit_loss_buf(c, loss, ldl, &l);
+    if (r == IAN_OK) r = run_fit_map(h, c.pl, c.f(0), c.f(1), prior, c.f(2), iters, l, c.st);
+    if (r == IAN_OK && z_out) {
+      if (has_flow(h))
+        LAUNCH_TRY(h, launch_made_iaf(c.f(2), h->made_w, h->made_b, c.f(3), nullptr, 0, c.cn, c.st));
+      else
+        CUDA_TRY(h, cudaMemcpyAsync(c.f(3), c.f(2), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
+    }
+    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
   });
 }
 
@@ -2615,7 +2748,7 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->made_w); cudaFree(h->made_b); cudaFree(h->head_taps); cudaFree(h->head_wgb); cudaFree(h->head_wbb);
   cudaFree(h->head_tc_wt);
   cudaFree(h->train_ws);
-  cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part);
+  cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part); cudaFree(h->map_flow);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -2780,6 +2913,22 @@ int ian_fit_latent_dev(ian_handle* h, const float* x, int n, float* z, int iters
 }
 int ian_fit_latent_host(ian_handle* h, const float* x, int n, float* z, int iters, float* loss) {
   return call_fit_latent(h, true, x, n, z, iters, loss, nullptr);
+}
+int ian_map_gauss_newton_dev(ian_handle* h, const float* u, const float* x, const float* w, double prior, int n, double* A,
+                             double* g, double* e, void* stream) {
+  return call_map_gauss_newton(h, false, u, x, w, prior, n, A, g, e, stream);
+}
+int ian_map_gauss_newton_host(ian_handle* h, const float* u, const float* x, const float* w, double prior, int n, double* A,
+                              double* g, double* e) {
+  return call_map_gauss_newton(h, true, u, x, w, prior, n, A, g, e, nullptr);
+}
+int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w, double prior, int n, float* u, float* z_out, int iters,
+                           float* loss, void* stream) {
+  return call_fit_latent_map(h, false, x, w, prior, n, u, z_out, iters, loss, stream);
+}
+int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w, double prior, int n, float* u, float* z_out, int iters,
+                            float* loss) {
+  return call_fit_latent_map(h, true, x, w, prior, n, u, z_out, iters, loss, nullptr);
 }
 
 int ian_edit_loop_dev(ian_handle* h, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
