@@ -92,8 +92,11 @@ static_assert(TcCfg<128, 3>::kRound == 32 && TcCfg<128, 3>::kOutRoundBytes == 16
 
 // ---------------------------------------------------------------- kernel
 // Persistent, warp-specialised.  Work items w = blockIdx.x + i*gridDim.x over
-// (phase | k-split | n-tile | m-tile), longest phases first.  The smem ring runs ACROSS work items: the producer
-// prefetches the next tile's operands while the consumers run the epilogue of the current one.
+// (phase | k-split | m-tile | n-tile), longest phases first.  The n-tiles of one m-tile are neighbouring work items, so
+// they run at the same time on neighbouring CTAs and read the same activation boxes: HBM delivers each box once and L2
+// serves the rest.  (With m-tiles innermost, a layer whose input outgrows L2 -- enc_conv2 reads 134 MB at batch 256 --
+// fetches its activations from HBM once per n-tile.)  The order does not change any sum.  The smem ring runs ACROSS
+// work items: the producer prefetches the next tile's operands while the consumers run the epilogue of the current one.
 struct WorkItem {
   int phase, ks, co0, it0, it1;
   int n0, p0, q0, mtile;
@@ -134,8 +137,8 @@ __device__ __forceinline__ WorkItem decode_work(const TapGemm& g, const TcMaps& 
   const int per_phase = tiles_m * tiles_n * g.ksplit;
   wi.phase = w / per_phase;
   int r = w % per_phase;
-  int mt = r % tiles_m; r /= tiles_m;
   const int nt = r % tiles_n; r /= tiles_n;
+  int mt = r % tiles_m; r /= tiles_m;
   wi.ks = r;
   wi.mtile = mt;
   const int qb = mt % tiles_q; mt /= tiles_q;
