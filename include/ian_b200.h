@@ -340,6 +340,51 @@ int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w /*nulla
 int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int n, float* u,
                             float* z_out /*nullable*/, int iters, float* loss /*nullable*/);
 
+/* ---- the IAN's introspection features and the latent fit under its feature-wise loss ---------------------------------
+ * The features g_1..g_4 are l_introspect = [enc_conv1, enc_conv2, enc_conv3, enc_conv4] of the reference graphs
+ * (IAN_simple.py:240, IAN.py:227, IANv1.py:220): the deterministic encoder's activations after BatchNorm (inference
+ * statistics, as in Z_hat_fn) and LeakyReLU, with M_i = 131072, 65536, 32768, 16384 elements per image.  Their values are
+ * what the encoder stores (float32 mode: exact float32; bf16 mode: the bf16 values the next layer reads).
+ * ian_introspect_*: x (n,3,64,64) -> f1 (n,128,32,32), f2 (n,256,16,16), f3 (n,512,8,8), f4 (n,1024,4,4) float32 NCHW, each
+ *   nullable: the encoder forward stopped after enc_conv4.
+ * ian_introspect_jvp_*: the features (nullable) and their tangents t1..t4 along the image tangents v (n,3,64,64), in the
+ *   same layout: ian_encode_jvp_*'s tangent chain stopped after enc_conv4, with its derivative conventions.
+ * With z (n,100) the l_Z the decoder takes, x_hat = decode(z), r = x_hat - x, r_i = g_i(x_hat) - g_i(x), a = pixel_weight
+ * and b = feature_weight (doubles, finite, >= 0, not both 0):
+ *   l_f = (1/4) sum_i |r_i|^2 / M_i   (per sample; train_IAN.py:244 under deterministic=True)
+ *   E(z) = a |r|^2 + b 12288 l_f,   J = d x_hat / d z,   J_i = d g_i(x_hat) / d z,   c_i = 3072 b / M_i
+ * ian_feature_gauss_newton_*: A = a J^T J + sum_i c_i J_i^T J_i (n,100,100, both triangles), g = a J^T r + sum_i c_i J_i^T r_i
+ *   (n,100) and e = E (n, nullable), float64.  Per sample one batch-100 decoder JVP (ian_decode_gauss_newton_*'s pass) and
+ *   one batch-100 encoder JVP to enc_conv4 with those 100 rows x_hat as primal and J's columns as tangents; the features of
+ *   x and x_hat come from encoder forwards at the call's batch size.  Every product is formed in float64 and summed in a
+ *   fixed order.
+ * ian_fit_latent_features_*: `iters` Levenberg-Marquardt steps per sample in place on z with ian_fit_latent_*'s solve,
+ *   damping, constants and accept / reject rule applied to this A, g and E; loss (n, iters+1, nullable) receives
+ *   E / 12288 = a MSE + b l_f of the start and after every step: non-increasing, and a flat entry leaves z bit-unchanged.
+ * a = 1, b = 0 computes ian_decode_gauss_newton_* / ian_fit_latent_*'s bits.
+ * All four: all three graphs, both paths; bf16 precision on the flow graphs.  n == 0 does nothing; n < 0, iters < 0, a
+ * negative or non-finite weight, a = b = 0, or a NULL x, v, t_i, z, A or g -> IAN_ERR_INVALID; not finalized ->
+ * IAN_ERR_STATE.  Deterministic (a repeated call is bit-identical; the device form computes the host form's bits).
+ * Memory: the host forms of ian_introspect* stage 1.97 MB per image on their first call per batch size; ian_introspect_jvp_*
+ * allocates what ian_encode_jvp_* does.  The fit and its normal equations allocate what ian_fit_latent_* does, plus on the
+ * first call on a handle 11.2 MB of Gram partials and the batch-100 plan's encoder tangent planes, and on the first call per
+ * batch size 1.97 MB per image of stored features. */
+int ian_introspect_dev(ian_handle* h, const float* x, int n, float* f1, float* f2, float* f3, float* f4, void* stream);
+int ian_introspect_host(ian_handle* h, const float* x, int n, float* f1, float* f2, float* f3, float* f4);
+int ian_introspect_jvp_dev(ian_handle* h, const float* x, const float* v, int n, float* f1 /*nullable*/, float* f2 /*nullable*/,
+                           float* f3 /*nullable*/, float* f4 /*nullable*/, float* t1, float* t2, float* t3, float* t4,
+                           void* stream);
+int ian_introspect_jvp_host(ian_handle* h, const float* x, const float* v, int n, float* f1 /*nullable*/, float* f2 /*nullable*/,
+                            float* f3 /*nullable*/, float* f4 /*nullable*/, float* t1, float* t2, float* t3, float* t4);
+int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
+                                 double* A, double* g, double* e /*nullable*/, void* stream);
+int ian_feature_gauss_newton_host(ian_handle* h, const float* z, const float* x, int n, double pixel_weight,
+                                  double feature_weight, double* A, double* g, double* e /*nullable*/);
+int ian_fit_latent_features_dev(ian_handle* h, const float* x, int n, float* z, int iters, double pixel_weight,
+                                double feature_weight, float* loss /*nullable*/, void* stream);
+int ian_fit_latent_features_host(ian_handle* h, const float* x, int n, float* z, int iters, double pixel_weight,
+                                 double feature_weight, float* loss /*nullable*/);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -429,7 +474,9 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * tangent) and "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head"; in the latent fit "gn_gram"
  * (the normal equations' Gram of one sample, with its chunk reduction) and "gn_solve" (the Levenberg-Marquardt solve of
  * the batch); in the masked fit "map_gram" (the weighted Gram of one sample, with its reduction and the prior terms) and
- * "gn_solve") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * "gn_solve"; in the feature fit "feat_gram" (the feature layers' Gram of one sample, with its reduction and the pixel
+ * Gram's weighting), "feat_accept" (the trial objective and accept rule of the batch), "gn_gram" and "gn_solve") over the
+ * launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

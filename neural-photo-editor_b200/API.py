@@ -16,7 +16,9 @@ batched `grad` / `edit_steps`, the decoder VJP `decode_vjp` for any pixel-space 
 functions in the prior space l_Z_IAF -- `flow_vjp` / `flow_jvp` (Z_IAF_fn) and `encode_pre_vjp` / `encode_pre_jvp` (Zfn),
 torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, the decoder's Gauss-Newton normal equations `gauss_newton` and
 the batched Levenberg-Marquardt latent fit `fit_latent`, their pixel-weighted forms under the N(0, I) prior in the sampling
-space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), and `*_dev` variants taking device pointers.
+space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), the IAN's introspection features `introspect` /
+`introspect_jvp` / `feature_loss` and the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`,
+and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -46,6 +48,8 @@ _FULL_CFG = {
     'ags_weight': 1.0, 'n_shuffles': 1, 'ortho': 1e-3,
 }
 _FULL_MODEL_KEYS = _SIMPLE_MODEL_KEYS + ('l_IAF_mu', 'l_IAF_ls', 'l_Z_IAF')
+# l_introspect = [enc_conv1, enc_conv2, enc_conv3, enc_conv4] (IAN_simple.py:240): per-image shapes
+FEATURE_SHAPES = ((128, 32, 32), (256, 16, 16), (512, 8, 8), (1024, 4, 4))
 
 
 def made_ordering(seed=1234, n=100):
@@ -531,6 +535,96 @@ class IAN:
                                                           _fp(z), iters, _fp(loss)))
         return (u, z, loss) if return_loss else (u, z)
 
+    # ---- the introspection features and the fit under the feature-wise loss ------------------------------------------------
+    def introspect(self, images):
+        """The IAN's introspection features l_introspect (IAN_simple.py:240): images float32 (n,3,64,64) -> [f1 (n,128,32,32),
+        f2 (n,256,16,16), f3 (n,512,8,8), f4 (n,1024,4,4)] float32, the outputs of enc_conv1..4 after BatchNorm (inference
+        statistics, as in Z_hat_fn) and LeakyReLU -- what get_output(l_introspect, deterministic=True) returns.  One encoder
+        forward stopped after enc_conv4."""
+        x = _img(images)
+        n = x.shape[0]
+        f = [np.empty((n,) + s, np.float32) for s in FEATURE_SHAPES]
+        if n:
+            self._check(self._lib.ian_introspect_host(self._h, _fp(x), n, *[_fp(a) for a in f]))
+        return f
+
+    def introspect_jvp(self, images, v, return_features=False):
+        """Jacobian-vector product of the introspection features along image tangents: images and v float32 (n,3,64,64) ->
+        the tangents [t1..t4] in introspect()'s shapes, and introspect(images) bit for bit when return_features (returned as
+        (features, tangents)).  encode_jvp's tangent chain stopped after enc_conv4, with its derivative conventions."""
+        x = _img(images)
+        t = _img(v, 'v')
+        n = x.shape[0]
+        if t.shape[0] != n:
+            raise ValueError("v must be (%d,3,64,64), got %r" % (n, t.shape))
+        f = [np.empty((n,) + s, np.float32) for s in FEATURE_SHAPES] if return_features else [None] * 4
+        dt = [np.empty((n,) + s, np.float32) for s in FEATURE_SHAPES]
+        if n:
+            self._check(self._lib.ian_introspect_jvp_host(self._h, _fp(x), _fp(t), n,
+                                                          *([_fp(a) if a is not None else None for a in f] + [_fp(a) for a in dt])))
+        return (f, dt) if return_features else dt
+
+    def feature_loss(self, x_hat, images):
+        """The per-sample feature-wise loss of train_IAN.py:244 under deterministic=True: x_hat, images float32 (n,3,64,64)
+        -> (n,) float64 l_f = (1/4) sum_i mean((g_i(x_hat) - g_i(images))^2) over the four introspect() features."""
+        a, b = self.introspect(x_hat), self.introspect(images)
+        if a[0].shape[0] != b[0].shape[0]:
+            raise ValueError("x_hat and images must hold the same number of images")
+        n = a[0].shape[0]
+        return sum(((p.astype(np.float64) - q).reshape(n, -1) ** 2).mean(1) for p, q in zip(a, b)) / 4
+
+    @staticmethod
+    def _feature_weights(pixel_weight, feature_weight):
+        a, b = float(pixel_weight), float(feature_weight)
+        for name, w in (("pixel_weight", a), ("feature_weight", b)):
+            if not (np.isfinite(w) and w >= 0):
+                raise ValueError("%s must be finite and >= 0 (got %r)" % (name, w))
+        if a == 0 and b == 0:
+            raise ValueError("pixel_weight and feature_weight must not both be 0")
+        return a, b
+
+    def gauss_newton_features(self, z, images, pixel_weight=1.0, feature_weight=1.0):
+        """The Gauss-Newton normal equations of the pixel plus feature-wise objective at each latent: z float32 (n,100) (l_Z,
+        as for sample_at), images float32 (n,3,64,64), a = pixel_weight, b = feature_weight (>= 0, not both 0) ->
+        (A (n,100,100), g (n,100), e (n,)) float64 for E(z) = a |x_hat - x|^2 + 12288 b feature_loss(x_hat, x), x_hat =
+        sample_at(z): A = a J^T J + sum_i c_i J_i^T J_i, g = a J^T r + sum_i c_i J_i^T r_i, e = E, with J_i the Jacobian of
+        feature i at x_hat along the decoder and c_i = 3072 b / M_i.  a = 1, b = 0 is gauss_newton.  Costs one batch-100
+        decode_jvp and one batch-100 introspect_jvp per sample."""
+        z = _z(z)
+        x = _img(images)
+        a, b = self._feature_weights(pixel_weight, feature_weight)
+        n = z.shape[0]
+        if x.shape[0] != n:
+            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        A = np.empty((n, 100, 100), np.float64)
+        g = np.empty((n, 100), np.float64)
+        e = np.empty((n,), np.float64)
+        if n:
+            d = C.POINTER(C.c_double)
+            self._check(self._lib.ian_feature_gauss_newton_host(self._h, _fp(z), _fp(x), n, a, b, A.ctypes.data_as(d),
+                                                                g.ctypes.data_as(d), e.ctypes.data_as(d)))
+        return A, g, e
+
+    def fit_latent_features(self, images, z0=None, iters=10, pixel_weight=1.0, feature_weight=1.0, return_loss=False):
+        """Fit a latent to each image under the IAN's own reconstruction objective: `iters` Levenberg-Marquardt steps on
+        pixel_weight * MSE + feature_weight * feature_loss (gauss_newton_features' E / 12288), every decision on the GPU.
+        images float32 (n,3,64,64) in [-1,1]; z0 float32 (n,100) the start (default: encode_images(images)) -> z float32
+        (n,100), and with return_loss that objective of the start and after every step, float32 (n, iters+1),
+        non-increasing.  pixel_weight = 1, feature_weight = 0 is fit_latent."""
+        x = _img(images)
+        a, b = self._feature_weights(pixel_weight, feature_weight)
+        n = x.shape[0]
+        iters = _int_scalar(iters, 'iters')
+        if iters < 0:
+            raise ValueError("iters must not be negative (got %d)" % iters)
+        z = self.encode_images(x) if z0 is None else _z(z0, 'z0').copy()
+        if z.shape[0] != n:
+            raise ValueError("z0 must be (%d,100), got %r" % (n, z.shape))
+        loss = np.empty((n, iters + 1), np.float32)
+        if n:
+            self._check(self._lib.ian_fit_latent_features_host(self._h, _fp(x), n, _fp(z), iters, a, b, _fp(loss)))
+        return (z, loss) if return_loss else z
+
     def param_vjp_names(self):
         """names of the parameters decode_param_vjp returns gradients for, in ian_model_param_spec order: on IAN_simple
         the 13 tensors of train_IAN_simple.py:353 (`decoder_params`); empty on IAN.py / IANv1.py."""
@@ -868,6 +962,25 @@ class IAN:
         float32; w_ptr, z_ptr and loss_ptr may be 0"""
         self._check(self._lib.ian_fit_latent_map_dev(self._h, x_ptr, w_ptr or None, float(prior), int(n), u_ptr, z_ptr or None,
                                                      int(iters), loss_ptr or None, stream or None))
+
+    def introspect_dev(self, x_ptr, n, f_ptrs, stream=0):
+        """introspect() on device pointers: f_ptrs = 4 pointers (0: not wanted) to float32 outputs in FEATURE_SHAPES"""
+        self._check(self._lib.ian_introspect_dev(self._h, x_ptr, int(n), *[p or None for p in f_ptrs], stream or None))
+
+    def introspect_jvp_dev(self, x_ptr, v_ptr, n, t_ptrs, f_ptrs=(0, 0, 0, 0), stream=0):
+        """introspect_jvp() on device pointers: t_ptrs = the 4 tangent outputs, f_ptrs the features (0: not wanted)"""
+        self._check(self._lib.ian_introspect_jvp_dev(self._h, x_ptr, v_ptr, int(n), *([p or None for p in f_ptrs] + list(t_ptrs)),
+                                                     stream or None))
+
+    def gauss_newton_features_dev(self, z_ptr, x_ptr, n, A_ptr, g_ptr, e_ptr=0, pixel_weight=1.0, feature_weight=1.0, stream=0):
+        """gauss_newton_features() on device pointers: A (n,100,100), g (n,100), e (n,) float64 (e optional)"""
+        self._check(self._lib.ian_feature_gauss_newton_dev(self._h, z_ptr, x_ptr, int(n), float(pixel_weight), float(feature_weight),
+                                                           A_ptr, g_ptr, e_ptr or None, stream or None))
+
+    def fit_latent_features_dev(self, x_ptr, n, z_ptr, iters, loss_ptr=0, pixel_weight=1.0, feature_weight=1.0, stream=0):
+        """fit_latent_features() on device pointers, in place on z (n,100); loss (n, iters+1) float32 optional"""
+        self._check(self._lib.ian_fit_latent_features_dev(self._h, x_ptr, int(n), z_ptr, int(iters), float(pixel_weight),
+                                                          float(feature_weight), loss_ptr or None, stream or None))
 
     def edit_loop_dev(self, z_ptr, boxes_ptr, target_ptr, target_is_frame, n, n_steps, weight, stream=0):
         self._check(self._lib.ian_edit_loop_dev(self._h, z_ptr, boxes_ptr, target_ptr or None, int(target_is_frame),

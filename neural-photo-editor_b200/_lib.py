@@ -82,6 +82,17 @@ SIGNATURES = {
     "ian_fit_latent_map_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                          C.c_void_p, C.c_void_p]),
     "ian_fit_latent_map_host": (C.c_int, [_H, _F, _F, C.c_double, C.c_int, _F, _F, C.c_int, _F]),
+    "ian_introspect_dev": (C.c_int, [_H, C.c_void_p, C.c_int] + [C.c_void_p] * 5),
+    "ian_introspect_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F, _F]),
+    "ian_introspect_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 9),
+    "ian_introspect_jvp_host": (C.c_int, [_H, _F, _F, C.c_int] + [_F] * 8),
+    "ian_feature_gauss_newton_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_feature_gauss_newton_host": (C.c_int, [_H, _F, _F, C.c_int, C.c_double, C.c_double, C.POINTER(C.c_double),
+                                                C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "ian_fit_latent_features_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double,
+                                              C.c_void_p, C.c_void_p]),
+    "ian_fit_latent_features_host": (C.c_int, [_H, _F, C.c_int, _F, C.c_int, C.c_double, C.c_double, _F]),
     "ian_param_vjp_supported": (C.c_int, [C.c_int, C.c_int]),
     "ian_decode_param_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_param_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),

@@ -129,6 +129,36 @@ int launch_map_gram(const float* J, const float* xh, const float* x, const float
                     double* A, double* g, double* e, cudaStream_t st);
 int launch_map_accept(int init, const float* xht, const float* x, const float* w, double beta, float* xh, double* e, double* lam,
                       float* u, const float* ut, const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st);
+// the IAN's introspection features and the fit under its feature-wise loss (feat_kernels.cu; ian_introspect_*,
+// ian_feature_gauss_newton_*, ian_fit_latent_features_*): layer l = 0..3 is enc_conv{l+1}'s output a{l+1}, (32 >> l)^2
+// pixels of 128 << l channels, M_l elements per image
+constexpr int kFeatTotal = 245760;
+__host__ __device__ __forceinline__ long long feat_m(int l) { return 131072LL >> l; }
+struct FeatLayers {           // per layer: split planes (tan, plane) and float32 NHWC features (cur, tgt)
+  const __nv_bfloat16* tan[4];
+  long long plane[4];
+  float* cur[4];
+  const float* tgt[4];
+};
+struct FeatWeights {          // E = a |r|^2 + sum_l c[l] |r_l|^2
+  double a;
+  double c[4];
+};
+size_t feat_part_doubles();   // the feature Gram's chunk partials, per sample
+// layer `layer` of n images: split planes (hi only when passes == 1) -> float32, NCHW when nchw, else NHWC
+int launch_feat_store(const __nv_bfloat16* p, long long plane, int passes, int layer, int n, float* out, int nchw,
+                      cudaStream_t st);
+// one sample: t.tan = the 100 tangent rows of every layer (plan of 100), t.cur / t.tgt = the sample's features ->
+// A (100,100), g (100), e (nullable) = sum_l c[l] [J_l | r_l]^T [J_l | r_l] (feats == 0: no such terms, t unread), plus
+// c.a times what A, g, e hold when pixel != 0 (the pixel Gram of launch_gn_gram)
+int launch_feat_gram(const FeatLayers& t, const FeatWeights& c, int feats, int passes, int pixel, double* part, double* A,
+                     double* g, double* e, cudaStream_t st);
+// launch_gn_accept on E: f.tan = the trial's feature planes (plan of n), f.tgt the target's and f.cur the current features
+// (n samples each, float32 NHWC); the start and every accepted step copy the trial's features into f.cur.  feats == 0:
+// no feature terms; c.a == 0: no pixel term
+int launch_feat_accept(int init, const float* xht, const float* x, const FeatLayers& f, const FeatWeights& c, int feats,
+                       int passes, float* xh, double* e, double* lam, float* z, const float* zt, const int* ok, float* loss,
+                       long long ldl, int col, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

@@ -166,6 +166,8 @@ enum LayerId {
   T_CONV1_TANGENT,                                      // enc_conv1's tangent in the encoder JVP
   T_GN_GRAM, T_GN_SOLVE,                                // the latent fit's Gram (with its chunk reduction) and LM solve
   T_MAP_GRAM,                                           // the masked fit's weighted Gram (with its reduction and the prior)
+  T_FEAT_GRAM, T_FEAT_ACCEPT,                           // the feature fit's Gram over the four feature layers (with its
+                                                        // reduction) and its trial reduction and accept rule
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -183,7 +185,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
-                                    "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram"};
+                                    "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
+                                    "feat_gram", "feat_accept"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -268,6 +271,8 @@ struct ian_handle {
   double* gn_part = nullptr;
   // the masked fit on IAN.py / IANv1.py: the flow's outputs on the replicated u -- z = F(u) rows, then J_F's columns (2 x 100 x 100)
   float* map_flow = nullptr;
+  // the feature fit (ian_feature_gauss_newton_*, ian_fit_latent_features_*): the feature Gram's chunk partials (11.2 MB)
+  double* feat_part = nullptr;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -371,6 +376,12 @@ struct Plan {
   float *fxh = nullptr, *fxt = nullptr, *fzt = nullptr, *floss = nullptr;
   int* fok = nullptr;
   long long floss_cap = 0;
+  // feature fit (allocated on the plan's first ian_feature_gauss_newton_* / ian_fit_latent_features_* call): the target's
+  // features g(x) and the current ones g(x_hat), float32 NHWC, layer l's n samples at n * kFeatOff[l] (1.97 MB per image)
+  bool feat = false;
+  float *ftg = nullptr, *fcur = nullptr;
+  // ian_introspect*_host staging: the features, then their tangents, float32 NCHW, laid out as ftg (first host call)
+  float* ifeat = nullptr;
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -2008,8 +2019,10 @@ int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, cons
 //   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
 //   host form (ian_*_host): per chunk, the caller's inputs are copied into plan buffers, the body runs on those, its kernel
 //   chain (Chunk::graphed) replayed as a CUDA graph on small plans, the outputs are copied back; then one synchronise.
-enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ, S_GN_A, S_GN_G, S_GN_E };
+enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ, S_GN_A, S_GN_G, S_GN_E, S_F1, S_T1 = S_F1 + 4 };
+constexpr long long kFeatOff[4] = {0, 131072, 196608, 229376};   // layer l's offset in a sample's 245760 features
 void* stage_buf(Plan* pl, int s) {
+  if (s >= S_F1) return pl->ifeat + (long long)pl->n * ((s >= S_T1 ? kFeatTotal : 0) + kFeatOff[(s - S_F1) % 4]);
   switch (s) {
     case S_X: return pl->x;
     case S_EPS: return pl->eps;
@@ -2037,7 +2050,7 @@ struct Chunk {
   int off, cn;
   cudaStream_t st;
   bool host;
-  void* p[6];             // the Args' pointers for this chunk, in order (nullptr for an input left out)
+  void* p[10];            // the Args' pointers for this chunk, in order (nullptr for an input left out)
   float* f(int i) const { return (float*)p[i]; }
   const int32_t* i32(int i) const { return (const int32_t*)p[i]; }
   // a kernel chain: replayed from graph `slot` by the host form (run_graphed), launched as is by the device form
@@ -2613,6 +2626,256 @@ int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w
   });
 }
 
+// ---- the IAN's introspection features and the fit under its feature-wise loss (DESIGN section 5.6k) --------------------
+// g_1..g_4 are the encoder's activations a1..a4 (enc_conv1..4 after BatchNorm and LeakyReLU, inference BatchNorm): the
+// encoder forward stopped after enc_conv4, and the feature values are what it stores (hi + lo, or hi in bf16 mode).
+const Planes& feat_planes(Plan* pl, int l) { return l == 0 ? pl->a1 : l == 1 ? pl->a2 : l == 2 ? pl->a3 : pl->a4; }
+
+int run_introspect(ian_handle* h, Plan* pl, const float* x, cudaStream_t st) {
+  {
+    ScopedTimer tm(h, T_CONV1, st);
+    if (h->path == IAN_PATH_TC)
+      LAUNCH_TRY(h, launch_conv1_tc(h->conv1_maps, pl->conv1_out, x, h->conv1_b, pl->n, st));
+    else
+      LAUNCH_TRY(h, launch_conv1(x, h->conv1_wt, h->conv1_b, pl->a1.p, pl->a1.plane, pl->n, st));
+  }
+  int rc;
+  for (int k = 0; k < 3; ++k)
+    if ((rc = run_gemm(h, pl, kEncoder.l[k], st)) != IAN_OK) return rc;
+  return IAN_OK;
+}
+
+// run_encode_jvp's tangent chain truncated after jvp_enc_conv4: the tangents of a1..a4 in pl->jea[0..3]
+int run_introspect_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, cudaStream_t st) {
+  int rc = run_introspect(h, pl, x, st);
+  if (rc != IAN_OK) return rc;
+  {
+    ScopedTimer tm(h, T_CONV1_TANGENT, st);
+    if (h->path == IAN_PATH_TC)
+      LAUNCH_TRY(h, launch_conv1_tangent_tc(h->conv1_maps, pl->jconv1_out, v, pl->a1.p, pl->n, st));
+    else
+      LAUNCH_TRY(h, launch_conv1_tangent(v, h->conv1_wt, pl->a1.p, pl->jea[0].p, pl->jea[0].plane, pl->n, st));
+  }
+  for (int k = 0; k < 3; ++k)
+    if ((rc = run_gemm(h, pl, kEncoderJvp.l[k], st)) != IAN_OK) return rc;
+  return IAN_OK;
+}
+
+// the plan's four feature planes (tangent: their tangents) -> float32: out[l] nullable, NCHW per layer, or NHWC at
+// base + n * off_l
+int store_features(ian_handle* h, Plan* pl, bool tangent, float* const* out, float* base, int nchw, cudaStream_t st) {
+  for (int l = 0; l < 4; ++l) {
+    const Planes& src = tangent ? pl->jea[l] : feat_planes(pl, l);
+    float* o = base ? base + (long long)pl->n * kFeatOff[l] : out[l];
+    if (o) LAUNCH_TRY(h, launch_feat_store(src.p, src.plane, h->passes, l, pl->n, o, nchw, st));
+  }
+  return IAN_OK;
+}
+
+// The host forms stage the outputs in a plan buffer of 1.97 MB per image (features, then tangents), allocated on their
+// first call on the plan; the device forms allocate nothing for the features.
+template <bool kHost, bool kJvp>
+int ensure_introspect_plan(ian_handle* h, Plan* pl) {
+  int rc;
+  if (kJvp && (rc = ensure_enc_jvp_plan(h, pl)) != IAN_OK) return rc;
+  if (kHost && !pl->ifeat) {
+    if ((rc = alloc_buf(h, pl, pl->ifeat, (long long)pl->n * 2 * kFeatTotal)) != IAN_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return IAN_OK;
+}
+
+constexpr size_t kFeatBytes[4] = {131072 * 4, 65536 * 4, 32768 * 4, 16384 * 4};
+
+// No CUDA graphs: the features are a measurement and a building block, not an interactive call.
+int call_introspect(ian_handle* h, bool host, const float* x, int n, float* const* f, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {f[0], kFeatBytes[0], S_F1, OUT},
+                                        {f[1], kFeatBytes[1], S_F1 + 1, OUT}, {f[2], kFeatBytes[2], S_F1 + 2, OUT},
+                                        {f[3], kFeatBytes[3], S_F1 + 3, OUT}},
+                   host ? ensure_introspect_plan<true, false> : ensure_introspect_plan<false, false>, [&](const Chunk& c) {
+    const int r = run_introspect(h, c.pl, c.f(0), c.st);
+    float* o[4] = {c.f(1), c.f(2), c.f(3), c.f(4)};
+    return r != IAN_OK ? r : store_features(h, c.pl, false, o, nullptr, 1, c.st);
+  });
+}
+
+int call_introspect_jvp(ian_handle* h, bool host, const float* x, const float* v, int n, float* const* f, float* const* t,
+                        void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !v || !t[0] || !t[1] || !t[2] || !t[3]) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {v, kImageBytes, S_TARGET, IN},
+                                        {f[0], kFeatBytes[0], S_F1, OUT}, {f[1], kFeatBytes[1], S_F1 + 1, OUT},
+                                        {f[2], kFeatBytes[2], S_F1 + 2, OUT}, {f[3], kFeatBytes[3], S_F1 + 3, OUT},
+                                        {t[0], kFeatBytes[0], S_T1, OUT}, {t[1], kFeatBytes[1], S_T1 + 1, OUT},
+                                        {t[2], kFeatBytes[2], S_T1 + 2, OUT}, {t[3], kFeatBytes[3], S_T1 + 3, OUT}},
+                   host ? ensure_introspect_plan<true, true> : ensure_introspect_plan<false, true>, [&](const Chunk& c) {
+    int r = run_introspect_jvp(h, c.pl, c.f(0), c.f(1), c.st);
+    float* o[4] = {c.f(2), c.f(3), c.f(4), c.f(5)};
+    float* ot[4] = {c.f(6), c.f(7), c.f(8), c.f(9)};
+    if (r == IAN_OK) r = store_features(h, c.pl, false, o, nullptr, 1, c.st);
+    return r != IAN_OK ? r : store_features(h, c.pl, true, ot, nullptr, 1, c.st);
+  });
+}
+
+// E(z) = a |x_hat - x|^2 + sum_l c_l |g_l(x_hat) - g_l(x)|^2 with c_l = 3072 b / M_l (b * 12288 * l_f, l_f the per-sample
+// feature loss of train_IAN.py:244).  J_l = (d g_l / d x)(x_hat) J comes from the truncated encoder JVP on the batch-100
+// plan, with the decoder JVP's 100 rows x_hat as primal and J's columns as tangents.  The stored features g(x) and
+// g(x_hat) come from encoder forwards on the caller's plan.  The first call on a handle also allocates the Gram's 11.2 MB of
+// partials and the batch-100 plan's encoder tangent planes; the first call on a plan its 1.97 MB per image of features.
+int ensure_feat_plan(ian_handle* h, Plan* pl) {
+  int rc = ensure_gn_plan(h, pl);
+  if (rc != IAN_OK) return rc;
+  Plan* jp = nullptr;
+  if ((rc = get_plan(h, 100, &jp)) != IAN_OK || (rc = ensure_enc_jvp_plan(h, jp)) != IAN_OK) return rc;
+  if (!h->feat_part) CUDA_TRY(h, cudaMalloc((void**)&h->feat_part, feat_part_doubles() * sizeof(double)));
+  if (pl->feat) return IAN_OK;
+  const long long N = pl->n;
+  if ((rc = alloc_buf(h, pl, pl->ftg, N * kFeatTotal)) != IAN_OK || (rc = alloc_buf(h, pl, pl->fcur, N * kFeatTotal)) != IAN_OK)
+    return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  pl->feat = true;
+  return IAN_OK;
+}
+
+FeatWeights feat_weights(double a, double b) {
+  FeatWeights w{a, {}};
+  for (int l = 0; l < 4; ++l) w.c[l] = 3072.0 * b / (double)feat_m(l);
+  return w;
+}
+
+// the trial planes (the plan's a1..a4) against the plan's target features, current features kept in fcur
+FeatLayers plan_feat_layers(Plan* pl) {
+  FeatLayers f{};
+  for (int l = 0; l < 4; ++l) {
+    f.tan[l] = feat_planes(pl, l).p;
+    f.plane[l] = feat_planes(pl, l).plane;
+    f.cur[l] = pl->fcur + pl->n * kFeatOff[l];
+    f.tgt[l] = pl->ftg + pl->n * kFeatOff[l];
+  }
+  return f;
+}
+
+// A, g, e of the plan's n samples at z, with x_hat = decode(z) in xh and (b != 0) the features of x and x_hat in the plan's
+// ftg and fcur
+int run_feat_normal_eqs(ian_handle* h, Plan* pl, const float* z, const float* x, const float* xh, const FeatWeights& w,
+                        double* A, double* g, double* e, cudaStream_t st) {
+  Plan* jp = nullptr;
+  int rc = get_plan(h, 100, &jp);
+  if (rc != IAN_OK) return rc;
+  const bool feats = w.c[0] != 0.0, pixel = w.a != 0.0;
+  for (int k = 0; k < pl->n; ++k) {
+    double *Ak = A + (size_t)k * 10000, *gk = g + (size_t)k * 100, *ek = e + k;
+    LAUNCH_TRY(h, launch_gn_replicate(z + (size_t)k * 100, h->gn_zrep, st));
+    if ((rc = run_decode_jvp(h, jp, h->gn_zrep, h->gn_eye, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+    if (pixel) {
+      ScopedTimer tm(h, T_GN_GRAM, st);
+      LAUNCH_TRY(h, launch_gn_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, h->gn_part, Ak, gk, ek, st));
+    }
+    FeatLayers t{};
+    if (feats) {
+      if ((rc = run_introspect_jvp(h, jp, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+      for (int l = 0; l < 4; ++l) {
+        t.tan[l] = jp->jea[l].p;
+        t.plane[l] = jp->jea[l].plane;
+        t.cur[l] = pl->fcur + pl->n * kFeatOff[l] + k * feat_m(l);
+        t.tgt[l] = pl->ftg + pl->n * kFeatOff[l] + k * feat_m(l);
+      }
+    }
+    ScopedTimer tm(h, T_FEAT_GRAM, st);
+    LAUNCH_TRY(h, launch_feat_gram(t, w, feats, h->passes, pixel, h->feat_part, Ak, gk, ek, st));
+  }
+  return IAN_OK;
+}
+
+// run_fit on E: trial steps decode z_trial and run the encoder to enc_conv4 on the plan; feat_accept reduces E
+int run_fit_features(ian_handle* h, Plan* pl, const float* x, float* z, int iters, float* loss, const FeatWeights& w,
+                     cudaStream_t st) {
+  const int n = pl->n;
+  const long long ldl = (long long)iters + 1;
+  const bool feats = w.c[0] != 0.0;
+  const FeatLayers f = plan_feat_layers(pl);
+  int rc;
+  if (feats) {
+    if ((rc = run_introspect(h, pl, x, st)) != IAN_OK) return rc;
+    if ((rc = store_features(h, pl, false, nullptr, pl->ftg, 0, st)) != IAN_OK) return rc;
+  }
+  auto trial = [&](const float* zz, float* xo) {
+    int r = run_decode(h, pl, zz, xo, st);
+    return r != IAN_OK || !feats ? r : run_introspect(h, pl, xo, st);
+  };
+  if ((rc = trial(z, pl->fxh)) != IAN_OK) return rc;
+  {
+    ScopedTimer tm(h, T_FEAT_ACCEPT, st);
+    LAUNCH_TRY(h, launch_feat_accept(1, pl->fxh, x, f, w, feats, h->passes, pl->fxh, pl->fe, pl->flam, z, nullptr, nullptr, loss,
+                                     ldl, 0, n, st));
+  }
+  for (int it = 0; it < iters; ++it) {
+    if ((rc = run_feat_normal_eqs(h, pl, z, x, pl->fxh, w, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
+    {
+      ScopedTimer tm(h, T_GN_SOLVE, st);
+      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, z, pl->fzt, pl->fok, n, st));
+    }
+    if ((rc = trial(pl->fzt, pl->fxt)) != IAN_OK) return rc;
+    ScopedTimer tm(h, T_FEAT_ACCEPT, st);
+    LAUNCH_TRY(h, launch_feat_accept(0, pl->fxt, x, f, w, feats, h->passes, pl->fxh, pl->fe, pl->flam, z, pl->fzt, pl->fok, loss,
+                                     ldl, it + 1, n, st));
+  }
+  return IAN_OK;
+}
+
+int check_feat_weights(ian_handle* h, double a, double b) {
+  if (!(a >= 0.0) || !std::isfinite(a)) return fail(h, IAN_ERR_INVALID, "pixel_weight must be finite and >= 0 (got %g)", a);
+  if (!(b >= 0.0) || !std::isfinite(b)) return fail(h, IAN_ERR_INVALID, "feature_weight must be finite and >= 0 (got %g)", b);
+  if (a == 0.0 && b == 0.0) return fail(h, IAN_ERR_INVALID, "pixel_weight and feature_weight are both 0");
+  return IAN_OK;
+}
+
+// As call_gauss_newton.  a = 1, b = 0 is ian_decode_gauss_newton_* itself.
+int call_feature_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, int n, double a, double b, double* A,
+                              double* g, double* e, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || (rc = check_feat_weights(h, a, b)) != IAN_OK || n == 0) return rc;
+  if (!z || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if (a == 1.0 && b == 0.0) return call_gauss_newton(h, host, z, x, n, A, g, e, stream);
+  const FeatWeights w = feat_weights(a, b);
+  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {A, 80000, S_GN_A, OUT},
+                                        {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_feat_plan, [&](const Chunk& c) {
+    Plan* pl = c.pl;
+    int r = run_decode(h, pl, c.f(0), pl->fxh, c.st);
+    if (r == IAN_OK && w.c[0] != 0.0) {
+      if ((r = run_introspect(h, pl, c.f(1), c.st)) == IAN_OK && (r = store_features(h, pl, false, nullptr, pl->ftg, 0, c.st)) == IAN_OK &&
+          (r = run_introspect(h, pl, pl->fxh, c.st)) == IAN_OK)
+        r = store_features(h, pl, false, nullptr, pl->fcur, 0, c.st);
+    }
+    return r != IAN_OK ? r : run_feat_normal_eqs(h, pl, c.f(0), c.f(1), pl->fxh, w, (double*)c.p[2], (double*)c.p[3],
+                                                 c.p[4] ? (double*)c.p[4] : pl->gne, c.st);
+  });
+}
+
+// As call_fit_latent.  a = 1, b = 0 is ian_fit_latent_* itself.
+int call_fit_latent_features(ian_handle* h, bool host, const float* x, int n, float* z, int iters, double a, double b, float* loss,
+                             void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
+  if ((rc = check_feat_weights(h, a, b)) != IAN_OK || n == 0) return rc;
+  if (!x || !z) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if (a == 1.0 && b == 0.0) return call_fit_latent(h, host, x, n, z, iters, loss, stream);
+  const FeatWeights w = feat_weights(a, b);
+  const size_t ldl = (size_t)iters + 1;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z, kLatentBytes, S_Z, INOUT}}, ensure_feat_plan,
+                   [&](const Chunk& c) {
+    float* l = nullptr;
+    int r = fit_loss_buf(c, loss, ldl, &l);
+    if (r == IAN_OK) r = run_fit_features(h, c.pl, c.f(0), c.f(1), iters, l, w, c.st);
+    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
+  });
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -2748,7 +3011,7 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->made_w); cudaFree(h->made_b); cudaFree(h->head_taps); cudaFree(h->head_wgb); cudaFree(h->head_wbb);
   cudaFree(h->head_tc_wt);
   cudaFree(h->train_ws);
-  cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part); cudaFree(h->map_flow);
+  cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part); cudaFree(h->map_flow); cudaFree(h->feat_part);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -2929,6 +3192,43 @@ int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w, double
 int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w, double prior, int n, float* u, float* z_out, int iters,
                             float* loss) {
   return call_fit_latent_map(h, true, x, w, prior, n, u, z_out, iters, loss, nullptr);
+}
+
+int ian_introspect_dev(ian_handle* h, const float* x, int n, float* f1, float* f2, float* f3, float* f4, void* stream) {
+  float* f[4] = {f1, f2, f3, f4};
+  return call_introspect(h, false, x, n, f, stream);
+}
+int ian_introspect_host(ian_handle* h, const float* x, int n, float* f1, float* f2, float* f3, float* f4) {
+  float* f[4] = {f1, f2, f3, f4};
+  return call_introspect(h, true, x, n, f, nullptr);
+}
+int ian_introspect_jvp_dev(ian_handle* h, const float* x, const float* v, int n, float* f1, float* f2, float* f3, float* f4,
+                           float* t1, float* t2, float* t3, float* t4, void* stream) {
+  float* f[4] = {f1, f2, f3, f4};
+  float* t[4] = {t1, t2, t3, t4};
+  return call_introspect_jvp(h, false, x, v, n, f, t, stream);
+}
+int ian_introspect_jvp_host(ian_handle* h, const float* x, const float* v, int n, float* f1, float* f2, float* f3, float* f4,
+                            float* t1, float* t2, float* t3, float* t4) {
+  float* f[4] = {f1, f2, f3, f4};
+  float* t[4] = {t1, t2, t3, t4};
+  return call_introspect_jvp(h, true, x, v, n, f, t, nullptr);
+}
+int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
+                                 double* A, double* g, double* e, void* stream) {
+  return call_feature_gauss_newton(h, false, z, x, n, pixel_weight, feature_weight, A, g, e, stream);
+}
+int ian_feature_gauss_newton_host(ian_handle* h, const float* z, const float* x, int n, double pixel_weight,
+                                  double feature_weight, double* A, double* g, double* e) {
+  return call_feature_gauss_newton(h, true, z, x, n, pixel_weight, feature_weight, A, g, e, nullptr);
+}
+int ian_fit_latent_features_dev(ian_handle* h, const float* x, int n, float* z, int iters, double pixel_weight,
+                                double feature_weight, float* loss, void* stream) {
+  return call_fit_latent_features(h, false, x, n, z, iters, pixel_weight, feature_weight, loss, stream);
+}
+int ian_fit_latent_features_host(ian_handle* h, const float* x, int n, float* z, int iters, double pixel_weight,
+                                 double feature_weight, float* loss) {
+  return call_fit_latent_features(h, true, x, n, z, iters, pixel_weight, feature_weight, loss, nullptr);
 }
 
 int ian_edit_loop_dev(ian_handle* h, float* z, const int32_t* boxes, const float* target, int target_is_frame, int n,
