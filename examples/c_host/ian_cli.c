@@ -86,7 +86,8 @@ static int symbols(void) {
       (anyfn)ian_fit_latent_dev, (anyfn)ian_fit_latent_host, (anyfn)ian_map_gauss_newton_dev, (anyfn)ian_map_gauss_newton_host,
       (anyfn)ian_fit_latent_map_dev, (anyfn)ian_fit_latent_map_host, (anyfn)ian_introspect_dev, (anyfn)ian_introspect_host,
       (anyfn)ian_introspect_jvp_dev, (anyfn)ian_introspect_jvp_host, (anyfn)ian_feature_gauss_newton_dev,
-      (anyfn)ian_feature_gauss_newton_host, (anyfn)ian_fit_latent_features_dev, (anyfn)ian_fit_latent_features_host};
+      (anyfn)ian_feature_gauss_newton_host, (anyfn)ian_fit_latent_features_dev, (anyfn)ian_fit_latent_features_host,
+      (anyfn)ian_introspect_vjp_dev, (anyfn)ian_introspect_vjp_host};
   size_t i, n = sizeof(fn) / sizeof(fn[0]);
   for (i = 0; i < n; ++i)
     if (!fn[i]) return 1;

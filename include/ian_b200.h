@@ -385,6 +385,23 @@ int ian_fit_latent_features_dev(ian_handle* h, const float* x, int n, float* z, 
 int ian_fit_latent_features_host(ian_handle* h, const float* x, int n, float* z, int iters, double pixel_weight,
                                  double feature_weight, float* loss /*nullable*/);
 
+/* ---- vector-Jacobian product of the introspection features --------------------------------------------------------------
+ * dx (n,3,64,64) = sum_i (d g_i / d x)^T c_i, with c1..c4 float32 NCHW in ian_introspect_*'s shapes (n,128,32,32),
+ * (n,256,16,16), (n,512,8,8), (n,1024,4,4); each nullable (a zero cotangent).  The derivative conventions are
+ * ian_introspect_jvp_*'s (LeakyRectify 0.2 from the sign of the stored activation, inference BatchNorm scale), so
+ * <c, introspect_jvp(v)> = <introspect_vjp(c), v> up to float32 summation.  The chain is ian_encode_vjp_*'s, entered at the
+ * deepest supplied layer L: the encoder forward stops after enc_conv{L}, and each shallower c_i joins the backward chain
+ * before that layer's activation derivative.  All four NULL: dx = 0 and nothing else runs.  All three graphs, both paths;
+ * bf16 precision on the flow graphs (the cotangents are then rounded to bf16, as the encoder VJP's own gradients are;
+ * enc_conv1's adjoint stays float32).  n == 0 does nothing; n < 0 or a NULL x or dx -> IAN_ERR_INVALID; not finalized ->
+ * IAN_ERR_STATE.  Deterministic (a repeated call is bit-identical; the device form computes the host form's bits).
+ * Memory: the first call per batch size allocates what ian_encode_vjp_* does (shared with it) plus 0.92 MB per image of
+ * cotangent planes for layers 1-3; the host form stages its inputs in ian_introspect*_host's 1.97 MB per image. */
+int ian_introspect_vjp_dev(ian_handle* h, const float* x, int n, const float* c1 /*nullable*/, const float* c2 /*nullable*/,
+                           const float* c3 /*nullable*/, const float* c4 /*nullable*/, float* dx, void* stream);
+int ian_introspect_vjp_host(ian_handle* h, const float* x, int n, const float* c1 /*nullable*/, const float* c2 /*nullable*/,
+                            const float* c3 /*nullable*/, const float* c4 /*nullable*/, float* dx);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -475,7 +492,10 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * (the normal equations' Gram of one sample, with its chunk reduction) and "gn_solve" (the Levenberg-Marquardt solve of
  * the batch); in the masked fit "map_gram" (the weighted Gram of one sample, with its reduction and the prior terms) and
  * "gn_solve"; in the feature fit "feat_gram" (the feature layers' Gram of one sample, with its reduction and the pixel
- * Gram's weighting), "feat_accept" (the trial objective and accept rule of the batch), "gn_gram" and "gn_solve") over the
+ * Gram's weighting), "feat_accept" (the trial objective and accept rule of the batch), "gn_gram" and "gn_solve"; in
+ * ian_introspect_vjp_* "feat_cotangent" (the cotangents' conversion to split planes), "introspect_bwd_enc_conv4",
+ * "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2" (a backward GEMM joined by a supplied cotangent; one without
+ * runs as "bwd_enc_conv*"), "enc_conv1" and "enc_conv1_bwd") over the
  * launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);

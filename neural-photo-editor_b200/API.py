@@ -17,8 +17,9 @@ functions in the prior space l_Z_IAF -- `flow_vjp` / `flow_jvp` (Z_IAF_fn) and `
 torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, the decoder's Gauss-Newton normal equations `gauss_newton` and
 the batched Levenberg-Marquardt latent fit `fit_latent`, their pixel-weighted forms under the N(0, I) prior in the sampling
 space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), the IAN's introspection features `introspect` /
-`introspect_jvp` / `feature_loss` and the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`,
-and `*_dev` variants taking device pointers.
+`introspect_jvp` / `introspect_vjp` / `feature_loss` (torch binding: `torch_ops.introspect` / `torch_ops.feature_loss`) and
+the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`, and `*_dev` variants taking device
+pointers.
 """
 from __future__ import annotations
 
@@ -564,6 +565,29 @@ class IAN:
                                                           *([_fp(a) if a is not None else None for a in f] + [_fp(a) for a in dt])))
         return (f, dt) if return_features else dt
 
+    def introspect_vjp(self, images, cotangents):
+        """Vector-Jacobian product of the introspection features: images float32 (n,3,64,64), cotangents = 4 arrays in
+        introspect()'s shapes (each may be None, a zero cotangent) -> dx = sum_i (d g_i / d x)^T c_i float32 (n,3,64,64),
+        the gradient w.r.t. the images of any loss on the features with dL/dg_i = c_i.  introspect_jvp's derivative
+        conventions, so <c, introspect_jvp(x, v)> = <introspect_vjp(x, c), v>.  One encoder forward to the deepest supplied
+        feature and one backward from it."""
+        x = _img(images)
+        n = x.shape[0]
+        if len(cotangents) != 4:
+            raise ValueError("cotangents must hold 4 arrays or None (got %d)" % len(cotangents))
+        c = []
+        for i, (a, s) in enumerate(zip(cotangents, FEATURE_SHAPES)):
+            if a is not None:
+                a = _f32(a, 4, "cotangents[%d]" % i)
+                if a.shape != (n,) + s:
+                    raise ValueError("cotangents[%d] must be %r, got %r" % (i, (n,) + s, a.shape))
+            c.append(a)
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        if n:
+            self._check(self._lib.ian_introspect_vjp_host(self._h, _fp(x), n, *[_fp(a) if a is not None else None for a in c],
+                                                          _fp(dx)))
+        return dx
+
     def feature_loss(self, x_hat, images):
         """The per-sample feature-wise loss of train_IAN.py:244 under deterministic=True: x_hat, images float32 (n,3,64,64)
         -> (n,) float64 l_f = (1/4) sum_i mean((g_i(x_hat) - g_i(images))^2) over the four introspect() features."""
@@ -971,6 +995,10 @@ class IAN:
         """introspect_jvp() on device pointers: t_ptrs = the 4 tangent outputs, f_ptrs the features (0: not wanted)"""
         self._check(self._lib.ian_introspect_jvp_dev(self._h, x_ptr, v_ptr, int(n), *([p or None for p in f_ptrs] + list(t_ptrs)),
                                                      stream or None))
+
+    def introspect_vjp_dev(self, x_ptr, n, c_ptrs, dx_ptr, stream=0):
+        """introspect_vjp() on device pointers: c_ptrs = 4 pointers to float32 cotangents in FEATURE_SHAPES (0: zero)"""
+        self._check(self._lib.ian_introspect_vjp_dev(self._h, x_ptr, int(n), *[p or None for p in c_ptrs], dx_ptr, stream or None))
 
     def gauss_newton_features_dev(self, z_ptr, x_ptr, n, A_ptr, g_ptr, e_ptr=0, pixel_weight=1.0, feature_weight=1.0, stream=0):
         """gauss_newton_features() on device pointers: A (n,100,100), g (n,100), e (n,) float64 (e optional)"""

@@ -86,6 +86,8 @@ SIGNATURES = {
     "ian_introspect_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F, _F]),
     "ian_introspect_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 9),
     "ian_introspect_jvp_host": (C.c_int, [_H, _F, _F, C.c_int] + [_F] * 8),
+    "ian_introspect_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
+    "ian_introspect_vjp_host": (C.c_int, [_H, _F, C.c_int] + [_F] * 5),
     "ian_feature_gauss_newton_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_feature_gauss_newton_host": (C.c_int, [_H, _F, _F, C.c_int, C.c_double, C.c_double, C.POINTER(C.c_double),

@@ -159,6 +159,22 @@ int launch_feat_gram(const FeatLayers& t, const FeatWeights& c, int feats, int p
 int launch_feat_accept(int init, const float* xht, const float* x, const FeatLayers& f, const FeatWeights& c, int feats,
                        int passes, float* xh, double* e, double* lam, float* z, const float* zt, const int* ok, float* loss,
                        long long ldl, int col, int n, cudaStream_t st);
+// the features' vector-Jacobian product (ian_introspect_vjp_*): per layer l the cotangent c[l] (n, 128 << l, 32 >> l,
+// 32 >> l) float32 NCHW (nullptr: not supplied) -> split planes NHWC at out[l].  Layer `deep` is the chain's seed:
+// r * scale[ch] * (hi(mask) > 0 ? 1 : 0.2) with r = c as a backward GEMM reads it as `res` (hi + lo; hi when passes == 1),
+// the ACT_MASK epilogue on a_deep with a zero accumulator (scale nullptr: 1).  Its lo plane is written only when deep_lo
+// is set: exactly when the backward GEMM landing on that layer writes it (float32 mode, or a split-K finalize), since
+// those planes are the encoder VJP's and a later call may read them.  The others are stored as they are, for the backward
+// GEMMs' `res`.  One launch covers every supplied layer.
+struct FeatCotangents {
+  const float* c[4];
+  __nv_bfloat16* out[4];
+  long long plane[4];
+  int deep, deep_lo;
+  const __nv_bfloat16* mask;
+  const float* scale;
+};
+int launch_feat_cotangent(const FeatCotangents& c, int passes, int n, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

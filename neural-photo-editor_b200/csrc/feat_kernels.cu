@@ -10,6 +10,8 @@
 //   feat_gram_reduce  : A = sum_i c_i (chunk sums of layer i, in chunk order) [+ a A_pixel], likewise g and e
 //   feat_accept       : e_trial = a |x_hat_trial - x|^2 + sum_i c_i |g_i(x_hat_trial) - g_i(x)|^2 in a fixed order, then
 //                       gn_accept's rule; an accepted step (and the start) also keeps the trial's features as the current ones
+//   feat_cotangent    : the features' cotangents (ian_introspect_vjp_*) float32 NCHW -> split planes NHWC, transposed
+//                       through shared memory; the deepest supplied layer gets the backward GEMMs' ACT_MASK rule
 // Every product of two operands is formed in float64, where a product of two float32 values is exact; the only roundings
 // are the additions (in a fixed order) and the c_i and a scalings, applied once per layer sum.
 #include "edge.h"
@@ -227,6 +229,53 @@ __global__ void __launch_bounds__(256) feat_accept_kernel(int init, const float*
   if (t < kLat) z[(size_t)k * kLat + t] = zt[(size_t)k * kLat + t];
 }
 
+// The deepest layer's value is what its backward GEMM's epilogue would write from a zero accumulator with the cotangent as
+// `res`: (0 + res) * scale * lrelu'(a), res read as the GEMM reads it (hi + lo, or hi in bf16 mode), and it writes the
+// planes that GEMM writes (in bf16 mode the lo plane only under a split-K finalize).  So a zero cotangent above it gives
+// the same bits as leaving that layer out, and the encoder VJP's planes hold afterwards what its own GEMM leaves there.
+// grid (tiles of the supplied layers, n), kCotThreads.  A tile is kCotCh channels x kCotPix pixels of one image and layer;
+// layer l's tiles start at tile0.{x,y,z} for l = 1, 2, 3 (0 for l = 0).  The NCHW rows are read along pixels and the NHWC
+// planes written along channels, both coalesced, through a padded shared-memory tile.
+constexpr int kCotCh = 32, kCotPix = 16, kCotThreads = 128;
+constexpr int cot_tiles(int l) { return ((128 << l) / kCotCh) * ((1024 >> (2 * l)) / kCotPix); }   // 256, 128, 64, 32
+
+__global__ void __launch_bounds__(kCotThreads) feat_cotangent_kernel(FeatCotangents c, int passes, int3 tile0) {
+  pdl_trigger();
+  __shared__ float s[kCotCh][kCotPix + 1];
+  const int t = blockIdx.x, k = blockIdx.y, tid = threadIdx.x;
+  const int l = t >= tile0.z ? 3 : t >= tile0.y ? 2 : t >= tile0.x ? 1 : 0;
+  const int C = 128 << l, HW = 1024 >> (2 * l);
+  const int tt = t - (l == 3 ? tile0.z : l == 2 ? tile0.y : l == 1 ? tile0.x : 0);
+  const int ch0 = tt / (HW / kCotPix) * kCotCh, px0 = tt % (HW / kCotPix) * kCotPix;
+  const float* src = pick(c.c, l);
+  __nv_bfloat16* dst = pick(c.out, l);
+  const long long plane = pick(c.plane, l);
+  pdl_wait();
+#pragma unroll
+  for (int i = 0; i < kCotCh * kCotPix / kCotThreads; ++i) {
+    const int ch = tid / kCotPix + i * (kCotThreads / kCotPix), px = tid % kCotPix;
+    s[ch][px] = src[((long long)k * C + ch0 + ch) * HW + px0 + px];
+  }
+  __syncthreads();
+  const bool deep = l == c.deep;
+  const int ch = tid % kCotCh;
+  const float sc = deep && c.scale ? c.scale[ch0 + ch] : 1.f;
+#pragma unroll
+  for (int i = 0; i < kCotCh * kCotPix / kCotThreads; ++i) {
+    const int px = tid / kCotCh + i * (kCotThreads / kCotCh);
+    const long long o = ((long long)k * HW + px0 + px) * C + ch0 + ch;
+    float v = s[ch][px];
+    __nv_bfloat16 hi, lo;
+    split_bf16(v, hi, lo);
+    if (deep) {   // tapgemm's res + ACT_MASK epilogue on a zero accumulator: res as the GEMM reads it, then scale and mask
+      const float r = passes == 1 ? __bfloat162float(hi) : __bfloat162float(hi) + __bfloat162float(lo);
+      split_bf16(r * sc * (__bfloat162float(c.mask[o]) > 0.f ? 1.f : 0.2f), hi, lo);
+    }
+    dst[o] = hi;
+    if (!deep || c.deep_lo) dst[plane + o] = lo;
+  }
+}
+
 }  // namespace
 
 size_t feat_part_doubles() { return (size_t)kChunks * kTiles * kTile * kTile; }
@@ -256,6 +305,16 @@ int launch_feat_accept(int init, const float* xht, const float* x, const FeatLay
                        long long ldl, int col, int n, cudaStream_t st) {
   if (launch_pdl(feat_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, f, c, feats, passes, xh, e, lam, z, zt, ok, loss, ldl,
                  col) != cudaSuccess)
+    return -1;
+  return 1;
+}
+
+int launch_feat_cotangent(const FeatCotangents& c, int passes, int n, cudaStream_t st) {
+  int first[5] = {0, 0, 0, 0, 0};
+  for (int l = 0; l < 4; ++l) first[l + 1] = first[l] + (c.c[l] ? cot_tiles(l) : 0);
+  if (first[4] == 0 || n == 0) return 0;
+  if (launch_pdl(feat_cotangent_kernel, dim3(first[4], n), dim3(kCotThreads), 0, st, c, passes, make_int3(first[1], first[2], first[3])) !=
+      cudaSuccess)
     return -1;
   return 1;
 }

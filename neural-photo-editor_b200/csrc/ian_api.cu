@@ -157,6 +157,9 @@ enum LayerId {
   // encoder Jacobian-vector product (ian_encode_jvp_*): the tangent twins of enc_conv2..4, enc_fc1 and the encoder head
   // (kEncoderJvp); built on first use
   JE_ENC_CONV2, JE_ENC_CONV3, JE_ENC_CONV4, JE_ENC_FC1, JE_ENC_HEAD,
+  // the features' vector-Jacobian product (ian_introspect_vjp_*): E_BWD_CONV4..2 with a shallower feature's cotangent
+  // joining before the activation derivative (res); built on first use
+  IV_BWD_CONV4, IV_BWD_CONV3, IV_BWD_CONV2,
   L_COUNT,
   T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
@@ -168,6 +171,7 @@ enum LayerId {
   T_MAP_GRAM,                                           // the masked fit's weighted Gram (with its reduction and the prior)
   T_FEAT_GRAM, T_FEAT_ACCEPT,                           // the feature fit's Gram over the four feature layers (with its
                                                         // reduction) and its trial reduction and accept rule
+  T_FEAT_COTANGENT,                                     // the features' VJP: the cotangents' conversion to split planes
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -183,10 +187,11 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_dec_conv3a", "jvp_dec_conv3a2", "jvp_full_dec_conv3", "jvp_dec_conv4a", "jvp_dec_conv4a2",
                                     "jvp_full_dec_conv4", "rgb_head_jvp",
                                     "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
+                                    "introspect_bwd_enc_conv4", "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
                                     "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
-                                    "feat_gram", "feat_accept"};
+                                    "feat_gram", "feat_accept", "feat_cotangent"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -382,6 +387,10 @@ struct Plan {
   float *ftg = nullptr, *fcur = nullptr;
   // ian_introspect*_host staging: the features, then their tangents, float32 NCHW, laid out as ftg (first host call)
   float* ifeat = nullptr;
+  // the features' VJP (allocated on the plan's first ian_introspect_vjp_* call, with the encoder VJP's planes): the
+  // cotangents of a1..a3 as split planes NHWC, the res operand of IV_BWD_CONV2..4 (0.92 MB per image)
+  bool ivjp = false;
+  Planes ivc[3];
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -2631,7 +2640,8 @@ int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w
 // encoder forward stopped after enc_conv4, and the feature values are what it stores (hi + lo, or hi in bf16 mode).
 const Planes& feat_planes(Plan* pl, int l) { return l == 0 ? pl->a1 : l == 1 ? pl->a2 : l == 2 ? pl->a3 : pl->a4; }
 
-int run_introspect(ian_handle* h, Plan* pl, const float* x, cudaStream_t st) {
+// depth < 4: the forward stops after enc_conv{depth}
+int run_introspect(ian_handle* h, Plan* pl, const float* x, cudaStream_t st, int depth = 4) {
   {
     ScopedTimer tm(h, T_CONV1, st);
     if (h->path == IAN_PATH_TC)
@@ -2640,7 +2650,7 @@ int run_introspect(ian_handle* h, Plan* pl, const float* x, cudaStream_t st) {
       LAUNCH_TRY(h, launch_conv1(x, h->conv1_wt, h->conv1_b, pl->a1.p, pl->a1.plane, pl->n, st));
   }
   int rc;
-  for (int k = 0; k < 3; ++k)
+  for (int k = 0; k < depth - 1; ++k)
     if ((rc = run_gemm(h, pl, kEncoder.l[k], st)) != IAN_OK) return rc;
   return IAN_OK;
 }
@@ -2718,6 +2728,93 @@ int call_introspect_jvp(ian_handle* h, bool host, const float* x, const float* v
     float* ot[4] = {c.f(6), c.f(7), c.f(8), c.f(9)};
     if (r == IAN_OK) r = store_features(h, c.pl, false, o, nullptr, 1, c.st);
     return r != IAN_OK ? r : store_features(h, c.pl, true, ot, nullptr, 1, c.st);
+  });
+}
+
+// ---- the features' vector-Jacobian product (DESIGN section 5.6l) ---------------------------------------------------------
+// dx = sum_i (d g_i / d x)^T c_i: run_encode_vjp's chain entered at the deepest supplied layer L instead of at the head.
+// The forward stops after enc_conv{L}; feat_cotangent writes c_L times scale_L * lrelu'(a_L) into e_L -- exactly what the
+// GEMM landing on a_L would write from a zero accumulator with c_L as res, so a zero c_L above gives the same bits as
+// leaving it out -- and the shallower supplied c_l, as they are, into the staging planes ivc.  Each backward
+// GEMM that lands on a layer with a supplied cotangent runs as its IV_BWD_* copy, whose epilogue adds ivc before the
+// activation derivative: e_l = (acc + c_l) * scale_l * lrelu'(a_l) (res, res_after = 0, ACT_MASK, as the encoder JVP's
+// tangent twins use it); a layer without one runs the encoder VJP's own descriptor.  enc_conv1's adjoint ends the chain.
+// The first call on a plan allocates what ian_encode_vjp_* does (shared with it) and the staging planes; the host form
+// stages x in the plan's image buffer, the cotangents in the ian_introspect*_host buffer and dx in its x_hat buffer.
+template <bool kHost>
+int ensure_introspect_vjp_plan(ian_handle* h, Plan* pl) {
+  int rc;
+  if ((rc = ensure_enc_vjp_plan(h, pl)) != IAN_OK) return rc;
+  if (!pl->ivjp) {
+    const Planes* a[3] = {&pl->a1, &pl->a2, &pl->a3};
+    const int from[3] = {E_BWD_CONV2, E_BWD_CONV3, E_BWD_CONV4}, to[3] = {IV_BWD_CONV2, IV_BWD_CONV3, IV_BWD_CONV4};
+    for (int l = 0; l < 3; ++l) {
+      if ((rc = alloc_planes(h, pl, pl->ivc[l], a[l]->plane)) != IAN_OK) return rc;
+      TapGemm& g = pl->g[to[l]];
+      g = pl->g[from[l]];                                 // its split-K factor and slabs too: the two never run at once
+      g.res = pl->ivc[l].p; g.res_plane = pl->ivc[l].plane; g.res_after = 0;
+      char err[256] = {0};
+      if (!(pl->maps[to[l]] = tc_build_maps(g, err, sizeof(err)))) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[to[l]], err);
+    }
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    pl->ivjp = true;
+  }
+  return ensure_introspect_plan<kHost, false>(h, pl);
+}
+
+int run_introspect_vjp(ian_handle* h, Plan* pl, const float* x, const float* const* c, float* dx, cudaStream_t st) {
+  const int n = pl->n;
+  int L = 4;                                              // the deepest supplied layer, 1-based
+  while (L > 0 && !c[L - 1]) --L;
+  if (L == 0) {
+    CUDA_TRY(h, cudaMemsetAsync(dx, 0, (size_t)n * kImageBytes, st));
+    return IAN_OK;
+  }
+  int rc = run_introspect(h, pl, x, st, L);
+  if (rc != IAN_OK) return rc;
+  Planes* e[4] = {&pl->e1, &pl->e2, &pl->e3, &pl->e4};
+  FeatCotangents fc{};
+  for (int l = 0; l < L; ++l) {
+    fc.c[l] = c[l];
+    const Planes& o = l == L - 1 ? *e[l] : pl->ivc[l];
+    fc.out[l] = o.p;
+    fc.plane[l] = o.plane;
+  }
+  fc.deep = L - 1;
+  // e_L's lo plane as the GEMM landing on a_L leaves it: bf16 mode writes it only in a split-K finalize (tapgemm.h), and
+  // enc_conv1's adjoint reads hi + lo of e1, in later encoder VJP calls too
+  const int land[4] = {E_BWD_CONV2, E_BWD_CONV3, E_BWD_CONV4, E_BWD_FC1};
+  fc.deep_lo = h->passes != 1 || (h->path == IAN_PATH_TC && pl->g[land[L - 1]].ksplit > 1);
+  fc.mask = feat_planes(pl, L - 1).p;
+  fc.scale = L == 1 ? nullptr : h->w[kEncoder.l[L - 2]].scale;   // bnorm{L}; enc_conv1 has a bias and no BatchNorm
+  {
+    ScopedTimer tm(h, T_FEAT_COTANGENT, st);
+    LAUNCH_TRY(h, launch_feat_cotangent(fc, h->passes, n, st));
+  }
+  const int bwd[3][2] = {{E_BWD_CONV2, IV_BWD_CONV2}, {E_BWD_CONV3, IV_BWD_CONV3}, {E_BWD_CONV4, IV_BWD_CONV4}};
+  for (int l = L - 2; l >= 0; --l)                        // e_{l+2} -> e_{l+1} (1-based), joined by c_{l+1}
+    if ((rc = run_gemm(h, pl, bwd[l][c[l] ? 1 : 0], st)) != IAN_OK) return rc;
+  ScopedTimer tm(h, T_CONV1_BWD, st);
+  if (h->path == IAN_PATH_TC)
+    LAUNCH_TRY(h, launch_conv1_bwd_tc(pl->conv1_bwd_maps, dx, n, st));
+  else
+    LAUNCH_TRY(h, launch_conv1_bwd(pl->e1.p, pl->e1.plane, h->conv1_bwd_wt, dx, n, st));
+  return IAN_OK;
+}
+
+// No CUDA graphs, as for the other introspect entries.  All four cotangents NULL: dx = 0, nothing else runs.
+int call_introspect_vjp(ian_handle* h, bool host, const float* x, int n, const float* const* c, float* dx, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !dx) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  const bool any = c[0] || c[1] || c[2] || c[3];
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {c[0], kFeatBytes[0], S_F1, IN},
+                                        {c[1], kFeatBytes[1], S_F1 + 1, IN}, {c[2], kFeatBytes[2], S_F1 + 2, IN},
+                                        {c[3], kFeatBytes[3], S_F1 + 3, IN}, {dx, kImageBytes, S_XHAT, OUT}},
+                   !any ? nullptr : host ? ensure_introspect_vjp_plan<true> : ensure_introspect_vjp_plan<false>,
+                   [&](const Chunk& ch) {
+    const float* ct[4] = {ch.f(1), ch.f(2), ch.f(3), ch.f(4)};
+    return run_introspect_vjp(h, ch.pl, ch.f(0), ct, ch.f(5), ch.st);
   });
 }
 
@@ -3213,6 +3310,16 @@ int ian_introspect_jvp_host(ian_handle* h, const float* x, const float* v, int n
   float* f[4] = {f1, f2, f3, f4};
   float* t[4] = {t1, t2, t3, t4};
   return call_introspect_jvp(h, true, x, v, n, f, t, nullptr);
+}
+int ian_introspect_vjp_dev(ian_handle* h, const float* x, int n, const float* c1, const float* c2, const float* c3,
+                           const float* c4, float* dx, void* stream) {
+  const float* c[4] = {c1, c2, c3, c4};
+  return call_introspect_vjp(h, false, x, n, c, dx, stream);
+}
+int ian_introspect_vjp_host(ian_handle* h, const float* x, int n, const float* c1, const float* c2, const float* c3,
+                            const float* c4, float* dx) {
+  const float* c[4] = {c1, c2, c3, c4};
+  return call_introspect_vjp(h, true, x, n, c, dx, nullptr);
 }
 int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
                                  double* A, double* g, double* e, void* stream) {

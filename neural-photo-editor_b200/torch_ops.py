@@ -16,6 +16,13 @@
     in reverse and forward mode, so decode(model, flow(model, z_iaf)) -- the script's `sample` -- optimises in prior space,
     and flow(model, encode_pre(model, x)) is encode(model, x) with eps absent.
 
+  * introspect(model, x) = the IAN's introspection features l_introspect = [enc_conv1..4] (IAN_simple.py:240, what
+    model.introspect returns) as a differentiable torch op.  Its backward is the features' vector-Jacobian product
+    (ian_introspect_vjp_dev, one call for all four features; an unused feature costs nothing and the chain starts at the
+    deepest one used), its jvp ian_introspect_jvp_dev.  feature_loss(model, x_hat, x) is the per-sample feature-wise loss
+    of train_IAN.py:244 built on it, so feature_loss(model, decode(model, z), x).sum().backward() drives z -- or, with
+    params, the IAN_simple decoder's parameters -- under the generator's own reconstruction objective.
+
   * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
     (ian_decode_param_vjp_dev) that also returns dz.  Before each forward, every tensor whose in-place version moved since
@@ -33,6 +40,7 @@ from .train_ops import _lib_stream
 _Decode = None
 _Encode = None
 _DecodeParams = None
+_Introspect = None
 
 
 def _check_tensor(model, t, what):
@@ -265,6 +273,90 @@ def flow(model, z_iaf):
     so losses on a prior sample's image -- fitting z_iaf to a photo, a brush loss plus a |z_iaf|^2 prior term -- drive z_iaf
     through torch.autograd."""
     return _prior_function("flow").apply(model, z_iaf)
+
+
+def _introspect_function():
+    global _Introspect
+    if _Introspect is not None:
+        return _Introspect
+    import torch
+    from torch.autograd.function import once_differentiable
+    from .API import FEATURE_SHAPES
+
+    class Introspect(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, model, x):
+            _check_tensor(model, x, "x")
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 64, 64):
+                raise ValueError("x must be (n,3,64,64), got %r" % (tuple(x.shape),))
+            x = x.contiguous()
+            n = int(x.shape[0])
+            f = [torch.empty((n,) + s, dtype=torch.float32, device=x.device) for s in FEATURE_SHAPES]
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.introspect_dev(x.data_ptr(), n, [a.data_ptr() for a in f], st)
+            ctx.model = model
+            ctx.set_materialize_grads(False)              # an unused feature reaches backward as None: a NULL cotangent
+            ctx.save_for_backward(x)
+            ctx.save_for_forward(x)
+            return tuple(f)
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, *gs):
+            (x,) = ctx.saved_tensors
+            model = ctx.model
+            cs = []
+            for g in gs:
+                if g is not None:
+                    _check_tensor(model, g, "grad_output")
+                    g = g.contiguous()
+                cs.append(g)
+            n = int(x.shape[0])
+            dx = torch.empty_like(x)
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.introspect_vjp_dev(x.data_ptr(), n, [c.data_ptr() if c is not None else 0 for c in cs],
+                                             dx.data_ptr(), st)
+            return None, dx
+
+        @staticmethod
+        def jvp(ctx, _model_t, v):
+            (x,) = ctx.saved_tensors
+            model = ctx.model
+            n = int(x.shape[0])
+            if v is None:
+                return tuple(torch.zeros((n,) + s, dtype=torch.float32, device=x.device) for s in FEATURE_SHAPES)
+            _check_tensor(model, v, "tangent")
+            v = v.contiguous()
+            t = [torch.empty((n,) + s, dtype=torch.float32, device=x.device) for s in FEATURE_SHAPES]
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.introspect_jvp_dev(x.data_ptr(), v.data_ptr(), n, [a.data_ptr() for a in t], (0, 0, 0, 0), st)
+            return tuple(t)
+
+    _Introspect = Introspect
+    return Introspect
+
+
+def introspect(model, x):
+    """(f1, f2, f3, f4) = the IAN's introspection features of x (n,3,64,64) float32 CUDA on the model's device: enc_conv1..4
+    after inference BatchNorm and LeakyReLU, shapes (n,128,32,32), (n,256,16,16), (n,512,8,8), (n,1024,4,4) -- what
+    model.introspect returns.  Differentiable w.r.t. x in reverse mode (one ian_introspect_vjp_dev call per backward; a
+    feature the loss does not use passes a NULL cotangent, so the chain starts at the deepest feature used) and forward mode
+    (one ian_introspect_jvp_dev call)."""
+    return _introspect_function().apply(model, x)
+
+
+def feature_loss(model, x_hat, x):
+    """Per-sample feature-wise loss of train_IAN.py:244, (1/4) sum_i mean((g_i(x_hat) - g_i(x))^2) over introspect's four
+    features, (n,) float32; differentiable w.r.t. x_hat and x through introspect (the same formula as
+    model.feature_loss)."""
+    fa, fb = introspect(model, x_hat), introspect(model, x)
+    n = int(fa[0].shape[0])
+    if int(fb[0].shape[0]) != n:
+        raise ValueError("x_hat and x must hold the same number of images")
+    return sum(((a - b) ** 2).reshape(n, -1).mean(1) for a, b in zip(fa, fb)) / 4
 
 
 def _params_function():
