@@ -340,6 +340,51 @@ int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w /*nulla
 int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int n, float* u,
                             float* z_out /*nullable*/, int iters, float* loss /*nullable*/);
 
+/* ---- robust latent fit: Huber and Cauchy pixel losses by reweighted Levenberg-Marquardt ----------------------------------
+ * The masked fit above with a robust loss rho on each squared residual, so pixels the generator cannot draw (an occluder, a
+ * caption, a highlight) lose their pull on u without anyone marking them.  In the same fit space u, with r, w (NULL: all ones)
+ * and prior = beta as there, s = r^2 and a per-sample scale delta:
+ *   E(u) = sum_{p: w_p > 0} w_p rho(r_p^2) + beta |u|^2
+ *   IAN_ROBUST_HUBER:  rho(s) = s for s <= delta^2, else 2 delta sqrt(s) - delta^2;   rho'(s) = 1, or delta / sqrt(s)
+ *   IAN_ROBUST_CAUCHY: rho(s) = delta^2 log1p(s / delta^2);                            rho'(s) = 1 / (1 + s / delta^2)
+ * Both rho are concave in s, so with omega_p = w_p rho'(r_p^2) at the current u, sum_p omega_p r_p(u')^2 majorises E up to a
+ * constant and Gauss-Newton on it (iteratively reweighted least squares) is sound.
+ * scale (n doubles, nullable): delta per sample, > 0 and not NaN; +inf only for Huber, where the loss is exactly the squared
+ *   one.  NULL: automatic, taken once at the start and held for the whole fit: delta = max(m c, 1/255) with m the lower median
+ *   (rank floor((count - 1) / 2)) of float32 |x_hat - x| over the pixels with w > 0 at the start's x_hat, c = 1.345 * 1.4826
+ *   (Huber) or 2.3849 * 1.4826 (Cauchy) -- the 95 %-efficiency constants times the MAD's Gaussian consistency factor -- and
+ *   1/255 half an 8-bit level on [-1, 1]; 1/255 when no pixel is weighted (E is then the prior alone).  scale_out (n,
+ *   nullable) receives the delta used.
+ * ian_robust_gauss_newton_*: A = J_u^T Omega J_u + beta I (n,100,100, both triangles), g = J_u^T Omega r + beta u (n,100)
+ *   (= half the gradient of E) and e = E(u) (n, nullable), float64, from ian_map_gauss_newton_*'s J_u pass; omega multiplies
+ *   one factor of every product, formed in float64.  With scale NULL delta is automatic at u.
+ * ian_fit_latent_robust_*: `iters` Levenberg-Marquardt steps per sample in place on u, with ian_fit_latent_map_*'s solve,
+ *   damping, constants and accept / reject rule applied to this A, g and the true E: loss (n, iters+1, nullable) receives
+ *   E / 12288 of the start and after every step, non-increasing, and a flat entry leaves u bit-unchanged.  z_out as in
+ *   ian_fit_latent_map_*.  outlier_w (n,3,64,64, nullable) receives rho'(r^2) at the final u (1 where the loss is quadratic,
+ *   towards 0 on what the latent does not explain) and 0 where w == 0.
+ * Huber with every scale +inf computes ian_map_gauss_newton_*'s A and g and ian_fit_latent_map_*'s u, z and loss bits; its e
+ * differs from map's by summation order only.  Both: all three graphs, both paths; bf16 precision on the flow graphs.
+ * n == 0 does nothing; an unknown kind, n < 0, iters < 0, a negative or non-finite prior, or a NULL u, x, A or g ->
+ * IAN_ERR_INVALID; the host forms also check every weight (finite, >= 0) and every scale (the device forms take w and scale as
+ * given); not finalized -> IAN_ERR_STATE.  Deterministic (a repeated call is bit-identical; the device form computes the host
+ * form's bits); one sample's inputs never change another sample's outputs.  Memory: what ian_fit_latent_map_* allocates,
+ * shared with it, plus 8 bytes per image of the plan. */
+enum { IAN_ROBUST_HUBER = 1, IAN_ROBUST_CAUCHY = 2 };
+int ian_robust_gauss_newton_dev(ian_handle* h, const float* u, const float* x, const float* w /*nullable*/, double prior,
+                                int kind, const double* scale /*nullable*/, int n, double* A, double* g, double* e /*nullable*/,
+                                double* scale_out /*nullable*/, void* stream);
+int ian_robust_gauss_newton_host(ian_handle* h, const float* u, const float* x, const float* w /*nullable*/, double prior,
+                                 int kind, const double* scale /*nullable*/, int n, double* A, double* g,
+                                 double* e /*nullable*/, double* scale_out /*nullable*/);
+int ian_fit_latent_robust_dev(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int kind,
+                              const double* scale /*nullable*/, int n, float* u, float* z_out /*nullable*/, int iters,
+                              float* loss /*nullable*/, double* scale_out /*nullable*/, float* outlier_w /*nullable*/,
+                              void* stream);
+int ian_fit_latent_robust_host(ian_handle* h, const float* x, const float* w /*nullable*/, double prior, int kind,
+                               const double* scale /*nullable*/, int n, float* u, float* z_out /*nullable*/, int iters,
+                               float* loss /*nullable*/, double* scale_out /*nullable*/, float* outlier_w /*nullable*/);
+
 /* ---- the IAN's introspection features and the latent fit under its feature-wise loss ---------------------------------
  * The features g_1..g_4 are l_introspect = [enc_conv1, enc_conv2, enc_conv3, enc_conv4] of the reference graphs
  * (IAN_simple.py:240, IAN.py:227, IANv1.py:220): the deterministic encoder's activations after BatchNorm (inference
@@ -495,7 +540,8 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
  * Gram's weighting), "feat_accept" (the trial objective and accept rule of the batch), "gn_gram" and "gn_solve"; in
  * ian_introspect_vjp_* "feat_cotangent" (the cotangents' conversion to split planes), "introspect_bwd_enc_conv4",
  * "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2" (a backward GEMM joined by a supplied cotangent; one without
- * runs as "bwd_enc_conv*"), "enc_conv1" and "enc_conv1_bwd") over the
+ * runs as "bwd_enc_conv*"), "enc_conv1" and "enc_conv1_bwd"; in the robust fit "robust_gram" (the reweighted Gram of
+ * one sample, with its reduction and the prior terms), "robust_scale" (the automatic scale of the batch) and "gn_solve") over the
  * launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);

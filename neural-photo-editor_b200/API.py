@@ -51,6 +51,14 @@ _FULL_CFG = {
 _FULL_MODEL_KEYS = _SIMPLE_MODEL_KEYS + ('l_IAF_mu', 'l_IAF_ls', 'l_Z_IAF')
 # l_introspect = [enc_conv1, enc_conv2, enc_conv3, enc_conv4] (IAN_simple.py:240): per-image shapes
 FEATURE_SHAPES = ((128, 32, 32), (256, 16, 16), (512, 8, 8), (1024, 4, 4))
+# the robust fit's losses (include/ian_b200.h IAN_ROBUST_*)
+ROBUST_KINDS = {"huber": 1, "cauchy": 2}
+
+
+def _robust_kind(kind):
+    if kind not in ROBUST_KINDS:
+        raise ValueError("kind must be one of %s (got %r)" % (sorted(ROBUST_KINDS), kind))
+    return ROBUST_KINDS[kind]
 
 
 def made_ordering(seed=1234, n=100):
@@ -536,6 +544,76 @@ class IAN:
                                                           _fp(z), iters, _fp(loss)))
         return (u, z, loss) if return_loss else (u, z)
 
+    def _robust_args(self, kind, scale, n):
+        if scale is None:
+            return _robust_kind(kind), None
+        s = np.ascontiguousarray(np.broadcast_to(np.asarray(scale, np.float64), (n,)))
+        if not np.all(s > 0) or (kind == "cauchy" and not np.all(np.isfinite(s))):
+            raise ValueError("scale must be > 0 (and finite for the Cauchy loss), got %r" % (scale,))
+        return _robust_kind(kind), s
+
+    def gauss_newton_robust(self, u, images, kind="huber", scale=None, weights=None, prior=0.0):
+        """The normal equations of the robust fit at each fit-space point u (as for gauss_newton_map): kind "huber" or
+        "cauchy", scale None (automatic: from the lower median of |sample(u) - images| over the weighted pixels), a float for
+        every sample or an (n,) array, > 0 (+inf allowed for Huber: the squared loss) -> (A (n,100,100), g (n,100), e (n,),
+        scale (n,)) float64 with omega = w rho'(r^2), A = J_u^T Omega J_u + prior I, g = J_u^T Omega r + prior u and
+        e = sum w rho(r^2) + prior |u|^2 (include/ian_b200.h, ian_robust_gauss_newton_*)."""
+        u = _z(u, 'u')
+        x, w, prior = self._map_args(images, weights, prior)
+        n = u.shape[0]
+        if x.shape[0] != n:
+            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        k, s = self._robust_args(kind, scale, n)
+        A = np.empty((n, 100, 100), np.float64)
+        g = np.empty((n, 100), np.float64)
+        e = np.empty((n,), np.float64)
+        so = np.empty((n,), np.float64)
+        if n:
+            d = C.POINTER(C.c_double)
+            self._check(self._lib.ian_robust_gauss_newton_host(
+                self._h, _fp(u), _fp(x), _fp(w) if w is not None else None, prior, k,
+                s.ctypes.data_as(d) if s is not None else None, n, A.ctypes.data_as(d), g.ctypes.data_as(d),
+                e.ctypes.data_as(d), so.ctypes.data_as(d)))
+        return A, g, e, so
+
+    def fit_latent_robust(self, images, kind="huber", scale=None, weights=None, prior=0.0, u0=None, iters=10,
+                          return_loss=False, return_outliers=False):
+        """Fit the sampling-space latent to each image under a robust pixel loss: `iters` reweighted Levenberg-Marquardt
+        steps on sum_p w_p rho((sample(u) - images)_p^2) + prior |u|^2, so pixels the generator cannot draw (occluders,
+        captions, highlights) lose their pull without being masked.  kind "huber" (convex, for mild outliers) or "cauchy"
+        (redescending, for gross ones); scale as for gauss_newton_robust, automatic at the start when None; weights, prior
+        and u0 as for fit_latent_map -> (u, z = Z_IAF_fn(u) float32 (n,100), scale float64 (n,)), then with return_loss the
+        per-sample objective / 12288 of the start and after every step, float32 (n, iters+1), non-increasing, and with
+        return_outliers rho'(r^2) at the fit, float32 (n,3,64,64): near 1 where the latent explains the pixel, near 0 on
+        outliers, 0 where the weight is 0."""
+        x, w, prior = self._map_args(images, weights, prior)
+        n = x.shape[0]
+        iters = _int_scalar(iters, 'iters')
+        if iters < 0:
+            raise ValueError("iters must not be negative (got %d)" % iters)
+        k, s = self._robust_args(kind, scale, n)
+        if u0 is None:
+            u = self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x))
+        else:
+            u = _z(u0, 'u0').copy()
+        if u.shape[0] != n:
+            raise ValueError("u0 must be (%d,100), got %r" % (n, u.shape))
+        z = np.empty((n, 100), np.float32)
+        so = np.empty((n,), np.float64)
+        loss = np.empty((n, iters + 1), np.float32)
+        out = np.empty((n, 3, 64, 64), np.float32) if return_outliers else None
+        if n:
+            d = C.POINTER(C.c_double)
+            self._check(self._lib.ian_fit_latent_robust_host(
+                self._h, _fp(x), _fp(w) if w is not None else None, prior, k, s.ctypes.data_as(d) if s is not None else None,
+                n, _fp(u), _fp(z), iters, _fp(loss), so.ctypes.data_as(d), _fp(out) if out is not None else None))
+        res = (u, z, so)
+        if return_loss:
+            res += (loss,)
+        if return_outliers:
+            res += (out,)
+        return res
+
     # ---- the introspection features and the fit under the feature-wise loss ------------------------------------------------
     def introspect(self, images):
         """The IAN's introspection features l_introspect (IAN_simple.py:240): images float32 (n,3,64,64) -> [f1 (n,128,32,32),
@@ -986,6 +1064,23 @@ class IAN:
         float32; w_ptr, z_ptr and loss_ptr may be 0"""
         self._check(self._lib.ian_fit_latent_map_dev(self._h, x_ptr, w_ptr or None, float(prior), int(n), u_ptr, z_ptr or None,
                                                      int(iters), loss_ptr or None, stream or None))
+
+    def gauss_newton_robust_dev(self, u_ptr, x_ptr, w_ptr, prior, kind, scale_ptr, n, A_ptr, g_ptr, e_ptr=0, scale_out_ptr=0,
+                                stream=0):
+        """device-pointer form of gauss_newton_robust: kind "huber" / "cauchy", scale (n) float64 or 0 (automatic), A
+        (n,100,100), g (n,100), e (n), scale_out (n) float64; w_ptr, e_ptr and scale_out_ptr may be 0"""
+        self._check(self._lib.ian_robust_gauss_newton_dev(self._h, u_ptr, x_ptr, w_ptr or None, float(prior), _robust_kind(kind),
+                                                          scale_ptr or None, int(n), A_ptr, g_ptr, e_ptr or None,
+                                                          scale_out_ptr or None, stream or None))
+
+    def fit_latent_robust_dev(self, x_ptr, w_ptr, prior, kind, scale_ptr, n, u_ptr, iters, z_ptr=0, loss_ptr=0,
+                              scale_out_ptr=0, outliers_ptr=0, stream=0):
+        """device-pointer form of fit_latent_robust: u (n,100) in place (in: the start), z (n,100) = F(u), loss (n, iters+1)
+        float32, scale_out (n) float64, outliers (n,3,64,64) float32; every pointer but x_ptr and u_ptr may be 0"""
+        self._check(self._lib.ian_fit_latent_robust_dev(self._h, x_ptr, w_ptr or None, float(prior), _robust_kind(kind),
+                                                        scale_ptr or None, int(n), u_ptr, z_ptr or None, int(iters),
+                                                        loss_ptr or None, scale_out_ptr or None, outliers_ptr or None,
+                                                        stream or None))
 
     def introspect_dev(self, x_ptr, n, f_ptrs, stream=0):
         """introspect() on device pointers: f_ptrs = 4 pointers (0: not wanted) to float32 outputs in FEATURE_SHAPES"""

@@ -82,6 +82,14 @@ SIGNATURES = {
     "ian_fit_latent_map_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                          C.c_void_p, C.c_void_p]),
     "ian_fit_latent_map_host": (C.c_int, [_H, _F, _F, C.c_double, C.c_int, _F, _F, C.c_int, _F]),
+    "ian_robust_gauss_newton_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_int]
+                                    + [C.c_void_p] * 5),
+    "ian_robust_gauss_newton_host": (C.c_int, [_H, _F, _F, _F, C.c_double, C.c_int, C.POINTER(C.c_double), C.c_int]
+                                     + [C.POINTER(C.c_double)] * 4),
+    "ian_fit_latent_robust_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_fit_latent_robust_host": (C.c_int, [_H, _F, _F, C.c_double, C.c_int, C.POINTER(C.c_double), C.c_int, _F, _F, C.c_int,
+                                             _F, C.POINTER(C.c_double), _F]),
     "ian_introspect_dev": (C.c_int, [_H, C.c_void_p, C.c_int] + [C.c_void_p] * 5),
     "ian_introspect_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F, _F]),
     "ian_introspect_jvp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 9),

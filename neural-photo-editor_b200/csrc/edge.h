@@ -129,6 +129,23 @@ int launch_map_gram(const float* J, const float* xh, const float* x, const float
                     double* A, double* g, double* e, cudaStream_t st);
 int launch_map_accept(int init, const float* xht, const float* x, const float* w, double beta, float* xh, double* e, double* lam,
                       float* u, const float* ut, const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st);
+// the robust fit (ian_robust_gauss_newton_* / ian_fit_latent_robust_*): launch_map_gram and launch_map_accept with
+// omega = w rho'(r^2) as the pixel weight and E = sum w rho(r^2) + beta |u|^2, kind kRobustHuber or kRobustCauchy (the
+// header's IAN_ROBUST_*), dl the per-sample scale delta (robust_gram: the one sample's).  The automatic scale is
+// max(m c, kRobustScaleFloor) with m the lower median of float32 |r| over the weighted pixels and c the loss's 95 %-efficiency
+// constant times 1.4826 (the MAD's Gaussian consistency); the floor is half an 8-bit level on [-1, 1].
+constexpr int kRobustHuber = 1, kRobustCauchy = 2;
+constexpr double kRobustHuberC = 1.345 * 1.4826, kRobustCauchyC = 2.3849 * 1.4826, kRobustScaleFloor = 1.0 / 255.0;
+int launch_robust_gram(const float* J, const float* xh, const float* x, const float* w, int kind, const double* dl, double beta,
+                       const float* u, double* part, double* A, double* g, cudaStream_t st);
+int launch_robust_accept(int init, const float* xht, const float* x, const float* w, double beta, int kind, const double* dl,
+                         float* xh, double* e, double* lam, float* u, const float* ut, const int* ok, float* loss, long long ldl,
+                         int col, int n, cudaStream_t st);
+// dl (n) from x_hat and x (n,12288), w (nullable)
+int launch_robust_scale(const float* xh, const float* x, const float* w, int kind, double* dl, int n, cudaStream_t st);
+// out (n,12288) = rho'(r^2) per element, 0 where w == 0
+int launch_robust_outliers(const float* xh, const float* x, const float* w, int kind, const double* dl, float* out, int n,
+                           cudaStream_t st);
 // the IAN's introspection features and the fit under its feature-wise loss (feat_kernels.cu; ian_introspect_*,
 // ian_feature_gauss_newton_*, ian_fit_latent_features_*): layer l = 0..3 is enc_conv{l+1}'s output a{l+1}, (32 >> l)^2
 // pixels of 128 << l channels, M_l elements per image

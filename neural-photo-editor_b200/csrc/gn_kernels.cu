@@ -14,6 +14,11 @@
 // map_gram_reduce adds beta I, beta u and beta |u|^2 after the chunk sums, and map_accept reduces
 // sum_p w_p (x_hat_p - x_p)^2 + beta |u|^2.  Pixels with w_p == 0 are staged or summed as nothing at all, so x there may
 // hold anything, NaN included.  The unweighted kernels instantiate the bodies without a weight.
+// The robust fit (ian_robust_gauss_newton_*, ian_fit_latent_robust_*; DESIGN section 5.6m) is iteratively reweighted least
+// squares on E(u) = sum_p w_p rho(r_p^2) + beta |u|^2 with a per-sample scale delta (Huber or Cauchy rho): robust_gram runs
+// gram_body with omega_p = w_p rho'(d^2) in place of w_p (then map_gram_reduce), robust_accept reduces the true E, and
+// robust_scale picks delta from the lower median of |r| over the weighted pixels.  Where rho'(s) = 1 (Huber's quadratic
+// region) omega_p is w_p itself, so Huber with delta = +inf stages map_gram's operands and sums map_accept's terms.
 #include "edge.h"
 
 namespace ian {
@@ -29,6 +34,19 @@ constexpr int kChunks = 16;             // pixel chunks per sample: kPairs x kCh
 constexpr int kChunkPix = kPix / kChunks;
 constexpr int kSub = 64;                // pixels staged in shared memory per step
 constexpr int kLd = kLat + 1;           // row stride of the solver's matrix in shared memory
+
+// rho'(s) and rho(s) of the robust losses at s = d^2 (kind: IAN_ROBUST_HUBER / IAN_ROBUST_CAUCHY, dl the scale delta)
+__device__ __forceinline__ double robust_dw(int kind, double dl, double s) {
+  if (kind == kRobustHuber) return s <= dl * dl ? 1.0 : dl / sqrt(s);
+  return 1.0 / (1.0 + s / (dl * dl));
+}
+
+// s + wp rho(d^2), with Huber's quadratic region summed exactly as map_accept sums every pixel
+__device__ __forceinline__ double robust_add(int kind, double dl, double wp, double d, double s) {
+  const double q = d * d, d2 = dl * dl;
+  if (kind == kRobustHuber) return q <= d2 ? fma(wp * d, d, s) : fma(wp, 2.0 * dl * fabs(d) - d2, s);
+  return fma(wp, d2 * log1p(q / d2), s);
+}
 
 __device__ __forceinline__ double gram_row(const float* __restrict__ J, const float* __restrict__ xh,
                                            const float* __restrict__ x, int row, int p) {
@@ -46,9 +64,12 @@ __global__ void __launch_bounds__(256) gn_replicate_kernel(const float* __restri
 
 // grid (kPairs, kChunks), 256 threads, each a 2 x 2 tile of the 32 x 32 output block; part[chunk][pair][32][32].
 // kMap: w (nullable: all ones) multiplies the first factor of every product; a pixel with w == 0 stages zeros in both.
-template <bool kMap>
+// kRobust: omega = w rho'(d^2) at the sample's scale *dl does, in its place; omega == 0 stages zeros.  Thread t stages only
+// pixel p0 + t % kSub (256 is a multiple of kSub), so it forms that pixel's omega once per step.
+template <bool kMap, bool kRobust = false>
 __device__ __forceinline__ void gram_body(const float* __restrict__ J, const float* __restrict__ xh,
-                                          const float* __restrict__ x, const float* __restrict__ w, double* __restrict__ part) {
+                                          const float* __restrict__ x, const float* __restrict__ w, double* __restrict__ part,
+                                          int kind = 0, const double* __restrict__ dl = nullptr) {
   pdl_trigger();
   pdl_wait();
   __shared__ double sa[kSub][kBlk + 1], sb[kSub][kBlk + 1];
@@ -58,9 +79,18 @@ __device__ __forceinline__ void gram_body(const float* __restrict__ J, const flo
   const int ti = (t >> 4) * 2, tj = (t & 15) * 2;
   double acc00 = 0.0, acc01 = 0.0, acc10 = 0.0, acc11 = 0.0;
   for (int p0 = chunk * kChunkPix; p0 < (chunk + 1) * kChunkPix; p0 += kSub) {
+    double om = 0.0;
+    if constexpr (kRobust) {
+      const int p = p0 + t % kSub;
+      const double wp = w ? (double)w[p] : 1.0, d = (double)xh[p] - (double)x[p];
+      om = wp == 0.0 ? 0.0 : wp * robust_dw(kind, *dl, d * d);
+    }
     for (int e = t; e < kBlk * kSub; e += 256) {
       const int r = e / kSub, p = e % kSub;
-      if (kMap && w) {
+      if (kRobust) {
+        sa[p][r] = om == 0.0 ? 0.0 : om * gram_row(J, xh, x, bi * kBlk + r, p0 + p);
+        sb[p][r] = om == 0.0 ? 0.0 : gram_row(J, xh, x, bj * kBlk + r, p0 + p);
+      } else if (kMap && w) {
         const double wp = (double)w[p0 + p];
         sa[p][r] = wp == 0.0 ? 0.0 : wp * gram_row(J, xh, x, bi * kBlk + r, p0 + p);
         sb[p][r] = wp == 0.0 ? 0.0 : gram_row(J, xh, x, bj * kBlk + r, p0 + p);
@@ -96,6 +126,12 @@ __global__ void __launch_bounds__(256) map_gram_kernel(const float* __restrict__
                                                        const float* __restrict__ x, const float* __restrict__ w,
                                                        double* __restrict__ part) {
   gram_body<true>(J, xh, x, w, part);
+}
+
+__global__ void __launch_bounds__(256) robust_gram_kernel(const float* __restrict__ J, const float* __restrict__ xh,
+                                                          const float* __restrict__ x, const float* __restrict__ w, int kind,
+                                                          const double* __restrict__ dl, double* __restrict__ part) {
+  gram_body<true, true>(J, xh, x, w, part, kind, dl);
 }
 
 // beta |u|^2 of one sample's float32 u (100), in one fixed order
@@ -216,11 +252,13 @@ __global__ void __launch_bounds__(256) gn_solve_kernel(const double* __restrict_
 // Otherwise accept when the step was solved and e_trial < e: z <- z_trial, x_hat <- x_hat_trial, e <- e_trial,
 // lambda <- max(lambda / 10, min); else lambda <- min(10 lambda, max).  loss[k * ldl + col] = e / 12288 after the decision.
 // kMap: e_trial = sum over w != 0 of w (x_hat_trial - x)^2 (w nullable: all ones) + beta |z_trial|^2 (init: |z|^2).
-template <bool kMap>
+// kRobust: sum over w != 0 of w rho((x_hat_trial - x)^2) at the sample's scale dl[k] instead, in the same order.
+template <bool kMap, bool kRobust = false>
 __device__ __forceinline__ void accept_body(int init, const float* __restrict__ xht, const float* __restrict__ x,
                                             const float* __restrict__ w, double beta, float* xh, double* __restrict__ e,
                                             double* __restrict__ lam, float* __restrict__ z, const float* __restrict__ zt,
-                                            const int* __restrict__ ok, float* __restrict__ loss, long long ldl, int col) {
+                                            const int* __restrict__ ok, float* __restrict__ loss, long long ldl, int col,
+                                            int kind = 0, const double* __restrict__ dl = nullptr) {
   pdl_trigger();
   pdl_wait();
   __shared__ double red[256];
@@ -230,8 +268,13 @@ __device__ __forceinline__ void accept_body(int init, const float* __restrict__ 
   const float* b = x + (size_t)k * kPix;
   const float* wk = kMap && w ? w + (size_t)k * kPix : nullptr;
   double s = 0.0;
+  const double dk = kRobust ? dl[k] : 0.0;
   for (int p = t; p < kPix; p += 256) {
-    if (kMap && wk) {
+    if (kRobust) {
+      const double wp = wk ? (double)wk[p] : 1.0;
+      if (wp == 0.0) continue;
+      s = robust_add(kind, dk, wp, (double)a[p] - (double)b[p], s);
+    } else if (kMap && wk) {
       const double wp = (double)wk[p];
       if (wp == 0.0) continue;
       const double d = (double)a[p] - (double)b[p];
@@ -289,6 +332,81 @@ __global__ void __launch_bounds__(256) map_accept_kernel(int init, const float* 
   accept_body<true>(init, xht, x, w, beta, xh, e, lam, z, zt, ok, loss, ldl, col);
 }
 
+__global__ void __launch_bounds__(256) robust_accept_kernel(int init, const float* __restrict__ xht,
+                                                            const float* __restrict__ x, const float* __restrict__ w,
+                                                            double beta, int kind, const double* __restrict__ dl, float* xh,
+                                                            double* __restrict__ e, double* __restrict__ lam,
+                                                            float* __restrict__ z, const float* __restrict__ zt,
+                                                            const int* __restrict__ ok, float* __restrict__ loss,
+                                                            long long ldl, int col) {
+  accept_body<true, true>(init, xht, x, w, beta, xh, e, lam, z, zt, ok, loss, ldl, col, kind, dl);
+}
+
+// one CTA per sample: dl[k] = max(m c, kRobustScaleFloor), m the lower median (rank (count - 1) / 2) of float32 |x_hat - x|
+// over the pixels with w != 0, selected exactly on the bit patterns (monotone for non-negative floats) by four 8-bit radix
+// passes from the top byte; kRobustScaleFloor when no pixel is weighted.  The histograms count with shared-memory atomics,
+// whose totals do not depend on their order.
+__global__ void __launch_bounds__(256) robust_scale_kernel(const float* __restrict__ xh, const float* __restrict__ x,
+                                                           const float* __restrict__ w, double c, double* __restrict__ dl) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ unsigned hist[256];
+  __shared__ unsigned cnt, prefix, rank;
+  const int k = blockIdx.x, t = threadIdx.x;
+  const float* a = xh + (size_t)k * kPix;
+  const float* b = x + (size_t)k * kPix;
+  const float* wk = w ? w + (size_t)k * kPix : nullptr;
+  if (t == 0) cnt = prefix = 0;
+  __syncthreads();
+  unsigned mine = 0;
+  for (int p = t; p < kPix; p += 256) mine += !wk || wk[p] != 0.f;
+  atomicAdd(&cnt, mine);
+  __syncthreads();
+  if (cnt == 0) {
+    if (t == 0) dl[k] = kRobustScaleFloor;
+    return;
+  }
+  if (t == 0) rank = (cnt - 1) / 2;
+  unsigned mask = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    hist[t] = 0;
+    __syncthreads();
+    const unsigned pre = prefix;
+    for (int p = t; p < kPix; p += 256) {
+      if (wk && wk[p] == 0.f) continue;
+      const unsigned v = __float_as_uint(fabsf(a[p] - b[p]));
+      if ((v & mask) == pre) atomicAdd(&hist[(v >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (t == 0) {
+      unsigned below = 0, j = 0;
+      while (below + hist[j] <= rank) below += hist[j++];
+      rank -= below;
+      prefix = pre | (j << shift);
+    }
+    mask |= 255u << shift;
+    __syncthreads();
+  }
+  if (t == 0) dl[k] = fmax((double)__uint_as_float(prefix) * c, kRobustScaleFloor);
+}
+
+// out (n,12288) = rho'((x_hat - x)^2) at the sample's scale dl[k] as float32, 0 where w == 0
+__global__ void __launch_bounds__(256) robust_outliers_kernel(const float* __restrict__ xh, const float* __restrict__ x,
+                                                              const float* __restrict__ w, int kind,
+                                                              const double* __restrict__ dl, float* __restrict__ out,
+                                                              long long total) {
+  pdl_trigger();
+  pdl_wait();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  if (w && w[i] == 0.f) {
+    out[i] = 0.f;
+    return;
+  }
+  const double d = (double)xh[i] - (double)x[i];
+  out[i] = (float)robust_dw(kind, dl[i / kPix], d * d);
+}
+
 constexpr size_t kSolveSmem = (size_t)kLat * kLd * sizeof(double);
 
 }  // namespace
@@ -318,6 +436,31 @@ int launch_map_gram(const float* J, const float* xh, const float* x, const float
   return 2;
 }
 
+int launch_robust_gram(const float* J, const float* xh, const float* x, const float* w, int kind, const double* dl, double beta,
+                       const float* u, double* part, double* A, double* g, cudaStream_t st) {
+  if (launch_pdl(robust_gram_kernel, dim3(kPairs, kChunks), dim3(256), 0, st, J, xh, x, w, kind, dl, part) != cudaSuccess)
+    return -1;
+  if (launch_pdl(map_gram_reduce_kernel, dim3(((kLat + 1) * (kLat + 1) + 255) / 256), dim3(256), 0, st, (const double*)part,
+                 beta, u, A, g, (double*)nullptr) != cudaSuccess)
+    return -1;
+  return 2;
+}
+
+int launch_robust_scale(const float* xh, const float* x, const float* w, int kind, double* dl, int n, cudaStream_t st) {
+  const double c = kind == kRobustHuber ? kRobustHuberC : kRobustCauchyC;
+  if (launch_pdl(robust_scale_kernel, dim3(n), dim3(256), 0, st, xh, x, w, c, dl) != cudaSuccess) return -1;
+  return 1;
+}
+
+int launch_robust_outliers(const float* xh, const float* x, const float* w, int kind, const double* dl, float* out, int n,
+                           cudaStream_t st) {
+  const long long total = (long long)n * kPix;
+  if (launch_pdl(robust_outliers_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, st, xh, x, w, kind, dl, out,
+                 total) != cudaSuccess)
+    return -1;
+  return 1;
+}
+
 int launch_gn_solve(const double* A, const double* g, const double* lam, const float* z, float* zt, int* ok, int n,
                     cudaStream_t st) {
   static DeviceOnce attr_set;
@@ -342,6 +485,15 @@ int launch_map_accept(int init, const float* xht, const float* x, const float* w
                       float* u, const float* ut, const int* ok, float* loss, long long ldl, int col, int n, cudaStream_t st) {
   if (launch_pdl(map_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, w, beta, xh, e, lam, u, ut, ok, loss, ldl, col) !=
       cudaSuccess)
+    return -1;
+  return 1;
+}
+
+int launch_robust_accept(int init, const float* xht, const float* x, const float* w, double beta, int kind, const double* dl,
+                         float* xh, double* e, double* lam, float* u, const float* ut, const int* ok, float* loss, long long ldl,
+                         int col, int n, cudaStream_t st) {
+  if (launch_pdl(robust_accept_kernel, dim3(n), dim3(256), 0, st, init, xht, x, w, beta, kind, dl, xh, e, lam, u, ut, ok, loss,
+                 ldl, col) != cudaSuccess)
     return -1;
   return 1;
 }

@@ -172,6 +172,8 @@ enum LayerId {
   T_FEAT_GRAM, T_FEAT_ACCEPT,                           // the feature fit's Gram over the four feature layers (with its
                                                         // reduction) and its trial reduction and accept rule
   T_FEAT_COTANGENT,                                     // the features' VJP: the cotangents' conversion to split planes
+  T_ROBUST_GRAM, T_ROBUST_SCALE,                        // the robust fit's reweighted Gram (with its reduction and the
+                                                        // prior) and its automatic per-sample scale
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -191,7 +193,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
                                     "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
-                                    "feat_gram", "feat_accept", "feat_cotangent"};
+                                    "feat_gram", "feat_accept", "feat_cotangent",
+                                    "robust_gram", "robust_scale"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -381,6 +384,9 @@ struct Plan {
   float *fxh = nullptr, *fxt = nullptr, *fzt = nullptr, *floss = nullptr;
   int* fok = nullptr;
   long long floss_cap = 0;
+  // robust fit (allocated on the plan's first ian_robust_gauss_newton_* / ian_fit_latent_robust_* call): the per-sample
+  // scale when the caller passes none and asks for none back, and the host form's staging of scale and scale_out
+  double* rdl = nullptr;
   // feature fit (allocated on the plan's first ian_feature_gauss_newton_* / ian_fit_latent_features_* call): the target's
   // features g(x) and the current ones g(x_hat), float32 NHWC, layer l's n samples at n * kFeatOff[l] (1.97 MB per image)
   bool feat = false;
@@ -2028,7 +2034,7 @@ int run_encode_jvp(ian_handle* h, Plan* pl, const float* x, const float* v, cons
 //   device form (ian_*_dev): the body on the caller's pointers, offset by the chunk, on the caller's stream;
 //   host form (ian_*_host): per chunk, the caller's inputs are copied into plan buffers, the body runs on those, its kernel
 //   chain (Chunk::graphed) replayed as a CUDA graph on small plans, the outputs are copied back; then one synchronise.
-enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ, S_GN_A, S_GN_G, S_GN_E, S_F1, S_T1 = S_F1 + 4 };
+enum StageBuf { S_X, S_EPS, S_Z, S_XHAT, S_BOXES, S_TARGET, S_EDZ, S_GN_A, S_GN_G, S_GN_E, S_SCALE, S_F1, S_T1 = S_F1 + 4 };
 constexpr long long kFeatOff[4] = {0, 131072, 196608, 229376};   // layer l's offset in a sample's 245760 features
 void* stage_buf(Plan* pl, int s) {
   if (s >= S_F1) return pl->ifeat + (long long)pl->n * ((s >= S_T1 ? kFeatTotal : 0) + kFeatOff[(s - S_F1) % 4]);
@@ -2042,6 +2048,7 @@ void* stage_buf(Plan* pl, int s) {
     case S_GN_A: return pl->gnA;
     case S_GN_G: return pl->gng;
     case S_GN_E: return pl->gne;
+    case S_SCALE: return pl->rdl;
     default: return pl->edz;
   }
 }
@@ -2537,9 +2544,18 @@ int run_map_decode(ian_handle* h, Plan* pl, const float* u, float* xh, cudaStrea
   return run_decode_from_planes(h, pl, xh, st);
 }
 
-// A (n,100,100), g (n,100) and e (n, nullable) of n samples at u, with x_hat = decode(F(u)) already in xh; w nullable
+// The robust fit's loss (DESIGN section 5.6m): kind IAN_ROBUST_HUBER / IAN_ROBUST_CAUCHY and the per-sample scale dl (n),
+// the caller's or, when automatic, written by robust_scale from the start's x_hat before anything reads it.
+struct RobustLoss {
+  int kind;
+  double* dl;
+  bool automatic;
+};
+
+// A (n,100,100), g (n,100) and e (n, nullable) of n samples at u, with x_hat = decode(F(u)) already in xh; w nullable.
+// rl (nullable): the robust fit's A and g, reweighted by rho' at rl's scale (e is then not written: its Gram corner is not E)
 int run_map_normal_eqs(ian_handle* h, int n, const float* u, const float* x, const float* w, double beta, const float* xh,
-                       double* A, double* g, double* e, cudaStream_t st) {
+                       double* A, double* g, double* e, cudaStream_t st, const RobustLoss* rl = nullptr) {
   Plan* jp = nullptr;
   int rc = get_plan(h, 100, &jp);
   if (rc != IAN_OK) return rc;
@@ -2554,6 +2570,12 @@ int run_map_normal_eqs(ian_handle* h, int n, const float* u, const float* x, con
       LAUNCH_TRY(h, launch_made_iaf_tangent(h->gn_zrep, h->gn_eye, h->made_w, h->made_b, h->map_flow + 10000, 100, st));
     }
     if ((rc = run_decode_jvp(h, jp, zr, tan, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+    if (rl) {
+      ScopedTimer tm(h, T_ROBUST_GRAM, st);
+      LAUNCH_TRY(h, launch_robust_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, w ? w + (size_t)k * 12288 : nullptr,
+                                       rl->kind, rl->dl + k, beta, uk, h->gn_part, A + (size_t)k * 10000, g + (size_t)k * 100, st));
+      continue;
+    }
     ScopedTimer tm(h, T_MAP_GRAM, st);
     LAUNCH_TRY(h, launch_map_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, w ? w + (size_t)k * 12288 : nullptr,
                                   beta, uk, h->gn_part, A + (size_t)k * 10000, g + (size_t)k * 100, e ? e + k : nullptr, st));
@@ -2561,23 +2583,42 @@ int run_map_normal_eqs(ian_handle* h, int n, const float* u, const float* x, con
   return IAN_OK;
 }
 
-// run_fit on E(u) = sum_p w_p r_p^2 + beta |u|^2: the same solve and rule, trial steps decoded from F(u_trial)
+// map_accept, or with rl robust_accept: the fit's objective at x_hat_trial and its accept rule (n samples)
+int launch_fit_accept(const RobustLoss* rl, int init, const float* xht, const float* x, const float* w, double beta, float* xh,
+                      double* e, double* lam, float* u, const float* ut, const int* ok, float* loss, long long ldl, int col,
+                      int n, cudaStream_t st) {
+  if (rl) return launch_robust_accept(init, xht, x, w, beta, rl->kind, rl->dl, xh, e, lam, u, ut, ok, loss, ldl, col, n, st);
+  return launch_map_accept(init, xht, x, w, beta, xh, e, lam, u, ut, ok, loss, ldl, col, n, st);
+}
+
+// rl's automatic scale (if it is) from x_hat and x of n samples
+int run_robust_scale(ian_handle* h, const RobustLoss* rl, const float* xh, const float* x, const float* w, int n,
+                     cudaStream_t st) {
+  if (!rl || !rl->automatic) return IAN_OK;
+  ScopedTimer tm(h, T_ROBUST_SCALE, st);
+  LAUNCH_TRY(h, launch_robust_scale(xh, x, w, rl->kind, rl->dl, n, st));
+  return IAN_OK;
+}
+
+// run_fit on E(u) = sum_p w_p r_p^2 + beta |u|^2: the same solve and rule, trial steps decoded from F(u_trial).
+// rl (nullable): on the robust E(u) = sum_p w_p rho(r_p^2) + beta |u|^2 instead, the scale taken at the start when automatic
 int run_fit_map(ian_handle* h, Plan* pl, const float* x, const float* w, double beta, float* u, int iters, float* loss,
-                cudaStream_t st) {
+                cudaStream_t st, const RobustLoss* rl = nullptr) {
   const int n = pl->n;
   const long long ldl = (long long)iters + 1;
   int rc;
   if ((rc = run_map_decode(h, pl, u, pl->fxh, st)) != IAN_OK) return rc;
-  LAUNCH_TRY(h, launch_map_accept(1, pl->fxh, x, w, beta, pl->fxh, pl->fe, pl->flam, u, nullptr, nullptr, loss, ldl, 0, n, st));
+  if ((rc = run_robust_scale(h, rl, pl->fxh, x, w, n, st)) != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_fit_accept(rl, 1, pl->fxh, x, w, beta, pl->fxh, pl->fe, pl->flam, u, nullptr, nullptr, loss, ldl, 0, n, st));
   for (int it = 0; it < iters; ++it) {
-    if ((rc = run_map_normal_eqs(h, n, u, x, w, beta, pl->fxh, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
+    if ((rc = run_map_normal_eqs(h, n, u, x, w, beta, pl->fxh, pl->gnA, pl->gng, pl->gne, st, rl)) != IAN_OK) return rc;
     {
       ScopedTimer tm(h, T_GN_SOLVE, st);
       LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, u, pl->fzt, pl->fok, n, st));
     }
     if ((rc = run_map_decode(h, pl, pl->fzt, pl->fxt, st)) != IAN_OK) return rc;
-    LAUNCH_TRY(h, launch_map_accept(0, pl->fxt, x, w, beta, pl->fxh, pl->fe, pl->flam, u, pl->fzt, pl->fok, loss, ldl, it + 1, n,
-                                    st));
+    LAUNCH_TRY(h, launch_fit_accept(rl, 0, pl->fxt, x, w, beta, pl->fxh, pl->fe, pl->flam, u, pl->fzt, pl->fok, loss, ldl, it + 1,
+                                    n, st));
   }
   return IAN_OK;
 }
@@ -2632,6 +2673,101 @@ int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w
         CUDA_TRY(h, cudaMemcpyAsync(c.f(3), c.f(2), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
     }
     return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
+  });
+}
+
+// ---- robust latent fit: Huber / Cauchy pixel losses by reweighted Levenberg-Marquardt (DESIGN section 5.6m) -------------
+// The masked fit's passes, plan and rule with the Gram reweighted by rho' and the accept rule on the true robust E.
+static_assert(IAN_ROBUST_HUBER == kRobustHuber && IAN_ROBUST_CAUCHY == kRobustCauchy,
+              "the kernels compare the header's loss ids with edge.h's");
+int ensure_robust_plan(ian_handle* h, Plan* pl) {
+  int rc = ensure_map_plan(h, pl);
+  if (rc != IAN_OK || pl->rdl) return rc;
+  if ((rc = alloc_buf(h, pl, pl->rdl, pl->n)) != IAN_OK) return rc;
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return IAN_OK;
+}
+
+// kind, and (host form) every scale: > 0 and not NaN, +inf for Huber only
+int check_robust_args(ian_handle* h, bool host, int n, int kind, const double* scale) {
+  if (kind != IAN_ROBUST_HUBER && kind != IAN_ROBUST_CAUCHY) return fail(h, IAN_ERR_INVALID, "unknown robust loss kind %d", kind);
+  if (host && scale)
+    for (int k = 0; k < n; ++k)
+      if (!(scale[k] > 0.0) || (std::isinf(scale[k]) && kind == IAN_ROBUST_CAUCHY))
+        return fail(h, IAN_ERR_INVALID, "scale %d is %g: scales must be > 0, and finite for the Cauchy loss", k, scale[k]);
+  return IAN_OK;
+}
+
+// The chunk's loss: the caller's scale (Arg is), or automatic into scale_out (Arg io; the plan's when left out).  In the host
+// form both stage in the plan's scale buffer.
+RobustLoss robust_loss(const Chunk& c, int kind, int is, int io) {
+  double* s = (double*)c.p[is];
+  double* o = (double*)c.p[io];
+  return {kind, s ? s : o ? o : c.pl->rdl, !s};
+}
+
+// scale_out of a passed scale: a copy of it
+int robust_scale_out(const Chunk& c, const RobustLoss& rl, int io) {
+  double* o = (double*)c.p[io];
+  if (!rl.automatic && o && o != rl.dl)
+    CUDA_TRY(c.h, cudaMemcpyAsync(o, rl.dl, (size_t)c.cn * sizeof(double), cudaMemcpyDeviceToDevice, c.st));
+  return IAN_OK;
+}
+
+// As call_map_gauss_newton; e comes from robust_accept's reduction (the fit's init form), not from the Gram.
+int call_robust_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int kind,
+                             const double* scale, int n, double* A, double* g, double* e, double* scale_out, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if ((rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK || n == 0) return rc;
+  if (!u || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{u, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
+                                        {scale, 8, S_SCALE, IN}, {A, 80000, S_GN_A, OUT}, {g, 800, S_GN_G, OUT},
+                                        {e, 8, S_GN_E, OUT}, {scale_out, 8, S_SCALE, OUT}}, ensure_robust_plan,
+                   [&](const Chunk& c) {
+    Plan* pl = c.pl;
+    const RobustLoss rl = robust_loss(c, kind, 3, 7);
+    int r = run_map_decode(h, pl, c.f(0), pl->fxh, c.st);
+    if (r == IAN_OK) r = run_robust_scale(h, &rl, pl->fxh, c.f(1), c.f(2), c.cn, c.st);
+    if (r == IAN_OK)
+      r = run_map_normal_eqs(h, c.cn, c.f(0), c.f(1), c.f(2), prior, pl->fxh, (double*)c.p[4], (double*)c.p[5], nullptr, c.st, &rl);
+    if (r != IAN_OK) return r;
+    LAUNCH_TRY(h, launch_robust_accept(1, pl->fxh, c.f(1), c.f(2), prior, kind, rl.dl, pl->fxh, c.p[6] ? (double*)c.p[6] : pl->gne,
+                                       pl->flam, c.f(0), nullptr, nullptr, nullptr, 1, 0, c.cn, c.st));
+    return robust_scale_out(c, rl, 7);
+  });
+}
+
+// As call_fit_latent_map; the host form also stages outlier_w in the plan's x_hat buffer, which the fit does not use.
+int call_fit_latent_robust(ian_handle* h, bool host, const float* x, const float* w, double prior, int kind, const double* scale,
+                           int n, float* u, float* z_out, int iters, float* loss, double* scale_out, float* outlier_w,
+                           void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
+  if ((rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK || n == 0) return rc;
+  if (!x || !u) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
+  const size_t ldl = (size_t)iters + 1;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN}, {scale, 8, S_SCALE, IN},
+                                        {u, kLatentBytes, S_Z, INOUT}, {z_out, kLatentBytes, S_EPS, OUT},
+                                        {scale_out, 8, S_SCALE, OUT}, {outlier_w, kImageBytes, S_XHAT, OUT}},
+                   ensure_robust_plan, [&](const Chunk& c) {
+    const RobustLoss rl = robust_loss(c, kind, 2, 5);
+    float* l = nullptr;
+    int r = fit_loss_buf(c, loss, ldl, &l);
+    if (r == IAN_OK) r = run_fit_map(h, c.pl, c.f(0), c.f(1), prior, c.f(3), iters, l, c.st, &rl);
+    if (r != IAN_OK) return r;
+    if (outlier_w) LAUNCH_TRY(h, launch_robust_outliers(c.pl->fxh, c.f(0), c.f(1), kind, rl.dl, c.f(6), c.cn, c.st));
+    if (z_out) {
+      if (has_flow(h))
+        LAUNCH_TRY(h, launch_made_iaf(c.f(3), h->made_w, h->made_b, c.f(4), nullptr, 0, c.cn, c.st));
+      else
+        CUDA_TRY(h, cudaMemcpyAsync(c.f(4), c.f(3), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
+    }
+    if ((r = robust_scale_out(c, rl, 5)) != IAN_OK) return r;
+    return fit_loss_out(c, loss, ldl, l);
   });
 }
 
@@ -3289,6 +3425,23 @@ int ian_fit_latent_map_dev(ian_handle* h, const float* x, const float* w, double
 int ian_fit_latent_map_host(ian_handle* h, const float* x, const float* w, double prior, int n, float* u, float* z_out, int iters,
                             float* loss) {
   return call_fit_latent_map(h, true, x, w, prior, n, u, z_out, iters, loss, nullptr);
+}
+
+int ian_robust_gauss_newton_dev(ian_handle* h, const float* u, const float* x, const float* w, double prior, int kind,
+                                const double* scale, int n, double* A, double* g, double* e, double* scale_out, void* stream) {
+  return call_robust_gauss_newton(h, false, u, x, w, prior, kind, scale, n, A, g, e, scale_out, stream);
+}
+int ian_robust_gauss_newton_host(ian_handle* h, const float* u, const float* x, const float* w, double prior, int kind,
+                                 const double* scale, int n, double* A, double* g, double* e, double* scale_out) {
+  return call_robust_gauss_newton(h, true, u, x, w, prior, kind, scale, n, A, g, e, scale_out, nullptr);
+}
+int ian_fit_latent_robust_dev(ian_handle* h, const float* x, const float* w, double prior, int kind, const double* scale, int n,
+                              float* u, float* z_out, int iters, float* loss, double* scale_out, float* outlier_w, void* stream) {
+  return call_fit_latent_robust(h, false, x, w, prior, kind, scale, n, u, z_out, iters, loss, scale_out, outlier_w, stream);
+}
+int ian_fit_latent_robust_host(ian_handle* h, const float* x, const float* w, double prior, int kind, const double* scale, int n,
+                               float* u, float* z_out, int iters, float* loss, double* scale_out, float* outlier_w) {
+  return call_fit_latent_robust(h, true, x, w, prior, kind, scale, n, u, z_out, iters, loss, scale_out, outlier_w, nullptr);
 }
 
 int ian_introspect_dev(ian_handle* h, const float* x, int n, float* f1, float* f2, float* f3, float* f4, void* stream) {
