@@ -524,6 +524,35 @@ int ian_bn_train_normalize_dev(ian_handle* h, const float* x, int n, int c, int 
 int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const float* theta, const float* log_weight_scale,
                               const float* b, int num_kernels, int dim_per_kernel, float* out, void* stream);
 
+/* ---- reverse mode of the two training-mode ops (DESIGN §5.6b).  Same conventions as the forward calls: device pointers,
+ * float32 tensors, float64 sums, the handle's workspace and stream; bit-reproducible; what the forward rejects ->
+ * IAN_ERR_INVALID; n == 0 does nothing.  Gradients flow through the batch mean and variance (Theano's T.grad through
+ * lasagne's input.mean / input.var); the running-average update has none.
+ *   ian_bn_backward_sums_dev    this rank's per-channel Σdy and Σdy·x (float64 [c] each) over (n, hw): exact products,
+ *                               float64 from the first term, the forward's split order.  sum / sumsq / count / eps are the
+ *                               forward's (global after an all-reduce).  dgamma = Σ dy·x̂ = s (Σdy·x - mean Σdy), evaluated in
+ *                               float64, and dbeta = Σdy (nullable, float32 [c]) are this rank's: DDP reduces them itself.
+ *                               Data-parallel ranks all-reduce sum_dy / sum_dyx here.
+ *   ian_bn_backward_dx_dev      from the (global) backward sums, N = count, s = 1/sqrt(var + eps), x̂ = (x - mean) s:
+ *                               dx = gamma s (dy - Σdy/N - x̂ Σ(dy x̂)/N), per element in float64, one rounding.
+ *                               gamma NULL means 1 (its gradient is then not wanted either).
+ * ian_minibatch_discrim_bwd_dev g = dL/d[x | f] (n, d+K) -> dx (n,d), dtheta (d,K,P), dlog_weight_scale (K,P), db (K), each
+ *                               nullable.  Recomputes A = x W; each pair i < j forms e_ijk = exp(-Σ_p|A_ikp - A_jkp|) once;
+ *                               dA_ikp = -Σ_{j≠i} (g_f[i,k] + g_f[j,k]) e_ijk sgn(A_ikp - A_jkp) with sgn(0) = 0; dx = g_x + dA Wᵀ,
+ *                               dW = xᵀ dA, then through W = theta exp(lws) / |theta[:,k,p]|.  FFMA, fixed-order chunked sums,
+ *                               no atomics.  b is the forward's (no gradient depends on it).  Workspace: 4 (K P (2n + d) +
+ *                               K n (n-1)/2) bytes. */
+int ian_bn_backward_sums_dev(ian_handle* h, const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq,
+                             double count, float eps, double* sum_dy, double* sum_dyx, float* dgamma /*nullable*/,
+                             float* dbeta /*nullable*/, void* stream);
+int ian_bn_backward_dx_dev(ian_handle* h, const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq,
+                           double count, const double* sum_dy, const double* sum_dyx, const float* gamma /*nullable*/, float eps,
+                           float* dx, void* stream);
+int ian_minibatch_discrim_bwd_dev(ian_handle* h, const float* x, int n, int d, const float* theta, const float* log_weight_scale,
+                                  const float* b, int num_kernels, int dim_per_kernel, const float* g, float* dx /*nullable*/,
+                                  float* dtheta /*nullable*/, float* dlog_weight_scale /*nullable*/, float* db /*nullable*/,
+                                  void* stream);
+
 /* ---- measurement helpers ----------------------------------------------------------------------- */
 /* Average device time (ms, CUDA events on the launch stream) of the tap-GEMM kernel of layer
  * `layer_name` ("enc_conv2", "dec_conv1", ...; the encoder VJP's "bwd_enc_head", "bwd_enc_fc1", "bwd_enc_conv4",

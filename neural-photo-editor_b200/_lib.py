@@ -119,6 +119,12 @@ SIGNATURES = {
                                              C.c_void_p]),
     "ian_minibatch_discrim_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                             C.c_void_p, C.c_void_p]),
+    "ian_bn_backward_sums_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_double, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_bn_backward_dx_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                         C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
+    "ian_minibatch_discrim_bwd_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_set_layer_timing": (C.c_int, [_H, C.c_int]),
     "ian_layer_time_ms": (C.c_double, [_H, C.c_char_p, C.c_int]),
 }

@@ -203,6 +203,14 @@ int launch_bn_train_normalize(const float* x, int n, int c, int hw, const double
 size_t mb_workspace_bytes(int n, int K, int P);
 int launch_minibatch_discrim(const float* x, int n, int d, const float* theta, const float* lws, const float* b, int K, int P,
                              float* out, void* ws, cudaStream_t st);
+// their reverse mode: BatchNorm backward sums (+ local dgamma / dbeta) and dx; MinibatchLayer dx, dtheta, dlws, db
+int launch_bn_backward_sums(const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq, double count,
+                            float eps, double* sum_dy, double* sum_dyx, float* dgamma, float* dbeta, void* ws, cudaStream_t st);
+int launch_bn_backward_dx(const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq, double count,
+                          const double* sum_dy, const double* sum_dyx, const float* gamma, float eps, float* dx, void* ws, cudaStream_t st);
+size_t mb_bwd_workspace_bytes(int n, int d, int K, int P);
+int launch_minibatch_discrim_bwd(const float* x, int n, int d, const float* theta, const float* lws, int K, int P, const float* g,
+                                 float* dx, float* dtheta, float* dlws, float* db, void* ws, cudaStream_t st);
 // pipelined all-gather: copy this rank's decoded shard (src, n_floats) into every peer's gather buffer from a small
 // side-stream kernel + free/pushed flag handshake (see decout_tc.cu); returns after enqueueing push + wait kernels
 int launch_peer_push(const float* src, float* const* dsts, float* const* flag_ptrs, long long n_floats, int world, int rank,

@@ -3825,6 +3825,50 @@ int ian_minibatch_discrim_dev(ian_handle* h, const float* x, int n, int d, const
   return IAN_OK;
 }
 
+int ian_bn_backward_sums_dev(ian_handle* h, const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq,
+                             double count, float eps, double* sum_dy, double* sum_dyx, float* dgamma, float* dbeta, void* stream) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!x || !dy || !sum || !sumsq || !sum_dy || !sum_dyx || n < 0 || c < 1 || hw < 1 || !(count >= 1.0))
+    return fail(h, IAN_ERR_INVALID, "bad argument (n=%d c=%d hw=%d count=%g)", n, c, hw, count);
+  if (n == 0) return IAN_OK;
+  DeviceGuard dg(h->device);
+  int rc = ensure_train_ws(h, bn_workspace_bytes(c));
+  if (rc != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_bn_backward_sums(x, dy, n, c, hw, sum, sumsq, count, eps, sum_dy, sum_dyx, dgamma, dbeta, h->train_ws,
+                                        stream ? (cudaStream_t)stream : h->stream));
+  return IAN_OK;
+}
+
+int ian_bn_backward_dx_dev(ian_handle* h, const float* x, const float* dy, int n, int c, int hw, const double* sum, const double* sumsq,
+                           double count, const double* sum_dy, const double* sum_dyx, const float* gamma, float eps, float* dx,
+                           void* stream) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!x || !dy || !dx || !sum || !sumsq || !sum_dy || !sum_dyx || n < 0 || c < 1 || hw < 1 || !(count >= 1.0))
+    return fail(h, IAN_ERR_INVALID, "bad argument (n=%d c=%d hw=%d count=%g)", n, c, hw, count);
+  if (n == 0) return IAN_OK;
+  DeviceGuard dg(h->device);
+  int rc = ensure_train_ws(h, bn_workspace_bytes(c));
+  if (rc != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_bn_backward_dx(x, dy, n, c, hw, sum, sumsq, count, sum_dy, sum_dyx, gamma, eps, dx, h->train_ws,
+                                      stream ? (cudaStream_t)stream : h->stream));
+  return IAN_OK;
+}
+
+int ian_minibatch_discrim_bwd_dev(ian_handle* h, const float* x, int n, int d, const float* theta, const float* log_weight_scale,
+                                  const float* b, int num_kernels, int dim_per_kernel, const float* g, float* dx, float* dtheta,
+                                  float* dlog_weight_scale, float* db, void* stream) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!x || !theta || !log_weight_scale || !b || !g || n < 0 || d < 1 || num_kernels < 1 || dim_per_kernel < 1)
+    return fail(h, IAN_ERR_INVALID, "bad argument");
+  if (n == 0) return IAN_OK;
+  DeviceGuard dg(h->device);
+  int rc = ensure_train_ws(h, mb_bwd_workspace_bytes(n, d, num_kernels, dim_per_kernel));
+  if (rc != IAN_OK) return rc;
+  LAUNCH_TRY(h, launch_minibatch_discrim_bwd(x, n, d, theta, log_weight_scale, num_kernels, dim_per_kernel, g, dx, dtheta,
+                                             dlog_weight_scale, db, h->train_ws, stream ? (cudaStream_t)stream : h->stream));
+  return IAN_OK;
+}
+
 // ---- one NPE paint stroke in one call (reference NPE.py:192-235, photo mode) ---------------------------------
 int ian_paint_stroke_host(ian_handle* h, float* z, const int32_t* box, const float* rgb_frame, float weight,
                           const uint8_t* recon_u8, const float* error, uint8_t* im_u8, uint8_t* display_u8) {
