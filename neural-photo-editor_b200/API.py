@@ -94,6 +94,10 @@ def _fp(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
 
+def _dp(a):
+    return a.ctypes.data_as(C.POINTER(C.c_double)) if a is not None else None
+
+
 def _z(a, what='z'):
     """latents: float32 (n,100).  The C side assumes the trailing dimension; theano would raise a shape error."""
     a = _f32(a, 2, what)
@@ -458,16 +462,9 @@ class IAN:
         sample_at.  Costs one batch-100 decode_jvp per sample."""
         z = _z(z)
         x = _img(images)
-        n = z.shape[0]
-        if x.shape[0] != n:
-            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
-        A = np.empty((n, 100, 100), np.float64)
-        g = np.empty((n, 100), np.float64)
-        e = np.empty((n,), np.float64)
+        n, A, g, e = self._normal_eqs(z, x)
         if n:
-            d = C.POINTER(C.c_double)
-            self._check(self._lib.ian_decode_gauss_newton_host(self._h, _fp(z), _fp(x), n, A.ctypes.data_as(d),
-                                                               g.ctypes.data_as(d), e.ctypes.data_as(d)))
+            self._check(self._lib.ian_decode_gauss_newton_host(self._h, _fp(z), _fp(x), n, _dp(A), _dp(g), _dp(e)))
         return A, g, e
 
     def fit_latent(self, images, z0=None, iters=10, return_loss=False):
@@ -477,16 +474,31 @@ class IAN:
         (n, iters+1), non-increasing.  z is l_Z, as for sample_at (on IAN.py / IANv1.py after the MADE/IAF flow)."""
         x = _img(images)
         n = x.shape[0]
-        iters = _int_scalar(iters, 'iters')
-        if iters < 0:
-            raise ValueError("iters must not be negative (got %d)" % iters)
-        z = self.encode_images(x) if z0 is None else _z(z0, 'z0').copy()
-        if z.shape[0] != n:
-            raise ValueError("z0 must be (%d,100), got %r" % (n, z.shape))
-        loss = np.empty((n, iters + 1), np.float32)
+        iters, z, loss = self._fit_start(iters, z0, 'z0', n, lambda: self.encode_images(x))
         if n:
             self._check(self._lib.ian_fit_latent_host(self._h, _fp(x), n, _fp(z), iters, _fp(loss)))
         return (z, loss) if return_loss else z
+
+    @staticmethod
+    def _normal_eqs(u, x):
+        """n and the float64 outputs A (n,100,100), g (n,100), e (n,) of the normal equations at u's n points for the
+        images x, once their batch sizes agree"""
+        n = u.shape[0]
+        if x.shape[0] != n:
+            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        return n, np.empty((n, 100, 100), np.float64), np.empty((n, 100), np.float64), np.empty((n,), np.float64)
+
+    @staticmethod
+    def _fit_start(iters, start, name, n, default):
+        """iters checked, the fit's start (a copy of `start`, default() when None) checked against the n images, and the
+        (n, iters+1) float32 loss history"""
+        iters = _int_scalar(iters, 'iters')
+        if iters < 0:
+            raise ValueError("iters must not be negative (got %d)" % iters)
+        u = default() if start is None else _z(start, name).copy()
+        if u.shape[0] != n:
+            raise ValueError("%s must be (%d,100), got %r" % (name, n, u.shape))
+        return iters, u, np.empty((n, iters + 1), np.float32)
 
     def _map_args(self, images, weights, prior):
         x = _img(images)
@@ -506,16 +518,10 @@ class IAN:
         A = J_u^T W J_u + beta I, g = J_u^T W r + beta u and e = r^T W r + beta |u|^2."""
         u = _z(u, 'u')
         x, w, prior = self._map_args(images, weights, prior)
-        n = u.shape[0]
-        if x.shape[0] != n:
-            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
-        A = np.empty((n, 100, 100), np.float64)
-        g = np.empty((n, 100), np.float64)
-        e = np.empty((n,), np.float64)
+        n, A, g, e = self._normal_eqs(u, x)
         if n:
-            d = C.POINTER(C.c_double)
             self._check(self._lib.ian_map_gauss_newton_host(self._h, _fp(u), _fp(x), _fp(w) if w is not None else None, prior,
-                                                            n, A.ctypes.data_as(d), g.ctypes.data_as(d), e.ctypes.data_as(d)))
+                                                            n, _dp(A), _dp(g), _dp(e)))
         return A, g, e
 
     def fit_latent_map(self, images, weights=None, prior=0.0, u0=None, iters=10, return_loss=False):
@@ -528,17 +534,9 @@ class IAN:
         non-increasing."""
         x, w, prior = self._map_args(images, weights, prior)
         n = x.shape[0]
-        iters = _int_scalar(iters, 'iters')
-        if iters < 0:
-            raise ValueError("iters must not be negative (got %d)" % iters)
-        if u0 is None:
-            u = self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x))
-        else:
-            u = _z(u0, 'u0').copy()
-        if u.shape[0] != n:
-            raise ValueError("u0 must be (%d,100), got %r" % (n, u.shape))
+        iters, u, loss = self._fit_start(iters, u0, 'u0', n,
+                                          lambda: self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x)))
         z = np.empty((n, 100), np.float32)
-        loss = np.empty((n, iters + 1), np.float32)
         if n:
             self._check(self._lib.ian_fit_latent_map_host(self._h, _fp(x), _fp(w) if w is not None else None, prior, n, _fp(u),
                                                           _fp(z), iters, _fp(loss)))
@@ -560,20 +558,12 @@ class IAN:
         e = sum w rho(r^2) + prior |u|^2 (include/ian_b200.h, ian_robust_gauss_newton_*)."""
         u = _z(u, 'u')
         x, w, prior = self._map_args(images, weights, prior)
-        n = u.shape[0]
-        if x.shape[0] != n:
-            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
+        n, A, g, e = self._normal_eqs(u, x)
         k, s = self._robust_args(kind, scale, n)
-        A = np.empty((n, 100, 100), np.float64)
-        g = np.empty((n, 100), np.float64)
-        e = np.empty((n,), np.float64)
         so = np.empty((n,), np.float64)
         if n:
-            d = C.POINTER(C.c_double)
-            self._check(self._lib.ian_robust_gauss_newton_host(
-                self._h, _fp(u), _fp(x), _fp(w) if w is not None else None, prior, k,
-                s.ctypes.data_as(d) if s is not None else None, n, A.ctypes.data_as(d), g.ctypes.data_as(d),
-                e.ctypes.data_as(d), so.ctypes.data_as(d)))
+            self._check(self._lib.ian_robust_gauss_newton_host(self._h, _fp(u), _fp(x), _fp(w) if w is not None else None,
+                                                               prior, k, _dp(s), n, _dp(A), _dp(g), _dp(e), _dp(so)))
         return A, g, e, so
 
     def fit_latent_robust(self, images, kind="huber", scale=None, weights=None, prior=0.0, u0=None, iters=10,
@@ -588,25 +578,16 @@ class IAN:
         outliers, 0 where the weight is 0."""
         x, w, prior = self._map_args(images, weights, prior)
         n = x.shape[0]
-        iters = _int_scalar(iters, 'iters')
-        if iters < 0:
-            raise ValueError("iters must not be negative (got %d)" % iters)
         k, s = self._robust_args(kind, scale, n)
-        if u0 is None:
-            u = self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x))
-        else:
-            u = _z(u0, 'u0').copy()
-        if u.shape[0] != n:
-            raise ValueError("u0 must be (%d,100), got %r" % (n, u.shape))
+        iters, u, loss = self._fit_start(iters, u0, 'u0', n,
+                                          lambda: self.Zfn(x if w is None else np.where(w == 0, np.float32(0), x)))
         z = np.empty((n, 100), np.float32)
         so = np.empty((n,), np.float64)
-        loss = np.empty((n, iters + 1), np.float32)
         out = np.empty((n, 3, 64, 64), np.float32) if return_outliers else None
         if n:
-            d = C.POINTER(C.c_double)
             self._check(self._lib.ian_fit_latent_robust_host(
-                self._h, _fp(x), _fp(w) if w is not None else None, prior, k, s.ctypes.data_as(d) if s is not None else None,
-                n, _fp(u), _fp(z), iters, _fp(loss), so.ctypes.data_as(d), _fp(out) if out is not None else None))
+                self._h, _fp(x), _fp(w) if w is not None else None, prior, k, _dp(s), n, _fp(u), _fp(z), iters, _fp(loss),
+                _dp(so), _fp(out) if out is not None else None))
         res = (u, z, so)
         if return_loss:
             res += (loss,)
@@ -695,16 +676,9 @@ class IAN:
         z = _z(z)
         x = _img(images)
         a, b = self._feature_weights(pixel_weight, feature_weight)
-        n = z.shape[0]
-        if x.shape[0] != n:
-            raise ValueError("images must be (%d,3,64,64), got %r" % (n, x.shape))
-        A = np.empty((n, 100, 100), np.float64)
-        g = np.empty((n, 100), np.float64)
-        e = np.empty((n,), np.float64)
+        n, A, g, e = self._normal_eqs(z, x)
         if n:
-            d = C.POINTER(C.c_double)
-            self._check(self._lib.ian_feature_gauss_newton_host(self._h, _fp(z), _fp(x), n, a, b, A.ctypes.data_as(d),
-                                                                g.ctypes.data_as(d), e.ctypes.data_as(d)))
+            self._check(self._lib.ian_feature_gauss_newton_host(self._h, _fp(z), _fp(x), n, a, b, _dp(A), _dp(g), _dp(e)))
         return A, g, e
 
     def fit_latent_features(self, images, z0=None, iters=10, pixel_weight=1.0, feature_weight=1.0, return_loss=False):
@@ -716,13 +690,7 @@ class IAN:
         x = _img(images)
         a, b = self._feature_weights(pixel_weight, feature_weight)
         n = x.shape[0]
-        iters = _int_scalar(iters, 'iters')
-        if iters < 0:
-            raise ValueError("iters must not be negative (got %d)" % iters)
-        z = self.encode_images(x) if z0 is None else _z(z0, 'z0').copy()
-        if z.shape[0] != n:
-            raise ValueError("z0 must be (%d,100), got %r" % (n, z.shape))
-        loss = np.empty((n, iters + 1), np.float32)
+        iters, z, loss = self._fit_start(iters, z0, 'z0', n, lambda: self.encode_images(x))
         if n:
             self._check(self._lib.ian_fit_latent_features_host(self._h, _fp(x), n, _fp(z), iters, a, b, _fp(loss)))
         return (z, loss) if return_loss else z

@@ -109,6 +109,28 @@ int launch_dec_out_jvp_tc(const DecOutMaps* maps, const float* xhat, float* dxha
 // lambda starts at 1e-3, is divided by 10 on an accepted step (not below 1e-7) and multiplied by 10 on a rejected one (not
 // above 1e10); the damping is lambda * diag(max(A_ii, 1e-9 * max_j A_jj)).
 constexpr double kGnLambda0 = 1e-3, kGnLambdaMin = 1e-7, kGnLambdaMax = 1e10, kGnLambdaFactor = 10.0, kGnDampFloor = 1e-9;
+// Thread 0 of sample k's accept CTA, with et the objective at the trial (init: at the start): init sets e and lambda;
+// otherwise the step is taken when it was solved (ok) and et < e, e <- et and lambda <- max(lambda / 10, min), else
+// lambda <- min(10 lambda, max).  loss[k * ldl + col] (nullable) = e / 12288 after the decision.  Returns whether the
+// step is taken; every accept kernel decides through this.
+__device__ __forceinline__ int gn_decide(int init, double et, const int* ok, double* e, double* lam, float* loss, long long ldl,
+                                         int col, int k) {
+  int take = 0;
+  if (init) {
+    e[k] = et;
+    lam[k] = kGnLambda0;
+  } else {
+    take = ok[k] && et < e[k];
+    if (take) {
+      e[k] = et;
+      lam[k] = fmax(lam[k] / kGnLambdaFactor, kGnLambdaMin);
+    } else {
+      lam[k] = fmin(lam[k] * kGnLambdaFactor, kGnLambdaMax);
+    }
+  }
+  if (loss) loss[(size_t)k * ldl + col] = (float)(e[k] / 12288.0);
+  return take;
+}
 size_t gn_part_doubles();                              // the Gram's chunk partials, per JVP pass
 // z (100) -> zrep (100,100), every row z
 int launch_gn_replicate(const float* z, float* zrep, cudaStream_t st);

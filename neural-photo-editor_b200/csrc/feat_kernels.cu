@@ -201,21 +201,7 @@ __global__ void __launch_bounds__(256) feat_accept_kernel(int init, const float*
   }
   if (t == 0) {
     const double et = c.a != 0.0 ? fma(c.a, red[0], redf[0]) : redf[0];
-    int take = 0;
-    if (init) {
-      e[k] = et;
-      lam[k] = kGnLambda0;
-    } else {
-      take = ok[k] && et < e[k];
-      if (take) {
-        e[k] = et;
-        lam[k] = fmax(lam[k] / kGnLambdaFactor, kGnLambdaMin);
-      } else {
-        lam[k] = fmin(lam[k] * kGnLambdaFactor, kGnLambdaMax);
-      }
-    }
-    if (loss) loss[(size_t)k * ldl + col] = (float)(e[k] / (double)kPix);
-    acc = take || init;
+    acc = gn_decide(init, et, ok, e, lam, loss, ldl, col, k) || init;
   }
   __syncthreads();
   if (!acc) return;

@@ -248,9 +248,8 @@ __global__ void __launch_bounds__(256) gn_solve_kernel(const double* __restrict_
   if (t == 0) ok[k] = good;
 }
 
-// one CTA per sample.  init: x_hat_trial is the start's decode (x_hat itself): e, lambda and loss column 0 are set.
-// Otherwise accept when the step was solved and e_trial < e: z <- z_trial, x_hat <- x_hat_trial, e <- e_trial,
-// lambda <- max(lambda / 10, min); else lambda <- min(10 lambda, max).  loss[k * ldl + col] = e / 12288 after the decision.
+// one CTA per sample.  init: x_hat_trial is the start's decode (x_hat itself).  e_trial, then gn_decide (edge.h); a taken
+// step also copies z <- z_trial, x_hat <- x_hat_trial.
 // kMap: e_trial = sum over w != 0 of w (x_hat_trial - x)^2 (w nullable: all ones) + beta |z_trial|^2 (init: |z|^2).
 // kRobust: sum over w != 0 of w rho((x_hat_trial - x)^2) at the sample's scale dl[k] instead, in the same order.
 template <bool kMap, bool kRobust = false>
@@ -293,21 +292,7 @@ __device__ __forceinline__ void accept_body(int init, const float* __restrict__ 
   if (t == 0) {
     double et = red[0];
     if (kMap) et = fma(beta, prior_sq((init ? z : zt) + (size_t)k * kLat), et);
-    int take = 0;
-    if (init) {
-      e[k] = et;
-      lam[k] = kGnLambda0;
-    } else {
-      take = ok[k] && et < e[k];
-      if (take) {
-        e[k] = et;
-        lam[k] = fmax(lam[k] / kGnLambdaFactor, kGnLambdaMin);
-      } else {
-        lam[k] = fmin(lam[k] * kGnLambdaFactor, kGnLambdaMax);
-      }
-    }
-    if (loss) loss[(size_t)k * ldl + col] = (float)(e[k] / (double)kPix);
-    acc = take;
+    acc = gn_decide(init, et, ok, e, lam, loss, ldl, col, k);
   }
   __syncthreads();
   if (!acc) return;

@@ -2265,15 +2265,22 @@ int call_encode_pre(ian_handle* h, bool host, const float* x, int n, float* z_ia
   });
 }
 
+// z = F(u) as ian_flow_* computes it, with made_iaf_kernel also writing zp when given; a copy of u on IAN_simple
+int flow_z(ian_handle* h, const float* u, float* z, Planes* zp, int n, cudaStream_t st) {
+  if (has_flow(h)) {
+    LAUNCH_TRY(h, launch_made_iaf(u, h->made_w, h->made_b, z, zp ? zp->p : nullptr, zp ? zp->plane : 0, n, st));
+    return IAN_OK;
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(z, u, (size_t)n * 400, cudaMemcpyDeviceToDevice, st));
+  return IAN_OK;
+}
+
 // l_Z_IAF -> l_Z (Z_IAF_fn) into z_out or the plan's z buffer, and the latent planes; x_out != NULL also decodes them
 // (`sample`).  The host form stages z_iaf in the plan's eps buffer; it decides on the caller's pointers, because it stages
 // every output whether asked for or not.
 int run_flow(ian_handle* h, Plan* pl, const float* z_iaf, float* z, cudaStream_t st) {
-  if (has_flow(h)) {
-    LAUNCH_TRY(h, launch_made_iaf(z_iaf, h->made_w, h->made_b, z, pl->zp.p, pl->zp.plane, pl->n, st));
-    return IAN_OK;
-  }
-  CUDA_TRY(h, cudaMemcpyAsync(z, z_iaf, (size_t)pl->n * 400, cudaMemcpyDeviceToDevice, st));
+  const int rc = flow_z(h, z_iaf, z, &pl->zp, pl->n, st);
+  if (rc != IAN_OK || has_flow(h)) return rc;
   LAUNCH_TRY(h, launch_z_to_planes(z, pl->zp.p, pl->zp.plane, pl->n, st));
   return IAN_OK;
 }
@@ -2422,64 +2429,14 @@ int ensure_gn_plan(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
-// A (n,100,100), g (n,100) and e (n, nullable) of n samples at z, with x_hat = decode(z) already in xh
-int run_normal_eqs(ian_handle* h, int n, const float* z, const float* x, const float* xh, double* A, double* g, double* e,
-                   cudaStream_t st) {
-  Plan* jp = nullptr;
-  int rc = get_plan(h, 100, &jp);
-  if (rc != IAN_OK) return rc;
-  for (int k = 0; k < n; ++k) {
-    LAUNCH_TRY(h, launch_gn_replicate(z + (size_t)k * 100, h->gn_zrep, st));
-    if ((rc = run_decode_jvp(h, jp, h->gn_zrep, h->gn_eye, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
-    ScopedTimer tm(h, T_GN_GRAM, st);
-    LAUNCH_TRY(h, launch_gn_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, h->gn_part, A + (size_t)k * 10000,
-                                 g + (size_t)k * 100, e ? e + k : nullptr, st));
-  }
-  return IAN_OK;
-}
-
-// iters Levenberg-Marquardt steps in place on z (pl->n samples); loss (nullable) row k receives e / 12288 of the start and
-// after every step, row stride iters + 1.  The fit's e is only ever set from gn_accept_kernel's reduction, so the history
-// cannot increase.
-int run_fit(ian_handle* h, Plan* pl, const float* x, float* z, int iters, float* loss, cudaStream_t st) {
-  const int n = pl->n;
-  const long long ldl = (long long)iters + 1;
-  int rc;
-  if ((rc = run_decode(h, pl, z, pl->fxh, st)) != IAN_OK) return rc;
-  LAUNCH_TRY(h, launch_gn_accept(1, pl->fxh, x, pl->fxh, pl->fe, pl->flam, z, nullptr, nullptr, loss, ldl, 0, n, st));
-  for (int it = 0; it < iters; ++it) {
-    if ((rc = run_normal_eqs(h, n, z, x, pl->fxh, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
-    {
-      ScopedTimer tm(h, T_GN_SOLVE, st);
-      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, z, pl->fzt, pl->fok, n, st));
-    }
-    if ((rc = run_decode(h, pl, pl->fzt, pl->fxt, st)) != IAN_OK) return rc;
-    LAUNCH_TRY(h, launch_gn_accept(0, pl->fxt, x, pl->fxh, pl->fe, pl->flam, z, pl->fzt, pl->fok, loss, ldl, it + 1, n, st));
-  }
-  return IAN_OK;
-}
-
-int check_fit_args(ian_handle* h, int n) {
+// The first checks of the fit and introspection entries: the handle, n and iters (the fits).  The fits then check their
+// objective's own arguments (check_robust_args, check_feat_weights), then n == 0 and the rest (check_fit_inputs).
+int check_fit_args(ian_handle* h, int n, int iters = 0) {
   if (!h) return IAN_ERR_INVALID;
   if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
   if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
   return IAN_OK;
-}
-
-// No CUDA graphs: the JVP passes run on the 100-row plan, whose schedule (stream-K) a capture would change, so both forms
-// launch the same kernels.  The host form stages z in the plan's z buffer, x in its image buffer and A, g, e in the plan's
-// own normal-equation buffers.
-int call_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, int n, double* A, double* g, double* e,
-                      void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK || n == 0) return rc;
-  if (!z || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {A, 80000, S_GN_A, OUT},
-                                        {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_gn_plan, [&](const Chunk& c) {
-    const int r = run_decode(h, c.pl, c.f(0), c.pl->fxh, c.st);
-    return r != IAN_OK ? r : run_normal_eqs(h, c.cn, c.f(0), c.f(1), c.pl->fxh, (double*)c.p[2], (double*)c.p[3],
-                                            c.p[4] ? (double*)c.p[4] : c.pl->gne, c.st);
-  });
 }
 
 // The fit's loss history (nullable) of one chunk, row stride ldl: the caller's rows in the device form; in the host form a
@@ -2506,23 +2463,6 @@ int fit_loss_out(const Chunk& c, float* loss, size_t ldl, const float* l) {
   return IAN_OK;
 }
 
-// The host form stages x in the plan's image buffer and z in its z buffer.
-int call_fit_latent(ian_handle* h, bool host, const float* x, int n, float* z, int iters, float* loss, void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK) return rc;
-  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
-  if (n == 0) return IAN_OK;
-  if (!x || !z) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  const size_t ldl = (size_t)iters + 1;
-  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z, kLatentBytes, S_Z, INOUT}}, ensure_gn_plan,
-                   [&](const Chunk& c) {
-    float* l = nullptr;
-    int r = fit_loss_buf(c, loss, ldl, &l);
-    if (r == IAN_OK) r = run_fit(h, c.pl, c.f(0), c.f(1), iters, l, c.st);
-    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
-  });
-}
-
 // ---- masked latent fit under the prior: pixel-weighted Levenberg-Marquardt in the fit space u (DESIGN section 5.6j) -------
 // u is l_Z on IAN_simple and l_Z_IAF on IAN.py / IANv1.py, and z = F(u) the MADE/IAF flow (the identity on IAN_simple).
 // x_hat = decode(F(u)) on the caller's batch plan: made_iaf_kernel writes the latent planes as `sample` does, so x_hat has
@@ -2535,145 +2475,6 @@ int ensure_map_plan(ian_handle* h, Plan* pl) {
   if (rc != IAN_OK) return rc;
   if (has_flow(h) && !h->map_flow) CUDA_TRY(h, cudaMalloc((void**)&h->map_flow, 20000 * sizeof(float)));
   return IAN_OK;
-}
-
-// x_hat = decode(F(u)) of the plan's n samples
-int run_map_decode(ian_handle* h, Plan* pl, const float* u, float* xh, cudaStream_t st) {
-  if (!has_flow(h)) return run_decode(h, pl, u, xh, st);
-  LAUNCH_TRY(h, launch_made_iaf(u, h->made_w, h->made_b, nullptr, pl->zp.p, pl->zp.plane, pl->n, st));
-  return run_decode_from_planes(h, pl, xh, st);
-}
-
-// The robust fit's loss (DESIGN section 5.6m): kind IAN_ROBUST_HUBER / IAN_ROBUST_CAUCHY and the per-sample scale dl (n),
-// the caller's or, when automatic, written by robust_scale from the start's x_hat before anything reads it.
-struct RobustLoss {
-  int kind;
-  double* dl;
-  bool automatic;
-};
-
-// A (n,100,100), g (n,100) and e (n, nullable) of n samples at u, with x_hat = decode(F(u)) already in xh; w nullable.
-// rl (nullable): the robust fit's A and g, reweighted by rho' at rl's scale (e is then not written: its Gram corner is not E)
-int run_map_normal_eqs(ian_handle* h, int n, const float* u, const float* x, const float* w, double beta, const float* xh,
-                       double* A, double* g, double* e, cudaStream_t st, const RobustLoss* rl = nullptr) {
-  Plan* jp = nullptr;
-  int rc = get_plan(h, 100, &jp);
-  if (rc != IAN_OK) return rc;
-  for (int k = 0; k < n; ++k) {
-    const float* uk = u + (size_t)k * 100;
-    const float *zr = h->gn_zrep, *tan = h->gn_eye;
-    LAUNCH_TRY(h, launch_gn_replicate(uk, h->gn_zrep, st));
-    if (has_flow(h)) {
-      zr = h->map_flow;
-      tan = h->map_flow + 10000;
-      LAUNCH_TRY(h, launch_made_iaf(h->gn_zrep, h->made_w, h->made_b, h->map_flow, nullptr, 0, 100, st));
-      LAUNCH_TRY(h, launch_made_iaf_tangent(h->gn_zrep, h->gn_eye, h->made_w, h->made_b, h->map_flow + 10000, 100, st));
-    }
-    if ((rc = run_decode_jvp(h, jp, zr, tan, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
-    if (rl) {
-      ScopedTimer tm(h, T_ROBUST_GRAM, st);
-      LAUNCH_TRY(h, launch_robust_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, w ? w + (size_t)k * 12288 : nullptr,
-                                       rl->kind, rl->dl + k, beta, uk, h->gn_part, A + (size_t)k * 10000, g + (size_t)k * 100, st));
-      continue;
-    }
-    ScopedTimer tm(h, T_MAP_GRAM, st);
-    LAUNCH_TRY(h, launch_map_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, w ? w + (size_t)k * 12288 : nullptr,
-                                  beta, uk, h->gn_part, A + (size_t)k * 10000, g + (size_t)k * 100, e ? e + k : nullptr, st));
-  }
-  return IAN_OK;
-}
-
-// map_accept, or with rl robust_accept: the fit's objective at x_hat_trial and its accept rule (n samples)
-int launch_fit_accept(const RobustLoss* rl, int init, const float* xht, const float* x, const float* w, double beta, float* xh,
-                      double* e, double* lam, float* u, const float* ut, const int* ok, float* loss, long long ldl, int col,
-                      int n, cudaStream_t st) {
-  if (rl) return launch_robust_accept(init, xht, x, w, beta, rl->kind, rl->dl, xh, e, lam, u, ut, ok, loss, ldl, col, n, st);
-  return launch_map_accept(init, xht, x, w, beta, xh, e, lam, u, ut, ok, loss, ldl, col, n, st);
-}
-
-// rl's automatic scale (if it is) from x_hat and x of n samples
-int run_robust_scale(ian_handle* h, const RobustLoss* rl, const float* xh, const float* x, const float* w, int n,
-                     cudaStream_t st) {
-  if (!rl || !rl->automatic) return IAN_OK;
-  ScopedTimer tm(h, T_ROBUST_SCALE, st);
-  LAUNCH_TRY(h, launch_robust_scale(xh, x, w, rl->kind, rl->dl, n, st));
-  return IAN_OK;
-}
-
-// run_fit on E(u) = sum_p w_p r_p^2 + beta |u|^2: the same solve and rule, trial steps decoded from F(u_trial).
-// rl (nullable): on the robust E(u) = sum_p w_p rho(r_p^2) + beta |u|^2 instead, the scale taken at the start when automatic
-int run_fit_map(ian_handle* h, Plan* pl, const float* x, const float* w, double beta, float* u, int iters, float* loss,
-                cudaStream_t st, const RobustLoss* rl = nullptr) {
-  const int n = pl->n;
-  const long long ldl = (long long)iters + 1;
-  int rc;
-  if ((rc = run_map_decode(h, pl, u, pl->fxh, st)) != IAN_OK) return rc;
-  if ((rc = run_robust_scale(h, rl, pl->fxh, x, w, n, st)) != IAN_OK) return rc;
-  LAUNCH_TRY(h, launch_fit_accept(rl, 1, pl->fxh, x, w, beta, pl->fxh, pl->fe, pl->flam, u, nullptr, nullptr, loss, ldl, 0, n, st));
-  for (int it = 0; it < iters; ++it) {
-    if ((rc = run_map_normal_eqs(h, n, u, x, w, beta, pl->fxh, pl->gnA, pl->gng, pl->gne, st, rl)) != IAN_OK) return rc;
-    {
-      ScopedTimer tm(h, T_GN_SOLVE, st);
-      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, u, pl->fzt, pl->fok, n, st));
-    }
-    if ((rc = run_map_decode(h, pl, pl->fzt, pl->fxt, st)) != IAN_OK) return rc;
-    LAUNCH_TRY(h, launch_fit_accept(rl, 0, pl->fxt, x, w, beta, pl->fxh, pl->fe, pl->flam, u, pl->fzt, pl->fok, loss, ldl, it + 1,
-                                    n, st));
-  }
-  return IAN_OK;
-}
-
-// the prior weight; in the host form also every pixel weight (the device form cannot read them)
-int check_map_args(ian_handle* h, bool host, int n, const float* w, double prior) {
-  if (!(prior >= 0.0) || !std::isfinite(prior)) return fail(h, IAN_ERR_INVALID, "prior must be finite and >= 0 (got %g)", prior);
-  if (host && w)
-    for (size_t i = 0; i < (size_t)n * 12288; ++i)
-      if (!(w[i] >= 0.f) || !std::isfinite(w[i]))
-        return fail(h, IAN_ERR_INVALID, "weight %zu (sample %zu) is %g: weights must be finite and >= 0", i, i / 12288, (double)w[i]);
-  return IAN_OK;
-}
-
-// As call_gauss_newton; the host form stages w in the plan's frame-target buffer.
-int call_map_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int n,
-                          double* A, double* g, double* e, void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK || n == 0) return rc;
-  if (!u || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
-  return run_entry(h, host, stream, n, {{u, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
-                                        {A, 80000, S_GN_A, OUT}, {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_map_plan,
-                   [&](const Chunk& c) {
-    const int r = run_map_decode(h, c.pl, c.f(0), c.pl->fxh, c.st);
-    return r != IAN_OK ? r : run_map_normal_eqs(h, c.cn, c.f(0), c.f(1), c.f(2), prior, c.pl->fxh, (double*)c.p[3],
-                                                (double*)c.p[4], c.p[5] ? (double*)c.p[5] : c.pl->gne, c.st);
-  });
-}
-
-// As call_fit_latent; the host form stages w in the plan's frame-target buffer and z_out in its eps buffer.  z_out = F(u)
-// comes from made_iaf_kernel on the final u, as ian_flow_* computes it (a copy of u on IAN_simple).
-int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w, double prior, int n, float* u, float* z_out,
-                        int iters, float* loss, void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK) return rc;
-  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
-  if (n == 0) return IAN_OK;
-  if (!x || !u) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
-  const size_t ldl = (size_t)iters + 1;
-  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
-                                        {u, kLatentBytes, S_Z, INOUT}, {z_out, kLatentBytes, S_EPS, OUT}}, ensure_map_plan,
-                   [&](const Chunk& c) {
-    float* l = nullptr;
-    int r = fit_loss_buf(c, loss, ldl, &l);
-    if (r == IAN_OK) r = run_fit_map(h, c.pl, c.f(0), c.f(1), prior, c.f(2), iters, l, c.st);
-    if (r == IAN_OK && z_out) {
-      if (has_flow(h))
-        LAUNCH_TRY(h, launch_made_iaf(c.f(2), h->made_w, h->made_b, c.f(3), nullptr, 0, c.cn, c.st));
-      else
-        CUDA_TRY(h, cudaMemcpyAsync(c.f(3), c.f(2), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
-    }
-    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
-  });
 }
 
 // ---- robust latent fit: Huber / Cauchy pixel losses by reweighted Levenberg-Marquardt (DESIGN section 5.6m) -------------
@@ -2696,79 +2497,6 @@ int check_robust_args(ian_handle* h, bool host, int n, int kind, const double* s
       if (!(scale[k] > 0.0) || (std::isinf(scale[k]) && kind == IAN_ROBUST_CAUCHY))
         return fail(h, IAN_ERR_INVALID, "scale %d is %g: scales must be > 0, and finite for the Cauchy loss", k, scale[k]);
   return IAN_OK;
-}
-
-// The chunk's loss: the caller's scale (Arg is), or automatic into scale_out (Arg io; the plan's when left out).  In the host
-// form both stage in the plan's scale buffer.
-RobustLoss robust_loss(const Chunk& c, int kind, int is, int io) {
-  double* s = (double*)c.p[is];
-  double* o = (double*)c.p[io];
-  return {kind, s ? s : o ? o : c.pl->rdl, !s};
-}
-
-// scale_out of a passed scale: a copy of it
-int robust_scale_out(const Chunk& c, const RobustLoss& rl, int io) {
-  double* o = (double*)c.p[io];
-  if (!rl.automatic && o && o != rl.dl)
-    CUDA_TRY(c.h, cudaMemcpyAsync(o, rl.dl, (size_t)c.cn * sizeof(double), cudaMemcpyDeviceToDevice, c.st));
-  return IAN_OK;
-}
-
-// As call_map_gauss_newton; e comes from robust_accept's reduction (the fit's init form), not from the Gram.
-int call_robust_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int kind,
-                             const double* scale, int n, double* A, double* g, double* e, double* scale_out, void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK) return rc;
-  if ((rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK || n == 0) return rc;
-  if (!u || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
-  return run_entry(h, host, stream, n, {{u, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
-                                        {scale, 8, S_SCALE, IN}, {A, 80000, S_GN_A, OUT}, {g, 800, S_GN_G, OUT},
-                                        {e, 8, S_GN_E, OUT}, {scale_out, 8, S_SCALE, OUT}}, ensure_robust_plan,
-                   [&](const Chunk& c) {
-    Plan* pl = c.pl;
-    const RobustLoss rl = robust_loss(c, kind, 3, 7);
-    int r = run_map_decode(h, pl, c.f(0), pl->fxh, c.st);
-    if (r == IAN_OK) r = run_robust_scale(h, &rl, pl->fxh, c.f(1), c.f(2), c.cn, c.st);
-    if (r == IAN_OK)
-      r = run_map_normal_eqs(h, c.cn, c.f(0), c.f(1), c.f(2), prior, pl->fxh, (double*)c.p[4], (double*)c.p[5], nullptr, c.st, &rl);
-    if (r != IAN_OK) return r;
-    LAUNCH_TRY(h, launch_robust_accept(1, pl->fxh, c.f(1), c.f(2), prior, kind, rl.dl, pl->fxh, c.p[6] ? (double*)c.p[6] : pl->gne,
-                                       pl->flam, c.f(0), nullptr, nullptr, nullptr, 1, 0, c.cn, c.st));
-    return robust_scale_out(c, rl, 7);
-  });
-}
-
-// As call_fit_latent_map; the host form also stages outlier_w in the plan's x_hat buffer, which the fit does not use.
-int call_fit_latent_robust(ian_handle* h, bool host, const float* x, const float* w, double prior, int kind, const double* scale,
-                           int n, float* u, float* z_out, int iters, float* loss, double* scale_out, float* outlier_w,
-                           void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK) return rc;
-  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
-  if ((rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK || n == 0) return rc;
-  if (!x || !u) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if ((rc = check_map_args(h, host, n, w, prior)) != IAN_OK) return rc;
-  const size_t ldl = (size_t)iters + 1;
-  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN}, {scale, 8, S_SCALE, IN},
-                                        {u, kLatentBytes, S_Z, INOUT}, {z_out, kLatentBytes, S_EPS, OUT},
-                                        {scale_out, 8, S_SCALE, OUT}, {outlier_w, kImageBytes, S_XHAT, OUT}},
-                   ensure_robust_plan, [&](const Chunk& c) {
-    const RobustLoss rl = robust_loss(c, kind, 2, 5);
-    float* l = nullptr;
-    int r = fit_loss_buf(c, loss, ldl, &l);
-    if (r == IAN_OK) r = run_fit_map(h, c.pl, c.f(0), c.f(1), prior, c.f(3), iters, l, c.st, &rl);
-    if (r != IAN_OK) return r;
-    if (outlier_w) LAUNCH_TRY(h, launch_robust_outliers(c.pl->fxh, c.f(0), c.f(1), kind, rl.dl, c.f(6), c.cn, c.st));
-    if (z_out) {
-      if (has_flow(h))
-        LAUNCH_TRY(h, launch_made_iaf(c.f(3), h->made_w, h->made_b, c.f(4), nullptr, 0, c.cn, c.st));
-      else
-        CUDA_TRY(h, cudaMemcpyAsync(c.f(4), c.f(3), (size_t)c.cn * 400, cudaMemcpyDeviceToDevice, c.st));
-    }
-    if ((r = robust_scale_out(c, rl, 5)) != IAN_OK) return r;
-    return fit_loss_out(c, loss, ldl, l);
-  });
 }
 
 // ---- the IAN's introspection features and the fit under its feature-wise loss (DESIGN section 5.6k) --------------------
@@ -2974,12 +2702,6 @@ int ensure_feat_plan(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
-FeatWeights feat_weights(double a, double b) {
-  FeatWeights w{a, {}};
-  for (int l = 0; l < 4; ++l) w.c[l] = 3072.0 * b / (double)feat_m(l);
-  return w;
-}
-
 // the trial planes (the plan's a1..a4) against the plan's target features, current features kept in fcur
 FeatLayers plan_feat_layers(Plan* pl) {
   FeatLayers f{};
@@ -2992,22 +2714,111 @@ FeatLayers plan_feat_layers(Plan* pl) {
   return f;
 }
 
-// A, g, e of the plan's n samples at z, with x_hat = decode(z) in xh and (b != 0) the features of x and x_hat in the plan's
-// ftg and fcur
-int run_feat_normal_eqs(ian_handle* h, Plan* pl, const float* z, const float* x, const float* xh, const FeatWeights& w,
-                        double* A, double* g, double* e, cudaStream_t st) {
+int check_feat_weights(ian_handle* h, double a, double b) {
+  if (!(a >= 0.0) || !std::isfinite(a)) return fail(h, IAN_ERR_INVALID, "pixel_weight must be finite and >= 0 (got %g)", a);
+  if (!(b >= 0.0) || !std::isfinite(b)) return fail(h, IAN_ERR_INVALID, "feature_weight must be finite and >= 0 (got %g)", b);
+  if (a == 0.0 && b == 0.0) return fail(h, IAN_ERR_INVALID, "pixel_weight and feature_weight are both 0");
+  return IAN_OK;
+}
+
+// ---- one driver for every latent fit (DESIGN section 5.6i) ---------------------------------------------------------------
+// run_lm runs every objective: a start decode and an init accept, then per step the normal equations, the damped solve,
+// a trial decode and the accept rule.  Each entry builds a Fit and runs one of two bodies, call_normal_eqs or call_fit.
+
+// The objective of one fit entry, built once per call from its arguments; the kind picks the Gram and the accept kernel.
+//   PLAIN     E(z) = |x_hat - x|^2                                       gn_gram, gn_accept
+//   MAP       E(u) = sum_p w_p r_p^2 + beta |u|^2                          map_gram, map_accept
+//   ROBUST    E(u) = sum_p w_p rho(r_p^2) + beta |u|^2, rho at scale dl     robust_gram, robust_accept
+//   FEATURES  E(z) = a |x_hat - x|^2 + sum_l c_l |g_l(x_hat) - g_l(x)|^2     gn_gram (a != 0) + feat_gram, feat_accept
+// w and dl are the chunk's (fit_at).
+struct Fit {
+  enum Kind { PLAIN, MAP, ROBUST, FEATURES } kind;
+  bool flow = false;          // x_hat = decode(F(u)): MAP and ROBUST on the flow graphs
+  double beta = 0.0;
+  int loss = 0;               // ROBUST: IAN_ROBUST_HUBER or IAN_ROBUST_CAUCHY
+  FeatWeights fw{};
+  const float* w = nullptr;   // MAP, ROBUST: pixel weights, nullable
+  double* dl = nullptr;       // ROBUST: the per-sample scale, the caller's or (automatic) robust_scale's from the start
+  bool automatic = false;
+  bool feats() const { return kind == FEATURES && fw.c[0] != 0.0; }
+};
+int (*const kFitPlan[4])(ian_handle*, Plan*) = {ensure_gn_plan, ensure_map_plan, ensure_robust_plan, ensure_feat_plan};
+
+// c_l = 3072 b / M_l (b * 12288 * l_f, l_f the per-sample feature loss of train_IAN.py:244).  a = 1, b = 0 is the plain fit.
+Fit feature_fit(double a, double b) {
+  if (a == 1.0 && b == 0.0) return Fit{Fit::PLAIN};
+  Fit f{Fit::FEATURES};
+  f.fw.a = a;
+  for (int l = 0; l < 4; ++l) f.fw.c[l] = 3072.0 * b / (double)feat_m(l);
+  return f;
+}
+
+// fit with the chunk's pixel weights (Arg iw) and robust scale: the caller's (Arg is), or automatic into scale_out (Arg io;
+// the plan's when left out).  In the host form both stage in the plan's scale buffer.
+Fit fit_at(const Fit& fit, const Chunk& c, int iw, int is, int io) {
+  Fit f = fit;
+  double* s = (double*)c.p[is];
+  double* o = (double*)c.p[io];
+  f.w = c.f(iw);
+  f.dl = s ? s : o ? o : c.pl->rdl;
+  f.automatic = !s;
+  return f;
+}
+
+// x_hat = decode(u) of the plan's n samples; with f.flow decode(F(u)), made_iaf_kernel writing the latent planes as
+// `sample` does, so x_hat has ian_flow_*'s bits with x_out at that batch size
+int fit_decode(ian_handle* h, Plan* pl, const Fit& f, const float* u, float* xo, cudaStream_t st) {
+  if (!f.flow) return run_decode(h, pl, u, xo, st);
+  LAUNCH_TRY(h, launch_made_iaf(u, h->made_w, h->made_b, nullptr, pl->zp.p, pl->zp.plane, pl->n, st));
+  return run_decode_from_planes(h, pl, xo, st);
+}
+
+// the feature fit's target features, of x, into the plan's ftg
+int feat_targets(ian_handle* h, Plan* pl, const float* x, cudaStream_t st) {
+  const int rc = run_introspect(h, pl, x, st);
+  return rc != IAN_OK ? rc : store_features(h, pl, false, nullptr, pl->ftg, 0, st);
+}
+
+// the robust fit's automatic scale, from x_hat and x of n samples
+int robust_scale(ian_handle* h, const Fit& f, const float* xh, const float* x, int n, cudaStream_t st) {
+  if (f.kind != Fit::ROBUST || !f.automatic) return IAN_OK;
+  ScopedTimer tm(h, T_ROBUST_SCALE, st);
+  LAUNCH_TRY(h, launch_robust_scale(xh, x, f.w, f.loss, f.dl, n, st));
+  return IAN_OK;
+}
+
+// A (n,100,100), g (n,100) and e (n) of the plan's n samples at u, with x_hat already in xh and, for the feature fit with
+// b != 0, the features of x and x_hat in the plan's ftg and fcur.  The robust Gram does not write e: its corner is not E.
+int fit_normal_eqs(ian_handle* h, Plan* pl, const Fit& f, const float* u, const float* x, const float* xh, double* A,
+                   double* g, double* e, cudaStream_t st) {
   Plan* jp = nullptr;
   int rc = get_plan(h, 100, &jp);
   if (rc != IAN_OK) return rc;
-  const bool feats = w.c[0] != 0.0, pixel = w.a != 0.0;
+  const bool feats = f.feats();
   for (int k = 0; k < pl->n; ++k) {
+    const float *uk = u + (size_t)k * 100, *xk = x + (size_t)k * 12288, *xhk = xh + (size_t)k * 12288;
+    const float* wk = f.w ? f.w + (size_t)k * 12288 : nullptr;
     double *Ak = A + (size_t)k * 10000, *gk = g + (size_t)k * 100, *ek = e + k;
-    LAUNCH_TRY(h, launch_gn_replicate(z + (size_t)k * 100, h->gn_zrep, st));
-    if ((rc = run_decode_jvp(h, jp, h->gn_zrep, h->gn_eye, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
-    if (pixel) {
-      ScopedTimer tm(h, T_GN_GRAM, st);
-      LAUNCH_TRY(h, launch_gn_gram(h->gn_J, xh + (size_t)k * 12288, x + (size_t)k * 12288, h->gn_part, Ak, gk, ek, st));
+    const float *zr = h->gn_zrep, *tan = h->gn_eye;
+    LAUNCH_TRY(h, launch_gn_replicate(uk, h->gn_zrep, st));
+    if (f.flow) {
+      zr = h->map_flow;
+      tan = h->map_flow + 10000;
+      LAUNCH_TRY(h, launch_made_iaf(h->gn_zrep, h->made_w, h->made_b, h->map_flow, nullptr, 0, 100, st));
+      LAUNCH_TRY(h, launch_made_iaf_tangent(h->gn_zrep, h->gn_eye, h->made_w, h->made_b, h->map_flow + 10000, 100, st));
     }
+    if ((rc = run_decode_jvp(h, jp, zr, tan, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
+    if (f.kind == Fit::MAP) {
+      ScopedTimer tm(h, T_MAP_GRAM, st);
+      LAUNCH_TRY(h, launch_map_gram(h->gn_J, xhk, xk, wk, f.beta, uk, h->gn_part, Ak, gk, ek, st));
+    } else if (f.kind == Fit::ROBUST) {
+      ScopedTimer tm(h, T_ROBUST_GRAM, st);
+      LAUNCH_TRY(h, launch_robust_gram(h->gn_J, xhk, xk, wk, f.loss, f.dl + k, f.beta, uk, h->gn_part, Ak, gk, st));
+    } else if (f.kind == Fit::PLAIN || f.fw.a != 0.0) {
+      ScopedTimer tm(h, T_GN_GRAM, st);
+      LAUNCH_TRY(h, launch_gn_gram(h->gn_J, xhk, xk, h->gn_part, Ak, gk, ek, st));
+    }
+    if (f.kind != Fit::FEATURES) continue;
     FeatLayers t{};
     if (feats) {
       if ((rc = run_introspect_jvp(h, jp, jp->xhat, h->gn_J, st)) != IAN_OK) return rc;
@@ -3019,94 +2830,195 @@ int run_feat_normal_eqs(ian_handle* h, Plan* pl, const float* z, const float* x,
       }
     }
     ScopedTimer tm(h, T_FEAT_GRAM, st);
-    LAUNCH_TRY(h, launch_feat_gram(t, w, feats, h->passes, pixel, h->feat_part, Ak, gk, ek, st));
+    LAUNCH_TRY(h, launch_feat_gram(t, f.fw, feats, h->passes, f.fw.a != 0.0, h->feat_part, Ak, gk, ek, st));
   }
   return IAN_OK;
 }
 
-// run_fit on E: trial steps decode z_trial and run the encoder to enc_conv4 on the plan; feat_accept reduces E
-int run_fit_features(ian_handle* h, Plan* pl, const float* x, float* z, int iters, float* loss, const FeatWeights& w,
-                     cudaStream_t st) {
+// the kind's accept kernel on the plan's n samples: E of the trial (x_hat_trial in fxt, u_trial in fzt), or with init of
+// the start (x_hat in fxh), and the Levenberg-Marquardt decision on e, the plan's lambda and loss column col
+int fit_accept(ian_handle* h, Plan* pl, const Fit& f, int init, const float* x, double* e, float* u, float* loss,
+               long long ldl, int col, cudaStream_t st) {
+  const float* xht = init ? pl->fxh : pl->fxt;
+  const float* ut = init ? nullptr : pl->fzt;
+  const int* ok = init ? nullptr : pl->fok;
   const int n = pl->n;
-  const long long ldl = (long long)iters + 1;
-  const bool feats = w.c[0] != 0.0;
-  const FeatLayers f = plan_feat_layers(pl);
-  int rc;
-  if (feats) {
-    if ((rc = run_introspect(h, pl, x, st)) != IAN_OK) return rc;
-    if ((rc = store_features(h, pl, false, nullptr, pl->ftg, 0, st)) != IAN_OK) return rc;
+  switch (f.kind) {
+    case Fit::PLAIN:
+      LAUNCH_TRY(h, launch_gn_accept(init, xht, x, pl->fxh, e, pl->flam, u, ut, ok, loss, ldl, col, n, st));
+      break;
+    case Fit::MAP:
+      LAUNCH_TRY(h, launch_map_accept(init, xht, x, f.w, f.beta, pl->fxh, e, pl->flam, u, ut, ok, loss, ldl, col, n, st));
+      break;
+    case Fit::ROBUST:
+      LAUNCH_TRY(h, launch_robust_accept(init, xht, x, f.w, f.beta, f.loss, f.dl, pl->fxh, e, pl->flam, u, ut, ok, loss, ldl,
+                                         col, n, st));
+      break;
+    case Fit::FEATURES: {
+      ScopedTimer tm(h, T_FEAT_ACCEPT, st);
+      LAUNCH_TRY(h, launch_feat_accept(init, xht, x, plan_feat_layers(pl), f.fw, f.feats(), h->passes, pl->fxh, e, pl->flam,
+                                       u, ut, ok, loss, ldl, col, n, st));
+    }
   }
-  auto trial = [&](const float* zz, float* xo) {
-    int r = run_decode(h, pl, zz, xo, st);
+  return IAN_OK;
+}
+
+// iters Levenberg-Marquardt steps in place on u (pl->n samples); loss (nullable) row k receives E / 12288 of the start and
+// after every step, row stride iters + 1.  The fit's e is only ever set from the accept kernel's reduction, so the history
+// cannot increase.  The feature fit's targets come first, the robust fit's automatic scale from the start's x_hat.
+int run_lm(ian_handle* h, Plan* pl, const Fit& f, const float* x, float* u, int iters, float* loss, cudaStream_t st) {
+  const long long ldl = (long long)iters + 1;
+  const bool feats = f.feats();
+  auto trial = [&](const float* uu, float* xo) {        // x_hat of uu and, for the feature fit, its features in the planes
+    const int r = fit_decode(h, pl, f, uu, xo, st);
     return r != IAN_OK || !feats ? r : run_introspect(h, pl, xo, st);
   };
-  if ((rc = trial(z, pl->fxh)) != IAN_OK) return rc;
-  {
-    ScopedTimer tm(h, T_FEAT_ACCEPT, st);
-    LAUNCH_TRY(h, launch_feat_accept(1, pl->fxh, x, f, w, feats, h->passes, pl->fxh, pl->fe, pl->flam, z, nullptr, nullptr, loss,
-                                     ldl, 0, n, st));
-  }
+  int rc;
+  if (feats && (rc = feat_targets(h, pl, x, st)) != IAN_OK) return rc;
+  if ((rc = trial(u, pl->fxh)) != IAN_OK || (rc = robust_scale(h, f, pl->fxh, x, pl->n, st)) != IAN_OK ||
+      (rc = fit_accept(h, pl, f, 1, x, pl->fe, u, loss, ldl, 0, st)) != IAN_OK)
+    return rc;
   for (int it = 0; it < iters; ++it) {
-    if ((rc = run_feat_normal_eqs(h, pl, z, x, pl->fxh, w, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
+    if ((rc = fit_normal_eqs(h, pl, f, u, x, pl->fxh, pl->gnA, pl->gng, pl->gne, st)) != IAN_OK) return rc;
     {
       ScopedTimer tm(h, T_GN_SOLVE, st);
-      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, z, pl->fzt, pl->fok, n, st));
+      LAUNCH_TRY(h, launch_gn_solve(pl->gnA, pl->gng, pl->flam, u, pl->fzt, pl->fok, pl->n, st));
     }
-    if ((rc = trial(pl->fzt, pl->fxt)) != IAN_OK) return rc;
-    ScopedTimer tm(h, T_FEAT_ACCEPT, st);
-    LAUNCH_TRY(h, launch_feat_accept(0, pl->fxt, x, f, w, feats, h->passes, pl->fxh, pl->fe, pl->flam, z, pl->fzt, pl->fok, loss,
-                                     ldl, it + 1, n, st));
+    if ((rc = trial(pl->fzt, pl->fxt)) != IAN_OK || (rc = fit_accept(h, pl, f, 0, x, pl->fe, u, loss, ldl, it + 1, st)) != IAN_OK)
+      return rc;
   }
   return IAN_OK;
 }
 
-int check_feat_weights(ian_handle* h, double a, double b) {
-  if (!(a >= 0.0) || !std::isfinite(a)) return fail(h, IAN_ERR_INVALID, "pixel_weight must be finite and >= 0 (got %g)", a);
-  if (!(b >= 0.0) || !std::isfinite(b)) return fail(h, IAN_ERR_INVALID, "feature_weight must be finite and >= 0 (got %g)", b);
-  if (a == 0.0 && b == 0.0) return fail(h, IAN_ERR_INVALID, "pixel_weight and feature_weight are both 0");
+// n == 0, the NULL pointers, then for the masked and robust fits the prior weight and, in the host form, every pixel
+// weight (the device form cannot read them)
+int check_fit_inputs(ian_handle* h, bool host, const Fit& f, int n, const float* w, bool null_ptr) {
+  if (n == 0) return IAN_OK;
+  if (null_ptr) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  if (f.kind != Fit::MAP && f.kind != Fit::ROBUST) return IAN_OK;
+  if (!(f.beta >= 0.0) || !std::isfinite(f.beta))
+    return fail(h, IAN_ERR_INVALID, "prior must be finite and >= 0 (got %g)", f.beta);
+  if (host && w)
+    for (size_t i = 0; i < (size_t)n * 12288; ++i)
+      if (!(w[i] >= 0.f) || !std::isfinite(w[i]))
+        return fail(h, IAN_ERR_INVALID, "weight %zu (sample %zu) is %g: weights must be finite and >= 0", i, i / 12288, (double)w[i]);
   return IAN_OK;
 }
 
-// As call_gauss_newton.  a = 1, b = 0 is ian_decode_gauss_newton_* itself.
+// scale_out (Arg io) of a passed scale: a copy of it
+int robust_scale_out(const Chunk& c, const Fit& f, int io) {
+  double* o = (double*)c.p[io];
+  if (f.kind == Fit::ROBUST && !f.automatic && o && o != f.dl)
+    CUDA_TRY(c.h, cudaMemcpyAsync(o, f.dl, (size_t)c.cn * sizeof(double), cudaMemcpyDeviceToDevice, c.st));
+  return IAN_OK;
+}
+
+// The normal equations at u of every objective (ian_*gauss_newton_*).  No CUDA graphs: the JVP passes run on the 100-row
+// plan, whose schedule (stream-K) a capture would change, so both forms launch the same kernels.  The host form stages u
+// in the plan's z buffer, x in its image buffer, w in its frame-target buffer, the scales in its scale buffer and A, g, e
+// in the plan's own normal-equation buffers.  The robust fit's e comes from robust_accept's reduction (the fit's init form).
+int call_normal_eqs(ian_handle* h, bool host, const Fit& fit, const float* u, const float* x, const float* w, const double* scale,
+                    int n, double* A, double* g, double* e, double* scale_out, void* stream) {
+  int rc = check_fit_inputs(h, host, fit, n, w, !u || !x || !A || !g);
+  if (rc != IAN_OK || n == 0) return rc;
+  return run_entry(h, host, stream, n, {{u, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN},
+                                        {scale, 8, S_SCALE, IN}, {A, 80000, S_GN_A, OUT}, {g, 800, S_GN_G, OUT},
+                                        {e, 8, S_GN_E, OUT}, {scale_out, 8, S_SCALE, OUT}}, kFitPlan[fit.kind],
+                   [&](const Chunk& c) {
+    Plan* pl = c.pl;
+    const Fit f = fit_at(fit, c, 2, 3, 7);
+    double* ec = c.p[6] ? (double*)c.p[6] : pl->gne;
+    int r = fit_decode(h, pl, f, c.f(0), pl->fxh, c.st);
+    if (r == IAN_OK && f.feats() && (r = feat_targets(h, pl, c.f(1), c.st)) == IAN_OK &&
+        (r = run_introspect(h, pl, pl->fxh, c.st)) == IAN_OK)
+      r = store_features(h, pl, false, nullptr, pl->fcur, 0, c.st);
+    if (r == IAN_OK) r = robust_scale(h, f, pl->fxh, c.f(1), c.cn, c.st);
+    if (r == IAN_OK) r = fit_normal_eqs(h, pl, f, c.f(0), c.f(1), pl->fxh, (double*)c.p[4], (double*)c.p[5], ec, c.st);
+    if (r != IAN_OK || f.kind != Fit::ROBUST) return r;
+    if ((r = fit_accept(h, pl, f, 1, c.f(1), ec, c.f(0), nullptr, 1, 0, c.st)) != IAN_OK) return r;
+    return robust_scale_out(c, f, 7);
+  });
+}
+
+// The fit of every objective (ian_fit_latent*_*), in place on u.  The host form stages x in the plan's image buffer, w in
+// its frame-target buffer, the scales in its scale buffer, u in its z buffer, z_out in its eps buffer and outlier_w in its
+// x_hat buffer, which the fit does not use.  After the fit: rho'(r^2) into outlier_w, z_out = F(u) on the final u, and
+// scale_out.
+int call_fit(ian_handle* h, bool host, const Fit& fit, const float* x, const float* w, const double* scale, int n, float* u,
+             float* z_out, int iters, float* loss, double* scale_out, float* outlier_w, void* stream) {
+  int rc = check_fit_inputs(h, host, fit, n, w, !x || !u);
+  if (rc != IAN_OK || n == 0) return rc;
+  const size_t ldl = (size_t)iters + 1;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {w, kImageBytes, S_TARGET, IN}, {scale, 8, S_SCALE, IN},
+                                        {u, kLatentBytes, S_Z, INOUT}, {z_out, kLatentBytes, S_EPS, OUT},
+                                        {scale_out, 8, S_SCALE, OUT}, {outlier_w, kImageBytes, S_XHAT, OUT}},
+                   kFitPlan[fit.kind], [&](const Chunk& c) {
+    const Fit f = fit_at(fit, c, 1, 2, 5);
+    float* l = nullptr;
+    int r = fit_loss_buf(c, loss, ldl, &l);
+    if (r == IAN_OK) r = run_lm(h, c.pl, f, c.f(0), c.f(3), iters, l, c.st);
+    if (r != IAN_OK) return r;
+    if (outlier_w) LAUNCH_TRY(h, launch_robust_outliers(c.pl->fxh, c.f(0), f.w, f.loss, f.dl, c.f(6), c.cn, c.st));
+    if (z_out && (r = flow_z(h, c.f(3), c.f(4), nullptr, c.cn, c.st)) != IAN_OK) return r;
+    if ((r = robust_scale_out(c, f, 5)) != IAN_OK) return r;
+    return fit_loss_out(c, loss, ldl, l);
+  });
+}
+
+int call_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, int n, double* A, double* g, double* e,
+                      void* stream) {
+  const int rc = check_fit_args(h, n);
+  return rc != IAN_OK ? rc : call_normal_eqs(h, host, Fit{Fit::PLAIN}, z, x, nullptr, nullptr, n, A, g, e, nullptr, stream);
+}
+
+int call_fit_latent(ian_handle* h, bool host, const float* x, int n, float* z, int iters, float* loss, void* stream) {
+  const int rc = check_fit_args(h, n, iters);
+  return rc != IAN_OK ? rc : call_fit(h, host, Fit{Fit::PLAIN}, x, nullptr, nullptr, n, z, nullptr, iters, loss, nullptr,
+                                      nullptr, stream);
+}
+
+int call_map_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int n,
+                          double* A, double* g, double* e, void* stream) {
+  const int rc = check_fit_args(h, n);
+  return rc != IAN_OK ? rc : call_normal_eqs(h, host, Fit{Fit::MAP, has_flow(h), prior}, u, x, w, nullptr, n, A, g, e,
+                                             nullptr, stream);
+}
+
+int call_fit_latent_map(ian_handle* h, bool host, const float* x, const float* w, double prior, int n, float* u, float* z_out,
+                        int iters, float* loss, void* stream) {
+  const int rc = check_fit_args(h, n, iters);
+  return rc != IAN_OK ? rc : call_fit(h, host, Fit{Fit::MAP, has_flow(h), prior}, x, w, nullptr, n, u, z_out, iters, loss,
+                                      nullptr, nullptr, stream);
+}
+
+int call_robust_gauss_newton(ian_handle* h, bool host, const float* u, const float* x, const float* w, double prior, int kind,
+                             const double* scale, int n, double* A, double* g, double* e, double* scale_out, void* stream) {
+  int rc = check_fit_args(h, n);
+  if (rc != IAN_OK || (rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK) return rc;
+  return call_normal_eqs(h, host, Fit{Fit::ROBUST, has_flow(h), prior, kind}, u, x, w, scale, n, A, g, e, scale_out, stream);
+}
+
+int call_fit_latent_robust(ian_handle* h, bool host, const float* x, const float* w, double prior, int kind, const double* scale,
+                           int n, float* u, float* z_out, int iters, float* loss, double* scale_out, float* outlier_w,
+                           void* stream) {
+  int rc = check_fit_args(h, n, iters);
+  if (rc != IAN_OK || (rc = check_robust_args(h, host, n, kind, scale)) != IAN_OK) return rc;
+  return call_fit(h, host, Fit{Fit::ROBUST, has_flow(h), prior, kind}, x, w, scale, n, u, z_out, iters, loss, scale_out,
+                  outlier_w, stream);
+}
+
 int call_feature_gauss_newton(ian_handle* h, bool host, const float* z, const float* x, int n, double a, double b, double* A,
                               double* g, double* e, void* stream) {
   int rc = check_fit_args(h, n);
-  if (rc != IAN_OK || (rc = check_feat_weights(h, a, b)) != IAN_OK || n == 0) return rc;
-  if (!z || !x || !A || !g) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if (a == 1.0 && b == 0.0) return call_gauss_newton(h, host, z, x, n, A, g, e, stream);
-  const FeatWeights w = feat_weights(a, b);
-  return run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}, {x, kImageBytes, S_X, IN}, {A, 80000, S_GN_A, OUT},
-                                        {g, 800, S_GN_G, OUT}, {e, 8, S_GN_E, OUT}}, ensure_feat_plan, [&](const Chunk& c) {
-    Plan* pl = c.pl;
-    int r = run_decode(h, pl, c.f(0), pl->fxh, c.st);
-    if (r == IAN_OK && w.c[0] != 0.0) {
-      if ((r = run_introspect(h, pl, c.f(1), c.st)) == IAN_OK && (r = store_features(h, pl, false, nullptr, pl->ftg, 0, c.st)) == IAN_OK &&
-          (r = run_introspect(h, pl, pl->fxh, c.st)) == IAN_OK)
-        r = store_features(h, pl, false, nullptr, pl->fcur, 0, c.st);
-    }
-    return r != IAN_OK ? r : run_feat_normal_eqs(h, pl, c.f(0), c.f(1), pl->fxh, w, (double*)c.p[2], (double*)c.p[3],
-                                                 c.p[4] ? (double*)c.p[4] : pl->gne, c.st);
-  });
+  if (rc != IAN_OK || (rc = check_feat_weights(h, a, b)) != IAN_OK) return rc;
+  return call_normal_eqs(h, host, feature_fit(a, b), z, x, nullptr, nullptr, n, A, g, e, nullptr, stream);
 }
 
-// As call_fit_latent.  a = 1, b = 0 is ian_fit_latent_* itself.
 int call_fit_latent_features(ian_handle* h, bool host, const float* x, int n, float* z, int iters, double a, double b, float* loss,
                              void* stream) {
-  int rc = check_fit_args(h, n);
-  if (rc != IAN_OK) return rc;
-  if (iters < 0) return fail(h, IAN_ERR_INVALID, "iters must not be negative (got %d)", iters);
-  if ((rc = check_feat_weights(h, a, b)) != IAN_OK || n == 0) return rc;
-  if (!x || !z) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
-  if (a == 1.0 && b == 0.0) return call_fit_latent(h, host, x, n, z, iters, loss, stream);
-  const FeatWeights w = feat_weights(a, b);
-  const size_t ldl = (size_t)iters + 1;
-  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {z, kLatentBytes, S_Z, INOUT}}, ensure_feat_plan,
-                   [&](const Chunk& c) {
-    float* l = nullptr;
-    int r = fit_loss_buf(c, loss, ldl, &l);
-    if (r == IAN_OK) r = run_fit_features(h, c.pl, c.f(0), c.f(1), iters, l, w, c.st);
-    return r != IAN_OK ? r : fit_loss_out(c, loss, ldl, l);
-  });
+  int rc = check_fit_args(h, n, iters);
+  if (rc != IAN_OK || (rc = check_feat_weights(h, a, b)) != IAN_OK) return rc;
+  return call_fit(h, host, feature_fit(a, b), x, nullptr, nullptr, n, z, nullptr, iters, loss, nullptr, nullptr, stream);
 }
 
 }  // namespace

@@ -14,7 +14,10 @@
         seeded inputs and synthetic oracle.weights, in one child process per build, and prints per array whether
         build/ab/<REV> ("base") and the in-tree build ("head") give the same bits: the three graphs; the tensor-core path
         by default and with IAN_STREAMK=0, IAN_STREAMK=2 and IAN_GRAPHS=0; the SIMT path; batches 1, 3, 47, 130 and 513.
-        Also the host forms of the sampling script's Zfn, Z_IAF_fn and sample on seeded images and N(0,1) latents.
+        Also the host forms of the sampling script's Zfn, Z_IAF_fn and sample on seeded images and N(0,1) latents, and
+        the eight latent-fit entry points (normal equations and fits: plain; masked with and without weights; robust,
+        Huber and Cauchy, automatic and given scale, with outliers; features at weights (1, 1), (0, 1), (1, 0)) in both
+        forms with 3 steps, each call's launch_count() delta one more array, at batches 1 and 3, and 20 under IAN_CHUNK=16.
 """
 import argparse
 import hashlib
@@ -129,6 +132,80 @@ def cmd_run(args):
 OUTPUT_CONFIGS = [("tc", {}), ("tc", {"IAN_STREAMK": "0"}), ("tc", {"IAN_STREAMK": "2"}), ("tc", {"IAN_GRAPHS": "0"}),
                   ("simt", {})]
 OUTPUT_BATCHES = (1, 3, 47, 130, 513)
+FIT_BATCHES = (1, 3)                       # a fit costs one batch-100 JVP pass per sample and step
+FIT_ITERS = 3
+
+
+def _fit_arrays(m, n, seed):
+    """(name, array) of every latent-fit entry point in its host and its device form on seeded inputs, each call
+    followed by its launch_count() delta"""
+    import numpy as np
+    import torch
+    import test_gpu_launch_forms as lf
+    rng = np.random.default_rng(seed)
+    x = np.tanh(rng.standard_normal((n, 3, 64, 64))).astype(np.float32)
+    u = (0.5 * rng.standard_normal((n, 100))).astype(np.float32)
+    w = np.where(rng.uniform(size=x.shape) < 0.25, 0, rng.uniform(size=x.shape)).astype(np.float32)
+    scale = rng.uniform(0.05, 0.5, n)
+    d = lf._Dev()
+    xp, up, wp, sp = d.put(x), d.put(u), d.put(w), d.put(scale)
+    it, prior = FIT_ITERS, 1e-2
+    out = []
+
+    def t(*shape, like=None, f64=False):
+        a = torch.zeros(shape, dtype=torch.float64 if f64 else torch.float32, device="cuda") if like is None else \
+            torch.from_numpy(like.copy()).cuda()
+        d.keep.append(a)
+        return a
+
+    def call(name, f, *res):
+        """f() runs one entry; its arrays are what it returns (host form) or the tensors res (device form)"""
+        c0 = m.launch_count()
+        torch.cuda.synchronize()
+        r = f()
+        torch.cuda.synchronize()
+        arrays = [a.cpu().numpy() for a in res] if res else list(r if isinstance(r, tuple) else (r,))
+        out.extend(("%s %d" % (name, i), a) for i, a in enumerate(arrays))
+        out.append((name + " launches", np.array([m.launch_count() - c0])))
+
+    def gn(name, host, dev):
+        A, g, e = t(n, 100, 100, f64=True), t(n, 100, f64=True), t(n, f64=True)
+        call(name + " host", host)
+        call(name + " dev", lambda: dev(A.data_ptr(), g.data_ptr(), e.data_ptr()), A, g, e)
+
+    gn("gauss_newton", lambda: m.gauss_newton(u, x), lambda A, g, e: m.gauss_newton_dev(up, xp, n, A, g, e))
+    z, loss = t(like=u), t(n, it + 1)
+    call("fit_latent host", lambda: m.fit_latent(x, u, iters=it, return_loss=True))
+    call("fit_latent dev", lambda: m.fit_latent_dev(xp, n, z.data_ptr(), it, loss.data_ptr()), z, loss)
+    for tag, wa, wd in (("", None, 0), ("_w", w, wp)):
+        gn("gauss_newton_map" + tag, lambda: m.gauss_newton_map(u, x, wa, prior),
+           lambda A, g, e: m.gauss_newton_map_dev(up, xp, wd, prior, n, A, g, e))
+        uu, z, loss = t(like=u), t(n, 100), t(n, it + 1)
+        call("fit_latent_map%s host" % tag, lambda: m.fit_latent_map(x, wa, prior, u, iters=it, return_loss=True))
+        call("fit_latent_map%s dev" % tag,
+             lambda: m.fit_latent_map_dev(xp, wd, prior, n, uu.data_ptr(), it, z.data_ptr(), loss.data_ptr()), uu, z, loss)
+    for kind in ("huber", "cauchy"):
+        for tag, sa, sd in (("auto", None, 0), ("given", scale, sp)):
+            name = "%s_%s" % (kind, tag)
+            so = t(n, f64=True)
+            gn("gauss_newton_robust_" + name, lambda: m.gauss_newton_robust(u, x, kind, sa, w, prior),
+               lambda A, g, e: m.gauss_newton_robust_dev(up, xp, wp, prior, kind, sd, n, A, g, e, so.data_ptr()))
+            out.append(("gauss_newton_robust_%s dev scale_out" % name, so.cpu().numpy()))
+            uu, z, loss, so, ow = t(like=u), t(n, 100), t(n, it + 1), t(n, f64=True), t(n, 3, 64, 64)
+            call("fit_latent_robust_%s host" % name,
+                 lambda: m.fit_latent_robust(x, kind, sa, w, prior, u, iters=it, return_loss=True, return_outliers=True))
+            call("fit_latent_robust_%s dev" % name,
+                 lambda: m.fit_latent_robust_dev(xp, wp, prior, kind, sd, n, uu.data_ptr(), it, z.data_ptr(), loss.data_ptr(),
+                                                 so.data_ptr(), ow.data_ptr()), uu, z, so, loss, ow)
+    for a, b in ((1.0, 1.0), (0.0, 1.0), (1.0, 0.0)):
+        name = "features_%g_%g" % (a, b)
+        gn("gauss_newton_" + name, lambda: m.gauss_newton_features(u, x, a, b),
+           lambda A, g, e: m.gauss_newton_features_dev(up, xp, n, A, g, e, a, b))
+        z, loss = t(like=u), t(n, it + 1)
+        call("fit_latent_%s host" % name, lambda: m.fit_latent_features(x, u, it, a, b, return_loss=True))
+        call("fit_latent_%s dev" % name,
+             lambda: m.fit_latent_features_dev(xp, n, z.data_ptr(), it, loss.data_ptr(), a, b), z, loss)
+    return out
 
 
 def cmd_dump(out):
@@ -145,6 +222,12 @@ def cmd_dump(out):
             del lib.SIGNATURES[name]
     npe = importlib.import_module("neural-photo-editor_b200")
     res = {}
+
+    def record(cfg, n, arrays):
+        for name, a in arrays:
+            a = np.ascontiguousarray(a)
+            res["%s n=%d %s" % (cfg, n, name)] = [hashlib.sha256(a.tobytes()).hexdigest(), list(a.shape),
+                                                  float(np.abs(a.astype(np.float64)).sum())]
     for graph in ("simple", "full", "v1"):
         for path, env in OUTPUT_CONFIGS:
             for k in lf.ENV:
@@ -160,11 +243,18 @@ def cmd_dump(out):
                 x = np.tanh(rng.standard_normal((n, 3, 64, 64))).astype(np.float32)
                 zi = rng.standard_normal((n, 100)).astype(np.float32)
                 arrays += [("Zfn host", m.Zfn(x)), ("Z_IAF_fn host", m.Z_IAF_fn(zi)), ("sample host", m.sample(zi))]
-                for name, a in arrays:
-                    a = np.ascontiguousarray(a)
-                    res["%s n=%d %s" % (cfg, n, name)] = [hashlib.sha256(a.tobytes()).hexdigest(), list(a.shape),
-                                                          float(np.abs(a.astype(np.float64)).sum())]
+                if n in FIT_BATCHES:
+                    arrays += _fit_arrays(m, n, 7200 + n)
+                record(cfg, n, arrays)
             m.close()
+        # the fits over two chunks, of 16 and 4 samples
+        for k in lf.ENV:
+            os.environ.pop(k, None)
+        os.environ["IAN_CHUNK"] = "16"
+        m = npe.IAN(lf.CONFIG[graph], True, weights=lf._weights(graph), path="tc")
+        record("%s-tc-IAN_CHUNK=16" % graph, 20, _fit_arrays(m, 20, 7220))
+        m.close()
+        os.environ.pop("IAN_CHUNK")
     with open(out, "w") as f:
         json.dump(res, f)
 

@@ -37,6 +37,81 @@ MAKE = {"simple": ow.make_simple_weights, "v1": ow.make_v1_weights, "full": ow.m
 ITERS = 10
 
 
+def alternated(fns, rounds, min_s):
+    """{key: [seconds per call, one per round]}: every fn warmed up and given enough calls per round for min_s, then all
+    of them timed in turn, round by round"""
+    reps = {}
+    for k, f in fns.items():
+        f()
+        reps[k] = max(2, int(np.ceil(min_s / timed(f, 1))))
+    sec = {k: [] for k in fns}
+    for _ in range(rounds):
+        for k, f in fns.items():
+            sec[k].append(timed(f, reps[k]) / reps[k])
+    return sec
+
+
+def spread(v):
+    return {"median": float(np.median(v)), "range": [float(min(v)), float(max(v))]}
+
+
+def step_ms(model, rounds, min_s, fits):
+    """{batch: {a, b, ratio}}: ms per step of two ITERS-step fits at batches 1 and 32, alternated round by round, and the
+    ratio a / b of their medians; fits(model, n, rng) -> {a: fn, b: fn} sets up both on the same targets"""
+    rng = np.random.default_rng(0)
+    fns = {(n, m): f for n in (1, 32) for m, f in fits(model, n, rng).items()}
+    sec = alternated(fns, rounds, min_s)
+    out = {}
+    for n in (1, 32):
+        r = {m: spread([t / ITERS * 1e3 for t in sec[(k, m)]]) for k, m in fns if k == n}
+        a, b = r
+        r["ratio"] = r[a]["median"] / r[b]["median"]
+        out[str(n)] = r
+    return out
+
+
+def open_model(npe, g, prec, weights):
+    m = npe.IAN(CONFIG[g], True, weights=weights)
+    if prec == "bf16":
+        m.set_precision("bf16")
+    return m
+
+
+def run(fields, measure, extra=None, after=None):
+    """the command line of every bench_fit*.py.  Per graph and precision, r = measure(model, prec, args) on a model with
+    seeded synthetic weights, closed before r.update(extra(npe, g, prec, args)); res = {"gpu", **fields, "<g>_<prec>": r},
+    after(res), then res as one JSON line on stdout and in --out"""
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--min-seconds", type=float, default=1.0)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("%s measures the GPU path and needs a CUDA device" % os.path.basename(sys.argv[0]))
+    npe = importlib.import_module("neural-photo-editor_b200")
+    res = dict({"gpu": gpu_info(0)}, **fields)
+    # a stream of its own: the legacy default stream's handle is 0, which the C-ABI reads as "the handle's own stream",
+    # and the timing events must be recorded on the stream the library calls are enqueued on
+    torch.cuda.set_stream(torch.cuda.Stream())
+    for g in ("simple", "v1", "full"):
+        for prec in (("fp32", "bf16") if g == "full" else ("fp32",)):
+            m = open_model(npe, g, prec, MAKE[g](0))
+            r = measure(m, prec, a)
+            m.close()
+            if extra:
+                r.update(extra(npe, g, prec, a))
+            res["%s_%s" % (g, prec)] = r
+            print(g, prec, json.dumps(r), file=sys.stderr, flush=True)
+    if after:
+        after(res)
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
 def fit_rates(model, rounds, min_s):
     """{batch: fits/s} of a 10-step fit_latent_dev at batches 1 and 32, alternated round by round"""
     rng = np.random.default_rng(0)
@@ -52,15 +127,7 @@ def fit_rates(model, rounds, min_s):
             z.copy_(z0)
             model.fit_latent_dev(x.data_ptr(), n, z.data_ptr(), ITERS, 0, st)
         fns[n] = f
-    reps = {}
-    for n, f in fns.items():
-        f()
-        reps[n] = max(2, int(np.ceil(min_s / timed(f, 1))))
-    rates = {n: [] for n in fns}
-    for _ in range(rounds):
-        for n, f in fns.items():
-            rates[n].append(n * reps[n] / timed(f, reps[n]))
-    return {str(n): {"median": float(np.median(v)), "range": [float(min(v)), float(max(v))]} for n, v in rates.items()}
+    return {str(n): spread([n / t for t in v]) for n, v in alternated(fns, rounds, min_s).items()}
 
 
 def step_split_ms(model, n, reps=10):
@@ -125,42 +192,17 @@ def convergence(model, g, rounds):
     return out
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--min-seconds", type=float, default=1.0)
-    ap.add_argument("--out", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_fit.py measures the GPU path and needs a CUDA device")
+def measure(m, prec, a):
+    return {"fits_per_s": fit_rates(m, a.rounds, a.min_seconds), "step_ms": {str(n): step_split_ms(m, n) for n in (1, 32)}}
+
+
+def recovery(npe, g, prec, a):
     import margin_weights as mw
-    npe = importlib.import_module("neural-photo-editor_b200")
-    res = {"gpu": gpu_info(0), "iters": ITERS}
-    # a stream of its own: the legacy default stream's handle is 0, which the C-ABI reads as "the handle's own stream",
-    # and the timing events must be recorded on the stream the library calls are enqueued on
-    torch.cuda.set_stream(torch.cuda.Stream())
-    for g in ("simple", "v1", "full"):
-        for prec in (("fp32", "bf16") if g == "full" else ("fp32",)):
-            m = npe.IAN(CONFIG[g], True, weights=MAKE[g](0))
-            if prec == "bf16":
-                m.set_precision("bf16")
-            r = {"fits_per_s": fit_rates(m, a.rounds, a.min_seconds),
-                 "step_ms": {str(n): step_split_ms(m, n) for n in (1, 32)}}
-            m.close()
-            mm = npe.IAN(CONFIG[g], True, weights=mw.weights(g, device="cuda"))
-            if prec == "bf16":
-                mm.set_precision("bf16")
-            r["mse_vs_time"] = convergence(mm, g, a.rounds)
-            mm.close()
-            res["%s_%s" % (g, prec)] = r
-            print(g, prec, json.dumps(r), file=sys.stderr, flush=True)
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    mm = open_model(npe, g, prec, mw.weights(g, device="cuda"))
+    r = {"mse_vs_time": convergence(mm, g, a.rounds)}
+    mm.close()
+    return r
 
 
 if __name__ == "__main__":
-    main()
+    run({"iters": ITERS}, measure, recovery)

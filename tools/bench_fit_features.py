@@ -14,9 +14,6 @@ Reported, with the card's name, power limit and SM clock read in the same run:
     101 * 102 / 2 * 245760 multiply-adds at 67 TFLOP/s (FP64 tensor cores) and 34 TFLOP/s (DFMA).
 Synthetic weights: nothing here says how well a trained model's latent fits a real photo.
 """
-import argparse
-import importlib
-import json
 import os
 import subprocess
 import sys
@@ -24,16 +21,10 @@ import sys
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from bench_fit import ITERS, run, step_ms  # noqa: E402
+from bench_vjp import timed  # noqa: E402
 
-from oracle import weights as ow  # noqa: E402
-from bench_vjp import gpu_info, timed  # noqa: E402
-
-CONFIG = {"simple": "IAN_simple.py", "v1": "IANv1.py", "full": "IAN.py"}
-MAKE = {"simple": ow.make_simple_weights, "v1": ow.make_v1_weights, "full": ow.make_full_weights}
-ITERS = 10
 FEAT = 245760
 MACS = 101 * 102 // 2 * FEAT
 
@@ -48,40 +39,22 @@ def sm_clock():
         return {}
 
 
-def step_ms(model, rounds, min_s):
-    """{batch: {features, fit, ratio}}: ms per step of the two 10-step fits at batches 1 and 32, alternated round by round"""
-    rng = np.random.default_rng(0)
+def fits(model, n, rng):
+    """a 10-step fit_latent_features_dev (pixel_weight 1, feature_weight 1) and a 10-step fit_latent_dev on its targets"""
     st = torch.cuda.current_stream().cuda_stream
-    fns = {}
-    for n in (1, 32):
-        zs = rng.standard_normal((n, 100)).astype(np.float32)
-        x = torch.from_numpy(model.sample_at(zs)).cuda()
-        z0 = torch.from_numpy((zs + 0.05 * rng.standard_normal((n, 100))).astype(np.float32)).cuda()
-        z = torch.empty_like(z0)
+    zs = rng.standard_normal((n, 100)).astype(np.float32)
+    x = torch.from_numpy(model.sample_at(zs)).cuda()
+    z0 = torch.from_numpy((zs + 0.05 * rng.standard_normal((n, 100))).astype(np.float32)).cuda()
+    z = torch.empty_like(z0)
 
-        def ffeat(n=n, x=x, z0=z0, z=z):
-            z.copy_(z0)
-            model.fit_latent_features_dev(x.data_ptr(), n, z.data_ptr(), ITERS, 0, 1.0, 1.0, st)
+    def ffeat():
+        z.copy_(z0)
+        model.fit_latent_features_dev(x.data_ptr(), n, z.data_ptr(), ITERS, 0, 1.0, 1.0, st)
 
-        def ffit(n=n, x=x, z0=z0, z=z):
-            z.copy_(z0)
-            model.fit_latent_dev(x.data_ptr(), n, z.data_ptr(), ITERS, 0, st)
-        fns[(n, "features")], fns[(n, "fit")] = ffeat, ffit
-    reps = {}
-    for k, f in fns.items():
-        f()
-        reps[k] = max(2, int(np.ceil(min_s / timed(f, 1))))
-    ms = {k: [] for k in fns}
-    for _ in range(rounds):
-        for k, f in fns.items():
-            ms[k].append(timed(f, reps[k]) / reps[k] / ITERS * 1e3)
-    out = {}
-    for n in (1, 32):
-        r = {m: {"median": float(np.median(ms[(n, m)])), "range": [float(min(ms[(n, m)])), float(max(ms[(n, m)]))]}
-             for m in ("features", "fit")}
-        r["ratio"] = r["features"]["median"] / r["fit"]["median"]
-        out[str(n)] = r
-    return out
+    def ffit():
+        z.copy_(z0)
+        model.fit_latent_dev(x.data_ptr(), n, z.data_ptr(), ITERS, 0, st)
+    return {"features": ffeat, "fit": ffit}
 
 
 def split_ms(model, n=4, reps=20):
@@ -127,40 +100,15 @@ def split_ms(model, n=4, reps=20):
     return out
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--min-seconds", type=float, default=1.0)
-    ap.add_argument("--out", default=None)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_fit_features.py measures the GPU path and needs a CUDA device")
-    npe = importlib.import_module("neural-photo-editor_b200")
-    res = {"gpu": gpu_info(0), "iters": ITERS, "pixel_weight": 1.0, "feature_weight": 1.0}
-    # a stream of its own: the legacy default stream's handle is 0, which the C-ABI reads as "the handle's own stream"
-    torch.cuda.set_stream(torch.cuda.Stream())
-    for g in ("simple", "v1", "full"):
-        for prec in (("fp32", "bf16") if g == "full" else ("fp32",)):
-            m = npe.IAN(CONFIG[g], True, weights=MAKE[g](0))
-            if prec == "bf16":
-                m.set_precision("bf16")
-            r = {"step_ms": step_ms(m, a.rounds, a.min_seconds), "split_ms": split_ms(m)}
-            planes = 2 if prec == "fp32" else 1
-            bounds = {"hbm_3.35TBps": 100 * FEAT * 2 * planes / 3.35e12 * 1e3, "fp64_tensor_67TFLOPs": 2 * MACS / 67e12 * 1e3,
-                      "dfma_34TFLOPs": 2 * MACS / 34e12 * 1e3}
-            r["feat_gram_bounds_ms"] = bounds
-            r["feat_gram_fp64_tflops"] = 2 * MACS / (r["split_ms"]["feat_gram"] * 1e-3) / 1e12
-            m.close()
-            res["%s_%s" % (g, prec)] = r
-            print(g, prec, json.dumps(r), file=sys.stderr, flush=True)
-    res["gpu"].update(sm_clock())                          # sampled right after the timed work
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+def measure(m, prec, a):
+    r = {"step_ms": step_ms(m, a.rounds, a.min_seconds, fits), "split_ms": split_ms(m)}
+    planes = 2 if prec == "fp32" else 1
+    r["feat_gram_bounds_ms"] = {"hbm_3.35TBps": 100 * FEAT * 2 * planes / 3.35e12 * 1e3,
+                                "fp64_tensor_67TFLOPs": 2 * MACS / 67e12 * 1e3, "dfma_34TFLOPs": 2 * MACS / 34e12 * 1e3}
+    r["feat_gram_fp64_tflops"] = 2 * MACS / (r["split_ms"]["feat_gram"] * 1e-3) / 1e12
+    return r
 
 
 if __name__ == "__main__":
-    main()
+    # the SM clock is sampled right after the timed work
+    run({"iters": ITERS, "pixel_weight": 1.0, "feature_weight": 1.0}, measure, after=lambda res: res["gpu"].update(sm_clock()))
