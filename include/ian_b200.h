@@ -447,6 +447,40 @@ int ian_introspect_vjp_dev(ian_handle* h, const float* x, int n, const float* c1
 int ian_introspect_vjp_host(ian_handle* h, const float* x, int n, const float* c1 /*nullable*/, const float* c2 /*nullable*/,
                             const float* c3 /*nullable*/, const float* c4 /*nullable*/, float* dx);
 
+/* ---- the discriminator head l_discrim (IAN_simple.py:225-231, IAN.py:210-216, IANv1.py:203-209) ------------------------
+ * ian_set_discriminator_param loads one of the head's four tensors, in the reference's checkpoint names and shapes:
+ *   minibatch_discrim.theta (1024,500,5), minibatch_discrim.log_weight_scale (500,5), minibatch_discrim.b (500),
+ *   discrimi.W (1524,U) with U = 1 on IAN_simple / IANv1 (sigmoid) and U = 3 on IAN.py (softmax; train_IAN.py:482-484's
+ *   classes: column 0 real, 1 reconstruction, 2 generated).
+ * Valid before or after ian_finalize; a second call replaces the tensor (after synchronising the device).  A wrong name or
+ * shape -> IAN_ERR_INVALID and nothing changes.  The head is not part of ian_model_param_spec's list.
+ *
+ * ian_discriminate_*: x (n,3,64,64) -> logits (n,U) = [pool(a4) | f] W and p (n,U, nullable) = sigmoid or softmax(logits),
+ *   l_discrim under deterministic=True: a4 is enc_conv4 after inference BatchNorm and LeakyReLU (introspect's f4), pool the
+ *   mean over its 4 x 4 pixels (GlobalPoolLayer), f (n,500) the MinibatchLayer's features of the pooled batch
+ *   (layers.py:486-524, as ian_minibatch_discrim_dev).  The trunk runs chunk by chunk; the MinibatchLayer and the dense
+ *   layer run once over the whole call, in float32 (FFMA, fixed summation order, softmax with its max subtracted).
+ * ian_discriminate_vjp_*: dx (n,3,64,64) = (d logits / d x)^T dlogits (n,U) over the whole coupled batch: per chunk the
+ *   trunk and pool, over the call the dense layer's and the MinibatchLayer's adjoints, per chunk again the trunk's reverse
+ *   chain from enc_conv4 (ian_introspect_vjp_*'s with c4 only).  The trunk's forward runs twice: 2 forwards + 1 backward.
+ * BATCH COUPLING: unlike every other entry point, one sample's result depends on the other samples of the call, which form
+ *   the MinibatchLayer's minibatch whatever the chunk size.  At n == 1, f = b exactly (the self-pair's exp(-1e6) is 0) and
+ *   the MinibatchLayer adds nothing to dx.  One non-finite image makes every sample's f, and so every logit, non-finite.  A
+ *   cotangent on sample i reaches every image.  The per-sample isolation that holds elsewhere does not apply here.
+ * Both graphs' trunks run on both paths; bf16 precision applies to the trunk where the handle allows it, the head always
+ *   runs in float32.  No CUDA graphs.  n == 0 does nothing; n < 0 or a NULL x, logits, dlogits or dx -> IAN_ERR_INVALID;
+ *   not finalized or no head loaded (all four tensors) -> IAN_ERR_STATE.  Deterministic (a repeated call is bit-identical;
+ *   the device form computes the host form's bits).
+ * Memory: 16.3 KB per image of whole-call buffers plus 64 KB per image of the largest chunk (grown to the largest n asked
+ *   for); the MinibatchLayer's workspace, shared with ian_minibatch_discrim*_dev: 4 (K P (n + 1)) bytes forward and
+ *   4 (K P (2n + d + 1) + K n (n-1)/2) bytes in the VJP (K = 500, P = 5, d = 1024): about 80 MB at n = 256 and 1.1 GB at
+ *   n = 1024; the VJP allocates what ian_introspect_vjp_* does for c4. */
+int ian_set_discriminator_param(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim);
+int ian_discriminate_dev(ian_handle* h, const float* x, int n, float* logits, float* p /*nullable*/, void* stream);
+int ian_discriminate_host(ian_handle* h, const float* x, int n, float* logits, float* p /*nullable*/);
+int ian_discriminate_vjp_dev(ian_handle* h, const float* x, int n, const float* dlogits, float* dx, void* stream);
+int ian_discriminate_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -570,8 +604,10 @@ int ian_minibatch_discrim_bwd_dev(ian_handle* h, const float* x, int n, int d, c
  * ian_introspect_vjp_* "feat_cotangent" (the cotangents' conversion to split planes), "introspect_bwd_enc_conv4",
  * "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2" (a backward GEMM joined by a supplied cotangent; one without
  * runs as "bwd_enc_conv*"), "enc_conv1" and "enc_conv1_bwd"; in the robust fit "robust_gram" (the reweighted Gram of
- * one sample, with its reduction and the prior terms), "robust_scale" (the automatic scale of the batch) and "gn_solve") over the
- * launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * one sample, with its reduction and the prior terms), "robust_scale" (the automatic scale of the batch) and "gn_solve"; in
+ * ian_discriminate_* "disc_pool" (a4's pool, per chunk), "disc_mb" (the MinibatchLayer), "disc_head" (the dense layer and
+ * its nonlinearity), and in ian_discriminate_vjp_* also "disc_head_bwd", "disc_mb_bwd" and "disc_cotangent" (enc_conv4's
+ * cotangent, per chunk) next to the trunk's own layers) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

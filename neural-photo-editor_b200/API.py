@@ -18,8 +18,9 @@ torch bindings `torch_ops.flow` / `torch_ops.encode_pre` --, the decoder's Gauss
 the batched Levenberg-Marquardt latent fit `fit_latent`, their pixel-weighted forms under the N(0, I) prior in the sampling
 space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), the IAN's introspection features `introspect` /
 `introspect_jvp` / `introspect_vjp` / `feature_loss` (torch binding: `torch_ops.introspect` / `torch_ops.feature_loss`) and
-the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`, and `*_dev` variants taking device
-pointers.
+the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`, the discriminator head l_discrim
+`load_discriminator` / `discriminate` / `discriminate_vjp` (torch binding: `torch_ops.discriminate`), and `*_dev` variants
+taking device pointers.
 """
 from __future__ import annotations
 
@@ -51,6 +52,8 @@ _FULL_CFG = {
 _FULL_MODEL_KEYS = _SIMPLE_MODEL_KEYS + ('l_IAF_mu', 'l_IAF_ls', 'l_Z_IAF')
 # l_introspect = [enc_conv1, enc_conv2, enc_conv3, enc_conv4] (IAN_simple.py:240): per-image shapes
 FEATURE_SHAPES = ((128, 32, 32), (256, 16, 16), (512, 8, 8), (1024, 4, 4))
+# the discriminator head's checkpoint tensors (IAN_simple.py:225-231, IAN.py:210-216, IANv1.py:203-209)
+DISCRIMINATOR_KEYS = ('minibatch_discrim.theta', 'minibatch_discrim.log_weight_scale', 'minibatch_discrim.b', 'discrimi.W')
 # the robust fit's losses (include/ian_b200.h IAN_ROBUST_*)
 ROBUST_KINDS = {"huber": 1, "cauchy": 2}
 
@@ -595,6 +598,57 @@ class IAN:
             res += (out,)
         return res
 
+    # ---- the discriminator head l_discrim --------------------------------------------------------------------------------
+    def discriminator_units(self):
+        """U: 3 on IAN.py (softmax over real / reconstruction / generated, train_IAN.py:482-484), else 1 (sigmoid)"""
+        return 3 if self.kind == _lib.IAN_MODEL_FULL else 1
+
+    def load_discriminator(self, weights=None):
+        """Load the discriminator head's four tensors (DISCRIMINATOR_KEYS) from weights_fname, or from a {name: ndarray}
+        dict.  Every key is looked up and every shape checked before anything is uploaded, so a missing key (IanError naming
+        it) or a wrong shape leaves the handle as it was: a head is never half-loaded."""
+        if weights is None:
+            weights = np.load(self.weights_fname, allow_pickle=False)
+        have = set(weights.keys() if hasattr(weights, 'keys') else weights)
+        shapes = {'minibatch_discrim.theta': (1024, 500, 5), 'minibatch_discrim.log_weight_scale': (500, 5),
+                  'minibatch_discrim.b': (500,), 'discrimi.W': (1524, self.discriminator_units())}
+        arrs = {}
+        for name in DISCRIMINATOR_KEYS:
+            if name not in have:
+                raise _lib.IanError("discriminator parameter '%s' is missing" % name)
+            arrs[name] = np.ascontiguousarray(np.asarray(weights[name], dtype=np.float32))
+            if arrs[name].shape != shapes[name]:
+                raise _lib.IanError("discriminator parameter '%s' must be %r, got %r" % (name, shapes[name], arrs[name].shape))
+        for name, arr in arrs.items():
+            shape = (C.c_int64 * arr.ndim)(*arr.shape)
+            self._check(self._lib.ian_set_discriminator_param(self._h, name.encode(), _fp(arr), shape, arr.ndim))
+
+    def discriminate(self, images, return_logits=False):
+        """l_discrim under deterministic=True: images float32 (n,3,64,64) -> p (n,U) float32, sigmoid (U = 1) or softmax
+        (U = 3) of the logits [pool(enc_conv4) | minibatch features] W; (p, logits) when return_logits.  The MinibatchLayer
+        compares every image of the call with every other, so one image's result depends on the rest of the batch (the
+        batch is the call's, whatever the library's chunk size); at n = 1 the minibatch features are exactly b."""
+        x = _img(images)
+        n, U = x.shape[0], self.discriminator_units()
+        p, logits = np.empty((n, U), np.float32), np.empty((n, U), np.float32)
+        if n:
+            self._check(self._lib.ian_discriminate_host(self._h, _fp(x), n, _fp(logits), _fp(p)))
+        return (p, logits) if return_logits else p
+
+    def discriminate_vjp(self, images, dlogits):
+        """Vector-Jacobian product of the discriminator's logits over the whole coupled batch: images float32 (n,3,64,64),
+        dlogits (n,U) -> dx (n,3,64,64) = (d logits / d x)^T dlogits; a cotangent on one sample reaches every image.  The
+        trunk's forward runs twice (2 forwards + 1 backward)."""
+        x = _img(images)
+        n = x.shape[0]
+        d = _f32(dlogits, 2, 'dlogits')
+        if d.shape != (n, self.discriminator_units()):
+            raise ValueError("dlogits must be (%d,%d), got %r" % (n, self.discriminator_units(), d.shape))
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        if n:
+            self._check(self._lib.ian_discriminate_vjp_host(self._h, _fp(x), n, _fp(d), _fp(dx)))
+        return dx
+
     # ---- the introspection features and the fit under the feature-wise loss ------------------------------------------------
     def introspect(self, images):
         """The IAN's introspection features l_introspect (IAN_simple.py:240): images float32 (n,3,64,64) -> [f1 (n,128,32,32),
@@ -1062,6 +1116,14 @@ class IAN:
     def introspect_vjp_dev(self, x_ptr, n, c_ptrs, dx_ptr, stream=0):
         """introspect_vjp() on device pointers: c_ptrs = 4 pointers to float32 cotangents in FEATURE_SHAPES (0: zero)"""
         self._check(self._lib.ian_introspect_vjp_dev(self._h, x_ptr, int(n), *[p or None for p in c_ptrs], dx_ptr, stream or None))
+
+    def discriminate_dev(self, x_ptr, n, logits_ptr, p_ptr=0, stream=0):
+        """discriminate() on device pointers: logits (n,U) float32, p (n,U) float32 (0: not wanted)"""
+        self._check(self._lib.ian_discriminate_dev(self._h, x_ptr, int(n), logits_ptr, p_ptr or None, stream or None))
+
+    def discriminate_vjp_dev(self, x_ptr, dlogits_ptr, n, dx_ptr, stream=0):
+        """discriminate_vjp() on device pointers"""
+        self._check(self._lib.ian_discriminate_vjp_dev(self._h, x_ptr, int(n), dlogits_ptr, dx_ptr, stream or None))
 
     def gauss_newton_features_dev(self, z_ptr, x_ptr, n, A_ptr, g_ptr, e_ptr=0, pixel_weight=1.0, feature_weight=1.0, stream=0):
         """gauss_newton_features() on device pointers: A (n,100,100), g (n,100), e (n,) float64 (e optional)"""

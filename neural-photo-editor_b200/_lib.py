@@ -103,6 +103,11 @@ SIGNATURES = {
     "ian_fit_latent_features_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double,
                                               C.c_void_p, C.c_void_p]),
     "ian_fit_latent_features_host": (C.c_int, [_H, _F, C.c_int, _F, C.c_int, C.c_double, C.c_double, _F]),
+    "ian_set_discriminator_param": (C.c_int, [_H, C.c_char_p, _F, C.POINTER(C.c_int64), C.c_int]),
+    "ian_discriminate_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_discriminate_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
+    "ian_discriminate_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_discriminate_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
     "ian_param_vjp_supported": (C.c_int, [C.c_int, C.c_int]),
     "ian_decode_param_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_param_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),

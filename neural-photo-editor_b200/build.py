@@ -15,7 +15,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = ["ian_api.cu", "tapgemm_simt.cu", "tapgemm_tc.cu", "decout_tc.cu", "conv1_tc.cu", "edge_kernels.cu",
        "head_tc.cu", "train_kernels.cu", "enc_vjp.cu", "wgrad_tc.cu", "param_vjp.cu",
-       "gn_kernels.cu", "feat_kernels.cu"]
+       "gn_kernels.cu", "feat_kernels.cu", "disc_kernels.cu"]
 HDR = ["tapgemm.h", "edge.h", "tc_ptx.cuh", "../../include/ian_b200.h"]
 LIB = os.path.join(HERE, "libian_b200.so")
 OBJ_DIR = os.path.join(HERE, "csrc", "_obj")

@@ -214,6 +214,17 @@ struct FeatCotangents {
   const float* scale;
 };
 int launch_feat_cotangent(const FeatCotangents& c, int passes, int n, cudaStream_t st);
+// the discriminator head l_discrim (disc_kernels.cu; ian_discriminate_*): its MinibatchLayer has kDiscKernels kernels of 5
+// dimensions on the 1024 pooled channels of a4, its dense layer 1024 + kDiscKernels -> U (1 or kDiscMaxUnits) units
+constexpr int kDiscKernels = 500, kDiscDims = 5, kDiscMaxUnits = 3;
+// a4 (split planes of n images; hi only when passes == 1) -> pooled (n,1024), the mean over the 4 x 4 pixels
+int launch_disc_pool(const __nv_bfloat16* a4, long long plane, int passes, int n, float* out, cudaStream_t st);
+// in (n,1524) = [pool | f], W (1524,U) -> logits (n,U) and p (n,U, nullable) = sigmoid (U = 1) or softmax (U = 3)
+int launch_disc_head(const float* in, const float* W, int U, int n, float* logits, float* p, cudaStream_t st);
+// g (n,1524) = dlogits (n,U) W^T
+int launch_disc_head_bwd(const float* dlogits, const float* W, int U, int n, float* g, cudaStream_t st);
+// c4 (n,1024,4,4) NCHW = dpool (n,1024) / 16 at every pixel
+int launch_disc_cotangent(const float* dpool, int n, float* c4, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

@@ -174,6 +174,8 @@ enum LayerId {
   T_FEAT_COTANGENT,                                     // the features' VJP: the cotangents' conversion to split planes
   T_ROBUST_GRAM, T_ROBUST_SCALE,                        // the robust fit's reweighted Gram (with its reduction and the
                                                         // prior) and its automatic per-sample scale
+  T_DISC_POOL, T_DISC_HEAD, T_DISC_HEAD_BWD, T_DISC_MB, T_DISC_MB_BWD,   // the discriminator head: a4's pool, the dense
+  T_DISC_COTANGENT,                                     // layer, their adjoints, the MinibatchLayer, and enc_conv4's cotangent
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -194,7 +196,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
                                     "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
                                     "feat_gram", "feat_accept", "feat_cotangent",
-                                    "robust_gram", "robust_scale"};
+                                    "robust_gram", "robust_scale",
+                                    "disc_pool", "disc_head", "disc_head_bwd", "disc_mb", "disc_mb_bwd", "disc_cotangent"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -281,6 +284,14 @@ struct ian_handle {
   float* map_flow = nullptr;
   // the feature fit (ian_feature_gauss_newton_*, ian_fit_latent_features_*): the feature Gram's chunk partials (11.2 MB)
   double* feat_part = nullptr;
+  // the discriminator head (ian_set_discriminator_param): theta, log_weight_scale, b, W on the device in the reference
+  // layout, and which of the four are loaded (bit i: kDiscParams[i])
+  float* disc_w[4] = {};
+  int disc_set = 0;
+  // ian_discriminate*'s whole-call buffers (grown to the largest batch asked for, disc_cap samples): the pooled features,
+  // [pool | f], its cotangent, the pool's cotangent, the host forms' logits / p / dlogits, and one chunk's enc_conv4 cotangent
+  float* disc_buf = nullptr;
+  int disc_cap = 0;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -2429,6 +2440,15 @@ int ensure_gn_plan(ian_handle* h, Plan* pl) {
   return IAN_OK;
 }
 
+// the workspace of the training-mode ops and the discriminator head's MinibatchLayer
+int ensure_train_ws(ian_handle* h, size_t bytes) {
+  if (bytes <= h->train_ws_bytes) return IAN_OK;
+  if (h->train_ws) { CUDA_TRY(h, cudaDeviceSynchronize()); CUDA_TRY(h, cudaFree(h->train_ws)); h->train_ws = nullptr; h->train_ws_bytes = 0; }
+  CUDA_TRY(h, cudaMalloc(&h->train_ws, bytes));
+  h->train_ws_bytes = bytes;
+  return IAN_OK;
+}
+
 // The first checks of the fit and introspection entries: the handle, n and iters (the fits).  The fits then check their
 // objective's own arguments (check_robust_args, check_feat_weights), then n == 0 and the rest (check_fit_inputs).
 int check_fit_args(ian_handle* h, int n, int iters = 0) {
@@ -2679,6 +2699,132 @@ int call_introspect_vjp(ian_handle* h, bool host, const float* x, int n, const f
                    [&](const Chunk& ch) {
     const float* ct[4] = {ch.f(1), ch.f(2), ch.f(3), ch.f(4)};
     return run_introspect_vjp(h, ch.pl, ch.f(0), ct, ch.f(5), ch.st);
+  });
+}
+
+// ---- the discriminator head l_discrim (DESIGN section 5.6n) ---------------------------------------------------------
+// logits = [pool(a4) | f] W with f the MinibatchLayer's features of the pooled batch, p = sigmoid / softmax(logits), under
+// deterministic=True.  The MinibatchLayer couples the samples of the call, so the entries run in phases: per chunk the trunk
+// (run_introspect) and the pool into a whole-call buffer at the chunk's offset; over the whole call the MinibatchLayer and
+// the dense layer (and, in the VJP, their adjoints); per chunk again the trunk's reverse chain from enc_conv4's cotangent.
+// The minibatch is therefore the call's batch whatever IAN_CHUNK is.  No CUDA graphs, as for the introspect entries.
+const char* const kDiscParams[4] = {"minibatch_discrim.theta", "minibatch_discrim.log_weight_scale", "minibatch_discrim.b",
+                                    "discrimi.W"};
+constexpr int kDiscIn = 1024 + kDiscKernels;
+inline int disc_units(const ian_handle* h) { return h->model_kind == IAN_MODEL_FULL ? kDiscMaxUnits : 1; }
+
+struct DiscBufs { float *pool, *in, *g, *dpool, *logits, *p, *dlogits, *c4; };
+DiscBufs disc_bufs(ian_handle* h, int cap) {
+  DiscBufs b;
+  const long long N = cap;
+  b.pool = h->disc_buf;
+  b.in = b.pool + N * 1024;
+  b.g = b.in + N * kDiscIn;
+  b.dpool = b.g + N * kDiscIn;
+  b.logits = b.dpool + N * 1024;
+  b.p = b.logits + N * kDiscMaxUnits;
+  b.dlogits = b.p + N * kDiscMaxUnits;
+  b.c4 = b.dlogits + N * kDiscMaxUnits;
+  return b;
+}
+
+int ensure_disc_bufs(ian_handle* h, int n, DiscBufs* out) {
+  if (n > h->disc_cap) {
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaFree(h->disc_buf));
+    h->disc_buf = nullptr;
+    h->disc_cap = 0;
+    const long long N = n, chunk = std::min(n, h->max_chunk);
+    CUDA_TRY(h, cudaMalloc((void**)&h->disc_buf, (size_t)(N * (2 * 1024 + 2 * kDiscIn + 3 * kDiscMaxUnits) + chunk * 16384) * sizeof(float)));
+    h->disc_cap = n;
+  }
+  *out = disc_bufs(h, h->disc_cap);
+  return IAN_OK;
+}
+
+int check_discriminate(ian_handle* h, int n) {
+  const int rc = check_fit_args(h, n);
+  if (rc != IAN_OK) return rc;
+  if (h->disc_set != 15) return fail(h, IAN_ERR_STATE, "no discriminator head loaded (ian_set_discriminator_param)");
+  return IAN_OK;
+}
+
+// phase 1: per chunk, the trunk to enc_conv4 and the pool of a4 into b.pool at the chunk's offset
+int disc_pool_phase(ian_handle* h, bool host, const float* x, int n, const DiscBufs& b, void* stream) {
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}}, nullptr, [&](const Chunk& c) {
+    const int r = run_introspect(h, c.pl, c.f(0), c.st);
+    if (r != IAN_OK) return r;
+    ScopedTimer tm(h, T_DISC_POOL, c.st);
+    LAUNCH_TRY(h, launch_disc_pool(c.pl->a4.p, c.pl->a4.plane, h->passes, c.cn, b.pool + (size_t)c.off * 1024, c.st));
+    return (int)IAN_OK;
+  });
+}
+
+int call_discriminate(ian_handle* h, bool host, const float* x, int n, float* logits, float* p, void* stream) {
+  int rc = check_discriminate(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !logits) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  const int U = disc_units(h);
+  DiscBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &b)) != IAN_OK || (rc = ensure_train_ws(h, mb_workspace_bytes(n, kDiscKernels, kDiscDims))) != IAN_OK ||
+      (rc = disc_pool_phase(h, host, x, n, b, stream)) != IAN_OK)
+    return rc;
+  float* lo = host ? b.logits : logits;
+  float* po = !p ? nullptr : host ? b.p : p;
+  {
+    ScopedTimer tm(h, T_DISC_MB, st);
+    LAUNCH_TRY(h, launch_minibatch_discrim(b.pool, n, 1024, h->disc_w[0], h->disc_w[1], h->disc_w[2], kDiscKernels, kDiscDims, b.in,
+                                           h->train_ws, st));
+  }
+  {
+    ScopedTimer tm(h, T_DISC_HEAD, st);
+    LAUNCH_TRY(h, launch_disc_head(b.in, h->disc_w[3], U, n, lo, po, st));
+  }
+  if (!host) return IAN_OK;
+  CUDA_TRY(h, cudaMemcpyAsync(logits, lo, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (p) CUDA_TRY(h, cudaMemcpyAsync(p, po, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+// phase 2 over the whole call, dlogits -> d[pool | f] -> d pool; phase 3 per chunk, c4 from d pool and run_introspect_vjp
+// with c = {0, 0, 0, c4}.  The trunk's forward runs twice: 2 forwards and 1 backward.
+int call_discriminate_vjp(ian_handle* h, bool host, const float* x, int n, const float* dlogits, float* dx, void* stream) {
+  int rc = check_discriminate(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !dlogits || !dx) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  const int U = disc_units(h);
+  DiscBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &b)) != IAN_OK ||
+      (rc = ensure_train_ws(h, mb_bwd_workspace_bytes(n, 1024, kDiscKernels, kDiscDims))) != IAN_OK ||
+      (rc = disc_pool_phase(h, host, x, n, b, stream)) != IAN_OK)
+    return rc;
+  const float* dl = dlogits;
+  if (host) {
+    CUDA_TRY(h, cudaMemcpyAsync(b.dlogits, dlogits, (size_t)n * U * sizeof(float), cudaMemcpyHostToDevice, st));
+    dl = b.dlogits;
+  }
+  {
+    ScopedTimer tm(h, T_DISC_HEAD_BWD, st);
+    LAUNCH_TRY(h, launch_disc_head_bwd(dl, h->disc_w[3], U, n, b.g, st));
+  }
+  {
+    ScopedTimer tm(h, T_DISC_MB_BWD, st);
+    LAUNCH_TRY(h, launch_minibatch_discrim_bwd(b.pool, n, 1024, h->disc_w[0], h->disc_w[1], kDiscKernels, kDiscDims, b.g, b.dpool,
+                                               nullptr, nullptr, nullptr, h->train_ws, st));
+  }
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {dx, kImageBytes, S_XHAT, OUT}}, ensure_introspect_vjp_plan<false>,
+                   [&](const Chunk& c) {
+    {
+      ScopedTimer tm(h, T_DISC_COTANGENT, c.st);
+      LAUNCH_TRY(h, launch_disc_cotangent(b.dpool + (size_t)c.off * 1024, c.cn, b.c4, c.st));
+    }
+    const float* ct[4] = {nullptr, nullptr, nullptr, b.c4};
+    return run_introspect_vjp(h, c.pl, c.f(0), ct, c.f(1), c.st);
   });
 }
 
@@ -3157,6 +3303,8 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->head_tc_wt);
   cudaFree(h->train_ws);
   cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part); cudaFree(h->map_flow); cudaFree(h->feat_part);
+  for (float* p : h->disc_w) cudaFree(p);
+  cudaFree(h->disc_buf);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -3385,6 +3533,41 @@ int ian_introspect_vjp_host(ian_handle* h, const float* x, int n, const float* c
                             const float* c4, float* dx) {
   const float* c[4] = {c1, c2, c3, c4};
   return call_introspect_vjp(h, true, x, n, c, dx, nullptr);
+}
+int ian_set_discriminator_param(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!name || !data || !shape) return fail(h, IAN_ERR_INVALID, "NULL argument");
+  int k = 0;
+  while (k < 4 && strcmp(name, kDiscParams[k])) ++k;
+  if (k == 4) return fail(h, IAN_ERR_INVALID, "'%s' is not a discriminator parameter", name);
+  const int64_t want[4][3] = {{1024, kDiscKernels, kDiscDims}, {kDiscKernels, kDiscDims}, {kDiscKernels}, {kDiscIn, disc_units(h)}};
+  const int nd[4] = {3, 2, 1, 2};
+  bool ok = ndim == nd[k];
+  int64_t elems = 1;
+  for (int i = 0; ok && i < ndim; ++i) {
+    ok = shape[i] == want[k][i];
+    elems *= want[k][i];
+  }
+  if (!ok) return fail(h, IAN_ERR_INVALID, "'%s' has the wrong shape (want %d dims: %lld %lld %lld)", name, nd[k],
+                       (long long)want[k][0], (long long)want[k][1], (long long)want[k][2]);
+  DeviceGuard dg(h->device);
+  if (h->disc_w[k]) CUDA_TRY(h, cudaDeviceSynchronize());   // ordered after all work enqueued before the call
+  else CUDA_TRY(h, cudaMalloc((void**)&h->disc_w[k], (size_t)elems * sizeof(float)));
+  CUDA_TRY(h, cudaMemcpy(h->disc_w[k], data, (size_t)elems * sizeof(float), cudaMemcpyHostToDevice));
+  h->disc_set |= 1 << k;
+  return IAN_OK;
+}
+int ian_discriminate_dev(ian_handle* h, const float* x, int n, float* logits, float* p, void* stream) {
+  return call_discriminate(h, false, x, n, logits, p, stream);
+}
+int ian_discriminate_host(ian_handle* h, const float* x, int n, float* logits, float* p) {
+  return call_discriminate(h, true, x, n, logits, p, nullptr);
+}
+int ian_discriminate_vjp_dev(ian_handle* h, const float* x, int n, const float* dlogits, float* dx, void* stream) {
+  return call_discriminate_vjp(h, false, x, n, dlogits, dx, stream);
+}
+int ian_discriminate_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx) {
+  return call_discriminate_vjp(h, true, x, n, dlogits, dx, nullptr);
 }
 int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
                                  double* A, double* g, double* e, void* stream) {
@@ -3692,13 +3875,6 @@ int ian_gather_wait_dev(ian_handle* h, float** gathered_out, void* stream) {
 }
 
 // ---- training-mode pieces (SURVEY 8f rank 4; the trainers themselves stay the reference's) ------------------------------
-static int ensure_train_ws(ian_handle* h, size_t bytes) {
-  if (bytes <= h->train_ws_bytes) return IAN_OK;
-  if (h->train_ws) { CUDA_TRY(h, cudaDeviceSynchronize()); CUDA_TRY(h, cudaFree(h->train_ws)); h->train_ws = nullptr; h->train_ws_bytes = 0; }
-  CUDA_TRY(h, cudaMalloc(&h->train_ws, bytes));
-  h->train_ws_bytes = bytes;
-  return IAN_OK;
-}
 
 int ian_bn_batch_stats_dev(ian_handle* h, const float* x, int n, int c, int hw, double* sum, double* sumsq, void* stream) {
   if (!h) return IAN_ERR_INVALID;

@@ -23,6 +23,11 @@
     of train_IAN.py:244 built on it, so feature_loss(model, decode(model, z), x).sum().backward() drives z -- or, with
     params, the IAN_simple decoder's parameters -- under the generator's own reconstruction objective.
 
+  * discriminate(model, x) = the logits of the IAN's discriminator head l_discrim (what model.discriminate(x,
+    return_logits=True) returns) as a differentiable torch op; F.logsigmoid / log_softmax of them is the realism score.  Its
+    backward is one ian_discriminate_vjp_dev call over the whole batch: the MinibatchLayer couples the samples, so a
+    loss on one sample's logits moves every image of the call.  Reverse mode only.
+
   * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
     (ian_decode_param_vjp_dev) that also returns dz.  Before each forward, every tensor whose in-place version moved since
@@ -41,6 +46,7 @@ _Decode = None
 _Encode = None
 _DecodeParams = None
 _Introspect = None
+_Discriminate = None
 
 
 def _check_tensor(model, t, what):
@@ -357,6 +363,59 @@ def feature_loss(model, x_hat, x):
     if int(fb[0].shape[0]) != n:
         raise ValueError("x_hat and x must hold the same number of images")
     return sum(((a - b) ** 2).reshape(n, -1).mean(1) for a, b in zip(fa, fb)) / 4
+
+
+def _discriminate_function():
+    global _Discriminate
+    if _Discriminate is not None:
+        return _Discriminate
+    import torch
+    from torch.autograd.function import once_differentiable
+
+    class Discriminate(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, model, x):
+            _check_tensor(model, x, "x")
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 64, 64):
+                raise ValueError("x must be (n,3,64,64), got %r" % (tuple(x.shape),))
+            x = x.contiguous()
+            n = int(x.shape[0])
+            logits = torch.empty(n, model.discriminator_units(), dtype=torch.float32, device=x.device)
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.discriminate_dev(x.data_ptr(), n, logits.data_ptr(), 0, st)
+            ctx.model = model
+            ctx.save_for_backward(x)
+            return logits
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            (x,) = ctx.saved_tensors
+            model = ctx.model
+            _check_tensor(model, g, "grad_output")
+            g = g.contiguous()
+            n = int(x.shape[0])
+            dx = torch.empty_like(x)
+            if n:
+                with _lib_stream(model, x) as st:
+                    model.discriminate_vjp_dev(x.data_ptr(), g.data_ptr(), n, dx.data_ptr(), st)
+            return None, dx
+
+        @staticmethod
+        def jvp(ctx, *tangents):
+            raise NotImplementedError("torch_ops.discriminate has no forward mode (the library has no JVP of the discriminator)")
+
+    _Discriminate = Discriminate
+    return Discriminate
+
+
+def discriminate(model, x):
+    """logits (n,U) of the discriminator head for x (n,3,64,64) float32 CUDA on the model's device, after
+    model.load_discriminator(): U = 1 (sigmoid) on IAN_simple / IANv1, 3 (softmax: real, reconstruction, generated) on IAN.py.
+    Differentiable w.r.t. x in reverse mode (one ian_discriminate_vjp_dev per backward: two trunk forwards and one
+    backward).  The batch is coupled: every sample's logits depend on every image of the call."""
+    return _discriminate_function().apply(model, x)
 
 
 def _params_function():
