@@ -481,6 +481,30 @@ int ian_discriminate_host(ian_handle* h, const float* x, int n, float* logits, f
 int ian_discriminate_vjp_dev(ian_handle* h, const float* x, int n, const float* dlogits, float* dx, void* stream);
 int ian_discriminate_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx);
 
+/* ---- the discriminator in training mode: l_discrim under deterministic=False (train_IAN.py:139-149, train_IAN_simple.py:405)
+ * ian_discriminate_train_*: logits and p (nullable) as ian_discriminate_*, with bnorm2..4 in the trunk normalising with the
+ *   BATCH's statistics: per channel mean and biased variance over (n, h, w) of enc_conv{2,3,4}'s raw output, inv_std =
+ *   1/sqrt(var + 1e-4), y = (x - mean) (gamma inv_std) + beta, then LeakyReLU(0.2); enc_conv1, GlobalPool, the MinibatchLayer
+ *   and the dense head are unchanged.  The handle's running mean / inv_std are neither used nor changed.
+ *   stats (nullable) receives the statistics used, float32 (2,1792): row 0 the means of bnorm2 (256) | bnorm3 (512) |
+ *   bnorm4 (1024), row 1 their inv_std -- Lasagne's running-average update (alpha = 0.1) is the caller's to apply.
+ * ian_discriminate_train_vjp_*: dx (n,3,64,64) = (d logits / d x)^T dlogits (n,U) over the whole batch, the gradient flowing
+ *   through the batch mean and variance as Theano's T.grad gives it.  1 trunk forward + 1 backward.
+ * The sums are float64 per image, added in image order: the statistics, and so every result, do not depend on IAN_CHUNK.
+ * BATCH COUPLING as for ian_discriminate_*, and more: every BatchNorm of the trunk couples the samples, so even at n == 1
+ *   a sample's result is its own batch's (a 1-image batch normalises over its pixels alone).
+ * Precision, paths, argument checks, error codes and IAN_ERR_STATE without a head are ian_discriminate_*'s; n == 0 does
+ *   nothing.  Deterministic.  No CUDA graphs.
+ * Memory: the whole-call buffers of ian_discriminate_* plus 852 KB per image (enc_conv2..4's raw sums, two cotangent
+ *   buffers, float32) and 16 KB per image of partial sums: about 220 MB at n = 256; the VJP allocates what
+ *   ian_encode_vjp_* does on each chunk's plan. */
+int ian_discriminate_train_dev(ian_handle* h, const float* x, int n, float* logits, float* p /*nullable*/,
+                               float* stats /*nullable*/, void* stream);
+int ian_discriminate_train_host(ian_handle* h, const float* x, int n, float* logits, float* p /*nullable*/,
+                                float* stats /*nullable*/);
+int ian_discriminate_train_vjp_dev(ian_handle* h, const float* x, int n, const float* dlogits, float* dx, void* stream);
+int ian_discriminate_train_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx);
+
 /* ---- decoder parameter vector-Jacobian product (IAN_MODEL_SIMPLE): dL/dtheta for the decoder's trainable tensors -----
  * The parameters train_IAN_simple.py:353 hands to the optimiser (`decoder_params`): l_dec_fc2.W, dec_conv1..3.W, dec_out.W
  * and bnorm_dec_fc2 / bnorm_dc1..3 .beta / .gamma, on the deterministic graph of X_hat_fn (API.py:46): inference
@@ -607,7 +631,9 @@ int ian_minibatch_discrim_bwd_dev(ian_handle* h, const float* x, int n, int d, c
  * one sample, with its reduction and the prior terms), "robust_scale" (the automatic scale of the batch) and "gn_solve"; in
  * ian_discriminate_* "disc_pool" (a4's pool, per chunk), "disc_mb" (the MinibatchLayer), "disc_head" (the dense layer and
  * its nonlinearity), and in ian_discriminate_vjp_* also "disc_head_bwd", "disc_mb_bwd" and "disc_cotangent" (enc_conv4's
- * cotangent, per chunk) next to the trunk's own layers) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * cotangent, per chunk) next to the trunk's own layers; in ian_discriminate_train* "disc_train_enc_conv2..4" (the
+ * layers' raw sums), "disc_train_stats", "disc_train_norm" (BatchNorm + LeakyReLU into the next layer's planes), and in the
+ * VJP also "disc_train_cotangent", "disc_train_bn_bwd" (Σdy, Σdy·x), "disc_train_bn_dx", "disc_train_bwd_enc_conv4..3") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

@@ -19,8 +19,8 @@ the batched Levenberg-Marquardt latent fit `fit_latent`, their pixel-weighted fo
 space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), the IAN's introspection features `introspect` /
 `introspect_jvp` / `introspect_vjp` / `feature_loss` (torch binding: `torch_ops.introspect` / `torch_ops.feature_loss`) and
 the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`, the discriminator head l_discrim
-`load_discriminator` / `discriminate` / `discriminate_vjp` (torch binding: `torch_ops.discriminate`), and `*_dev` variants
-taking device pointers.
+`load_discriminator` / `discriminate` / `discriminate_vjp` and their training-mode forms `discriminate_train` /
+`discriminate_train_vjp` (torch binding: `torch_ops.discriminate`), and `*_dev` variants taking device pointers.
 """
 from __future__ import annotations
 
@@ -649,6 +649,37 @@ class IAN:
             self._check(self._lib.ian_discriminate_vjp_host(self._h, _fp(x), n, _fp(d), _fp(dx)))
         return dx
 
+    def discriminate_train(self, images, return_logits=False, return_stats=False):
+        """l_discrim in training mode (deterministic=False, as train_IAN.py:139-149 evaluates it): bnorm2..4 in the trunk
+        normalise with the batch's mean and biased variance over (n, h, w), inv_std = 1/sqrt(var + 1e-4); the running
+        statistics are neither used nor changed.  images float32 (n,3,64,64) -> p (n,U); with return_logits also the logits,
+        with return_stats also stats float32 (2,1792): row 0 the batch means of bnorm2 | bnorm3 | bnorm4, row 1 their
+        inv_std (for Lasagne's running-average update, alpha = 0.1, which is the caller's).  Returns p alone, or the tuple
+        (p[, logits][, stats])."""
+        x = _img(images)
+        n, U = x.shape[0], self.discriminator_units()
+        p, logits = np.empty((n, U), np.float32), np.empty((n, U), np.float32)
+        stats = np.empty((2, 1792), np.float32)
+        if n:
+            self._check(self._lib.ian_discriminate_train_host(self._h, _fp(x), n, _fp(logits), _fp(p), _fp(stats)))
+        else:
+            stats.fill(np.nan)
+        res = (p,) + ((logits,) if return_logits else ()) + ((stats,) if return_stats else ())
+        return res if len(res) > 1 else p
+
+    def discriminate_train_vjp(self, images, dlogits):
+        """Vector-Jacobian product of discriminate_train()'s logits over the whole batch: dx (n,3,64,64) = (d logits / d x)^T
+        dlogits, through the batch statistics as Theano's T.grad gives it.  1 trunk forward + 1 backward."""
+        x = _img(images)
+        n = x.shape[0]
+        d = _f32(dlogits, 2, 'dlogits')
+        if d.shape != (n, self.discriminator_units()):
+            raise ValueError("dlogits must be (%d,%d), got %r" % (n, self.discriminator_units(), d.shape))
+        dx = np.empty((n, 3, 64, 64), np.float32)
+        if n:
+            self._check(self._lib.ian_discriminate_train_vjp_host(self._h, _fp(x), n, _fp(d), _fp(dx)))
+        return dx
+
     # ---- the introspection features and the fit under the feature-wise loss ------------------------------------------------
     def introspect(self, images):
         """The IAN's introspection features l_introspect (IAN_simple.py:240): images float32 (n,3,64,64) -> [f1 (n,128,32,32),
@@ -1124,6 +1155,15 @@ class IAN:
     def discriminate_vjp_dev(self, x_ptr, dlogits_ptr, n, dx_ptr, stream=0):
         """discriminate_vjp() on device pointers"""
         self._check(self._lib.ian_discriminate_vjp_dev(self._h, x_ptr, int(n), dlogits_ptr, dx_ptr, stream or None))
+
+    def discriminate_train_dev(self, x_ptr, n, logits_ptr, p_ptr=0, stats_ptr=0, stream=0):
+        """discriminate_train() on device pointers: logits (n,U), p (n,U) and stats (2,1792) float32 (0: not wanted)"""
+        self._check(self._lib.ian_discriminate_train_dev(self._h, x_ptr, int(n), logits_ptr, p_ptr or None, stats_ptr or None,
+                                                         stream or None))
+
+    def discriminate_train_vjp_dev(self, x_ptr, dlogits_ptr, n, dx_ptr, stream=0):
+        """discriminate_train_vjp() on device pointers"""
+        self._check(self._lib.ian_discriminate_train_vjp_dev(self._h, x_ptr, int(n), dlogits_ptr, dx_ptr, stream or None))
 
     def gauss_newton_features_dev(self, z_ptr, x_ptr, n, A_ptr, g_ptr, e_ptr=0, pixel_weight=1.0, feature_weight=1.0, stream=0):
         """gauss_newton_features() on device pointers: A (n,100,100), g (n,100), e (n,) float64 (e optional)"""

@@ -108,6 +108,10 @@ SIGNATURES = {
     "ian_discriminate_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
     "ian_discriminate_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_discriminate_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
+    "ian_discriminate_train_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_discriminate_train_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F]),
+    "ian_discriminate_train_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_discriminate_train_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
     "ian_param_vjp_supported": (C.c_int, [C.c_int, C.c_int]),
     "ian_decode_param_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_param_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),

@@ -7,6 +7,17 @@
 //   disc_head_bwd   : its adjoint d[pool | f] = dlogits W^T, U products per element in u order
 //   disc_cotangent  : d pool -> the cotangent of a4, c4 = broadcast(d pool / 16) (n,1024,4,4) float32 NCHW
 // A feature value is what the encoder stores: hi + lo of the split planes, or hi alone in bf16 mode (launch_feat_store's rule).
+//
+// The training-mode trunk (ian_discriminate_train*; DESIGN section 5.6o): batch-statistics BatchNorm on enc_conv2..4's raw
+// sums, whole-call float32 NHWC buffers (n, HW, C), channel c of pixel p of image i at (i HW + p) C + c.
+//   disc_bn_partial  : per image and channel, Σu and Σu·v in float64 over the image's pixels in order (u = v = x: the
+//                      forward's Σx, Σx²; u = dy, v = x: the backward's Σdy, Σdy·x)
+//   disc_bn_stats    : the images' partials added in image order, so the sums do not depend on the chunking; mean and
+//                      inv_std = 1/sqrt(var + eps) as bn_finalize_kernel forms them (biased var), float32 copies for the callers
+//   disc_bn_act      : y = (x - mean) (gamma inv_std) + beta, a = LeakyReLU(0.2)(y) -> split planes (hi only in bf16 mode)
+//   disc_train_cot   : the pool's adjoint times lrelu'(y4): dy4 = d pool / 16 * (y4 > 0 ? 1 : 0.2), float32
+//   disc_bn_coef     : bn_bwd_coef_kernel's coefficients from the whole-call sums
+//   disc_bn_dx       : dx per element in float64, rounded once as bn_bwd_apply_kernel does -> split planes
 #include "edge.h"
 
 namespace ian {
@@ -100,6 +111,101 @@ __global__ void __launch_bounds__(256) disc_cotangent_kernel(const float* __rest
 
 unsigned blocks_of(long long total) { return (unsigned)((total + 255) / 256); }
 
+// thread (image, channel): coalesced over channels, the image's pixels in order
+__global__ void __launch_bounds__(128) disc_bn_partial_kernel(const float* __restrict__ u, const float* __restrict__ v, int hw, int c,
+                                                              double* __restrict__ part /*[n][2][c]*/) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
+  if (ch >= c) return;
+  const long long base = (long long)i * hw * c + ch;
+  double s = 0.0, q = 0.0;                               // float64 from the first term: a product of two float32 is exact
+  for (int p = 0; p < hw; ++p) {
+    const double a = (double)__ldg(u + base + (long long)p * c);
+    s += a;
+    q += a * (double)__ldg(v + base + (long long)p * c);
+  }
+  part[((long long)i * 2) * c + ch] = s;
+  part[((long long)i * 2 + 1) * c + ch] = q;
+}
+
+// sums[2][c] = the partials of images 0..n-1 in order; with count > 0 also mean_f / inv_std_f (the forward's statistics)
+__global__ void disc_bn_stats_kernel(const double* __restrict__ part, int n, int c, double count, float eps, double* __restrict__ sums,
+                                     float* __restrict__ mean_f, float* __restrict__ inv_std_f) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= c) return;
+  double s = 0.0, q = 0.0;
+  for (int i = 0; i < n; ++i) {
+    s += part[((long long)i * 2) * c + ch];
+    q += part[((long long)i * 2 + 1) * c + ch];
+  }
+  sums[ch] = s;
+  sums[c + ch] = q;
+  if (!mean_f) return;
+  const double mean = s / count;
+  double var = q / count - mean * mean;                  // biased variance, as theano's x.var(axes)
+  if (var < 0.0) var = 0.0;
+  mean_f[ch] = (float)mean;
+  inv_std_f[ch] = (float)(1.0 / sqrt(var + (double)eps));
+}
+
+// lasagne's order: (x - mean) * (gamma * inv_std) + beta
+__device__ __forceinline__ float bn_train_y(float x, int ch, const float* mean, const float* inv_std, const float* gamma,
+                                            const float* beta) {
+  return (x - __ldg(mean + ch)) * (__ldg(gamma + ch) * __ldg(inv_std + ch)) + __ldg(beta + ch);
+}
+
+__global__ void __launch_bounds__(256) disc_bn_act_kernel(const float* __restrict__ x, long long total, int c, const float* __restrict__ mean,
+                                                          const float* __restrict__ inv_std, const float* __restrict__ gamma,
+                                                          const float* __restrict__ beta, int passes, __nv_bfloat16* __restrict__ out,
+                                                          long long plane) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float y = bn_train_y(x[i], (int)(i % c), mean, inv_std, gamma, beta);
+  const float a = fmaf(0.4f, fabsf(y), 0.6f * y);       // LeakyRectify(0.2) as the tap-GEMM epilogue forms it
+  __nv_bfloat16 hi, lo;
+  split_bf16(a, hi, lo);
+  out[i] = hi;
+  if (passes != 1) out[plane + i] = lo;
+}
+
+__global__ void __launch_bounds__(256) disc_train_cot_kernel(const float* __restrict__ dpool, const float* __restrict__ x4, int n,
+                                                             const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                             float* __restrict__ dy) {
+  const long long o = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (o >= (long long)n * kPool * kC4) return;
+  const int ch = (int)(o % kC4);
+  const float y = bn_train_y(x4[o], ch, mean, inv_std, gamma, beta);
+  dy[o] = dpool[(o / (kPool * kC4)) * kC4 + ch] * (1.f / kPool) * (y > 0.f ? 1.f : 0.2f);
+}
+
+// dx = a (dy - m - (x - mean) k), a = gamma s, m = Σdy/N, k = s² (Σdy·x - mean Σdy)/N, s = inv_std in float64
+__global__ void disc_bn_coef_kernel(const double* __restrict__ fsum, const double* __restrict__ bsum, double count, float eps,
+                                    const float* __restrict__ gamma, int c, double* __restrict__ coef /*[4][c]*/) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= c) return;
+  const double mean = fsum[ch] / count;
+  double var = fsum[c + ch] / count - mean * mean;
+  if (var < 0.0) var = 0.0;
+  const double s = 1.0 / sqrt(var + (double)eps);
+  coef[ch] = (double)gamma[ch] * s;
+  coef[c + ch] = bsum[ch] / count;
+  coef[2 * c + ch] = mean;
+  coef[3 * c + ch] = s * s * (bsum[c + ch] - mean * bsum[ch]) / count;
+}
+
+__global__ void __launch_bounds__(256) disc_bn_dx_kernel(const float* __restrict__ x, const float* __restrict__ dy, long long total, int c,
+                                                         const double* __restrict__ coef, int passes, __nv_bfloat16* __restrict__ out,
+                                                         long long plane) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int ch = (int)(i % c);
+  const double t = (double)dy[i] - coef[c + ch] - ((double)x[i] - coef[2 * c + ch]) * coef[3 * c + ch];
+  __nv_bfloat16 hi, lo;
+  split_bf16((float)(coef[ch] * t), hi, lo);
+  out[i] = hi;
+  if (passes != 1) out[plane + i] = lo;
+}
+
 }  // namespace
 
 int launch_disc_pool(const __nv_bfloat16* a4, long long plane, int passes, int n, float* out, cudaStream_t st) {
@@ -120,6 +226,37 @@ int launch_disc_head_bwd(const float* dlogits, const float* W, int U, int n, flo
 int launch_disc_cotangent(const float* dpool, int n, float* c4, cudaStream_t st) {
   return launch_pdl(disc_cotangent_kernel, dim3(blocks_of((long long)n * kC4 * kPool)), dim3(256), 0, st, dpool, n, c4) ==
                  cudaSuccess ? 1 : -1;
+}
+
+int launch_disc_bn_sums(const float* u, const float* v, int n, int hw, int c, double count, float eps, double* part, double* sums,
+                        float* mean_f, float* inv_std_f, cudaStream_t st) {
+  disc_bn_partial_kernel<<<dim3((c + 127) / 128, n), 128, 0, st>>>(u, v, hw, c, part);
+  disc_bn_stats_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, n, c, count, eps, sums, mean_f, inv_std_f);
+  return cudaGetLastError() == cudaSuccess ? 2 : -1;
+}
+
+int launch_disc_bn_act(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
+                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st) {
+  disc_bn_act_kernel<<<blocks_of(total), 256, 0, st>>>(x, total, c, mean, inv_std, gamma, beta, passes, out, plane);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_disc_train_cotangent(const float* dpool, const float* x4, int n, const float* mean, const float* inv_std,
+                                const float* gamma, const float* beta, float* dy, cudaStream_t st) {
+  disc_train_cot_kernel<<<blocks_of((long long)n * kPool * kC4), 256, 0, st>>>(dpool, x4, n, mean, inv_std, gamma, beta, dy);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_disc_bn_coef(const double* fsum, const double* bsum, double count, float eps, const float* gamma, int c, double* coef,
+                        cudaStream_t st) {
+  disc_bn_coef_kernel<<<(c + 127) / 128, 128, 0, st>>>(fsum, bsum, count, eps, gamma, c, coef);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_disc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
+                      long long plane, cudaStream_t st) {
+  disc_bn_dx_kernel<<<blocks_of(total), 256, 0, st>>>(x, dy, total, c, coef, passes, out, plane);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 }  // namespace ian

@@ -160,6 +160,9 @@ enum LayerId {
   // the features' vector-Jacobian product (ian_introspect_vjp_*): E_BWD_CONV4..2 with a shallower feature's cotangent
   // joining before the activation derivative (res); built on first use
   IV_BWD_CONV4, IV_BWD_CONV3, IV_BWD_CONV2,
+  // the training-mode discriminator (ian_discriminate_train*): enc_conv2..4 with unit scale, no shift and no activation
+  // into a float32 raw buffer, and E_BWD_CONV4 / E_BWD_CONV3 with unit scale into a float32 buffer; built on first use
+  DT_ENC_CONV2, DT_ENC_CONV3, DT_ENC_CONV4, DT_BWD_CONV4, DT_BWD_CONV3,
   L_COUNT,
   T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
@@ -176,6 +179,8 @@ enum LayerId {
                                                         // prior) and its automatic per-sample scale
   T_DISC_POOL, T_DISC_HEAD, T_DISC_HEAD_BWD, T_DISC_MB, T_DISC_MB_BWD,   // the discriminator head: a4's pool, the dense
   T_DISC_COTANGENT,                                     // layer, their adjoints, the MinibatchLayer, and enc_conv4's cotangent
+  T_DT_STATS, T_DT_NORM, T_DT_COTANGENT, T_DT_BN_BWD, T_DT_BN_DX,   // the training-mode trunk: batch statistics, normalise +
+                                                        // LeakyReLU, the pool's adjoint, BatchNorm backward sums and dx
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -192,12 +197,16 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "jvp_full_dec_conv4", "rgb_head_jvp",
                                     "jvp_enc_conv2", "jvp_enc_conv3", "jvp_enc_conv4", "jvp_enc_fc1", "jvp_enc_head",
                                     "introspect_bwd_enc_conv4", "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2",
+                                    "disc_train_enc_conv2", "disc_train_enc_conv3", "disc_train_enc_conv4",
+                                    "disc_train_bwd_enc_conv4", "disc_train_bwd_enc_conv3",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
                                     "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
                                     "feat_gram", "feat_accept", "feat_cotangent",
                                     "robust_gram", "robust_scale",
-                                    "disc_pool", "disc_head", "disc_head_bwd", "disc_mb", "disc_mb_bwd", "disc_cotangent"};
+                                    "disc_pool", "disc_head", "disc_head_bwd", "disc_mb", "disc_mb_bwd", "disc_cotangent",
+                                    "disc_train_stats", "disc_train_norm", "disc_train_cotangent", "disc_train_bn_bwd",
+                                    "disc_train_bn_dx"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -292,6 +301,11 @@ struct ian_handle {
   // [pool | f], its cotangent, the pool's cotangent, the host forms' logits / p / dlogits, and one chunk's enc_conv4 cotangent
   float* disc_buf = nullptr;
   int disc_cap = 0;
+  // bnorm2..4's gamma | beta (1792 + 1792 floats, uploaded with the encoder), and ian_discriminate_train*'s whole-call
+  // buffers (grown to the largest batch asked for, disc_tcap samples; see TrainBufs)
+  float* enc_bn_gb = nullptr;
+  char* disc_tbuf = nullptr;
+  int disc_tcap = 0;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -408,6 +422,9 @@ struct Plan {
   // cotangents of a1..a3 as split planes NHWC, the res operand of IV_BWD_CONV2..4 (0.92 MB per image)
   bool ivjp = false;
   Planes ivc[3];
+  // the training-mode discriminator's tap-GEMM twins (DT_ENC_CONV2..4 on the first ian_discriminate_train* call on the plan,
+  // DT_BWD_CONV4..3 with the encoder VJP's planes on the first ian_discriminate_train_vjp_* call)
+  bool dtrain = false, dtrain_vjp = false;
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -1060,6 +1077,18 @@ int prepare_encoder(ian_handle* h) {
         for (int t = 0; t < 25; ++t) B[((size_t)t * c.Cout + o) * c.Cin + ci] = W[((size_t)o * c.Cin + ci) * 25 + t];
     fold_bn(h, c.bn, c.Cout, sc, sf);
     if ((rc = upload_gemm_weights(h, c.l, B, 25, c.Cout, c.Cin, sc, sf)) != IAN_OK) return rc;
+  }
+  {   // bnorm2..4's gamma | beta for the training-mode discriminator, which normalises with the batch's statistics
+    std::vector<float> gb(2 * 1792);
+    int off = 0;
+    for (auto& c : convs) {
+      const auto& ga = P(h, (std::string(c.bn) + ".gamma").c_str()).data;
+      const auto& be = P(h, (std::string(c.bn) + ".beta").c_str()).data;
+      std::copy(ga.begin(), ga.begin() + c.Cout, gb.begin() + off);
+      std::copy(be.begin(), be.begin() + c.Cout, gb.begin() + 1792 + off);
+      off += c.Cout;
+    }
+    if ((rc = put_dev(h, h->enc_bn_gb, gb.data(), gb.size() * sizeof(float))) != IAN_OK) return rc;
   }
   // enc_fc1: rows of W are flatten(NCHW) = c*16 + hw; our A is NHWC = hw*1024 + c.  Cout 1000 -> 1024.
   {
@@ -2828,6 +2857,244 @@ int call_discriminate_vjp(ian_handle* h, bool host, const float* x, int n, const
   });
 }
 
+// ---- the discriminator in training mode (DESIGN section 5.6o) ----------------------------------------------------------
+// l_discrim under deterministic=False: bnorm2..4 normalise with the batch's statistics, so the trunk couples the call's
+// samples at three more points than the MinibatchLayer does and runs layer by layer over the whole call.  For each of
+// enc_conv2..4: per chunk, the layer's twin (unit scale, no shift, no activation) writes its raw sums into a whole-call float32
+// buffer; over the call, per-image float64 sums added in image order give mean and inv_std (so they do not depend on
+// IAN_CHUNK); per chunk again disc_bn_act writes the next layer's input planes.  The head then runs as in inference.
+// The VJP keeps the forward's raw buffers and recomputes each chunk's activation planes (the masks of the backward GEMMs)
+// from them: the pool's adjoint times lrelu'(y4); per layer whole-call float64 Σdy, Σdy·x, then per chunk dx as split planes
+// and the backward GEMM's twin (unit scale, the training-mode activations as LeakyReLU masks) into a float32 buffer;
+// enc_conv2's backward (its scale is 1 already) and enc_conv1's adjoint end the chain on the chunk's planes.
+constexpr int kTrainC[3] = {256, 512, 1024}, kTrainHW[3] = {256, 64, 16}, kTrainOff[3] = {0, 256, 768};
+constexpr long long kTrainElems[3] = {65536, 32768, 16384};   // per image, enc_conv2..4's outputs
+constexpr float kBnEps = 1e-4f;
+
+// raw[l]: enc_conv{l+2}'s raw sums (n,HW,C); dy[0] (the size of raw[0]) holds dy of bnorm4, then bnorm2; dy[1] bnorm3's;
+// part: the per-image partial sums; fsum: the forward's [2][C] per layer; bsum: the backward's; coef: [4][1024];
+// stats: [2][1792] float32, the means of bnorm2 | bnorm3 | bnorm4, then their inv_std
+struct TrainBufs {
+  float *raw[3], *dy[2], *stats;
+  double *part, *fsum, *bsum, *coef;
+};
+
+int ensure_train_bufs(ian_handle* h, int n, TrainBufs* b) {
+  const long long per_img = 2 * kTrainElems[0] + 2 * kTrainElems[1] + kTrainElems[2];   // floats
+  if (n > h->disc_tcap) {
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaFree(h->disc_tbuf));
+    h->disc_tbuf = nullptr;
+    h->disc_tcap = 0;
+    const size_t bytes = (size_t)n * (per_img * sizeof(float) + 2 * 1024 * sizeof(double)) +
+                         (2 * 1792 + 2 * 1024 + 4 * 1024) * sizeof(double) + 2 * 1792 * sizeof(float);
+    CUDA_TRY(h, cudaMalloc((void**)&h->disc_tbuf, bytes));
+    h->disc_tcap = n;
+  }
+  const long long N = h->disc_tcap;
+  double* d = (double*)h->disc_tbuf;
+  b->part = d;
+  b->fsum = b->part + N * 2 * 1024;
+  b->bsum = b->fsum + 2 * 1792;
+  b->coef = b->bsum + 2 * 1024;
+  float* f = (float*)(b->coef + 4 * 1024);
+  b->stats = f;
+  b->raw[0] = f + 2 * 1792;
+  b->raw[1] = b->raw[0] + N * kTrainElems[0];
+  b->raw[2] = b->raw[1] + N * kTrainElems[1];
+  b->dy[0] = b->raw[2] + N * kTrainElems[2];
+  b->dy[1] = b->dy[0] + N * kTrainElems[0];
+  return IAN_OK;
+}
+
+// the twins share the originals' B tiles, taps and split-K slabs (the two never run at once); only the epilogue differs
+int build_twin(ian_handle* h, Plan* pl, int to, int from) {
+  TapGemm& g = pl->g[to];
+  g = pl->g[from];
+  g.scale = nullptr; g.shift = nullptr; g.out = nullptr; g.out_plane = 0; g.out_f32 = nullptr;
+  if (g.act != ACT_MASK) g.act = ACT_NONE;
+  char err[256] = {0};
+  if (!(pl->maps[to] = tc_build_maps(g, err, sizeof(err)))) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[to], err);
+  return IAN_OK;
+}
+
+template <bool kVjp>
+int ensure_disc_train_plan(ian_handle* h, Plan* pl) {
+  int rc;
+  if (!pl->dtrain) {
+    for (int k = 0; k < 3; ++k)
+      if ((rc = build_twin(h, pl, DT_ENC_CONV2 + k, kEncoder.l[k])) != IAN_OK) return rc;
+    pl->dtrain = true;
+  }
+  if (kVjp && !pl->dtrain_vjp) {
+    if ((rc = ensure_enc_vjp_plan(h, pl)) != IAN_OK) return rc;
+    if ((rc = build_twin(h, pl, DT_BWD_CONV4, E_BWD_CONV4)) != IAN_OK || (rc = build_twin(h, pl, DT_BWD_CONV3, E_BWD_CONV3)) != IAN_OK)
+      return rc;
+    pl->dtrain_vjp = true;
+  }
+  return IAN_OK;
+}
+
+int run_gemm_into(ian_handle* h, Plan* pl, int l, float* out, cudaStream_t st) {
+  pl->g[l].out_f32 = out;
+  return run_gemm(h, pl, l, st);
+}
+
+// bnorm{l+2}'s batch-normalised, LeakyReLU'd output of the chunk at `off` -> the planes `a`
+int train_act(ian_handle* h, const TrainBufs& b, int l, int off, int cn, const Planes& a, cudaStream_t st) {
+  ScopedTimer tm(h, T_DT_NORM, st);
+  const float* gb = h->enc_bn_gb;
+  LAUNCH_TRY(h, launch_disc_bn_act(b.raw[l] + off * kTrainElems[l], cn * kTrainElems[l], kTrainC[l], b.stats + kTrainOff[l],
+                                   b.stats + 1792 + kTrainOff[l], gb + kTrainOff[l], gb + 1792 + kTrainOff[l], h->passes, a.p,
+                                   a.plane, st));
+  return IAN_OK;
+}
+
+// u = v = raw[l] (forward: statistics into b.stats) or u = dy, v = raw[l] (backward: Σdy, Σdy·x into b.bsum, then coef)
+int train_sums(ian_handle* h, const TrainBufs& b, int l, int n, const float* dy, cudaStream_t st) {
+  const double count = (double)n * kTrainHW[l];
+  ScopedTimer tm(h, dy ? T_DT_BN_BWD : T_DT_STATS, st);
+  if (!dy) {
+    LAUNCH_TRY(h, launch_disc_bn_sums(b.raw[l], b.raw[l], n, kTrainHW[l], kTrainC[l], count, kBnEps, b.part, b.fsum + 2 * kTrainOff[l],
+                                      b.stats + kTrainOff[l], b.stats + 1792 + kTrainOff[l], st));
+    return IAN_OK;
+  }
+  LAUNCH_TRY(h, launch_disc_bn_sums(dy, b.raw[l], n, kTrainHW[l], kTrainC[l], 0.0, kBnEps, b.part, b.bsum, nullptr, nullptr, st));
+  LAUNCH_TRY(h, launch_disc_bn_coef(b.fsum + 2 * kTrainOff[l], b.bsum, count, kBnEps, h->enc_bn_gb + kTrainOff[l], kTrainC[l], b.coef, st));
+  return IAN_OK;
+}
+
+// the whole forward to the pooled features b.pool: enc_conv1 and the three training-mode layers, then a4's pool
+template <bool kVjp>
+int disc_train_trunk(ian_handle* h, bool host, const float* x, int n, const DiscBufs& d, const TrainBufs& b, void* stream) {
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  int rc = run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}}, ensure_disc_train_plan<kVjp>, [&](const Chunk& c) {
+    const int r = run_introspect(h, c.pl, c.f(0), c.st, 1);
+    return r != IAN_OK ? r : run_gemm_into(h, c.pl, DT_ENC_CONV2, b.raw[0] + c.off * kTrainElems[0], c.st);
+  });
+  if (rc != IAN_OK || (rc = train_sums(h, b, 0, n, nullptr, st)) != IAN_OK) return rc;
+  for (int l = 1; l < 3; ++l) {
+    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+      int r = ensure_disc_train_plan<kVjp>(h, pl);
+      if (r == IAN_OK) r = train_act(h, b, l - 1, off, cn, l == 1 ? pl->a2 : pl->a3, st);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, DT_ENC_CONV2 + l, b.raw[l] + off * kTrainElems[l], st);
+    });
+    if (rc != IAN_OK || (rc = train_sums(h, b, l, n, nullptr, st)) != IAN_OK) return rc;
+  }
+  return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+    const int r = train_act(h, b, 2, off, cn, pl->a4, st);
+    if (r != IAN_OK) return r;
+    ScopedTimer tm(h, T_DISC_POOL, st);
+    LAUNCH_TRY(h, launch_disc_pool(pl->a4.p, pl->a4.plane, h->passes, cn, d.pool + (size_t)off * 1024, st));
+    return (int)IAN_OK;
+  });
+}
+
+int call_discriminate_train(ian_handle* h, bool host, const float* x, int n, float* logits, float* p, float* stats, void* stream) {
+  int rc = check_discriminate(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !logits) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  const int U = disc_units(h);
+  DiscBufs d;
+  TrainBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_train_bufs(h, n, &b)) != IAN_OK ||
+      (rc = ensure_train_ws(h, mb_workspace_bytes(n, kDiscKernels, kDiscDims))) != IAN_OK ||
+      (rc = disc_train_trunk<false>(h, host, x, n, d, b, stream)) != IAN_OK)
+    return rc;
+  float* lo = host ? d.logits : logits;
+  float* po = !p ? nullptr : host ? d.p : p;
+  {
+    ScopedTimer tm(h, T_DISC_MB, st);
+    LAUNCH_TRY(h, launch_minibatch_discrim(d.pool, n, 1024, h->disc_w[0], h->disc_w[1], h->disc_w[2], kDiscKernels, kDiscDims, d.in,
+                                           h->train_ws, st));
+  }
+  {
+    ScopedTimer tm(h, T_DISC_HEAD, st);
+    LAUNCH_TRY(h, launch_disc_head(d.in, h->disc_w[3], U, n, lo, po, st));
+  }
+  const cudaMemcpyKind k = host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  if (stats) CUDA_TRY(h, cudaMemcpyAsync(stats, b.stats, 2 * 1792 * sizeof(float), k, st));
+  if (!host) return IAN_OK;
+  CUDA_TRY(h, cudaMemcpyAsync(logits, lo, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (p) CUDA_TRY(h, cudaMemcpyAsync(p, po, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
+}
+
+// 1 forward + 1 backward: the forward's raw buffers stay for the backward, whose masks are recomputed per chunk from them
+int call_discriminate_train_vjp(ian_handle* h, bool host, const float* x, int n, const float* dlogits, float* dx, void* stream) {
+  int rc = check_discriminate(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!x || !dlogits || !dx) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  const int U = disc_units(h);
+  DiscBufs d;
+  TrainBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_train_bufs(h, n, &b)) != IAN_OK ||
+      (rc = ensure_train_ws(h, mb_bwd_workspace_bytes(n, 1024, kDiscKernels, kDiscDims))) != IAN_OK ||
+      (rc = disc_train_trunk<true>(h, host, x, n, d, b, stream)) != IAN_OK)
+    return rc;
+  const float* dl = dlogits;
+  if (host) {
+    CUDA_TRY(h, cudaMemcpyAsync(d.dlogits, dlogits, (size_t)n * U * sizeof(float), cudaMemcpyHostToDevice, st));
+    dl = d.dlogits;
+  }
+  {
+    ScopedTimer tm(h, T_DISC_HEAD_BWD, st);
+    LAUNCH_TRY(h, launch_disc_head_bwd(dl, h->disc_w[3], U, n, d.g, st));
+  }
+  {
+    ScopedTimer tm(h, T_DISC_MB_BWD, st);
+    LAUNCH_TRY(h, launch_minibatch_discrim_bwd(d.pool, n, 1024, h->disc_w[0], h->disc_w[1], kDiscKernels, kDiscDims, d.g, d.dpool,
+                                               nullptr, nullptr, nullptr, h->train_ws, st));
+  }
+  {
+    ScopedTimer tm(h, T_DT_COTANGENT, st);
+    const float* gb = h->enc_bn_gb;
+    LAUNCH_TRY(h, launch_disc_train_cotangent(d.dpool, b.raw[2], n, b.stats + kTrainOff[2], b.stats + 1792 + kTrainOff[2],
+                                              gb + kTrainOff[2], gb + 1792 + kTrainOff[2], b.dy[0], st));
+  }
+  // bnorm4 -> a3 (dy of bnorm3 into dy[1]), bnorm3 -> a2 (dy of bnorm2 into dy[0])
+  const int bwd[2] = {DT_BWD_CONV4, DT_BWD_CONV3};
+  for (int l = 2; l >= 1; --l) {
+    const float* dy = b.dy[l == 2 ? 0 : 1];
+    float* dy_next = b.dy[l == 2 ? 1 : 0];
+    if ((rc = train_sums(h, b, l, n, dy, st)) != IAN_OK) return rc;
+    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+      const Planes& e = l == 2 ? pl->e4 : pl->e3;
+      {
+        ScopedTimer tm(h, T_DT_BN_DX, st);
+        LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[l] + off * kTrainElems[l], dy + off * kTrainElems[l], cn * kTrainElems[l], kTrainC[l], b.coef,
+                                        h->passes, e.p, e.plane, st));
+      }
+      const int r = train_act(h, b, l - 1, off, cn, l == 2 ? pl->a3 : pl->a2, st);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, bwd[2 - l], dy_next + off * kTrainElems[l - 1], st);
+    });
+    if (rc != IAN_OK) return rc;
+  }
+  if ((rc = train_sums(h, b, 0, n, b.dy[0], st)) != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {dx, kImageBytes, S_XHAT, OUT}}, ensure_disc_train_plan<true>,
+                   [&](const Chunk& c) {
+    {
+      ScopedTimer tm(h, T_DT_BN_DX, c.st);
+      LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[0] + c.off * kTrainElems[0], b.dy[0] + c.off * kTrainElems[0], c.cn * kTrainElems[0],
+                                      kTrainC[0], b.coef, h->passes, c.pl->e2.p, c.pl->e2.plane, c.st));
+    }
+    int r = run_introspect(h, c.pl, c.f(0), c.st, 1);     // a1: the mask of enc_conv2's backward
+    if (r == IAN_OK) r = run_gemm(h, c.pl, E_BWD_CONV2, c.st);
+    if (r != IAN_OK) return r;
+    ScopedTimer tm(h, T_CONV1_BWD, c.st);
+    if (h->path == IAN_PATH_TC)
+      LAUNCH_TRY(h, launch_conv1_bwd_tc(c.pl->conv1_bwd_maps, c.f(1), c.cn, c.st));
+    else
+      LAUNCH_TRY(h, launch_conv1_bwd(c.pl->e1.p, c.pl->e1.plane, h->conv1_bwd_wt, c.f(1), c.cn, c.st));
+    return (int)IAN_OK;
+  });
+}
+
 // E(z) = a |x_hat - x|^2 + sum_l c_l |g_l(x_hat) - g_l(x)|^2 with c_l = 3072 b / M_l (b * 12288 * l_f, l_f the per-sample
 // feature loss of train_IAN.py:244).  J_l = (d g_l / d x)(x_hat) J comes from the truncated encoder JVP on the batch-100
 // plan, with the decoder JVP's 100 rows x_hat as primal and J's columns as tangents.  The stored features g(x) and
@@ -3305,6 +3572,8 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->gn_eye); cudaFree(h->gn_zrep); cudaFree(h->gn_J); cudaFree(h->gn_part); cudaFree(h->map_flow); cudaFree(h->feat_part);
   for (float* p : h->disc_w) cudaFree(p);
   cudaFree(h->disc_buf);
+  cudaFree(h->enc_bn_gb);
+  cudaFree(h->disc_tbuf);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -3568,6 +3837,18 @@ int ian_discriminate_vjp_dev(ian_handle* h, const float* x, int n, const float* 
 }
 int ian_discriminate_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx) {
   return call_discriminate_vjp(h, true, x, n, dlogits, dx, nullptr);
+}
+int ian_discriminate_train_dev(ian_handle* h, const float* x, int n, float* logits, float* p, float* stats, void* stream) {
+  return call_discriminate_train(h, false, x, n, logits, p, stats, stream);
+}
+int ian_discriminate_train_host(ian_handle* h, const float* x, int n, float* logits, float* p, float* stats) {
+  return call_discriminate_train(h, true, x, n, logits, p, stats, nullptr);
+}
+int ian_discriminate_train_vjp_dev(ian_handle* h, const float* x, int n, const float* dlogits, float* dx, void* stream) {
+  return call_discriminate_train_vjp(h, false, x, n, dlogits, dx, stream);
+}
+int ian_discriminate_train_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx) {
+  return call_discriminate_train_vjp(h, true, x, n, dlogits, dx, nullptr);
 }
 int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
                                  double* A, double* g, double* e, void* stream) {

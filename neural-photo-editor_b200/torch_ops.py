@@ -23,10 +23,11 @@
     of train_IAN.py:244 built on it, so feature_loss(model, decode(model, z), x).sum().backward() drives z -- or, with
     params, the IAN_simple decoder's parameters -- under the generator's own reconstruction objective.
 
-  * discriminate(model, x) = the logits of the IAN's discriminator head l_discrim (what model.discriminate(x,
+  * discriminate(model, x, training=False) = the logits of the IAN's discriminator head l_discrim (what model.discriminate(x,
     return_logits=True) returns) as a differentiable torch op; F.logsigmoid / log_softmax of them is the realism score.  Its
     backward is one ian_discriminate_vjp_dev call over the whole batch: the MinibatchLayer couples the samples, so a
-    loss on one sample's logits moves every image of the call.  Reverse mode only.
+    loss on one sample's logits moves every image of the call.  Reverse mode only.  training=True evaluates it as the
+    reference's trainers do (batch-statistics BatchNorm in the trunk), for the generator's adversarial term.
 
   * decoder_parameters(model, weights) + decode(model, z, params): the IAN_simple decoder's 13 trainable tensors
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
@@ -374,7 +375,7 @@ def _discriminate_function():
 
     class Discriminate(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, model, x):
+        def forward(ctx, model, x, training):
             _check_tensor(model, x, "x")
             if x.dim() != 4 or tuple(x.shape[1:]) != (3, 64, 64):
                 raise ValueError("x must be (n,3,64,64), got %r" % (tuple(x.shape),))
@@ -383,8 +384,12 @@ def _discriminate_function():
             logits = torch.empty(n, model.discriminator_units(), dtype=torch.float32, device=x.device)
             if n:
                 with _lib_stream(model, x) as st:
-                    model.discriminate_dev(x.data_ptr(), n, logits.data_ptr(), 0, st)
+                    if training:
+                        model.discriminate_train_dev(x.data_ptr(), n, logits.data_ptr(), 0, 0, st)
+                    else:
+                        model.discriminate_dev(x.data_ptr(), n, logits.data_ptr(), 0, st)
             ctx.model = model
+            ctx.training = training
             ctx.save_for_backward(x)
             return logits
 
@@ -399,8 +404,9 @@ def _discriminate_function():
             dx = torch.empty_like(x)
             if n:
                 with _lib_stream(model, x) as st:
-                    model.discriminate_vjp_dev(x.data_ptr(), g.data_ptr(), n, dx.data_ptr(), st)
-            return None, dx
+                    vjp = model.discriminate_train_vjp_dev if ctx.training else model.discriminate_vjp_dev
+                    vjp(x.data_ptr(), g.data_ptr(), n, dx.data_ptr(), st)
+            return None, dx, None
 
         @staticmethod
         def jvp(ctx, *tangents):
@@ -410,12 +416,15 @@ def _discriminate_function():
     return Discriminate
 
 
-def discriminate(model, x):
+def discriminate(model, x, training=False):
     """logits (n,U) of the discriminator head for x (n,3,64,64) float32 CUDA on the model's device, after
     model.load_discriminator(): U = 1 (sigmoid) on IAN_simple / IANv1, 3 (softmax: real, reconstruction, generated) on IAN.py.
     Differentiable w.r.t. x in reverse mode (one ian_discriminate_vjp_dev per backward: two trunk forwards and one
-    backward).  The batch is coupled: every sample's logits depend on every image of the call."""
-    return _discriminate_function().apply(model, x)
+    backward).  The batch is coupled: every sample's logits depend on every image of the call.
+    training=True: l_discrim as the reference's trainers evaluate it (deterministic=False): bnorm2..4 normalise with the
+    batch's statistics, and the backward (ian_discriminate_train_vjp_dev: one trunk forward and one backward) flows through
+    them.  The model's running statistics are neither used nor changed."""
+    return _discriminate_function().apply(model, x, bool(training))
 
 
 def _params_function():
