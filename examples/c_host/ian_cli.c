@@ -92,7 +92,9 @@ static int symbols(void) {
       (anyfn)ian_bn_backward_sums_dev, (anyfn)ian_bn_backward_dx_dev, (anyfn)ian_minibatch_discrim_bwd_dev,
       (anyfn)ian_set_discriminator_param, (anyfn)ian_discriminate_dev, (anyfn)ian_discriminate_host,
       (anyfn)ian_discriminate_vjp_dev, (anyfn)ian_discriminate_vjp_host, (anyfn)ian_discriminate_train_dev,
-      (anyfn)ian_discriminate_train_host, (anyfn)ian_discriminate_train_vjp_dev, (anyfn)ian_discriminate_train_vjp_host};
+      (anyfn)ian_discriminate_train_host, (anyfn)ian_discriminate_train_vjp_dev, (anyfn)ian_discriminate_train_vjp_host,
+      (anyfn)ian_decode_train_dev, (anyfn)ian_decode_train_host, (anyfn)ian_decode_train_vjp_dev,
+      (anyfn)ian_decode_train_vjp_host};
   size_t i, n = sizeof(fn) / sizeof(fn[0]);
   for (i = 0; i < n; ++i)
     if (!fn[i]) return 1;

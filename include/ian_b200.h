@@ -528,6 +528,37 @@ int ian_decode_param_vjp_host(ian_handle* h, const float* z, const float* dx_hat
  * Other names -> IAN_ERR_INVALID; not finalized -> IAN_ERR_STATE; IAN_MODEL_FULL / IAN_MODEL_V1 -> IAN_ERR_UNSUPPORTED. */
 int ian_update_param_host(ian_handle* h, const char* name, const float* data, const int64_t* shape, int ndim);
 
+/* ---- the IAN_simple decoder in training mode: get_output(l_out, {l_Z: z}) under deterministic=False, as the reference's
+ * trainers build X_hat and the generated samples (train_IAN_simple.py:217-224, 253) ------------------------------------
+ * ian_decode_train_*: x_hat (n,3,64,64) float32 NCHW for z (n,100), with bnorm_dec_fc2 and bnorm_dc1..3 normalising with
+ *   the BATCH's statistics: bnorm_dec_fc2 each of its 16384 features over the n samples, bnorm_dc1..3 each channel over
+ *   (n, h, w); biased variance, inv_std = 1/sqrt(var + 1e-4), y = (x - mean) (gamma inv_std) + beta, then rectify.
+ *   The handle's running mean / inv_std are neither used nor changed.
+ *   stats (nullable) receives the statistics used, float32 (2,17280): row 0 the means of bnorm_dec_fc2 (16384, in the
+ *   reference's feature order) | bnorm_dc1 (512) | bnorm_dc2 (256) | bnorm_dc3 (128), row 1 their inv_std.  Lasagne's
+ *   running-average update, r <- 0.9 r + 0.1 batch for both mean and inv_std, is the caller's to apply
+ *   (ian_update_param_host).
+ * ian_decode_train_vjp_*: dz (n,100, nullable) = (d x_hat / d z)^T dx_hat through the batch statistics, and the gradients
+ *   of ian_decode_param_vjp_*'s 13 tensors on this graph: grads indexed and laid out as there, with its error rules (a
+ *   pointer for a parameter without a gradient -> IAN_ERR_INVALID).  Weight gradients run only for the tensors asked for.
+ *   1 forward + 1 backward.
+ * The sums are float64 per image, added in image order: the statistics, x_hat and dz do not depend on IAN_CHUNK; the
+ * weight gradients add the chunks in chunk order.
+ * BATCH COUPLING: one sample's z changes every sample's x_hat, and one non-finite z makes every output non-finite.  At
+ *   n == 1 bnorm_dec_fc2 sees a single sample, so x_hat = h(beta) does not depend on z: dz and l_dec_fc2.W's gradient are
+ *   exactly 0.
+ * IAN_MODEL_FULL / IAN_MODEL_V1 -> IAN_ERR_UNSUPPORTED; n == 0 does nothing.  Float32 on both paths.  Deterministic.  No
+ *   CUDA graphs.
+ * Memory: whole-call buffers of 2.1 MB per image (the four layers' raw sums, 245 760 floats, their cotangents of the same
+ *   size, and 256 KB of float64 partial sums) plus 0.9 MB fixed, grown to the largest batch asked for; the VJP also
+ *   allocates ian_decode_param_vjp_*'s buffers on each chunk's plan. */
+int ian_decode_train_dev(ian_handle* h, const float* z, int n, float* x_hat, float* stats /*nullable*/, void* stream);
+int ian_decode_train_host(ian_handle* h, const float* z, int n, float* x_hat, float* stats /*nullable*/);
+int ian_decode_train_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz /*nullable*/,
+                             float* const* grads /*nullable*/, void* stream);
+int ian_decode_train_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz /*nullable*/,
+                              float* const* grads /*nullable*/);
+
 /* ---- encoder vector-Jacobian product: reverse mode through the encoder from the image (reference Z_hat, API.py:50) ------
  *   dx = (d z / d x)^T . dz
  * x (n,3,64,64) float32 NCHW, eps (n,100) nullable, dz (n,100), dx (n,3,64,64).  z is exactly what ian_encode_* returns for
@@ -633,7 +664,11 @@ int ian_minibatch_discrim_bwd_dev(ian_handle* h, const float* x, int n, int d, c
  * its nonlinearity), and in ian_discriminate_vjp_* also "disc_head_bwd", "disc_mb_bwd" and "disc_cotangent" (enc_conv4's
  * cotangent, per chunk) next to the trunk's own layers; in ian_discriminate_train* "disc_train_enc_conv2..4" (the
  * layers' raw sums), "disc_train_stats", "disc_train_norm" (BatchNorm + LeakyReLU into the next layer's planes), and in the
- * VJP also "disc_train_cotangent", "disc_train_bn_bwd" (Σdy, Σdy·x), "disc_train_bn_dx", "disc_train_bwd_enc_conv4..3") over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
+ * VJP also "disc_train_cotangent", "disc_train_bn_bwd" (Σdy, Σdy·x), "disc_train_bn_dx", "disc_train_bwd_enc_conv4..3"; in
+ * ian_decode_train* "dec_train_l_dec_fc2", "dec_train_dec_conv1..3" (the layers' raw sums), "dec_train_stats",
+ * "dec_train_norm" (BatchNorm + rectify into the next layer's planes) and "dec_out", and in the VJP also "brush_seed",
+ * "dec_train_cotangent" (bnorm_dc3's dy), "dec_train_bn_bwd" (Σdy, Σdy·x), "dec_train_bn_grads" (d beta, d gamma),
+ * "dec_train_bn_dx", "dec_train_bwd_dec_conv3..1" and the "wgrad_*" of ian_decode_param_vjp_*) over the launches since the last reset; returns <0 if the layer was never timed.  Timing is enabled with ian_set_layer_timing(h, 1). */
 int ian_set_layer_timing(ian_handle* h, int enable);
 double ian_layer_time_ms(ian_handle* h, const char* layer_name, int reset);
 

@@ -20,7 +20,9 @@ space `gauss_newton_map` / `fit_latent_map` (masked fits and inpainting), the IA
 `introspect_jvp` / `introspect_vjp` / `feature_loss` (torch binding: `torch_ops.introspect` / `torch_ops.feature_loss`) and
 the fit under its feature-wise loss `gauss_newton_features` / `fit_latent_features`, the discriminator head l_discrim
 `load_discriminator` / `discriminate` / `discriminate_vjp` and their training-mode forms `discriminate_train` /
-`discriminate_train_vjp` (torch binding: `torch_ops.discriminate`), and `*_dev` variants taking device pointers.
+`discriminate_train_vjp` (torch binding: `torch_ops.discriminate`), the IAN_simple decoder in training mode
+`decode_train` / `decode_train_vjp` (torch binding: `torch_ops.decode(..., training=True)`), and `*_dev` variants taking
+device pointers.
 """
 from __future__ import annotations
 
@@ -814,6 +816,43 @@ class IAN:
         self._check(self._lib.ian_decode_param_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz), ptrs))
         return dz, grads
 
+    def decode_train(self, z, return_stats=False):
+        """The IAN_simple decoder in training mode (deterministic=False, as train_IAN_simple.py:217-224 builds X_hat):
+        bnorm_dec_fc2 and bnorm_dc1..3 normalise with the batch's mean and biased variance, inv_std = 1/sqrt(var + 1e-4);
+        the running statistics are neither used nor changed.  z float32 (n,100) -> x_hat (n,3,64,64); with return_stats
+        also stats float32 (2,17280): row 0 the batch means of bnorm_dec_fc2 (reference feature order) | bnorm_dc1 |
+        bnorm_dc2 | bnorm_dc3, row 1 their inv_std (for Lasagne's running-average update, alpha = 0.1, which is the
+        caller's: update_params).  The batch is coupled: every sample's x_hat depends on every z of the call."""
+        z = _z(z)
+        n = z.shape[0]
+        x = np.empty((n, 3, 64, 64), np.float32)
+        stats = np.empty((2, 17280), np.float32)
+        if n:
+            self._check(self._lib.ian_decode_train_host(self._h, _fp(z), n, _fp(x), _fp(stats)))
+        else:
+            stats.fill(np.nan)
+        return (x, stats) if return_stats else x
+
+    def decode_train_vjp(self, z, dx_hat, grads=True):
+        """Reverse mode through decode_train(): (dz (n,100), {name: dL/dparam}) for dx_hat = dL/dx_hat (n,3,64,64), the
+        gradient flowing through the batch statistics as Theano's T.grad gives it.  grads: True (every name of
+        param_vjp_names()), False (none) or an iterable of names; weight gradients run only for those.  1 forward + 1
+        backward."""
+        z = _z(z)
+        dx = _img(dx_hat, 'dx_hat')
+        n = z.shape[0]
+        if dx.shape[0] != n:
+            raise ValueError("dx_hat must be (%d,3,64,64), got %r" % (n, dx.shape))
+        names = self.param_vjp_names() if grads is True else [] if grads is False else list(grads)
+        specs, index = self._param_slots(names)
+        out = {name: np.zeros(specs[index[name]][1], np.float32) for name in names}
+        dz = np.zeros_like(z)
+        ptrs = (C.c_void_p * len(specs))()
+        for name, g in out.items():
+            ptrs[index[name]] = g.ctypes.data
+        self._check(self._lib.ian_decode_train_vjp_host(self._h, _fp(z), _fp(dx), n, _fp(dz), ptrs))
+        return dz, out
+
     def update_params(self, params):
         """Replace IAN_simple decoder parameters of this finalized model in place: {name: array in the reference shape}
         for any of param_vjp_names() and bnorm_dec_fc2 / bnorm_dc1..3 .mean / .inv_std.  Afterwards every call computes
@@ -1066,6 +1105,19 @@ class IAN:
         for name, p in grad_ptrs.items():
             ptrs[index[name]] = p
         self._check(self._lib.ian_decode_param_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr or None, ptrs, stream or None))
+
+    def decode_train_dev(self, z_ptr, n, x_ptr, stats_ptr=0, stream=0):
+        """decode_train() on device pointers: x_hat (n,3,64,64) and stats (2,17280) float32 (0: not wanted)"""
+        self._check(self._lib.ian_decode_train_dev(self._h, z_ptr, int(n), x_ptr, stats_ptr or None, stream or None))
+
+    def decode_train_vjp_dev(self, z_ptr, dx_ptr, n, dz_ptr, grad_ptrs, stream=0):
+        """decode_train_vjp() on device pointers: grad_ptrs {name: device pointer} (any subset of param_vjp_names()),
+        dz_ptr may be 0."""
+        specs, index = self._param_slots(grad_ptrs)
+        ptrs = (C.c_void_p * len(specs))()
+        for name, p in grad_ptrs.items():
+            ptrs[index[name]] = p
+        self._check(self._lib.ian_decode_train_vjp_dev(self._h, z_ptr, dx_ptr, int(n), dz_ptr or None, ptrs, stream or None))
 
     def encode_vjp_dev(self, x_ptr, dz_ptr, n, dx_ptr, eps_ptr=0, stream=0):
         self._check(self._lib.ian_encode_vjp_dev(self._h, x_ptr, int(n), eps_ptr or None, dz_ptr, dx_ptr, stream or None))

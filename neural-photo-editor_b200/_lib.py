@@ -115,6 +115,10 @@ SIGNATURES = {
     "ian_param_vjp_supported": (C.c_int, [C.c_int, C.c_int]),
     "ian_decode_param_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_decode_param_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),
+    "ian_decode_train_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_decode_train_host": (C.c_int, [_H, _F, C.c_int, _F, _F]),
+    "ian_decode_train_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ian_decode_train_vjp_host": (C.c_int, [_H, _F, _F, C.c_int, _F, C.c_void_p]),
     "ian_update_param_host": (C.c_int, [_H, C.c_char_p, _F, C.POINTER(C.c_int64), C.c_int]),
     "ian_encode_vjp_dev": (C.c_int, [_H, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ian_encode_vjp_host": (C.c_int, [_H, _F, C.c_int, _F, _F, _F]),

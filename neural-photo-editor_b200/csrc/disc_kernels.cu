@@ -18,6 +18,15 @@
 //   disc_train_cot   : the pool's adjoint times lrelu'(y4): dy4 = d pool / 16 * (y4 > 0 ? 1 : 0.2), float32
 //   disc_bn_coef     : bn_bwd_coef_kernel's coefficients from the whole-call sums
 //   disc_bn_dx       : dx per element in float64, rounded once as bn_bwd_apply_kernel does -> split planes
+//
+// The IAN_simple decoder in training mode (ian_decode_train*; DESIGN section 5.6p) uses disc_bn_partial / disc_bn_stats /
+// disc_bn_coef / disc_bn_dx on l_dec_fc2 and dec_conv1..3's raw sums (l_dec_fc2: hw = 1, c = 16384 library columns), and:
+//   dec_bn_relu      : disc_bn_act with rectify in place of LeakyReLU(0.2)
+//   dec_train_dy     : dy = dL/dh (hi + lo of split planes) * (y > 0), float32: bnorm_dc3's cotangent from the seed kernel
+//   dec_bn_grads     : d beta = Σdy, d gamma = inv_std (Σdy·x - mean Σdy) in float64 from the whole-call sums, written in
+//                      the reference's feature order
+//   dec_stats_out    : the statistics in the reference's feature order
+// bnorm_dec_fc2's library column c = hw 1024 + ch is the reference's feature ch 16 + hw.
 #include "edge.h"
 
 namespace ian {
@@ -206,6 +215,54 @@ __global__ void __launch_bounds__(256) disc_bn_dx_kernel(const float* __restrict
   if (passes != 1) out[plane + i] = lo;
 }
 
+__global__ void __launch_bounds__(256) dec_bn_relu_kernel(const float* __restrict__ x, long long total, int c, const float* __restrict__ mean,
+                                                          const float* __restrict__ inv_std, const float* __restrict__ gamma,
+                                                          const float* __restrict__ beta, int passes, __nv_bfloat16* __restrict__ out,
+                                                          long long plane) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float y = bn_train_y(x[i], (int)(i % c), mean, inv_std, gamma, beta);
+  const float a = fmaf(0.5f, fabsf(y), 0.5f * y);       // rectify as the tap-GEMM epilogue forms it
+  __nv_bfloat16 hi, lo;
+  split_bf16(a, hi, lo);
+  out[i] = hi;
+  if (passes != 1) out[plane + i] = lo;
+}
+
+__global__ void __launch_bounds__(256) dec_train_dy_kernel(const __nv_bfloat16* __restrict__ dh, long long plane,
+                                                           const float* __restrict__ x, long long total, int c,
+                                                           const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                                           const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                           float* __restrict__ dy) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float y = bn_train_y(x[i], (int)(i % c), mean, inv_std, gamma, beta);
+  dy[i] = y > 0.f ? __bfloat162float(dh[i]) + __bfloat162float(dh[plane + i]) : 0.f;
+}
+
+__device__ __forceinline__ int ref_feature(int col, int fc2) { return fc2 ? (col % 1024) * 16 + col / 1024 : col; }
+
+__global__ void dec_bn_grads_kernel(const double* __restrict__ fsum, const double* __restrict__ bsum, double count, float eps,
+                                    int c, int fc2, float* __restrict__ dbeta, float* __restrict__ dgamma) {
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ch >= c) return;
+  const int j = ref_feature(ch, fc2);
+  if (dbeta) dbeta[j] = (float)bsum[ch];
+  if (!dgamma) return;
+  const double mean = fsum[ch] / count;
+  double var = fsum[c + ch] / count - mean * mean;
+  if (var < 0.0) var = 0.0;
+  dgamma[j] = (float)((bsum[c + ch] - mean * bsum[ch]) / sqrt(var + (double)eps));
+}
+
+// in, out: [2][total] (mean | inv_std); the first fc2_cols columns are bnorm_dec_fc2's
+__global__ void dec_stats_out_kernel(const float* __restrict__ in, int total, int fc2_cols, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * total) return;
+  const int r = i / total, col = i % total;
+  out[r * total + (col < fc2_cols ? ref_feature(col, 1) : col)] = in[i];
+}
+
 }  // namespace
 
 int launch_disc_pool(const __nv_bfloat16* a4, long long plane, int passes, int n, float* out, cudaStream_t st) {
@@ -256,6 +313,29 @@ int launch_disc_bn_coef(const double* fsum, const double* bsum, double count, fl
 int launch_disc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
                       long long plane, cudaStream_t st) {
   disc_bn_dx_kernel<<<blocks_of(total), 256, 0, st>>>(x, dy, total, c, coef, passes, out, plane);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_dec_bn_relu(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
+                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st) {
+  dec_bn_relu_kernel<<<blocks_of(total), 256, 0, st>>>(x, total, c, mean, inv_std, gamma, beta, passes, out, plane);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_dec_train_dy(const __nv_bfloat16* dh, long long plane, const float* x, long long total, int c, const float* mean,
+                        const float* inv_std, const float* gamma, const float* beta, float* dy, cudaStream_t st) {
+  dec_train_dy_kernel<<<blocks_of(total), 256, 0, st>>>(dh, plane, x, total, c, mean, inv_std, gamma, beta, dy);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_dec_bn_grads(const double* fsum, const double* bsum, double count, float eps, int c, int fc2, float* dbeta,
+                        float* dgamma, cudaStream_t st) {
+  dec_bn_grads_kernel<<<(c + 127) / 128, 128, 0, st>>>(fsum, bsum, count, eps, c, fc2, dbeta, dgamma);
+  return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+int launch_dec_stats_out(const float* in, int total, int fc2_cols, float* out, cudaStream_t st) {
+  dec_stats_out_kernel<<<blocks_of(2LL * total), 256, 0, st>>>(in, total, fc2_cols, out);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -240,6 +240,18 @@ int launch_disc_bn_coef(const double* fsum, const double* bsum, double count, fl
                         cudaStream_t st);
 int launch_disc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
                       long long plane, cudaStream_t st);
+// the IAN_simple decoder in training mode (ian_decode_train*): launch_disc_bn_act with rectify in place of LeakyReLU(0.2)
+int launch_dec_bn_relu(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
+                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st);
+// dy (float32) = (hi + lo of the split planes dh) * (y > 0), y the batch-normalised x
+int launch_dec_train_dy(const __nv_bfloat16* dh, long long plane, const float* x, long long total, int c, const float* mean,
+                        const float* inv_std, const float* gamma, const float* beta, float* dy, cudaStream_t st);
+// d beta, d gamma (nullable each) from the forward's and the backward's [2][c] sums; fc2: columns in bnorm_dec_fc2's library
+// order, written at their reference feature
+int launch_dec_bn_grads(const double* fsum, const double* bsum, double count, float eps, int c, int fc2, float* dbeta,
+                        float* dgamma, cudaStream_t st);
+// [2][total] statistics with bnorm_dec_fc2's first fc2_cols columns moved to their reference feature
+int launch_dec_stats_out(const float* in, int total, int fc2_cols, float* out, cudaStream_t st);
 // signal + wait kernels of the peer-memory barrier (flag_ptrs[r] = rank r's flag array, int[8])
 int launch_peer_barrier(float* const* flag_ptrs, int world, int rank, int epoch, cudaStream_t st);
 // training-mode pieces (train_kernels.cu): BatchNorm batch statistics / normalisation, MinibatchLayer forward

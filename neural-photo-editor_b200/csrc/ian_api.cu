@@ -163,6 +163,9 @@ enum LayerId {
   // the training-mode discriminator (ian_discriminate_train*): enc_conv2..4 with unit scale, no shift and no activation
   // into a float32 raw buffer, and E_BWD_CONV4 / E_BWD_CONV3 with unit scale into a float32 buffer; built on first use
   DT_ENC_CONV2, DT_ENC_CONV3, DT_ENC_CONV4, DT_BWD_CONV4, DT_BWD_CONV3,
+  // the IAN_simple decoder in training mode (ian_decode_train*): l_dec_fc2 and dec_conv1..3 with unit scale, no shift and no
+  // activation into a float32 raw buffer, and L_BWD_CONV3..1 with unit scale into a float32 buffer; built on first use
+  DD_DEC_FC2, DD_DEC_CONV1, DD_DEC_CONV2, DD_DEC_CONV3, DD_BWD_CONV3, DD_BWD_CONV2, DD_BWD_CONV1,
   L_COUNT,
   T_CONV1 = L_COUNT, T_DEC_OUT, T_BRUSH_SEED, T_CONV1_BWD,   // timing-only slots of the edge kernels (brush_seed: the
                                                         // loss-seed kernel of every decoder backward, box or dense VJP seed;
@@ -181,6 +184,9 @@ enum LayerId {
   T_DISC_COTANGENT,                                     // layer, their adjoints, the MinibatchLayer, and enc_conv4's cotangent
   T_DT_STATS, T_DT_NORM, T_DT_COTANGENT, T_DT_BN_BWD, T_DT_BN_DX,   // the training-mode trunk: batch statistics, normalise +
                                                         // LeakyReLU, the pool's adjoint, BatchNorm backward sums and dx
+  T_DD_STATS, T_DD_NORM, T_DD_COTANGENT, T_DD_BN_BWD, T_DD_BN_DX,   // the same steps of the training-mode decoder (cotangent:
+                                                        // bnorm_dc3's dy from the seed), and its BatchNorm beta / gamma
+  T_DD_BN_GRADS,
   T_COUNT
 };
 const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_fc1", "enc_head", "l_dec_fc2", "dec_conv1",
@@ -199,6 +205,8 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "introspect_bwd_enc_conv4", "introspect_bwd_enc_conv3", "introspect_bwd_enc_conv2",
                                     "disc_train_enc_conv2", "disc_train_enc_conv3", "disc_train_enc_conv4",
                                     "disc_train_bwd_enc_conv4", "disc_train_bwd_enc_conv3",
+                                    "dec_train_l_dec_fc2", "dec_train_dec_conv1", "dec_train_dec_conv2", "dec_train_dec_conv3",
+                                    "dec_train_bwd_dec_conv3", "dec_train_bwd_dec_conv2", "dec_train_bwd_dec_conv1",
                                     "enc_conv1", "dec_out", "brush_seed", "enc_conv1_bwd",
                                     "wgrad_l_dec_fc2", "wgrad_dec_conv1", "wgrad_dec_conv2", "wgrad_dec_conv3", "wgrad_dec_out",
                                     "dec_out_jvp", "jvp_enc_conv1", "gn_gram", "gn_solve", "map_gram",
@@ -206,7 +214,9 @@ const char* kLayerNames[T_COUNT] = {"enc_conv2", "enc_conv3", "enc_conv4", "enc_
                                     "robust_gram", "robust_scale",
                                     "disc_pool", "disc_head", "disc_head_bwd", "disc_mb", "disc_mb_bwd", "disc_cotangent",
                                     "disc_train_stats", "disc_train_norm", "disc_train_cotangent", "disc_train_bn_bwd",
-                                    "disc_train_bn_dx"};
+                                    "disc_train_bn_dx",
+                                    "dec_train_stats", "dec_train_norm", "dec_train_cotangent", "dec_train_bn_bwd",
+                                    "dec_train_bn_dx", "dec_train_bn_grads"};
 
 struct DevWeights {           // one GEMM layer's B operand + epilogue vectors
   __nv_bfloat16* b = nullptr;
@@ -306,6 +316,11 @@ struct ian_handle {
   float* enc_bn_gb = nullptr;
   char* disc_tbuf = nullptr;
   int disc_tcap = 0;
+  // bnorm_dec_fc2 / bnorm_dc1..3's gamma | beta in the library's column order (2 x 17280 floats, IAN_simple, written with
+  // the folded vectors), and ian_decode_train*'s whole-call buffers (grown to dec_tcap samples; see DecTrainBufs)
+  float* dec_bn_gb = nullptr;
+  char* dec_tbuf = nullptr;
+  int dec_tcap = 0;
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -425,6 +440,8 @@ struct Plan {
   // the training-mode discriminator's tap-GEMM twins (DT_ENC_CONV2..4 on the first ian_discriminate_train* call on the plan,
   // DT_BWD_CONV4..3 with the encoder VJP's planes on the first ian_discriminate_train_vjp_* call)
   bool dtrain = false, dtrain_vjp = false;
+  // the training-mode decoder's twins (DD_DEC_*, then DD_BWD_* with the parameter VJP's planes and weight-gradient maps)
+  bool dectrain = false, dectrain_vjp = false;
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -947,12 +964,8 @@ int run_head(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
   return IAN_OK;
 }
 
-// zp must already hold the latent planes
-int run_decode_from_planes(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
-  int rc;
-  for (int l : decoder_layers(h).fwd)
-    if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
-  if (has_flow(h)) return run_head(h, pl, xhat, st);
+// IAN_simple's dec_out and tanh from the h3 planes
+int run_dec_out(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
   ScopedTimer tm(h, T_DEC_OUT, st);
   if (h->path == IAN_PATH_TC) {
     float* one[1] = {xhat};
@@ -961,6 +974,14 @@ int run_decode_from_planes(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st
   else
     LAUNCH_TRY(h, launch_dec_out(pl->h3.p, pl->h3.plane, h->decout_wt, xhat, pl->n, st));
   return IAN_OK;
+}
+
+// zp must already hold the latent planes
+int run_decode_from_planes(ian_handle* h, Plan* pl, float* xhat, cudaStream_t st) {
+  int rc;
+  for (int l : decoder_layers(h).fwd)
+    if ((rc = run_gemm(h, pl, l, st)) != IAN_OK) return rc;
+  return has_flow(h) ? run_head(h, pl, xhat, st) : run_dec_out(h, pl, xhat, st);
 }
 
 int run_decode(ian_handle* h, Plan* pl, const float* z, float* xhat, cudaStream_t st) {
@@ -1195,6 +1216,7 @@ inline int fc2_ref_col(int col, int C) { return (col % C) * 16 + col / C; }
 // Each writes every device buffer derived from its group: allocated by the first call, overwritten in place by later ones.
 const char* kDecBn[4] = {"bnorm_dec_fc2", "bnorm_dc1", "bnorm_dc2", "bnorm_dc3"};
 const int kDecBnC[4] = {16384, 512, 256, 128};
+constexpr int kDecBnOff[4] = {0, 16384, 16896, 17152}, kDecBnTotal = 17280;   // the four BatchNorms' columns, concatenated
 struct DecConv { int lf, lb; const char* w; int Cin, Cout; };
 const DecConv kDecConv[3] = {{L_DEC_CONV1, L_BWD_CONV1, "dec_conv1.W", 1024, 512},
                              {L_DEC_CONV2, L_BWD_CONV2, "dec_conv2.W", 512, 256},
@@ -1257,6 +1279,16 @@ int simple_bn(ian_handle* h, int k) {
   if (rc != IAN_OK) return rc;
   if ((rc = put_dev(h, h->w[lf].shift, sf.data(), C * 4)) != IAN_OK) return rc;
   if (k < 3 && (rc = put_dev(h, h->w[kDecConv[k].lb].scale, sc.data(), C * 4)) != IAN_OK) return rc;
+  {   // gamma | beta in the library's column order for the training-mode decoder, which normalises with the batch's statistics
+    if (!h->dec_bn_gb) CUDA_TRY(h, cudaMalloc((void**)&h->dec_bn_gb, 2 * kDecBnTotal * sizeof(float)));
+    for (int j = 0; j < C; ++j) {
+      const int i = k == 0 ? fc2_ref_col(j, 1024) : j;
+      sc[j] = f[1][i];
+      sf[j] = f[0][i];
+    }
+    CUDA_TRY(h, cudaMemcpy(h->dec_bn_gb + kDecBnOff[k], sc.data(), C * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->dec_bn_gb + kDecBnTotal + kDecBnOff[k], sf.data(), C * 4, cudaMemcpyHostToDevice));
+  }
   if (h->dec_bn_stats[k][0]) {
     if ((rc = put_dev(h, h->dec_bn_stats[k][0], f[2].data(), C * 4)) != IAN_OK) return rc;
     if ((rc = put_dev(h, h->dec_bn_stats[k][1], f[3].data(), C * 4)) != IAN_OK) return rc;
@@ -2911,7 +2943,7 @@ int ensure_train_bufs(ian_handle* h, int n, TrainBufs* b) {
 int build_twin(ian_handle* h, Plan* pl, int to, int from) {
   TapGemm& g = pl->g[to];
   g = pl->g[from];
-  g.scale = nullptr; g.shift = nullptr; g.out = nullptr; g.out_plane = 0; g.out_f32 = nullptr;
+  g.scale = nullptr; g.shift = nullptr; g.out = nullptr; g.out_plane = 0; g.out_f32 = nullptr; g.scale_pix_stride = 0;
   if (g.act != ACT_MASK) g.act = ACT_NONE;
   char err[256] = {0};
   if (!(pl->maps[to] = tc_build_maps(g, err, sizeof(err)))) return fail(h, IAN_ERR_CUDA, "layer %s: %s", kLayerNames[to], err);
@@ -3093,6 +3125,243 @@ int call_discriminate_train_vjp(ian_handle* h, bool host, const float* x, int n,
       LAUNCH_TRY(h, launch_conv1_bwd(c.pl->e1.p, c.pl->e1.plane, h->conv1_bwd_wt, c.f(1), c.cn, c.st));
     return (int)IAN_OK;
   });
+}
+
+// ---- the IAN_simple decoder in training mode (DESIGN section 5.6p) ----------------------------------------------------
+// get_output(l_out, {l_Z: z}) under deterministic=False: bnorm_dec_fc2 and bnorm_dc1..3 normalise with the batch's
+// statistics, so the decoder runs layer by layer over the whole call, as the training-mode discriminator's trunk does.  For
+// each of l_dec_fc2 and dec_conv1..3: per chunk, the layer's twin (unit scale, no shift, no activation) writes its raw sums
+// into a whole-call float32 buffer; over the call, per-image float64 sums added in image order give mean and inv_std; per
+// chunk again dec_bn_relu writes the next layer's input planes.  dec_out runs as ever on h3.
+// The VJP runs that forward, then per chunk the parameter VJP's dense seed (the seed image and dL/dh3 before the mask) and
+// dec_out's weight gradient; per layer from dc3 down to fc2: whole-call float64 Σdy, Σdy·x (d beta, d gamma and the
+// BatchNorm backward's coefficients), then per chunk dL/d(raw sum) as split planes (d3..d0), the layer's weight gradient
+// (wgrad on those planes and the training-mode activations, chunks added in order) and the backward-data GEMM's twin with
+// the training-mode activations as ReLU masks into a float32 buffer -- L_BWD_FC2 itself (unit scale already) for dz.
+constexpr int kDecTrainC[4] = {16384, 512, 256, 128}, kDecTrainHW[4] = {1, 64, 256, 1024};
+constexpr long long kDecTrainElems[4] = {16384, 32768, 65536, 131072};   // per image, l_dec_fc2 and dec_conv1..3's outputs
+constexpr long long kDecTrainPerImg = 245760;
+
+// raw[l], dy[l]: layer l's raw sums and dL/dy (n, HW, C); part: the per-image partial sums ([n][2][16384]); fsum: the
+// forward's [2][C] per layer; bsum: the backward's; coef: [4][16384]; stats: [2][17280] float32 in the library's column
+// order, sout: the same in the reference's feature order (the host form's staging)
+struct DecTrainBufs {
+  float *raw[4], *dy[4], *stats, *sout;
+  double *part, *fsum, *bsum, *coef;
+};
+
+int ensure_dec_train_bufs(ian_handle* h, int n, DecTrainBufs* b) {
+  if (n > h->dec_tcap) {
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaFree(h->dec_tbuf));
+    h->dec_tbuf = nullptr;
+    h->dec_tcap = 0;
+    const size_t bytes = (size_t)n * (2 * kDecTrainPerImg * sizeof(float) + 2 * 16384 * sizeof(double)) +
+                         (2 * kDecBnTotal + 2 * 16384 + 4 * 16384) * sizeof(double) + 4 * kDecBnTotal * sizeof(float);
+    CUDA_TRY(h, cudaMalloc((void**)&h->dec_tbuf, bytes));
+    h->dec_tcap = n;
+  }
+  const long long N = h->dec_tcap;
+  b->part = (double*)h->dec_tbuf;
+  b->fsum = b->part + N * 2 * 16384;
+  b->bsum = b->fsum + 2 * kDecBnTotal;
+  b->coef = b->bsum + 2 * 16384;
+  b->stats = (float*)(b->coef + 4 * 16384);
+  b->sout = b->stats + 2 * kDecBnTotal;
+  float* f = b->sout + 2 * kDecBnTotal;
+  for (int l = 0; l < 4; ++l) { b->raw[l] = f; f += N * kDecTrainElems[l]; }
+  for (int l = 0; l < 4; ++l) { b->dy[l] = f; f += N * kDecTrainElems[l]; }
+  return IAN_OK;
+}
+
+template <bool kVjp>
+int ensure_dec_train_plan(ian_handle* h, Plan* pl) {
+  int rc;
+  if (!pl->dectrain) {
+    for (int k = 0; k < 4; ++k)
+      if ((rc = build_twin(h, pl, DD_DEC_FC2 + k, kSimpleDecoder.fwd.l[k])) != IAN_OK) return rc;
+    pl->dectrain = true;
+  }
+  if (kVjp && !pl->dectrain_vjp) {
+    if ((rc = ensure_param_vjp_plan(h, pl)) != IAN_OK) return rc;
+    for (int k = 0; k < 3; ++k)
+      if ((rc = build_twin(h, pl, DD_BWD_CONV3 + k, kSimpleDecoder.bwd.l[k])) != IAN_OK) return rc;
+    pl->dectrain_vjp = true;
+  }
+  return IAN_OK;
+}
+
+const Planes& dec_planes(const Plan* pl, int l) { return l == 0 ? pl->h0 : l == 1 ? pl->h1 : l == 2 ? pl->h2 : pl->h3; }
+
+// layer l's batch-normalised, rectified output of the chunk at `off` -> its planes h_l
+int dec_train_act(ian_handle* h, const DecTrainBufs& b, int l, Plan* pl, int off, int cn, cudaStream_t st) {
+  ScopedTimer tm(h, T_DD_NORM, st);
+  const float* gb = h->dec_bn_gb;
+  const Planes& a = dec_planes(pl, l);
+  LAUNCH_TRY(h, launch_dec_bn_relu(b.raw[l] + off * kDecTrainElems[l], cn * kDecTrainElems[l], kDecTrainC[l], b.stats + kDecBnOff[l],
+                                   b.stats + kDecBnTotal + kDecBnOff[l], gb + kDecBnOff[l], gb + kDecBnTotal + kDecBnOff[l], h->passes,
+                                   a.p, a.plane, st));
+  return IAN_OK;
+}
+
+// forward (dy == nullptr): layer l's statistics into b.stats; backward: Σdy, Σdy·x into b.bsum, then the coefficients and
+// d beta / d gamma (out: the 13 gradient pointers, nullable)
+int dec_train_sums(ian_handle* h, const DecTrainBufs& b, int l, int n, const float* dy, float* const* out, cudaStream_t st) {
+  const double count = (double)n * kDecTrainHW[l];
+  const int C = kDecTrainC[l], off = kDecBnOff[l];
+  double* fsum = b.fsum + 2 * off;
+  if (!dy) {
+    ScopedTimer tm(h, T_DD_STATS, st);
+    LAUNCH_TRY(h, launch_disc_bn_sums(b.raw[l], b.raw[l], n, kDecTrainHW[l], C, count, kBnEps, b.part, fsum, b.stats + off,
+                                      b.stats + kDecBnTotal + off, st));
+    return IAN_OK;
+  }
+  {
+    ScopedTimer tm(h, T_DD_BN_BWD, st);
+    LAUNCH_TRY(h, launch_disc_bn_sums(dy, b.raw[l], n, kDecTrainHW[l], C, 0.0, kBnEps, b.part, b.bsum, nullptr, nullptr, st));
+    LAUNCH_TRY(h, launch_disc_bn_coef(fsum, b.bsum, count, kBnEps, h->dec_bn_gb + off, C, b.coef, st));
+  }
+  float *db = out[PV_BN0_B + 2 * l], *dg = out[PV_BN0_G + 2 * l];
+  if (db || dg) {
+    ScopedTimer tm(h, T_DD_BN_GRADS, st);
+    LAUNCH_TRY(h, launch_dec_bn_grads(fsum, b.bsum, count, kBnEps, C, l == 0 ? 1 : 0, db, dg, st));
+  }
+  return IAN_OK;
+}
+
+// the forward to every layer's raw sums and statistics (h3's planes are left to the caller, per chunk)
+template <bool kVjp>
+int dec_train_forward(ian_handle* h, bool host, const float* z, int n, const DecTrainBufs& b, void* stream) {
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  int rc = run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}}, ensure_dec_train_plan<kVjp>, [&](const Chunk& c) {
+    LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+    return run_gemm_into(h, c.pl, DD_DEC_FC2, b.raw[0] + c.off * kDecTrainElems[0], c.st);
+  });
+  if (rc != IAN_OK || (rc = dec_train_sums(h, b, 0, n, nullptr, nullptr, st)) != IAN_OK) return rc;
+  for (int l = 1; l < 4; ++l) {
+    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+      int r = ensure_dec_train_plan<kVjp>(h, pl);
+      if (r == IAN_OK) r = dec_train_act(h, b, l - 1, pl, off, cn, st);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, DD_DEC_FC2 + l, b.raw[l] + off * kDecTrainElems[l], st);
+    });
+    if (rc != IAN_OK || (rc = dec_train_sums(h, b, l, n, nullptr, nullptr, st)) != IAN_OK) return rc;
+  }
+  return IAN_OK;
+}
+
+int check_decode_train(ian_handle* h, int n) {
+  if (!h) return IAN_ERR_INVALID;
+  if (!h->finalized) return fail(h, IAN_ERR_STATE, "ian_finalize() has not been called");
+  if (h->model_kind != IAN_MODEL_SIMPLE)
+    return fail(h, IAN_ERR_UNSUPPORTED, "the training-mode decoder is implemented for IAN_simple only");
+  if (n < 0) return fail(h, IAN_ERR_INVALID, "batch size must not be negative (got %d)", n);
+  return IAN_OK;
+}
+
+int call_decode_train(ian_handle* h, bool host, const float* z, int n, float* x_hat, float* stats, void* stream) {
+  int rc = check_decode_train(h, n);
+  if (rc != IAN_OK || n == 0) return rc;
+  if (!z || !x_hat) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  DecTrainBufs b;
+  if ((rc = ensure_dec_train_bufs(h, n, &b)) != IAN_OK || (rc = dec_train_forward<false>(h, host, z, n, b, stream)) != IAN_OK)
+    return rc;
+  if (stats) {
+    LAUNCH_TRY(h, launch_dec_stats_out(b.stats, kDecBnTotal, 16384, host ? b.sout : stats, st));
+    if (host) CUDA_TRY(h, cudaMemcpyAsync(stats, b.sout, 2 * kDecBnTotal * sizeof(float), cudaMemcpyDeviceToHost, st));
+  }
+  return run_entry(h, host, stream, n, {{x_hat, kImageBytes, S_XHAT, OUT}}, ensure_dec_train_plan<false>, [&](const Chunk& c) {
+    const int r = dec_train_act(h, b, 3, c.pl, c.off, c.cn, c.st);
+    return r != IAN_OK ? r : run_dec_out(h, c.pl, c.f(0), c.st);
+  });
+}
+
+// 1 forward + 1 backward.  The host form computes the requested gradients into the handle's device buffers and copies them
+// out at the end.
+int call_decode_train_vjp(ian_handle* h, bool host, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                          void* stream) {
+  float* req[PV_COUNT];
+  int rc = check_param_vjp(h, z, dx_hat, n, grads, req);
+  if (rc != IAN_OK || n == 0) return rc;
+  DeviceGuard dg(h->device);
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  float* out[PV_COUNT];
+  for (int k = 0; k < PV_COUNT; ++k) {
+    out[k] = req[k];
+    if (!host || !req[k]) continue;
+    if (!h->pv_dev[k]) CUDA_TRY(h, cudaMalloc((void**)&h->pv_dev[k], (size_t)kPvSize[k] * 4));
+    out[k] = h->pv_dev[k];
+  }
+  DecTrainBufs b;
+  if ((rc = ensure_dec_train_bufs(h, n, &b)) != IAN_OK || (rc = dec_train_forward<true>(h, host, z, n, b, stream)) != IAN_OK)
+    return rc;
+  const float* gb = h->dec_bn_gb;
+  // h3, x_hat and the seed per chunk: dec_out's weight gradient, and bnorm_dc3's dy from dL/dh3 and the training-mode mask
+  rc = run_entry(h, host, stream, n, {{dx_hat, kImageBytes, S_TARGET, IN}}, ensure_dec_train_plan<true>, [&](const Chunk& c) {
+    Plan* pl = c.pl;
+    int r = dec_train_act(h, b, 3, pl, c.off, c.cn, c.st);
+    if (r == IAN_OK) r = run_dec_out(h, pl, pl->xhat, c.st);
+    if (r != IAN_OK) return r;
+    {
+      ScopedTimer tm(h, T_BRUSH_SEED, c.st);
+      LAUNCH_TRY(h, launch_brush_param_seed_bwd(pl->xhat, c.f(0), h->decout_wt, h->w[L_DEC_CONV3].scale, pl->h3.p, pl->d3.p,
+                                                pl->d3.plane, pl->pseed, pl->dh3.p, c.cn, c.st));
+    }
+    if (out[PV_OUT]) {
+      ScopedTimer tm(h, T_WGRAD_DEC_OUT, c.st);
+      LAUNCH_TRY(h, launch_decout_wgrad(pl->pseed, pl->h3.p, pl->h3.plane, c.cn, pl->ppart, out[PV_OUT], c.off > 0, c.st));
+    }
+    ScopedTimer tm(h, T_DD_COTANGENT, c.st);
+    const int o = kDecBnOff[3];
+    LAUNCH_TRY(h, launch_dec_train_dy(pl->dh3.p, pl->dh3.plane, b.raw[3] + c.off * kDecTrainElems[3], c.cn * kDecTrainElems[3],
+                                      kDecTrainC[3], b.stats + o, b.stats + kDecBnTotal + o, gb + o, gb + kDecBnTotal + o,
+                                      b.dy[3] + c.off * kDecTrainElems[3], c.st));
+    return (int)IAN_OK;
+  });
+  if (rc != IAN_OK) return rc;
+  // dL/d(raw sum) of layer l for the chunk -> its split planes d_l, then layer l's weight gradient (A: the layer's input)
+  auto grad_planes = [&](Plan* pl, int l, int off, int cn, cudaStream_t s) {
+    const Planes& d = l == 0 ? pl->d0 : l == 1 ? pl->d1 : l == 2 ? pl->d2 : pl->d3;
+    {
+      ScopedTimer tm(h, T_DD_BN_DX, s);
+      LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[l] + off * kDecTrainElems[l], b.dy[l] + off * kDecTrainElems[l], cn * kDecTrainElems[l],
+                                      kDecTrainC[l], b.coef, h->passes, d.p, d.plane, s));
+    }
+    if (l > 0) {
+      const int r = dec_train_act(h, b, l - 1, pl, off, cn, s);
+      if (r != IAN_OK) return r;
+    }
+    if (!out[PV_FC2 + l]) return (int)IAN_OK;
+    {
+      ScopedTimer tm(h, T_WGRAD_FC2 + l, s);
+      if (h->path == IAN_PATH_TC) LAUNCH_TRY(h, launch_wgrad_tc(pl->wg[l], pl->wmaps[l], s));
+      else LAUNCH_TRY(h, launch_wgrad_simt(pl->wg[l], s));
+    }
+    LAUNCH_TRY(h, launch_wgrad_finalize(pl->wg[l], l == 0 ? WG_FC2 : WG_DECONV, out[PV_FC2 + l], off > 0, s));
+    return (int)IAN_OK;
+  };
+  for (int l = 3; l >= 1; --l) {
+    if ((rc = dec_train_sums(h, b, l, n, b.dy[l], out, st)) != IAN_OK) return rc;
+    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+      int r = ensure_dec_train_plan<true>(h, pl);
+      if (r == IAN_OK) r = grad_planes(pl, l, off, cn, st);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, DD_BWD_CONV3 + (3 - l), b.dy[l - 1] + off * kDecTrainElems[l - 1], st);
+    });
+    if (rc != IAN_OK) return rc;
+  }
+  if ((rc = dec_train_sums(h, b, 0, n, b.dy[0], out, st)) != IAN_OK) return rc;
+  rc = run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}}, ensure_dec_train_plan<true>, [&](const Chunk& c) {
+    LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
+    int r = grad_planes(c.pl, 0, c.off, c.cn, c.st);
+    if (r == IAN_OK) r = run_gemm(h, c.pl, L_BWD_FC2, c.st);
+    return r != IAN_OK ? r : copy_dz(c, dz);
+  });
+  if (rc != IAN_OK || !host) return rc;
+  for (int k = 0; k < PV_COUNT; ++k)
+    if (req[k]) CUDA_TRY(h, cudaMemcpyAsync(req[k], out[k], (size_t)kPvSize[k] * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(h, cudaStreamSynchronize(st));
+  return IAN_OK;
 }
 
 // E(z) = a |x_hat - x|^2 + sum_l c_l |g_l(x_hat) - g_l(x)|^2 with c_l = 3072 b / M_l (b * 12288 * l_f, l_f the per-sample
@@ -3574,6 +3843,8 @@ int ian_destroy(ian_handle* h) {
   cudaFree(h->disc_buf);
   cudaFree(h->enc_bn_gb);
   cudaFree(h->disc_tbuf);
+  cudaFree(h->dec_bn_gb);
+  cudaFree(h->dec_tbuf);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }
@@ -3849,6 +4120,19 @@ int ian_discriminate_train_vjp_dev(ian_handle* h, const float* x, int n, const f
 }
 int ian_discriminate_train_vjp_host(ian_handle* h, const float* x, int n, const float* dlogits, float* dx) {
   return call_discriminate_train_vjp(h, true, x, n, dlogits, dx, nullptr);
+}
+int ian_decode_train_dev(ian_handle* h, const float* z, int n, float* x_hat, float* stats, void* stream) {
+  return call_decode_train(h, false, z, n, x_hat, stats, stream);
+}
+int ian_decode_train_host(ian_handle* h, const float* z, int n, float* x_hat, float* stats) {
+  return call_decode_train(h, true, z, n, x_hat, stats, nullptr);
+}
+int ian_decode_train_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads,
+                             void* stream) {
+  return call_decode_train_vjp(h, false, z, dx_hat, n, dz, grads, stream);
+}
+int ian_decode_train_vjp_host(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz, float* const* grads) {
+  return call_decode_train_vjp(h, true, z, dx_hat, n, dz, grads, nullptr);
 }
 int ian_feature_gauss_newton_dev(ian_handle* h, const float* z, const float* x, int n, double pixel_weight, double feature_weight,
                                  double* A, double* g, double* e, void* stream) {

@@ -33,7 +33,9 @@
     (train_IAN_simple.py:353, `decoder_params`) as leaf CUDA tensors, differentiable through one parameter VJP
     (ian_decode_param_vjp_dev) that also returns dz.  Before each forward, every tensor whose in-place version moved since
     its last upload is written back into the handle (ian_update_param_host), so a plain torch.optim loop over
-    params.values() fine-tunes the generator with no extra call.
+    params.values() fine-tunes the generator with no extra call.  decode(model, z, params, training=True) is the decoder
+    as the reference's trainers run it (batch-statistics BatchNorm: ian_decode_train_dev forward, one
+    ian_decode_train_vjp_dev backward), so that loop trains the reference's function.
 
 A backward costs one forward plus one backward of that half of the model: the library recomputes the forward from the
 saved input instead of keeping the activations of the forward call.  The op is once-differentiable (no double backward).  Inputs and outputs are
@@ -436,7 +438,7 @@ def _params_function():
 
     class DecodeParams(torch.autograd.Function):
         @staticmethod
-        def forward(ctx, model, z, names, *tensors):
+        def forward(ctx, model, z, training, names, *tensors):
             _check_tensor(model, z, "z")
             if z.dim() != 2 or z.shape[1] != 100:
                 raise ValueError("z must be (n,100), got %r" % (tuple(z.shape),))
@@ -446,8 +448,11 @@ def _params_function():
             x = torch.empty(n, 3, 64, 64, dtype=torch.float32, device=z.device)
             if n:
                 with _lib_stream(model, z) as st:
-                    model.decode_dev(z.data_ptr(), n, x.data_ptr(), st)
-            ctx.model, ctx.names = model, names
+                    if training:
+                        model.decode_train_dev(z.data_ptr(), n, x.data_ptr(), 0, st)
+                    else:
+                        model.decode_dev(z.data_ptr(), n, x.data_ptr(), st)
+            ctx.model, ctx.names, ctx.training = model, names, training
             ctx.save_for_backward(z, *tensors)
             return x
 
@@ -461,12 +466,13 @@ def _params_function():
             n = int(z.shape[0])
             want_z = ctx.needs_input_grad[1]
             dz = torch.zeros_like(z) if want_z else None
-            grads = [torch.zeros_like(t) if ctx.needs_input_grad[3 + i] else None for i, t in enumerate(tensors)]
+            grads = [torch.zeros_like(t) if ctx.needs_input_grad[4 + i] else None for i, t in enumerate(tensors)]
             if n:
                 ptrs = {name: gr.data_ptr() for name, gr in zip(ctx.names, grads) if gr is not None}
+                vjp = model.decode_train_vjp_dev if ctx.training else model.decode_param_vjp_dev
                 with _lib_stream(model, z) as st:
-                    model.decode_param_vjp_dev(z.data_ptr(), g.data_ptr(), n, dz.data_ptr() if want_z else 0, ptrs, st)
-            return (None, dz, None) + tuple(grads)
+                    vjp(z.data_ptr(), g.data_ptr(), n, dz.data_ptr() if want_z else 0, ptrs, st)
+            return (None, dz, None, None) + tuple(grads)
 
     _DecodeParams = DecodeParams
     return DecodeParams
@@ -502,13 +508,17 @@ def decoder_parameters(model, weights):
     return params
 
 
-def decode(model, z, params=None):
+def decode(model, z, params=None, training=False):
     """x_hat = decoder(z) for z (n,100) float32 CUDA on the model's device; differentiable w.r.t. z (one decoder forward +
     one backward per backward call).  Without params it also supports forward mode: under torch.autograd.forward_ad a
     dual z (make_dual(z, v)) gives x_hat with the tangent (d x_hat / d z) . v, from one ian_decode_jvp_dev call.
     With params (from decoder_parameters), also differentiable w.r.t. those tensors: one ian_decode_param_vjp_dev returns
-    dz and every gradient; tensors that do not require grad get None.  That form is reverse mode only."""
-    if params is None:
+    dz and every gradient; tensors that do not require grad get None.  That form is reverse mode only.
+    training=True (IAN_simple): the decoder as the reference's trainers evaluate it (deterministic=False): its four
+    BatchNorms normalise with the batch's statistics, so every sample's x_hat depends on every z of the call.  The forward
+    is ian_decode_train_dev and the backward one ian_decode_train_vjp_dev, for z and the params alike; reverse mode only.
+    The model's running statistics are neither used nor changed."""
+    if params is None and not training:
         return _function().apply(model, z)
-    names = list(params)
-    return _params_function().apply(model, z, tuple(names), *[params[n] for n in names])
+    names = list(params or ())
+    return _params_function().apply(model, z, bool(training), tuple(names), *[params[n] for n in names])
