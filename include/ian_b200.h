@@ -549,9 +549,10 @@ int ian_update_param_host(ian_handle* h, const char* name, const float* data, co
  *   exactly 0.
  * IAN_MODEL_FULL / IAN_MODEL_V1 -> IAN_ERR_UNSUPPORTED; n == 0 does nothing.  Float32 on both paths.  Deterministic.  No
  *   CUDA graphs.
- * Memory: whole-call buffers of 2.1 MB per image (the four layers' raw sums, 245 760 floats, their cotangents of the same
- *   size, and 256 KB of float64 partial sums) plus 0.9 MB fixed, grown to the largest batch asked for; the VJP also
- *   allocates ian_decode_param_vjp_*'s buffers on each chunk's plan. */
+ * Memory: whole-call buffers of 1.9 MB per image (the four layers' raw sums, 245 760 floats; two cotangent slots the
+ *   layers alternate between, 131 072 floats for bnorm_dc3 / bnorm_dc1 and 65 536 for bnorm_dc2 / bnorm_dec_fc2; 256 KB of
+ *   float64 partial sums) plus 1.3 MB fixed, grown to the largest batch asked for; the VJP also allocates
+ *   ian_decode_param_vjp_*'s buffers on each chunk's plan. */
 int ian_decode_train_dev(ian_handle* h, const float* z, int n, float* x_hat, float* stats /*nullable*/, void* stream);
 int ian_decode_train_host(ian_handle* h, const float* z, int n, float* x_hat, float* stats /*nullable*/);
 int ian_decode_train_vjp_dev(ian_handle* h, const float* z, const float* dx_hat, int n, float* dz /*nullable*/,

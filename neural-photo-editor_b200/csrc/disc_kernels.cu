@@ -8,20 +8,20 @@
 //   disc_cotangent  : d pool -> the cotangent of a4, c4 = broadcast(d pool / 16) (n,1024,4,4) float32 NCHW
 // A feature value is what the encoder stores: hi + lo of the split planes, or hi alone in bf16 mode (launch_feat_store's rule).
 //
-// The training-mode trunk (ian_discriminate_train*; DESIGN section 5.6o): batch-statistics BatchNorm on enc_conv2..4's raw
-// sums, whole-call float32 NHWC buffers (n, HW, C), channel c of pixel p of image i at (i HW + p) C + c.
-//   disc_bn_partial  : per image and channel, Σu and Σu·v in float64 over the image's pixels in order (u = v = x: the
+// The batch-statistics BatchNorm stacks (ian_api.cu's BnStack; DESIGN section 5.6o) -- the training-mode trunk
+// (ian_discriminate_train*: bnorm2..4 on enc_conv2..4) and the IAN_simple decoder in training mode (ian_decode_train*;
+// DESIGN section 5.6p: bnorm_dec_fc2 with hw = 1 and c = its 16384 library columns, bnorm_dc1..3) -- share these kernels on
+// the layers' raw sums in whole-call float32 NHWC buffers (n, HW, C), channel c of pixel p of image i at (i HW + p) C + c:
+//   nhwc_bn_partial  : per image and channel, Σu and Σu·v in float64 over the image's pixels in order (u = v = x: the
 //                      forward's Σx, Σx²; u = dy, v = x: the backward's Σdy, Σdy·x)
-//   disc_bn_stats    : the images' partials added in image order, so the sums do not depend on the chunking; mean and
+//   nhwc_bn_stats    : the images' partials added in image order, so the sums do not depend on the chunking; mean and
 //                      inv_std = 1/sqrt(var + eps) as bn_finalize_kernel forms them (biased var), float32 copies for the callers
-//   disc_bn_act      : y = (x - mean) (gamma inv_std) + beta, a = LeakyReLU(0.2)(y) -> split planes (hi only in bf16 mode)
+//   nhwc_bn_act      : y = (x - mean) (gamma inv_std) + beta, a = fmaf(act_abs, |y|, act_lin y) -> split planes (hi only in
+//                      bf16 mode): LeakyReLU(0.2) with 0.4, 0.6 (the trunk), rectify with 0.5, 0.5 (the decoder)
+//   nhwc_bn_coef     : bn_bwd_coef_kernel's coefficients (train_kernels.cu) from the whole-call sums, in its own rounding
+//   nhwc_bn_dx       : dx per element in float64, rounded once as bn_bwd_apply_kernel does -> split planes
+// Each stack's own kernels:
 //   disc_train_cot   : the pool's adjoint times lrelu'(y4): dy4 = d pool / 16 * (y4 > 0 ? 1 : 0.2), float32
-//   disc_bn_coef     : bn_bwd_coef_kernel's coefficients from the whole-call sums
-//   disc_bn_dx       : dx per element in float64, rounded once as bn_bwd_apply_kernel does -> split planes
-//
-// The IAN_simple decoder in training mode (ian_decode_train*; DESIGN section 5.6p) uses disc_bn_partial / disc_bn_stats /
-// disc_bn_coef / disc_bn_dx on l_dec_fc2 and dec_conv1..3's raw sums (l_dec_fc2: hw = 1, c = 16384 library columns), and:
-//   dec_bn_relu      : disc_bn_act with rectify in place of LeakyReLU(0.2)
 //   dec_train_dy     : dy = dL/dh (hi + lo of split planes) * (y > 0), float32: bnorm_dc3's cotangent from the seed kernel
 //   dec_bn_grads     : d beta = Σdy, d gamma = inv_std (Σdy·x - mean Σdy) in float64 from the whole-call sums, written in
 //                      the reference's feature order
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(256) disc_cotangent_kernel(const float* __rest
 unsigned blocks_of(long long total) { return (unsigned)((total + 255) / 256); }
 
 // thread (image, channel): coalesced over channels, the image's pixels in order
-__global__ void __launch_bounds__(128) disc_bn_partial_kernel(const float* __restrict__ u, const float* __restrict__ v, int hw, int c,
+__global__ void __launch_bounds__(128) nhwc_bn_partial_kernel(const float* __restrict__ u, const float* __restrict__ v, int hw, int c,
                                                               double* __restrict__ part /*[n][2][c]*/) {
   const int ch = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
   if (ch >= c) return;
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(128) disc_bn_partial_kernel(const float* __res
 }
 
 // sums[2][c] = the partials of images 0..n-1 in order; with count > 0 also mean_f / inv_std_f (the forward's statistics)
-__global__ void disc_bn_stats_kernel(const double* __restrict__ part, int n, int c, double count, float eps, double* __restrict__ sums,
+__global__ void nhwc_bn_stats_kernel(const double* __restrict__ part, int n, int c, double count, float eps, double* __restrict__ sums,
                                      float* __restrict__ mean_f, float* __restrict__ inv_std_f) {
   const int ch = blockIdx.x * blockDim.x + threadIdx.x;
   if (ch >= c) return;
@@ -162,14 +162,15 @@ __device__ __forceinline__ float bn_train_y(float x, int ch, const float* mean, 
   return (x - __ldg(mean + ch)) * (__ldg(gamma + ch) * __ldg(inv_std + ch)) + __ldg(beta + ch);
 }
 
-__global__ void __launch_bounds__(256) disc_bn_act_kernel(const float* __restrict__ x, long long total, int c, const float* __restrict__ mean,
+// act_abs, act_lin: the activation as the tap-GEMM epilogue forms it
+__global__ void __launch_bounds__(256) nhwc_bn_act_kernel(const float* __restrict__ x, long long total, int c, const float* __restrict__ mean,
                                                           const float* __restrict__ inv_std, const float* __restrict__ gamma,
-                                                          const float* __restrict__ beta, int passes, __nv_bfloat16* __restrict__ out,
-                                                          long long plane) {
+                                                          const float* __restrict__ beta, float act_abs, float act_lin, int passes,
+                                                          __nv_bfloat16* __restrict__ out, long long plane) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= total) return;
   const float y = bn_train_y(x[i], (int)(i % c), mean, inv_std, gamma, beta);
-  const float a = fmaf(0.4f, fabsf(y), 0.6f * y);       // LeakyRectify(0.2) as the tap-GEMM epilogue forms it
+  const float a = fmaf(act_abs, fabsf(y), act_lin * y);
   __nv_bfloat16 hi, lo;
   split_bf16(a, hi, lo);
   out[i] = hi;
@@ -187,8 +188,10 @@ __global__ void __launch_bounds__(256) disc_train_cot_kernel(const float* __rest
   dy[o] = dpool[(o / (kPool * kC4)) * kC4 + ch] * (1.f / kPool) * (y > 0.f ? 1.f : 0.2f);
 }
 
-// dx = a (dy - m - (x - mean) k), a = gamma s, m = Σdy/N, k = s² (Σdy·x - mean Σdy)/N, s = inv_std in float64
-__global__ void disc_bn_coef_kernel(const double* __restrict__ fsum, const double* __restrict__ bsum, double count, float eps,
+// dx = a (dy - m - (x - mean) k), a = gamma s, m = Σdy/N, k = s² (Σdy·x - mean Σdy)/N, s = inv_std in float64: the coefficients
+// of bn_bwd_coef_kernel (train_kernels.cu), kept apart because the two compile differently: here Σx²/N - mean² is one fused
+// multiply-add, there (bn_stats) mean² is rounded before the subtraction, so s can differ in its last bit
+__global__ void nhwc_bn_coef_kernel(const double* __restrict__ fsum, const double* __restrict__ bsum, double count, float eps,
                                     const float* __restrict__ gamma, int c, double* __restrict__ coef /*[4][c]*/) {
   const int ch = blockIdx.x * blockDim.x + threadIdx.x;
   if (ch >= c) return;
@@ -202,7 +205,7 @@ __global__ void disc_bn_coef_kernel(const double* __restrict__ fsum, const doubl
   coef[3 * c + ch] = s * s * (bsum[c + ch] - mean * bsum[ch]) / count;
 }
 
-__global__ void __launch_bounds__(256) disc_bn_dx_kernel(const float* __restrict__ x, const float* __restrict__ dy, long long total, int c,
+__global__ void __launch_bounds__(256) nhwc_bn_dx_kernel(const float* __restrict__ x, const float* __restrict__ dy, long long total, int c,
                                                          const double* __restrict__ coef, int passes, __nv_bfloat16* __restrict__ out,
                                                          long long plane) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -211,20 +214,6 @@ __global__ void __launch_bounds__(256) disc_bn_dx_kernel(const float* __restrict
   const double t = (double)dy[i] - coef[c + ch] - ((double)x[i] - coef[2 * c + ch]) * coef[3 * c + ch];
   __nv_bfloat16 hi, lo;
   split_bf16((float)(coef[ch] * t), hi, lo);
-  out[i] = hi;
-  if (passes != 1) out[plane + i] = lo;
-}
-
-__global__ void __launch_bounds__(256) dec_bn_relu_kernel(const float* __restrict__ x, long long total, int c, const float* __restrict__ mean,
-                                                          const float* __restrict__ inv_std, const float* __restrict__ gamma,
-                                                          const float* __restrict__ beta, int passes, __nv_bfloat16* __restrict__ out,
-                                                          long long plane) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const float y = bn_train_y(x[i], (int)(i % c), mean, inv_std, gamma, beta);
-  const float a = fmaf(0.5f, fabsf(y), 0.5f * y);       // rectify as the tap-GEMM epilogue forms it
-  __nv_bfloat16 hi, lo;
-  split_bf16(a, hi, lo);
   out[i] = hi;
   if (passes != 1) out[plane + i] = lo;
 }
@@ -285,16 +274,17 @@ int launch_disc_cotangent(const float* dpool, int n, float* c4, cudaStream_t st)
                  cudaSuccess ? 1 : -1;
 }
 
-int launch_disc_bn_sums(const float* u, const float* v, int n, int hw, int c, double count, float eps, double* part, double* sums,
+int launch_nhwc_bn_sums(const float* u, const float* v, int n, int hw, int c, double count, float eps, double* part, double* sums,
                         float* mean_f, float* inv_std_f, cudaStream_t st) {
-  disc_bn_partial_kernel<<<dim3((c + 127) / 128, n), 128, 0, st>>>(u, v, hw, c, part);
-  disc_bn_stats_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, n, c, count, eps, sums, mean_f, inv_std_f);
+  nhwc_bn_partial_kernel<<<dim3((c + 127) / 128, n), 128, 0, st>>>(u, v, hw, c, part);
+  nhwc_bn_stats_kernel<<<(c + 127) / 128, 128, 0, st>>>(part, n, c, count, eps, sums, mean_f, inv_std_f);
   return cudaGetLastError() == cudaSuccess ? 2 : -1;
 }
 
-int launch_disc_bn_act(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
-                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st) {
-  disc_bn_act_kernel<<<blocks_of(total), 256, 0, st>>>(x, total, c, mean, inv_std, gamma, beta, passes, out, plane);
+int launch_nhwc_bn_act(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
+                       const float* beta, float act_abs, float act_lin, int passes, __nv_bfloat16* out, long long plane,
+                       cudaStream_t st) {
+  nhwc_bn_act_kernel<<<blocks_of(total), 256, 0, st>>>(x, total, c, mean, inv_std, gamma, beta, act_abs, act_lin, passes, out, plane);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -304,21 +294,15 @@ int launch_disc_train_cotangent(const float* dpool, const float* x4, int n, cons
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
-int launch_disc_bn_coef(const double* fsum, const double* bsum, double count, float eps, const float* gamma, int c, double* coef,
+int launch_nhwc_bn_coef(const double* fsum, const double* bsum, double count, float eps, const float* gamma, int c, double* coef,
                         cudaStream_t st) {
-  disc_bn_coef_kernel<<<(c + 127) / 128, 128, 0, st>>>(fsum, bsum, count, eps, gamma, c, coef);
+  nhwc_bn_coef_kernel<<<(c + 127) / 128, 128, 0, st>>>(fsum, bsum, count, eps, gamma, c, coef);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
-int launch_disc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
+int launch_nhwc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
                       long long plane, cudaStream_t st) {
-  disc_bn_dx_kernel<<<blocks_of(total), 256, 0, st>>>(x, dy, total, c, coef, passes, out, plane);
-  return cudaGetLastError() == cudaSuccess ? 1 : -1;
-}
-
-int launch_dec_bn_relu(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
-                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st) {
-  dec_bn_relu_kernel<<<blocks_of(total), 256, 0, st>>>(x, total, c, mean, inv_std, gamma, beta, passes, out, plane);
+  nhwc_bn_dx_kernel<<<blocks_of(total), 256, 0, st>>>(x, dy, total, c, coef, passes, out, plane);
   return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

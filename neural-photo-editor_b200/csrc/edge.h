@@ -225,25 +225,25 @@ int launch_disc_head(const float* in, const float* W, int U, int n, float* logit
 int launch_disc_head_bwd(const float* dlogits, const float* W, int U, int n, float* g, cudaStream_t st);
 // c4 (n,1024,4,4) NCHW = dpool (n,1024) / 16 at every pixel
 int launch_disc_cotangent(const float* dpool, int n, float* c4, cudaStream_t st);
-// the training-mode trunk (ian_discriminate_train*): whole-call float32 NHWC (n, hw, c).  part: [n][2][c] doubles of per-image
-// Σu, Σu·v; sums[2][c] their image-ordered totals; count > 0 (the forward): also mean_f, inv_std_f (eps inside the root)
-int launch_disc_bn_sums(const float* u, const float* v, int n, int hw, int c, double count, float eps, double* part, double* sums,
+// the batch-statistics BatchNorm stacks (ian_discriminate_train*, ian_decode_train*): whole-call float32 NHWC (n, hw, c).
+// part: [n][2][c] doubles of per-image Σu, Σu·v; sums[2][c] their image-ordered totals; count > 0 (the forward): also mean_f,
+// inv_std_f (eps inside the root)
+int launch_nhwc_bn_sums(const float* u, const float* v, int n, int hw, int c, double count, float eps, double* part, double* sums,
                         float* mean_f, float* inv_std_f, cudaStream_t st);
-// x (total elements, channel fastest) -> LeakyReLU(0.2)((x - mean) (gamma inv_std) + beta) as split planes (hi only if passes == 1)
-int launch_disc_bn_act(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
-                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st);
+// x (total elements, channel fastest) -> fmaf(act_abs, |y|, act_lin y), y = (x - mean) (gamma inv_std) + beta, as split planes
+// (hi only if passes == 1)
+int launch_nhwc_bn_act(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
+                       const float* beta, float act_abs, float act_lin, int passes, __nv_bfloat16* out, long long plane,
+                       cudaStream_t st);
+// BatchNorm backward: coef[4][c] from the forward's sums and the backward's (Σdy, Σdy·x), then dx as split planes
+int launch_nhwc_bn_coef(const double* fsum, const double* bsum, double count, float eps, const float* gamma, int c, double* coef,
+                        cudaStream_t st);
+int launch_nhwc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
+                      long long plane, cudaStream_t st);
 // dy4 (n,4,4,1024) = dpool / 16 * lrelu'(y4), y4 the batch-normalised enc_conv4 of x4
 int launch_disc_train_cotangent(const float* dpool, const float* x4, int n, const float* mean, const float* inv_std,
                                 const float* gamma, const float* beta, float* dy, cudaStream_t st);
-// BatchNorm backward: coef[4][c] from the forward's sums and the backward's (Σdy, Σdy·x), then dx as split planes
-int launch_disc_bn_coef(const double* fsum, const double* bsum, double count, float eps, const float* gamma, int c, double* coef,
-                        cudaStream_t st);
-int launch_disc_bn_dx(const float* x, const float* dy, long long total, int c, const double* coef, int passes, __nv_bfloat16* out,
-                      long long plane, cudaStream_t st);
-// the IAN_simple decoder in training mode (ian_decode_train*): launch_disc_bn_act with rectify in place of LeakyReLU(0.2)
-int launch_dec_bn_relu(const float* x, long long total, int c, const float* mean, const float* inv_std, const float* gamma,
-                       const float* beta, int passes, __nv_bfloat16* out, long long plane, cudaStream_t st);
-// dy (float32) = (hi + lo of the split planes dh) * (y > 0), y the batch-normalised x
+// the IAN_simple decoder in training mode (ian_decode_train*): dy (float32) = (hi + lo of the split planes dh) * (y > 0), y the batch-normalised x
 int launch_dec_train_dy(const __nv_bfloat16* dh, long long plane, const float* x, long long total, int c, const float* mean,
                         const float* inv_std, const float* gamma, const float* beta, float* dy, cudaStream_t st);
 // d beta, d gamma (nullable each) from the forward's and the backward's [2][c] sums; fc2: columns in bnorm_dec_fc2's library

@@ -311,16 +311,14 @@ struct ian_handle {
   // [pool | f], its cotangent, the pool's cotangent, the host forms' logits / p / dlogits, and one chunk's enc_conv4 cotangent
   float* disc_buf = nullptr;
   int disc_cap = 0;
-  // bnorm2..4's gamma | beta (1792 + 1792 floats, uploaded with the encoder), and ian_discriminate_train*'s whole-call
-  // buffers (grown to the largest batch asked for, disc_tcap samples; see TrainBufs)
+  // bnorm2..4's gamma | beta (1792 + 1792 floats, uploaded with the encoder)
   float* enc_bn_gb = nullptr;
-  char* disc_tbuf = nullptr;
-  int disc_tcap = 0;
   // bnorm_dec_fc2 / bnorm_dc1..3's gamma | beta in the library's column order (2 x 17280 floats, IAN_simple, written with
-  // the folded vectors), and ian_decode_train*'s whole-call buffers (grown to dec_tcap samples; see DecTrainBufs)
+  // the folded vectors)
   float* dec_bn_gb = nullptr;
-  char* dec_tbuf = nullptr;
-  int dec_tcap = 0;
+  // the whole-call buffers of each batch-statistics stack (the training-mode discriminator's trunk, the IAN_simple decoder),
+  // grown to the largest batch asked for, cap samples; see BnBufs
+  struct { char* buf = nullptr; int cap = 0; } bn_bufs[2];
   int max_chunk = 512;
   bool timing = false;
   struct Timed { cudaEvent_t e0, e1; };
@@ -437,11 +435,9 @@ struct Plan {
   // cotangents of a1..a3 as split planes NHWC, the res operand of IV_BWD_CONV2..4 (0.92 MB per image)
   bool ivjp = false;
   Planes ivc[3];
-  // the training-mode discriminator's tap-GEMM twins (DT_ENC_CONV2..4 on the first ian_discriminate_train* call on the plan,
-  // DT_BWD_CONV4..3 with the encoder VJP's planes on the first ian_discriminate_train_vjp_* call)
-  bool dtrain = false, dtrain_vjp = false;
-  // the training-mode decoder's twins (DD_DEC_*, then DD_BWD_* with the parameter VJP's planes and weight-gradient maps)
-  bool dectrain = false, dectrain_vjp = false;
+  // each batch-statistics stack's tap-GEMM twins: [stack][0] the forward ones (DT_ENC_CONV2..4, DD_DEC_*) on the stack's first
+  // call on the plan, [stack][1] the backward-data ones (DT_BWD_*, DD_BWD_*) with their VJP's planes on its first VJP call
+  bool bn_twins[2][2] = {};
   enum { G_ENCODE, G_ENCODE_EPS, G_DECODE, G_RECON, G_GRAD, G_EDIT_STEP, G_STROKE, G_VJP, G_ENC_VJP, G_PARAM_VJP, G_JVP, G_ENC_JVP,
          G_ENCODE_PRE, G_FLOW, G_FLOW_VJP, G_FLOW_JVP, G_ENC_PRE_VJP, G_ENC_PRE_JVP, G_COUNT };
   GraphSlot graph[G_COUNT];
@@ -2889,53 +2885,88 @@ int call_discriminate_vjp(ian_handle* h, bool host, const float* x, int n, const
   });
 }
 
-// ---- the discriminator in training mode (DESIGN section 5.6o) ----------------------------------------------------------
-// l_discrim under deterministic=False: bnorm2..4 normalise with the batch's statistics, so the trunk couples the call's
-// samples at three more points than the MinibatchLayer does and runs layer by layer over the whole call.  For each of
-// enc_conv2..4: per chunk, the layer's twin (unit scale, no shift, no activation) writes its raw sums into a whole-call float32
-// buffer; over the call, per-image float64 sums added in image order give mean and inv_std (so they do not depend on
-// IAN_CHUNK); per chunk again disc_bn_act writes the next layer's input planes.  The head then runs as in inference.
-// The VJP keeps the forward's raw buffers and recomputes each chunk's activation planes (the masks of the backward GEMMs)
-// from them: the pool's adjoint times lrelu'(y4); per layer whole-call float64 Σdy, Σdy·x, then per chunk dx as split planes
-// and the backward GEMM's twin (unit scale, the training-mode activations as LeakyReLU masks) into a float32 buffer;
-// enc_conv2's backward (its scale is 1 already) and enc_conv1's adjoint end the chain on the chunk's planes.
-constexpr int kTrainC[3] = {256, 512, 1024}, kTrainHW[3] = {256, 64, 16}, kTrainOff[3] = {0, 256, 768};
-constexpr long long kTrainElems[3] = {65536, 32768, 16384};   // per image, enc_conv2..4's outputs
+// ---- batch-statistics BatchNorm stacks (DESIGN section 5.6o) -----------------------------------------------------------
+// The training-mode discriminator's trunk (bnorm2..4 on enc_conv2..4) and the IAN_simple decoder in training mode
+// (bnorm_dec_fc2, bnorm_dc1..3 on l_dec_fc2, dec_conv1..3) normalise with the call's own statistics, so they couple the
+// call's samples and run layer by layer over the whole call.  A BnStack holds what differs between the two as data; one set
+// of helpers runs both.
+// Forward, per layer: per chunk, the layer's twin (unit scale, no shift, no activation) writes its raw sums into a whole-call
+// float32 buffer; over the call, per-image float64 sums added in image order give mean and inv_std (so no result depends
+// on IAN_CHUNK); per chunk again bn_act normalises, activates and writes the next layer's input planes.
+// Backward, from the top layer down: whole-call float64 Σdy, Σdy·x and the coefficients; then per chunk dx as split planes,
+// the layer below's activation recomputed from its raw sums (the backward GEMM's mask) and the backward-data twin (unit
+// scale, float32 output) into the next cotangent slot.  The bottom layer's dx and what follows it are the caller's.
+struct BnStack {
+  int id;                                   // its slots in ian_handle::bn_bufs and Plan::bn_twins
+  int L, C[4], HW[4];                       // layers; each layer's channels and pixels
+  int off[4], total;                        // each layer's columns in the concatenated stats and gamma | beta
+  int fwd, fwd_of[4];                       // layer l's forward twin is fwd + l, a twin of fwd_of[l]
+  int bwd, bwd_of[3];                       // the backward-data twin from layer L-1-k down: bwd + k, a twin of bwd_of[k]
+  int (*vjp_plan)(ian_handle*, Plan*);      // the VJP planes the backward twins read and write
+  float act_abs, act_lin;                   // the activation fmaf(act_abs, |y|, act_lin y), as the tap-GEMM epilogue forms it
+  int t_stats, t_norm, t_bn_bwd, t_bn_dx;   // timer slots
+  float* ian_handle::*gb;                   // gamma | beta, [2][total]
+  Planes Plan::*act[4], Plan::*dx[4];       // layer l's activation planes (the next layer's input) and its dx planes
+};
+constexpr BnStack kDiscStack = {0, 3, {256, 512, 1024}, {256, 64, 16}, {0, 256, 768}, 1792,
+                                DT_ENC_CONV2, {L_ENC_CONV2, L_ENC_CONV3, L_ENC_CONV4}, DT_BWD_CONV4, {E_BWD_CONV4, E_BWD_CONV3},
+                                ensure_enc_vjp_plan, 0.4f, 0.6f,   // LeakyRectify(0.2)
+                                T_DT_STATS, T_DT_NORM, T_DT_BN_BWD, T_DT_BN_DX, &ian_handle::enc_bn_gb,
+                                {&Plan::a2, &Plan::a3, &Plan::a4}, {&Plan::e2, &Plan::e3, &Plan::e4}};
+constexpr BnStack kDecStack = {1, 4, {16384, 512, 256, 128}, {1, 64, 256, 1024},
+                               {kDecBnOff[0], kDecBnOff[1], kDecBnOff[2], kDecBnOff[3]}, kDecBnTotal,
+                               DD_DEC_FC2, {L_DEC_FC2, L_DEC_CONV1, L_DEC_CONV2, L_DEC_CONV3},
+                               DD_BWD_CONV3, {L_BWD_CONV3, L_BWD_CONV2, L_BWD_CONV1},
+                               ensure_param_vjp_plan, 0.5f, 0.5f,   // rectify
+                               T_DD_STATS, T_DD_NORM, T_DD_BN_BWD, T_DD_BN_DX, &ian_handle::dec_bn_gb,
+                               {&Plan::h0, &Plan::h1, &Plan::h2, &Plan::h3}, {&Plan::d0, &Plan::d1, &Plan::d2, &Plan::d3}};
 constexpr float kBnEps = 1e-4f;
 
-// raw[l]: enc_conv{l+2}'s raw sums (n,HW,C); dy[0] (the size of raw[0]) holds dy of bnorm4, then bnorm2; dy[1] bnorm3's;
-// part: the per-image partial sums; fsum: the forward's [2][C] per layer; bsum: the backward's; coef: [4][1024];
-// stats: [2][1792] float32, the means of bnorm2 | bnorm3 | bnorm4, then their inv_std
-struct TrainBufs {
-  float *raw[3], *dy[2], *stats;
+long long bn_elems(const BnStack& S, int l) { return (long long)S.C[l] * S.HW[l]; }   // per image
+
+// raw[l]: layer l's raw sums (n, HW, C).  dy: two cotangent slots, layer l's dy (n, HW, C) in dy[(L-1-l) % 2], each sized
+// for its largest layer: layer l's dy is last read by its own dx step, so layer l-1's twin writes the other slot and only
+// layer l-2's twin, after layer l is done, writes this one again.  part: the per-image partial sums [n][2][max C]; fsum,
+// bsum: the forward's and the backward's [2][C] sums of layer l at 2 off[l]; coef: [4][max C]; stats: [2][total] float32,
+// the means then the inv_std in the library's column order; sout: [2][total], the staging of a reordered copy of stats
+struct BnBufs {
+  float *raw[4], *dy[2], *stats, *sout;
   double *part, *fsum, *bsum, *coef;
 };
 
-int ensure_train_bufs(ian_handle* h, int n, TrainBufs* b) {
-  const long long per_img = 2 * kTrainElems[0] + 2 * kTrainElems[1] + kTrainElems[2];   // floats
-  if (n > h->disc_tcap) {
-    CUDA_TRY(h, cudaDeviceSynchronize());
-    CUDA_TRY(h, cudaFree(h->disc_tbuf));
-    h->disc_tbuf = nullptr;
-    h->disc_tcap = 0;
-    const size_t bytes = (size_t)n * (per_img * sizeof(float) + 2 * 1024 * sizeof(double)) +
-                         (2 * 1792 + 2 * 1024 + 4 * 1024) * sizeof(double) + 2 * 1792 * sizeof(float);
-    CUDA_TRY(h, cudaMalloc((void**)&h->disc_tbuf, bytes));
-    h->disc_tcap = n;
+float* bn_dy(const BnStack& S, const BnBufs& b, int l) { return b.dy[(S.L - 1 - l) % 2]; }
+
+int ensure_bn_bufs(ian_handle* h, const BnStack& S, int n, BnBufs* b) {
+  int maxc = 0;
+  long long slot[2] = {0, 0}, per_img = 0;   // floats
+  for (int l = 0; l < S.L; ++l) {
+    maxc = std::max(maxc, S.C[l]);
+    slot[(S.L - 1 - l) % 2] = std::max(slot[(S.L - 1 - l) % 2], bn_elems(S, l));
+    per_img += bn_elems(S, l);
   }
-  const long long N = h->disc_tcap;
-  double* d = (double*)h->disc_tbuf;
-  b->part = d;
-  b->fsum = b->part + N * 2 * 1024;
-  b->bsum = b->fsum + 2 * 1792;
-  b->coef = b->bsum + 2 * 1024;
-  float* f = (float*)(b->coef + 4 * 1024);
-  b->stats = f;
-  b->raw[0] = f + 2 * 1792;
-  b->raw[1] = b->raw[0] + N * kTrainElems[0];
-  b->raw[2] = b->raw[1] + N * kTrainElems[1];
-  b->dy[0] = b->raw[2] + N * kTrainElems[2];
-  b->dy[1] = b->dy[0] + N * kTrainElems[0];
+  per_img += slot[0] + slot[1];
+  auto& s = h->bn_bufs[S.id];
+  if (n > s.cap) {
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaFree(s.buf));
+    s.buf = nullptr;
+    s.cap = 0;
+    const size_t bytes = (size_t)n * (per_img * sizeof(float) + 2 * maxc * sizeof(double)) +
+                         (4 * S.total + 4 * maxc) * sizeof(double) + 4 * S.total * sizeof(float);
+    CUDA_TRY(h, cudaMalloc((void**)&s.buf, bytes));
+    s.cap = n;
+  }
+  const long long N = s.cap;
+  b->part = (double*)s.buf;
+  b->fsum = b->part + N * 2 * maxc;
+  b->bsum = b->fsum + 2 * S.total;
+  b->coef = b->bsum + 2 * S.total;
+  b->stats = (float*)(b->coef + 4 * maxc);
+  b->sout = b->stats + 2 * S.total;
+  float* f = b->sout + 2 * S.total;
+  for (int l = 0; l < S.L; ++l) { b->raw[l] = f; f += N * bn_elems(S, l); }
+  b->dy[0] = f;
+  b->dy[1] = f + N * slot[0];
   return IAN_OK;
 }
 
@@ -2950,71 +2981,125 @@ int build_twin(ian_handle* h, Plan* pl, int to, int from) {
   return IAN_OK;
 }
 
-template <bool kVjp>
-int ensure_disc_train_plan(ian_handle* h, Plan* pl) {
+// the stack's forward twins on the plan; with vjp also its backward-data twins, on the VJP's planes
+int ensure_bn_twins(ian_handle* h, Plan* pl, const BnStack& S, bool vjp) {
+  bool* built = pl->bn_twins[S.id];
   int rc;
-  if (!pl->dtrain) {
-    for (int k = 0; k < 3; ++k)
-      if ((rc = build_twin(h, pl, DT_ENC_CONV2 + k, kEncoder.l[k])) != IAN_OK) return rc;
-    pl->dtrain = true;
+  if (!built[0]) {
+    for (int l = 0; l < S.L; ++l)
+      if ((rc = build_twin(h, pl, S.fwd + l, S.fwd_of[l])) != IAN_OK) return rc;
+    built[0] = true;
   }
-  if (kVjp && !pl->dtrain_vjp) {
-    if ((rc = ensure_enc_vjp_plan(h, pl)) != IAN_OK) return rc;
-    if ((rc = build_twin(h, pl, DT_BWD_CONV4, E_BWD_CONV4)) != IAN_OK || (rc = build_twin(h, pl, DT_BWD_CONV3, E_BWD_CONV3)) != IAN_OK)
-      return rc;
-    pl->dtrain_vjp = true;
+  if (vjp && !built[1]) {
+    if ((rc = S.vjp_plan(h, pl)) != IAN_OK) return rc;
+    for (int k = 0; k < S.L - 1; ++k)
+      if ((rc = build_twin(h, pl, S.bwd + k, S.bwd_of[k])) != IAN_OK) return rc;
+    built[1] = true;
   }
   return IAN_OK;
 }
+
+// ensure_bn_twins as run_entry's prepare
+template <const BnStack& S, bool kVjp>
+int ensure_bn_plan(ian_handle* h, Plan* pl) { return ensure_bn_twins(h, pl, S, kVjp); }
 
 int run_gemm_into(ian_handle* h, Plan* pl, int l, float* out, cudaStream_t st) {
   pl->g[l].out_f32 = out;
   return run_gemm(h, pl, l, st);
 }
 
-// bnorm{l+2}'s batch-normalised, LeakyReLU'd output of the chunk at `off` -> the planes `a`
-int train_act(ian_handle* h, const TrainBufs& b, int l, int off, int cn, const Planes& a, cudaStream_t st) {
-  ScopedTimer tm(h, T_DT_NORM, st);
-  const float* gb = h->enc_bn_gb;
-  LAUNCH_TRY(h, launch_disc_bn_act(b.raw[l] + off * kTrainElems[l], cn * kTrainElems[l], kTrainC[l], b.stats + kTrainOff[l],
-                                   b.stats + 1792 + kTrainOff[l], gb + kTrainOff[l], gb + 1792 + kTrainOff[l], h->passes, a.p,
+// layer l's batch-normalised, activated output of the chunk at `off` -> its activation planes
+int bn_act(ian_handle* h, const BnStack& S, const BnBufs& b, int l, Plan* pl, int off, int cn, cudaStream_t st) {
+  ScopedTimer tm(h, S.t_norm, st);
+  const float* gb = h->*S.gb + S.off[l];
+  const Planes& a = pl->*S.act[l];
+  LAUNCH_TRY(h, launch_nhwc_bn_act(b.raw[l] + off * bn_elems(S, l), cn * bn_elems(S, l), S.C[l], b.stats + S.off[l],
+                                   b.stats + S.total + S.off[l], gb, gb + S.total, S.act_abs, S.act_lin, h->passes, a.p,
                                    a.plane, st));
   return IAN_OK;
 }
 
-// u = v = raw[l] (forward: statistics into b.stats) or u = dy, v = raw[l] (backward: Σdy, Σdy·x into b.bsum, then coef)
-int train_sums(ian_handle* h, const TrainBufs& b, int l, int n, const float* dy, cudaStream_t st) {
-  const double count = (double)n * kTrainHW[l];
-  ScopedTimer tm(h, dy ? T_DT_BN_BWD : T_DT_STATS, st);
-  if (!dy) {
-    LAUNCH_TRY(h, launch_disc_bn_sums(b.raw[l], b.raw[l], n, kTrainHW[l], kTrainC[l], count, kBnEps, b.part, b.fsum + 2 * kTrainOff[l],
-                                      b.stats + kTrainOff[l], b.stats + 1792 + kTrainOff[l], st));
+// forward: layer l's sums into b.fsum and its statistics into b.stats; backward: Σdy, Σdy·x into b.bsum, then the coefficients
+int bn_sums(ian_handle* h, const BnStack& S, const BnBufs& b, int l, int n, bool bwd, cudaStream_t st) {
+  const double count = (double)n * S.HW[l];
+  const int C = S.C[l], o = S.off[l];
+  ScopedTimer tm(h, bwd ? S.t_bn_bwd : S.t_stats, st);
+  if (!bwd) {
+    LAUNCH_TRY(h, launch_nhwc_bn_sums(b.raw[l], b.raw[l], n, S.HW[l], C, count, kBnEps, b.part, b.fsum + 2 * o, b.stats + o,
+                                      b.stats + S.total + o, st));
     return IAN_OK;
   }
-  LAUNCH_TRY(h, launch_disc_bn_sums(dy, b.raw[l], n, kTrainHW[l], kTrainC[l], 0.0, kBnEps, b.part, b.bsum, nullptr, nullptr, st));
-  LAUNCH_TRY(h, launch_disc_bn_coef(b.fsum + 2 * kTrainOff[l], b.bsum, count, kBnEps, h->enc_bn_gb + kTrainOff[l], kTrainC[l], b.coef, st));
+  LAUNCH_TRY(h, launch_nhwc_bn_sums(bn_dy(S, b, l), b.raw[l], n, S.HW[l], C, 0.0, kBnEps, b.part, b.bsum + 2 * o, nullptr, nullptr,
+                                    st));
+  LAUNCH_TRY(h, launch_nhwc_bn_coef(b.fsum + 2 * o, b.bsum + 2 * o, count, kBnEps, h->*S.gb + o, C, b.coef, st));
   return IAN_OK;
 }
 
-// the whole forward to the pooled features b.pool: enc_conv1 and the three training-mode layers, then a4's pool
-template <bool kVjp>
-int disc_train_trunk(ian_handle* h, bool host, const float* x, int n, const DiscBufs& d, const TrainBufs& b, void* stream) {
+// dL/d(raw sum) of layer l for the chunk at `off`, from its dy and the coefficients -> its dx planes
+int bn_dx(ian_handle* h, const BnStack& S, const BnBufs& b, int l, Plan* pl, int off, int cn, cudaStream_t st) {
+  ScopedTimer tm(h, S.t_bn_dx, st);
+  const Planes& d = pl->*S.dx[l];
+  const long long e = bn_elems(S, l);
+  LAUNCH_TRY(h, launch_nhwc_bn_dx(b.raw[l] + off * e, bn_dy(S, b, l) + off * e, cn * e, S.C[l], b.coef, h->passes, d.p, d.plane,
+                                  st));
+  return IAN_OK;
+}
+
+// the forward to every layer's raw sums and statistics; first(c) writes the chunk's input planes of layer 0's twin.  The
+// top layer's activation is the caller's, per chunk.
+template <const BnStack& S, bool kVjp, typename First>
+int bn_forward(ian_handle* h, bool host, const Arg& in, int n, const BnBufs& b, void* stream, First&& first) {
   const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
-  int rc = run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}}, ensure_disc_train_plan<kVjp>, [&](const Chunk& c) {
-    const int r = run_introspect(h, c.pl, c.f(0), c.st, 1);
-    return r != IAN_OK ? r : run_gemm_into(h, c.pl, DT_ENC_CONV2, b.raw[0] + c.off * kTrainElems[0], c.st);
+  int rc = run_entry(h, host, stream, n, {in}, ensure_bn_plan<S, kVjp>, [&](const Chunk& c) {
+    const int r = first(c);
+    return r != IAN_OK ? r : run_gemm_into(h, c.pl, S.fwd, b.raw[0] + c.off * bn_elems(S, 0), c.st);
   });
-  if (rc != IAN_OK || (rc = train_sums(h, b, 0, n, nullptr, st)) != IAN_OK) return rc;
-  for (int l = 1; l < 3; ++l) {
+  if (rc != IAN_OK || (rc = bn_sums(h, S, b, 0, n, false, st)) != IAN_OK) return rc;
+  for (int l = 1; l < S.L; ++l) {
     rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-      int r = ensure_disc_train_plan<kVjp>(h, pl);
-      if (r == IAN_OK) r = train_act(h, b, l - 1, off, cn, l == 1 ? pl->a2 : pl->a3, st);
-      return r != IAN_OK ? r : run_gemm_into(h, pl, DT_ENC_CONV2 + l, b.raw[l] + off * kTrainElems[l], st);
+      int r = ensure_bn_twins(h, pl, S, kVjp);
+      if (r == IAN_OK) r = bn_act(h, S, b, l - 1, pl, off, cn, st);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, S.fwd + l, b.raw[l] + off * bn_elems(S, l), st);
     });
-    if (rc != IAN_OK || (rc = train_sums(h, b, l, n, nullptr, st)) != IAN_OK) return rc;
+    if (rc != IAN_OK || (rc = bn_sums(h, S, b, l, n, false, st)) != IAN_OK) return rc;
   }
+  return IAN_OK;
+}
+
+// the backward from the top layer's dy, in its slot, to the bottom layer's coefficients.  hook(pl, l, off, cn) runs per
+// chunk once layer l's dx planes and layer l-1's activation planes are written, before the backward-data twin.
+template <typename Hook>
+int bn_backward(ian_handle* h, const BnStack& S, const BnBufs& b, int n, cudaStream_t st, Hook&& hook) {
+  int rc;
+  for (int l = S.L - 1; l >= 1; --l) {
+    if ((rc = bn_sums(h, S, b, l, n, true, st)) != IAN_OK) return rc;
+    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
+      int r = ensure_bn_twins(h, pl, S, true);
+      if (r == IAN_OK) r = bn_dx(h, S, b, l, pl, off, cn, st);
+      if (r == IAN_OK) r = bn_act(h, S, b, l - 1, pl, off, cn, st);
+      if (r == IAN_OK) r = hook(pl, l, off, cn);
+      return r != IAN_OK ? r : run_gemm_into(h, pl, S.bwd + (S.L - 1 - l), bn_dy(S, b, l - 1) + off * bn_elems(S, l - 1), st);
+    });
+    if (rc != IAN_OK) return rc;
+  }
+  return bn_sums(h, S, b, 0, n, true, st);
+}
+
+// ---- the discriminator in training mode (DESIGN section 5.6o) ----------------------------------------------------------
+// l_discrim under deterministic=False: enc_conv1 as ever, then kDiscStack, a4's pool and the head as in inference.  The VJP
+// keeps the forward's raw buffers: the head's and the MinibatchLayer's adjoints, then the pool's adjoint times lrelu'(y4) as
+// bnorm4's dy, the stack's backward, and per chunk bnorm2's dx, enc_conv2's backward (its scale is 1 already) and
+// enc_conv1's adjoint.
+
+// the whole forward to the pooled features d.pool
+template <bool kVjp>
+int disc_train_trunk(ian_handle* h, bool host, const float* x, int n, const DiscBufs& d, const BnBufs& b, void* stream) {
+  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
+  int rc = bn_forward<kDiscStack, kVjp>(h, host, {x, kImageBytes, S_X, IN}, n, b, stream,
+                                        [&](const Chunk& c) { return run_introspect(h, c.pl, c.f(0), c.st, 1); });
+  if (rc != IAN_OK) return rc;
   return for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-    const int r = train_act(h, b, 2, off, cn, pl->a4, st);
+    const int r = bn_act(h, kDiscStack, b, 2, pl, off, cn, st);
     if (r != IAN_OK) return r;
     ScopedTimer tm(h, T_DISC_POOL, st);
     LAUNCH_TRY(h, launch_disc_pool(pl->a4.p, pl->a4.plane, h->passes, cn, d.pool + (size_t)off * 1024, st));
@@ -3030,8 +3115,8 @@ int call_discriminate_train(ian_handle* h, bool host, const float* x, int n, flo
   const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
   const int U = disc_units(h);
   DiscBufs d;
-  TrainBufs b;
-  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_train_bufs(h, n, &b)) != IAN_OK ||
+  BnBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_bn_bufs(h, kDiscStack, n, &b)) != IAN_OK ||
       (rc = ensure_train_ws(h, mb_workspace_bytes(n, kDiscKernels, kDiscDims))) != IAN_OK ||
       (rc = disc_train_trunk<false>(h, host, x, n, d, b, stream)) != IAN_OK)
     return rc;
@@ -3047,7 +3132,7 @@ int call_discriminate_train(ian_handle* h, bool host, const float* x, int n, flo
     LAUNCH_TRY(h, launch_disc_head(d.in, h->disc_w[3], U, n, lo, po, st));
   }
   const cudaMemcpyKind k = host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-  if (stats) CUDA_TRY(h, cudaMemcpyAsync(stats, b.stats, 2 * 1792 * sizeof(float), k, st));
+  if (stats) CUDA_TRY(h, cudaMemcpyAsync(stats, b.stats, 2 * kDiscStack.total * sizeof(float), k, st));
   if (!host) return IAN_OK;
   CUDA_TRY(h, cudaMemcpyAsync(logits, lo, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (p) CUDA_TRY(h, cudaMemcpyAsync(p, po, (size_t)n * U * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -3063,9 +3148,10 @@ int call_discriminate_train_vjp(ian_handle* h, bool host, const float* x, int n,
   DeviceGuard dg(h->device);
   const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
   const int U = disc_units(h);
+  const BnStack& S = kDiscStack;
   DiscBufs d;
-  TrainBufs b;
-  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_train_bufs(h, n, &b)) != IAN_OK ||
+  BnBufs b;
+  if ((rc = ensure_disc_bufs(h, n, &d)) != IAN_OK || (rc = ensure_bn_bufs(h, S, n, &b)) != IAN_OK ||
       (rc = ensure_train_ws(h, mb_bwd_workspace_bytes(n, 1024, kDiscKernels, kDiscDims))) != IAN_OK ||
       (rc = disc_train_trunk<true>(h, host, x, n, d, b, stream)) != IAN_OK)
     return rc;
@@ -3085,37 +3171,15 @@ int call_discriminate_train_vjp(ian_handle* h, bool host, const float* x, int n,
   }
   {
     ScopedTimer tm(h, T_DT_COTANGENT, st);
-    const float* gb = h->enc_bn_gb;
-    LAUNCH_TRY(h, launch_disc_train_cotangent(d.dpool, b.raw[2], n, b.stats + kTrainOff[2], b.stats + 1792 + kTrainOff[2],
-                                              gb + kTrainOff[2], gb + 1792 + kTrainOff[2], b.dy[0], st));
+    const float* gb = h->enc_bn_gb + S.off[2];
+    LAUNCH_TRY(h, launch_disc_train_cotangent(d.dpool, b.raw[2], n, b.stats + S.off[2], b.stats + S.total + S.off[2], gb,
+                                              gb + S.total, bn_dy(S, b, 2), st));
   }
-  // bnorm4 -> a3 (dy of bnorm3 into dy[1]), bnorm3 -> a2 (dy of bnorm2 into dy[0])
-  const int bwd[2] = {DT_BWD_CONV4, DT_BWD_CONV3};
-  for (int l = 2; l >= 1; --l) {
-    const float* dy = b.dy[l == 2 ? 0 : 1];
-    float* dy_next = b.dy[l == 2 ? 1 : 0];
-    if ((rc = train_sums(h, b, l, n, dy, st)) != IAN_OK) return rc;
-    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-      const Planes& e = l == 2 ? pl->e4 : pl->e3;
-      {
-        ScopedTimer tm(h, T_DT_BN_DX, st);
-        LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[l] + off * kTrainElems[l], dy + off * kTrainElems[l], cn * kTrainElems[l], kTrainC[l], b.coef,
-                                        h->passes, e.p, e.plane, st));
-      }
-      const int r = train_act(h, b, l - 1, off, cn, l == 2 ? pl->a3 : pl->a2, st);
-      return r != IAN_OK ? r : run_gemm_into(h, pl, bwd[2 - l], dy_next + off * kTrainElems[l - 1], st);
-    });
-    if (rc != IAN_OK) return rc;
-  }
-  if ((rc = train_sums(h, b, 0, n, b.dy[0], st)) != IAN_OK) return rc;
-  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {dx, kImageBytes, S_XHAT, OUT}}, ensure_disc_train_plan<true>,
+  if ((rc = bn_backward(h, S, b, n, st, [](Plan*, int, int, int) { return (int)IAN_OK; })) != IAN_OK) return rc;
+  return run_entry(h, host, stream, n, {{x, kImageBytes, S_X, IN}, {dx, kImageBytes, S_XHAT, OUT}}, ensure_bn_plan<kDiscStack, true>,
                    [&](const Chunk& c) {
-    {
-      ScopedTimer tm(h, T_DT_BN_DX, c.st);
-      LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[0] + c.off * kTrainElems[0], b.dy[0] + c.off * kTrainElems[0], c.cn * kTrainElems[0],
-                                      kTrainC[0], b.coef, h->passes, c.pl->e2.p, c.pl->e2.plane, c.st));
-    }
-    int r = run_introspect(h, c.pl, c.f(0), c.st, 1);     // a1: the mask of enc_conv2's backward
+    int r = bn_dx(h, S, b, 0, c.pl, c.off, c.cn, c.st);
+    if (r == IAN_OK) r = run_introspect(h, c.pl, c.f(0), c.st, 1);     // a1: the mask of enc_conv2's backward
     if (r == IAN_OK) r = run_gemm(h, c.pl, E_BWD_CONV2, c.st);
     if (r != IAN_OK) return r;
     ScopedTimer tm(h, T_CONV1_BWD, c.st);
@@ -3128,125 +3192,19 @@ int call_discriminate_train_vjp(ian_handle* h, bool host, const float* x, int n,
 }
 
 // ---- the IAN_simple decoder in training mode (DESIGN section 5.6p) ----------------------------------------------------
-// get_output(l_out, {l_Z: z}) under deterministic=False: bnorm_dec_fc2 and bnorm_dc1..3 normalise with the batch's
-// statistics, so the decoder runs layer by layer over the whole call, as the training-mode discriminator's trunk does.  For
-// each of l_dec_fc2 and dec_conv1..3: per chunk, the layer's twin (unit scale, no shift, no activation) writes its raw sums
-// into a whole-call float32 buffer; over the call, per-image float64 sums added in image order give mean and inv_std; per
-// chunk again dec_bn_relu writes the next layer's input planes.  dec_out runs as ever on h3.
-// The VJP runs that forward, then per chunk the parameter VJP's dense seed (the seed image and dL/dh3 before the mask) and
-// dec_out's weight gradient; per layer from dc3 down to fc2: whole-call float64 Σdy, Σdy·x (d beta, d gamma and the
-// BatchNorm backward's coefficients), then per chunk dL/d(raw sum) as split planes (d3..d0), the layer's weight gradient
-// (wgrad on those planes and the training-mode activations, chunks added in order) and the backward-data GEMM's twin with
-// the training-mode activations as ReLU masks into a float32 buffer -- L_BWD_FC2 itself (unit scale already) for dz.
-constexpr int kDecTrainC[4] = {16384, 512, 256, 128}, kDecTrainHW[4] = {1, 64, 256, 1024};
-constexpr long long kDecTrainElems[4] = {16384, 32768, 65536, 131072};   // per image, l_dec_fc2 and dec_conv1..3's outputs
-constexpr long long kDecTrainPerImg = 245760;
-
-// raw[l], dy[l]: layer l's raw sums and dL/dy (n, HW, C); part: the per-image partial sums ([n][2][16384]); fsum: the
-// forward's [2][C] per layer; bsum: the backward's; coef: [4][16384]; stats: [2][17280] float32 in the library's column
-// order, sout: the same in the reference's feature order (the host form's staging)
-struct DecTrainBufs {
-  float *raw[4], *dy[4], *stats, *sout;
-  double *part, *fsum, *bsum, *coef;
-};
-
-int ensure_dec_train_bufs(ian_handle* h, int n, DecTrainBufs* b) {
-  if (n > h->dec_tcap) {
-    CUDA_TRY(h, cudaDeviceSynchronize());
-    CUDA_TRY(h, cudaFree(h->dec_tbuf));
-    h->dec_tbuf = nullptr;
-    h->dec_tcap = 0;
-    const size_t bytes = (size_t)n * (2 * kDecTrainPerImg * sizeof(float) + 2 * 16384 * sizeof(double)) +
-                         (2 * kDecBnTotal + 2 * 16384 + 4 * 16384) * sizeof(double) + 4 * kDecBnTotal * sizeof(float);
-    CUDA_TRY(h, cudaMalloc((void**)&h->dec_tbuf, bytes));
-    h->dec_tcap = n;
-  }
-  const long long N = h->dec_tcap;
-  b->part = (double*)h->dec_tbuf;
-  b->fsum = b->part + N * 2 * 16384;
-  b->bsum = b->fsum + 2 * kDecBnTotal;
-  b->coef = b->bsum + 2 * 16384;
-  b->stats = (float*)(b->coef + 4 * 16384);
-  b->sout = b->stats + 2 * kDecBnTotal;
-  float* f = b->sout + 2 * kDecBnTotal;
-  for (int l = 0; l < 4; ++l) { b->raw[l] = f; f += N * kDecTrainElems[l]; }
-  for (int l = 0; l < 4; ++l) { b->dy[l] = f; f += N * kDecTrainElems[l]; }
-  return IAN_OK;
-}
-
-template <bool kVjp>
-int ensure_dec_train_plan(ian_handle* h, Plan* pl) {
-  int rc;
-  if (!pl->dectrain) {
-    for (int k = 0; k < 4; ++k)
-      if ((rc = build_twin(h, pl, DD_DEC_FC2 + k, kSimpleDecoder.fwd.l[k])) != IAN_OK) return rc;
-    pl->dectrain = true;
-  }
-  if (kVjp && !pl->dectrain_vjp) {
-    if ((rc = ensure_param_vjp_plan(h, pl)) != IAN_OK) return rc;
-    for (int k = 0; k < 3; ++k)
-      if ((rc = build_twin(h, pl, DD_BWD_CONV3 + k, kSimpleDecoder.bwd.l[k])) != IAN_OK) return rc;
-    pl->dectrain_vjp = true;
-  }
-  return IAN_OK;
-}
-
-const Planes& dec_planes(const Plan* pl, int l) { return l == 0 ? pl->h0 : l == 1 ? pl->h1 : l == 2 ? pl->h2 : pl->h3; }
-
-// layer l's batch-normalised, rectified output of the chunk at `off` -> its planes h_l
-int dec_train_act(ian_handle* h, const DecTrainBufs& b, int l, Plan* pl, int off, int cn, cudaStream_t st) {
-  ScopedTimer tm(h, T_DD_NORM, st);
-  const float* gb = h->dec_bn_gb;
-  const Planes& a = dec_planes(pl, l);
-  LAUNCH_TRY(h, launch_dec_bn_relu(b.raw[l] + off * kDecTrainElems[l], cn * kDecTrainElems[l], kDecTrainC[l], b.stats + kDecBnOff[l],
-                                   b.stats + kDecBnTotal + kDecBnOff[l], gb + kDecBnOff[l], gb + kDecBnTotal + kDecBnOff[l], h->passes,
-                                   a.p, a.plane, st));
-  return IAN_OK;
-}
-
-// forward (dy == nullptr): layer l's statistics into b.stats; backward: Σdy, Σdy·x into b.bsum, then the coefficients and
-// d beta / d gamma (out: the 13 gradient pointers, nullable)
-int dec_train_sums(ian_handle* h, const DecTrainBufs& b, int l, int n, const float* dy, float* const* out, cudaStream_t st) {
-  const double count = (double)n * kDecTrainHW[l];
-  const int C = kDecTrainC[l], off = kDecBnOff[l];
-  double* fsum = b.fsum + 2 * off;
-  if (!dy) {
-    ScopedTimer tm(h, T_DD_STATS, st);
-    LAUNCH_TRY(h, launch_disc_bn_sums(b.raw[l], b.raw[l], n, kDecTrainHW[l], C, count, kBnEps, b.part, fsum, b.stats + off,
-                                      b.stats + kDecBnTotal + off, st));
-    return IAN_OK;
-  }
-  {
-    ScopedTimer tm(h, T_DD_BN_BWD, st);
-    LAUNCH_TRY(h, launch_disc_bn_sums(dy, b.raw[l], n, kDecTrainHW[l], C, 0.0, kBnEps, b.part, b.bsum, nullptr, nullptr, st));
-    LAUNCH_TRY(h, launch_disc_bn_coef(fsum, b.bsum, count, kBnEps, h->dec_bn_gb + off, C, b.coef, st));
-  }
-  float *db = out[PV_BN0_B + 2 * l], *dg = out[PV_BN0_G + 2 * l];
-  if (db || dg) {
-    ScopedTimer tm(h, T_DD_BN_GRADS, st);
-    LAUNCH_TRY(h, launch_dec_bn_grads(fsum, b.bsum, count, kBnEps, C, l == 0 ? 1 : 0, db, dg, st));
-  }
-  return IAN_OK;
-}
+// get_output(l_out, {l_Z: z}) under deterministic=False: kDecStack on the latent planes, then dec_out as ever on h3.  The VJP
+// runs that forward, then per chunk the parameter VJP's dense seed (the seed image and dL/dh3 before the mask), dec_out's
+// weight gradient and bnorm_dc3's dy; the stack's backward with each layer's weight gradient (wgrad on its dx planes and its
+// training-mode input, chunks added in order) as the hook; d beta and d gamma from the kept sums; and per chunk
+// bnorm_dec_fc2's dx, l_dec_fc2's weight gradient and L_BWD_FC2 itself (unit scale already) for dz.
 
 // the forward to every layer's raw sums and statistics (h3's planes are left to the caller, per chunk)
 template <bool kVjp>
-int dec_train_forward(ian_handle* h, bool host, const float* z, int n, const DecTrainBufs& b, void* stream) {
-  const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
-  int rc = run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}}, ensure_dec_train_plan<kVjp>, [&](const Chunk& c) {
+int dec_train_forward(ian_handle* h, bool host, const float* z, int n, const BnBufs& b, void* stream) {
+  return bn_forward<kDecStack, kVjp>(h, host, {z, kLatentBytes, S_Z, IN}, n, b, stream, [&](const Chunk& c) {
     LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
-    return run_gemm_into(h, c.pl, DD_DEC_FC2, b.raw[0] + c.off * kDecTrainElems[0], c.st);
+    return (int)IAN_OK;
   });
-  if (rc != IAN_OK || (rc = dec_train_sums(h, b, 0, n, nullptr, nullptr, st)) != IAN_OK) return rc;
-  for (int l = 1; l < 4; ++l) {
-    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-      int r = ensure_dec_train_plan<kVjp>(h, pl);
-      if (r == IAN_OK) r = dec_train_act(h, b, l - 1, pl, off, cn, st);
-      return r != IAN_OK ? r : run_gemm_into(h, pl, DD_DEC_FC2 + l, b.raw[l] + off * kDecTrainElems[l], st);
-    });
-    if (rc != IAN_OK || (rc = dec_train_sums(h, b, l, n, nullptr, nullptr, st)) != IAN_OK) return rc;
-  }
-  return IAN_OK;
 }
 
 int check_decode_train(ian_handle* h, int n) {
@@ -3264,15 +3222,15 @@ int call_decode_train(ian_handle* h, bool host, const float* z, int n, float* x_
   if (!z || !x_hat) return fail(h, IAN_ERR_INVALID, "NULL tensor pointer");
   DeviceGuard dg(h->device);
   const cudaStream_t st = !host && stream ? (cudaStream_t)stream : h->stream;
-  DecTrainBufs b;
-  if ((rc = ensure_dec_train_bufs(h, n, &b)) != IAN_OK || (rc = dec_train_forward<false>(h, host, z, n, b, stream)) != IAN_OK)
+  BnBufs b;
+  if ((rc = ensure_bn_bufs(h, kDecStack, n, &b)) != IAN_OK || (rc = dec_train_forward<false>(h, host, z, n, b, stream)) != IAN_OK)
     return rc;
   if (stats) {
     LAUNCH_TRY(h, launch_dec_stats_out(b.stats, kDecBnTotal, 16384, host ? b.sout : stats, st));
     if (host) CUDA_TRY(h, cudaMemcpyAsync(stats, b.sout, 2 * kDecBnTotal * sizeof(float), cudaMemcpyDeviceToHost, st));
   }
-  return run_entry(h, host, stream, n, {{x_hat, kImageBytes, S_XHAT, OUT}}, ensure_dec_train_plan<false>, [&](const Chunk& c) {
-    const int r = dec_train_act(h, b, 3, c.pl, c.off, c.cn, c.st);
+  return run_entry(h, host, stream, n, {{x_hat, kImageBytes, S_XHAT, OUT}}, ensure_bn_plan<kDecStack, false>, [&](const Chunk& c) {
+    const int r = bn_act(h, kDecStack, b, 3, c.pl, c.off, c.cn, c.st);
     return r != IAN_OK ? r : run_dec_out(h, c.pl, c.f(0), c.st);
   });
 }
@@ -3293,14 +3251,14 @@ int call_decode_train_vjp(ian_handle* h, bool host, const float* z, const float*
     if (!h->pv_dev[k]) CUDA_TRY(h, cudaMalloc((void**)&h->pv_dev[k], (size_t)kPvSize[k] * 4));
     out[k] = h->pv_dev[k];
   }
-  DecTrainBufs b;
-  if ((rc = ensure_dec_train_bufs(h, n, &b)) != IAN_OK || (rc = dec_train_forward<true>(h, host, z, n, b, stream)) != IAN_OK)
+  const BnStack& S = kDecStack;
+  BnBufs b;
+  if ((rc = ensure_bn_bufs(h, S, n, &b)) != IAN_OK || (rc = dec_train_forward<true>(h, host, z, n, b, stream)) != IAN_OK)
     return rc;
-  const float* gb = h->dec_bn_gb;
   // h3, x_hat and the seed per chunk: dec_out's weight gradient, and bnorm_dc3's dy from dL/dh3 and the training-mode mask
-  rc = run_entry(h, host, stream, n, {{dx_hat, kImageBytes, S_TARGET, IN}}, ensure_dec_train_plan<true>, [&](const Chunk& c) {
+  rc = run_entry(h, host, stream, n, {{dx_hat, kImageBytes, S_TARGET, IN}}, ensure_bn_plan<kDecStack, true>, [&](const Chunk& c) {
     Plan* pl = c.pl;
-    int r = dec_train_act(h, b, 3, pl, c.off, c.cn, c.st);
+    int r = bn_act(h, S, b, 3, pl, c.off, c.cn, c.st);
     if (r == IAN_OK) r = run_dec_out(h, pl, pl->xhat, c.st);
     if (r != IAN_OK) return r;
     {
@@ -3313,47 +3271,36 @@ int call_decode_train_vjp(ian_handle* h, bool host, const float* z, const float*
       LAUNCH_TRY(h, launch_decout_wgrad(pl->pseed, pl->h3.p, pl->h3.plane, c.cn, pl->ppart, out[PV_OUT], c.off > 0, c.st));
     }
     ScopedTimer tm(h, T_DD_COTANGENT, c.st);
-    const int o = kDecBnOff[3];
-    LAUNCH_TRY(h, launch_dec_train_dy(pl->dh3.p, pl->dh3.plane, b.raw[3] + c.off * kDecTrainElems[3], c.cn * kDecTrainElems[3],
-                                      kDecTrainC[3], b.stats + o, b.stats + kDecBnTotal + o, gb + o, gb + kDecBnTotal + o,
-                                      b.dy[3] + c.off * kDecTrainElems[3], c.st));
+    const float* gb = h->dec_bn_gb + S.off[3];
+    const long long e = bn_elems(S, 3);
+    LAUNCH_TRY(h, launch_dec_train_dy(pl->dh3.p, pl->dh3.plane, b.raw[3] + c.off * e, c.cn * e, S.C[3], b.stats + S.off[3],
+                                      b.stats + S.total + S.off[3], gb, gb + S.total, bn_dy(S, b, 3) + c.off * e, c.st));
     return (int)IAN_OK;
   });
   if (rc != IAN_OK) return rc;
-  // dL/d(raw sum) of layer l for the chunk -> its split planes d_l, then layer l's weight gradient (A: the layer's input)
-  auto grad_planes = [&](Plan* pl, int l, int off, int cn, cudaStream_t s) {
-    const Planes& d = l == 0 ? pl->d0 : l == 1 ? pl->d1 : l == 2 ? pl->d2 : pl->d3;
-    {
-      ScopedTimer tm(h, T_DD_BN_DX, s);
-      LAUNCH_TRY(h, launch_disc_bn_dx(b.raw[l] + off * kDecTrainElems[l], b.dy[l] + off * kDecTrainElems[l], cn * kDecTrainElems[l],
-                                      kDecTrainC[l], b.coef, h->passes, d.p, d.plane, s));
-    }
-    if (l > 0) {
-      const int r = dec_train_act(h, b, l - 1, pl, off, cn, s);
-      if (r != IAN_OK) return r;
-    }
+  // layer l's weight gradient from its dx planes and its input planes
+  auto wgrad = [&](Plan* pl, int l, int off, int) {
     if (!out[PV_FC2 + l]) return (int)IAN_OK;
     {
-      ScopedTimer tm(h, T_WGRAD_FC2 + l, s);
-      if (h->path == IAN_PATH_TC) LAUNCH_TRY(h, launch_wgrad_tc(pl->wg[l], pl->wmaps[l], s));
-      else LAUNCH_TRY(h, launch_wgrad_simt(pl->wg[l], s));
+      ScopedTimer tm(h, T_WGRAD_FC2 + l, st);
+      if (h->path == IAN_PATH_TC) LAUNCH_TRY(h, launch_wgrad_tc(pl->wg[l], pl->wmaps[l], st));
+      else LAUNCH_TRY(h, launch_wgrad_simt(pl->wg[l], st));
     }
-    LAUNCH_TRY(h, launch_wgrad_finalize(pl->wg[l], l == 0 ? WG_FC2 : WG_DECONV, out[PV_FC2 + l], off > 0, s));
+    LAUNCH_TRY(h, launch_wgrad_finalize(pl->wg[l], l == 0 ? WG_FC2 : WG_DECONV, out[PV_FC2 + l], off > 0, st));
     return (int)IAN_OK;
   };
-  for (int l = 3; l >= 1; --l) {
-    if ((rc = dec_train_sums(h, b, l, n, b.dy[l], out, st)) != IAN_OK) return rc;
-    rc = for_chunks(h, n, [&](Plan* pl, int off, int cn) {
-      int r = ensure_dec_train_plan<true>(h, pl);
-      if (r == IAN_OK) r = grad_planes(pl, l, off, cn, st);
-      return r != IAN_OK ? r : run_gemm_into(h, pl, DD_BWD_CONV3 + (3 - l), b.dy[l - 1] + off * kDecTrainElems[l - 1], st);
-    });
-    if (rc != IAN_OK) return rc;
+  if ((rc = bn_backward(h, S, b, n, st, wgrad)) != IAN_OK) return rc;
+  for (int l = 0; l < S.L; ++l) {
+    float *db = out[PV_BN0_B + 2 * l], *dg = out[PV_BN0_G + 2 * l];
+    if (!db && !dg) continue;
+    ScopedTimer tm(h, T_DD_BN_GRADS, st);
+    LAUNCH_TRY(h, launch_dec_bn_grads(b.fsum + 2 * S.off[l], b.bsum + 2 * S.off[l], (double)n * S.HW[l], kBnEps, S.C[l], l == 0 ? 1 : 0,
+                                      db, dg, st));
   }
-  if ((rc = dec_train_sums(h, b, 0, n, b.dy[0], out, st)) != IAN_OK) return rc;
-  rc = run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}}, ensure_dec_train_plan<true>, [&](const Chunk& c) {
+  rc = run_entry(h, host, stream, n, {{z, kLatentBytes, S_Z, IN}}, ensure_bn_plan<kDecStack, true>, [&](const Chunk& c) {
     LAUNCH_TRY(h, launch_z_to_planes(c.f(0), c.pl->zp.p, c.pl->zp.plane, c.cn, c.st));
-    int r = grad_planes(c.pl, 0, c.off, c.cn, c.st);
+    int r = bn_dx(h, S, b, 0, c.pl, c.off, c.cn, c.st);
+    if (r == IAN_OK) r = wgrad(c.pl, 0, c.off, c.cn);
     if (r == IAN_OK) r = run_gemm(h, c.pl, L_BWD_FC2, c.st);
     return r != IAN_OK ? r : copy_dz(c, dz);
   });
@@ -3842,9 +3789,8 @@ int ian_destroy(ian_handle* h) {
   for (float* p : h->disc_w) cudaFree(p);
   cudaFree(h->disc_buf);
   cudaFree(h->enc_bn_gb);
-  cudaFree(h->disc_tbuf);
   cudaFree(h->dec_bn_gb);
-  cudaFree(h->dec_tbuf);
+  for (auto& s : h->bn_bufs) cudaFree(s.buf);
   for (auto& v : h->timed) for (auto& t : v) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
   if (h->push_stream) { cudaStreamSynchronize(h->push_stream); cudaStreamDestroy(h->push_stream); }
   for (int b = 0; b < 2; ++b) { if (h->g_comp[b]) cudaEventDestroy(h->g_comp[b]); if (h->g_done[b]) cudaEventDestroy(h->g_done[b]); }

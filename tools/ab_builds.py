@@ -18,6 +18,10 @@
         the eight latent-fit entry points (normal equations and fits: plain; masked with and without weights; robust,
         Huber and Cauchy, automatic and given scale, with outliers; features at weights (1, 1), (0, 1), (1, 0)) in both
         forms with 3 steps, each call's launch_count() delta one more array, at batches 1 and 3, and 20 under IAN_CHUNK=16.
+        And the entry points whose batch is coupled, in both forms, each call's launch_count() delta one more array, at
+        every batch above and at 20 under IAN_CHUNK=16: the discriminator (tests/test_gpu_discriminate_train.py's seeded
+        head) in inference and in training mode, forward with the statistics and VJP; on IAN_simple the training-mode
+        decoder, x_hat with the statistics and its VJP with all 13 gradients and with l_dec_fc2.W's alone.
 """
 import argparse
 import hashlib
@@ -136,6 +140,21 @@ FIT_BATCHES = (1, 3)                       # a fit costs one batch-100 JVP pass 
 FIT_ITERS = 3
 
 
+def _counted(m, out, name, f, *res):
+    """runs f(), one entry point; appends to out its arrays -- what f returns (host form) or the device tensors res (device
+    form) -- and its launch_count() delta; returns what f returned"""
+    import numpy as np
+    import torch
+    c0 = m.launch_count()
+    torch.cuda.synchronize()
+    r = f()
+    torch.cuda.synchronize()
+    arrays = [a.cpu().numpy() for a in res] if res else list(r if isinstance(r, tuple) else (r,))
+    out.extend(("%s %d" % (name, i), a) for i, a in enumerate(arrays))
+    out.append((name + " launches", np.array([m.launch_count() - c0])))
+    return r
+
+
 def _fit_arrays(m, n, seed):
     """(name, array) of every latent-fit entry point in its host and its device form on seeded inputs, each call
     followed by its launch_count() delta"""
@@ -159,14 +178,7 @@ def _fit_arrays(m, n, seed):
         return a
 
     def call(name, f, *res):
-        """f() runs one entry; its arrays are what it returns (host form) or the tensors res (device form)"""
-        c0 = m.launch_count()
-        torch.cuda.synchronize()
-        r = f()
-        torch.cuda.synchronize()
-        arrays = [a.cpu().numpy() for a in res] if res else list(r if isinstance(r, tuple) else (r,))
-        out.extend(("%s %d" % (name, i), a) for i, a in enumerate(arrays))
-        out.append((name + " launches", np.array([m.launch_count() - c0])))
+        _counted(m, out, name, f, *res)
 
     def gn(name, host, dev):
         A, g, e = t(n, 100, 100, f64=True), t(n, 100, f64=True), t(n, f64=True)
@@ -208,12 +220,63 @@ def _fit_arrays(m, n, seed):
     return out
 
 
+def _train_arrays(m, n, seed):
+    """(name, array) of the discriminator's entry points, inference and training mode (the head loaded), and on IAN_simple
+    of the training-mode decoder's (x_hat with stats; dz with all 13 gradients, and with l_dec_fc2.W's alone), in their host
+    and their device form on seeded inputs, each call followed by its launch_count() delta"""
+    import importlib
+    import numpy as np
+    import test_gpu_launch_forms as lf
+    rng = np.random.default_rng(seed)
+    U = m.discriminator_units()
+    x = np.tanh(rng.standard_normal((n, 3, 64, 64))).astype(np.float32)
+    dl = rng.standard_normal((n, U)).astype(np.float32)
+    d = lf._Dev()
+    xp, dlp = d.put(x), d.put(dl)
+    out = []
+
+    def call(name, f, *res):
+        return _counted(m, out, name, f, *res)
+
+    lg, p = d.empty((n, U)), d.empty((n, U))
+    call("discriminate host", lambda: m.discriminate(x, return_logits=True))
+    call("discriminate dev", lambda: m.discriminate_dev(xp, n, lg.data_ptr(), p.data_ptr()), lg, p)
+    dx = d.empty((n, 3, 64, 64))
+    call("discriminate_vjp host", lambda: m.discriminate_vjp(x, dl))
+    call("discriminate_vjp dev", lambda: m.discriminate_vjp_dev(xp, dlp, n, dx.data_ptr()), dx)
+    lg, p, st = d.empty((n, U)), d.empty((n, U)), d.empty((2, 1792))
+    call("discriminate_train host", lambda: m.discriminate_train(x, return_logits=True, return_stats=True))
+    call("discriminate_train dev", lambda: m.discriminate_train_dev(xp, n, lg.data_ptr(), p.data_ptr(), st.data_ptr()), lg, p, st)
+    dx = d.empty((n, 3, 64, 64))
+    call("discriminate_train_vjp host", lambda: m.discriminate_train_vjp(x, dl))
+    call("discriminate_train_vjp dev", lambda: m.discriminate_train_vjp_dev(xp, dlp, n, dx.data_ptr()), dx)
+    if m.kind != importlib.import_module("neural-photo-editor_b200._lib").IAN_MODEL_SIMPLE:
+        return out
+    z = rng.standard_normal((n, 100)).astype(np.float32)
+    dxh = rng.standard_normal((n, 3, 64, 64)).astype(np.float32)
+    zp, dxhp = d.put(z), d.put(dxh)
+    xh, st = d.empty((n, 3, 64, 64)), d.empty((2, 17280))
+    call("decode_train host", lambda: m.decode_train(z, return_stats=True))
+    call("decode_train dev", lambda: m.decode_train_dev(zp, n, xh.data_ptr(), st.data_ptr()), xh, st)
+    def vjp_host(names):
+        dz, g = m.decode_train_vjp(z, dxh, names)
+        return (dz,) + tuple(g[k] for k in names)
+
+    for tag, names in (("all", m.param_vjp_names()), ("fc2_W", ["l_dec_fc2.W"])):
+        r = call("decode_train_vjp_%s host" % tag, lambda: vjp_host(names))
+        dz, g = d.empty((n, 100)), [d.empty(a.shape) for a in r[1:]]
+        call("decode_train_vjp_%s dev" % tag,
+             lambda: m.decode_train_vjp_dev(zp, dxhp, n, dz.data_ptr(), {k: t.data_ptr() for k, t in zip(names, g)}), dz, *g)
+    return out
+
+
 def cmd_dump(out):
     """child of `outputs`: sha256 and sum of |a| of every array, for the build IAN_B200_LIB names"""
     import importlib
     import numpy as np
     sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
     import ctypes
+    import discrim_train_oracle as dto
     import test_gpu_launch_forms as lf
     lib = importlib.import_module("neural-photo-editor_b200._lib")
     so = ctypes.CDLL(lib.LIB_PATH)
@@ -221,6 +284,7 @@ def cmd_dump(out):
         if not hasattr(so, name):
             del lib.SIGNATURES[name]
     npe = importlib.import_module("neural-photo-editor_b200")
+    heads = {g: f[2] for g, f in dto.fixture().items()}    # tests/test_gpu_discriminate_train.py's seeded heads
     res = {}
 
     def record(cfg, n, arrays):
@@ -234,6 +298,7 @@ def cmd_dump(out):
                 os.environ.pop(k, None)
             os.environ.update(env)
             m = npe.IAN(lf.CONFIG[graph], True, weights=lf._weights(graph), path=path)
+            m.load_discriminator(heads[graph])
             cfg = "%s-%s%s" % (graph, path, "".join("-%s=%s" % kv for kv in env.items()))
             for n in OUTPUT_BATCHES:
                 arrays = [("%s %s" % (name, form), a) for name, host, dev in lf._pairs(m, npe, lf._inputs(n, 7000 + n))
@@ -245,14 +310,16 @@ def cmd_dump(out):
                 arrays += [("Zfn host", m.Zfn(x)), ("Z_IAF_fn host", m.Z_IAF_fn(zi)), ("sample host", m.sample(zi))]
                 if n in FIT_BATCHES:
                     arrays += _fit_arrays(m, n, 7200 + n)
+                arrays += _train_arrays(m, n, 7300 + n)
                 record(cfg, n, arrays)
             m.close()
-        # the fits over two chunks, of 16 and 4 samples
+        # the fits and the coupled-batch entries over two chunks, of 16 and 4 samples
         for k in lf.ENV:
             os.environ.pop(k, None)
         os.environ["IAN_CHUNK"] = "16"
         m = npe.IAN(lf.CONFIG[graph], True, weights=lf._weights(graph), path="tc")
-        record("%s-tc-IAN_CHUNK=16" % graph, 20, _fit_arrays(m, 20, 7220))
+        m.load_discriminator(heads[graph])
+        record("%s-tc-IAN_CHUNK=16" % graph, 20, _fit_arrays(m, 20, 7220) + _train_arrays(m, 20, 7320))
         m.close()
         os.environ.pop("IAN_CHUNK")
     with open(out, "w") as f:
